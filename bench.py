@@ -8,10 +8,11 @@ workload's point sets.  Default workload: BASELINE.json configs[1] -- 2-D Poisso
 shard of a 128 x (128 N) grid (weak scaling).  --config cfg3 | cfg4 | cfg5 runs the other BASELINE
 configurations, each with its own roofline / e2e / cpu_baseline (see build_workload).
 
-  python bench.py --gpus N --steps K --warmup W [--config cfgK]            # our engine
-  python bench.py --impl reference --gpus N --steps K ... [--config cfgK]  # CPU restatement of the reference
+  python bench.py --gpus N --steps K --warmup W [--config cfgK] [--dump-outputs DIR]   # our engine
+  python bench.py --impl reference --gpus N --steps K ... [--config cfgK]               # CPU restatement of the reference
 
-Prints ONE JSON line (see the contract in the task statement).
+Prints ONE JSON line.  --dump-outputs DIR writes what the last timed step returned (gradient, term losses, total loss) as
+DIR/<name>.npy, so that two builds can be compared output for output on the same seeded inputs.
 """
 from __future__ import annotations
 
@@ -39,7 +40,8 @@ def peaks():
         with open(p) as f:
             d = json.load(f)
         return d, "measured"
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0}, "fallback"
+    # NVIDIA H100 SXM data sheet (700 W): HBM3 3.35 TB/s, dense BF16 989 TFLOP/s
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0}, "datasheet"
 
 
 class ClockSampler:
@@ -305,7 +307,7 @@ def run_ours(args, rank: int, local_rank: int, world: int):
     grad_d = torch.empty(n_theta, dtype=torch.float32, device=dev)
     terms_d = torch.empty(n_terms, dtype=torch.float32, device=dev)
     total_d = torch.empty(1, dtype=torch.float32, device=dev)
-    flush = torch.empty(256 * 1024 * 1024 // 4, dtype=torch.float32, device=dev)   # 256 MiB > 126 MB L2
+    flush = torch.empty(256 * 1024 * 1024 // 4, dtype=torch.float32, device=dev)   # 256 MiB > 50 MB L2
     stream = torch.cuda.current_stream().cuda_stream
 
     def step():
@@ -339,6 +341,10 @@ def run_ours(args, rank: int, local_rank: int, world: int):
     t_total = float(ms.sum()) * 1e-3
     loss_val = float(total_d.item())
     grad_h = grad_d.cpu().numpy().astype(np.float64)
+    if args.dump_outputs and rank == 0:
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        for name, t in (("grad", grad_d), ("term_losses", terms_d), ("loss", total_d)):
+            np.save(os.path.join(args.dump_outputs, name + ".npy"), t.cpu().numpy().astype(np.float32))
 
     # ---- main-kernel duration (for the roofline), events inside the library around the fused kernel ----
     eng.set_timing(True)
@@ -374,16 +380,7 @@ def run_ours(args, rank: int, local_rank: int, world: int):
         wide = mode != "ffma" and max(max(c.dims[1:-1]) for c in cfg.chains) > 64
         kernel = KERNEL_OF["ffma" if mode == "ffma" else ("wide" if wide else "narrow")]
         tensor_bound = mode != "ffma"
-        peak = pk["bf16_tflops"] if tensor_bound else 74.0            # fp32 FMA: 148 SMs x 128 lanes x 2 x 1.965 GHz
-        # DRAM traffic of the dominant kernel: measured once per round with `ncu --set full` (profiles/), not re-measured here
-        traffic, traffic_src = None, None
-        try:
-            with open(os.path.join(ROOT, "profiles", "r02_ncu_traffic.json")) as fh:
-                ent = json.load(fh).get("%s_%s_n%d" % (args.config, mode, args.n))
-            if ent and world == 1:
-                traffic, traffic_src = int(ent["dram_bytes_read"]) + int(ent["dram_bytes_write"]), ent["source"]
-        except (OSError, ValueError, KeyError):
-            pass
+        peak = pk["bf16_tflops"] if tensor_bound else 67.0            # fp32 FMA, H100 SXM data sheet
         line = {
             "metric": METRIC, "value": value, "unit": UNIT, "n_gpus": world, "steps": args.steps,
             "warmup": max(args.warmup, 3), "ms_per_step": 1e3 * t_total / args.steps, "higher_is_better": True,
@@ -400,11 +397,10 @@ def run_ours(args, rank: int, local_rank: int, world: int):
                     "ms_per_step": 1e3 * t_e2e / args.steps, "api": "pinn_loss_grad_host"},
             "gpu_launches": int(launches),
             "roofline": {"bound": "tensor" if tensor_bound else "fp32-fma", "achieved": achieved, "peak": peak, "unit": "TFLOP/s",
-                         "frac": achieved / peak, "traffic": traffic, "traffic_unit": "bytes (DRAM read + write per launch, ncu)",
-                         "traffic_source": traffic_src, "peak_source": pk_kind if tensor_bound else "nominal fp32 FMA",
+                         "frac": achieved / peak, "peak_source": pk_kind if tensor_bound else "datasheet",
                          "kernel": kernel,
-                         "arithmetic": {"ffma": "fp32 FMA on CUDA cores", "tc_bf16": "tcgen05 bf16 x bf16 -> fp32",
-                                        "tc_split": "tcgen05 split-bf16 (3 MMAs per product in the forward sweep)"}[mode],
+                         "arithmetic": {"ffma": "fp32 FMA on CUDA cores", "tc_bf16": "wgmma bf16 x bf16 -> fp32",
+                                        "tc_split": "wgmma split-bf16 (3 MMAs per product in the forward sweep)"}[mode],
                          "kernel_ms": kernel_ms, "flops_per_launch": flops,
                          "note": "algorithmic FLOPs 6*C*S per point (SURVEY 8(d)) / fused-kernel duration (the kernel "
                                  "includes the in-kernel gradient reduction%s)" % (" and peer sum" if fused_p2p else "")},
@@ -475,6 +471,8 @@ def main():
     ap.add_argument("--scaling", default="weak", choices=["weak", "strong"])
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-alt-modes", action="store_true")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the last timed step's gradient, term losses and loss as DIR/<name>.npy (float32)")
     args = ap.parse_args()
     # stdout carries exactly one JSON line: NCCL's version banner / debug output (printed to stdout when NCCL_DEBUG is
     # set in the environment) goes to stderr instead

@@ -50,7 +50,7 @@ check(rc) = rc == 0 || throw(ArgumentError(unsafe_string(@ccall lib.pinn_last_er
     B200PINN(inner::PhysicsInformedNN; mode = :tc_split)
 
 Sibling discretizer (extension rule: src/NeuralPDE.jl:64-71).  `mode`: `:ffma` (fp32 / fp64 parity path),
-`:tc_bf16`, `:tc_split` (tcgen05 paths, Float32 theta).
+`:tc_bf16`, `:tc_split` (tensor-core paths, Float32 theta).
 """
 struct B200PINN{P <: PhysicsInformedNN} <: AbstractPINN
     inner::P

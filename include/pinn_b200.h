@@ -1,5 +1,5 @@
 /*
- * pinn_b200.h -- C ABI of the B200-native PINN residual/loss engine.
+ * pinn_b200.h -- C ABI of the H100-native PINN residual/loss engine.
  *
  * This is the drop-in boundary for NeuralPDE.jl's PhysicsInformedNN hot path
  * (SURVEY.md section 8(b), boundary B1).  The reference has no FFI of its own:
@@ -72,15 +72,15 @@ typedef struct pinn_engine* pinn_handle;
 enum { PINN_F32 = 0, PINN_F64 = 1 };
 
 /* arithmetic mode of the layer contractions.
- * Shapes the tcgen05 modes accept (anything else: pinn_create fails with a message, never a silent fallback):
+ * Shapes the tensor-core modes accept (anything else: pinn_create fails with a message, never a silent fallback):
  *   1-output networks, linear last layer, >= 2 Dense layers, PINN_F32, <= 6 taps per term, and either
  *     - every hidden width in {16, 32, 48, 64} and <= 5 propagated channels per (term, network)      [both modes], or
  *     - every hidden width in {64, 128}, at least one hidden->hidden layer; terms that need more than 4 channels
  *       are evaluated in several passes over the same weights (pure second derivatives only)   [PINN_MODE_TC_BF16]. */
 enum {
   PINN_MODE_FFMA = 0,      /* CUDA-core FMA in the scalar type (parity mode, fp32 / fp64)   */
-  PINN_MODE_TC_BF16 = 1,   /* tcgen05, bf16 operands, fp32 accumulate                        */
-  PINN_MODE_TC_SPLIT = 2   /* tcgen05, split-bf16 x2 (3 MMAs per product), fp32 accumulate   */
+  PINN_MODE_TC_BF16 = 1,   /* wgmma, bf16 operands, fp32 accumulate                          */
+  PINN_MODE_TC_SPLIT = 2   /* wgmma, split-bf16 x2 (3 MMAs per product), fp32 accumulate     */
 };
 
 /* activations (Lux Dense: act.(W*x .+ b)) */

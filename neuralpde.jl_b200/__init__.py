@@ -1,4 +1,4 @@
-"""neuralpde.jl_b200 -- B200-native PINN residual/loss engine behind NeuralPDE.jl's
+"""neuralpde.jl_b200 -- H100-native PINN residual/loss engine behind NeuralPDE.jl's
 PhysicsInformedNN / discretize interface.
 
 The directory name contains a dot, so import it through the root-level alias module:

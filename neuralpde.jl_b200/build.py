@@ -1,4 +1,4 @@
-"""Build libpinn_b200.so (sm_100a) in-tree with nvcc.
+"""Build libpinn_b200.so (sm_90a) in-tree with nvcc.
 
 The library is the C-ABI product (include/pinn_b200.h).  Objects are rebuilt only when a
 source or header is newer, and translation units compile in parallel.
@@ -19,7 +19,7 @@ LIB = os.path.join(LIBDIR, "libpinn_b200.so")
 INCLUDE = os.path.join(os.path.dirname(HERE), "include")
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC",
     "-I", INCLUDE,
@@ -52,19 +52,15 @@ def _deps_mtime() -> float:
     return m
 
 
-def _extra_units(debug: bool):
-    """tcgen05 translation units; the descriptor probe (tc_probe.cu) only in debug builds."""
-    extra = []
-    for f in sorted(os.listdir(CSRC)):
-        if f.startswith("tc_") and f.endswith(".cu") and (debug or f != "tc_probe.cu"):
-            extra.append((f[:-3] + ".o", f, []))
-    return extra
+def _extra_units():
+    """tensor-core translation units (tc_*.cu)."""
+    return [(f[:-3] + ".o", f, []) for f in sorted(os.listdir(CSRC)) if f.startswith("tc_") and f.endswith(".cu")]
 
 
 def build(verbose: bool = False, force: bool = False, defines=(), debug: bool = False) -> str:
     """Default: the product library lib/libpinn_b200.so (no instrumentation).
-    debug=True: lib/libpinn_b200_debug.so with -DPINN_DEBUG (phase timestamps for scripts/tc_timeline.py, the tcgen05
-    descriptor probe for scripts/tc_probe*.py).  defines=("NAME=VAL", ...): a measurement variant
+    debug=True: lib/libpinn_b200_debug.so with -DPINN_DEBUG (phase timestamps for scripts/tc_timeline.py and
+    scripts/tail_timeline.py).  defines=("NAME=VAL", ...): a measurement variant
     lib/libpinn_b200_<tag>.so built in build_<tag>/ (select it with PINN_B200_LIB)."""
     objdir, lib, flags = OBJDIR, LIB, list(NVCC_FLAGS)
     tag = ("debug" if debug else "") + "".join(d.replace("=", "") for d in defines)
@@ -76,7 +72,7 @@ def build(verbose: bool = False, force: bool = False, defines=(), debug: bool = 
     os.makedirs(objdir, exist_ok=True)
     nvcc = _nvcc()
     hdr_m = _deps_mtime()
-    units = UNITS + _extra_units(debug)
+    units = UNITS + _extra_units()
     jobs = []
     for obj, src, defs in units:
         o = os.path.join(objdir, obj)
@@ -97,7 +93,7 @@ def build(verbose: bool = False, force: bool = False, defines=(), debug: bool = 
                     raise RuntimeError("nvcc failed: %s\n%s\n%s" % (" ".join(cmd), r.stdout, r.stderr))
     objs = [os.path.join(objdir, u[0]) for u in units]
     if jobs or not os.path.exists(lib) or any(os.path.getmtime(o) > os.path.getmtime(lib) for o in objs):
-        cmd = [nvcc, "-gencode", "arch=compute_100a,code=sm_100a", "-shared", "-o", lib, *objs, "-ldl"]
+        cmd = [nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-shared", "-o", lib, *objs, "-ldl"]
         r = subprocess.run(cmd, capture_output=True, text=True)
         if r.returncode != 0:
             raise RuntimeError("link failed: %s\n%s\n%s" % (" ".join(cmd), r.stdout, r.stderr))

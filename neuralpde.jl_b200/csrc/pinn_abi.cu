@@ -124,6 +124,7 @@ struct pinn_engine {
   void* tw_wpack = nullptr;
   int* tw_counter = nullptr;
   void* tw_zstash = nullptr;
+  float* tc_acc = nullptr;       // tensor-core paths: per-CTA fp32 accumulator regions (tc_prims.cuh)
   // workspaces (device)
   void* partial = nullptr;
   double* term_sums = nullptr;
@@ -479,12 +480,12 @@ static int lower_problem(const pinn_problem_desc* d, pinn_engine* e) {
     return 0;
   }
 
-  // ---- tcgen05 path: supported-shape check and shared-memory plan -----------------------------------
-  if (d->dtype != PINN_F32) return fail("pinn_create: the tcgen05 modes compute in bf16/fp32 and need dtype PINN_F32");
+  // ---- tensor-core path: supported-shape check and shared-memory plan -----------------------------------
+  if (d->dtype != PINN_F32) return fail("pinn_create: the tensor-core modes compute in bf16/fp32 and need dtype PINN_F32");
   for (int t = 0; t < d->n_terms; ++t)
     for (int s2 = 0; s2 < P.terms[t].n_used; ++s2)
       if (P.terms[t].chan[s2].n3 > 0)
-        return fail("pinn_create(tc): term %d takes a third derivative; the tcgen05 path propagates derivatives up to order 2 "
+        return fail("pinn_create(tc): term %d takes a third derivative; the tensor-core path propagates derivatives up to order 2 "
                     "(use PINN_MODE_FFMA)", t);
   e->tc_split = d->mode == PINN_MODE_TC_SPLIT ? 1 : 0;
   e->tile_pts = kTcPts;
@@ -507,14 +508,14 @@ static int lower_problem(const pinn_problem_desc* d, pinn_engine* e) {
     for (int l = 1; l < n.n_layers; ++l) {
       const int w = n.dims[l];
       if (!wide && (w % 16 != 0 || w < 16 || w > 64))
-        return fail("pinn_create(tc): net %d hidden width %d unsupported by the tcgen05 path (16, 32, 48, 64, or 64/128 "
+        return fail("pinn_create(tc): net %d hidden width %d unsupported by the tensor-core path (16, 32, 48, 64, or 64/128 "
                     "with PINN_MODE_TC_BF16; use PINN_MODE_FFMA for other shapes)", k, w);
       if (wide && w != 64 && w != 128)
         return fail("pinn_create(tc): net %d hidden width %d: networks with layers wider than 64 need every hidden width "
-                    "to be 64 or 128 on the tcgen05 path (use PINN_MODE_FFMA for other shapes)", k, w);
+                    "to be 64 or 128 on the tensor-core path (use PINN_MODE_FFMA for other shapes)", k, w);
     }
     if (wide && n.n_layers < 3)
-      return fail("pinn_create(tc): net %d: the 128-wide tcgen05 path needs at least one hidden->hidden layer", k);
+      return fail("pinn_create(tc): net %d: the 128-wide tensor-core path needs at least one hidden->hidden layer", k);
   }
   if (wide && d->mode != PINN_MODE_TC_BF16)
     return fail("pinn_create(tc): PINN_MODE_TC_SPLIT supports hidden widths up to 64; 128-wide layers run in "
@@ -543,7 +544,7 @@ static int lower_problem(const pinn_problem_desc* d, pinn_engine* e) {
           continue;
         }
         if (!ch.pure)
-          return fail("pinn_create(tc): term %d needs %d channels including mixed second derivatives; the 128-wide tcgen05 "
+          return fail("pinn_create(tc): term %d needs %d channels including mixed second derivatives; the 128-wide tensor-core "
                       "path splits only pure second derivatives into passes (use PINN_MODE_FFMA)", t, ch.C);
         bool placed[PINN_MAX_IN] = {false};
         int left = ch.n1;
@@ -584,7 +585,7 @@ static int lower_problem(const pinn_problem_desc* d, pinn_engine* e) {
   int n_used_max = 1;
   for (int t = 0; t < d->n_terms; ++t) {
     const DevTerm& T = P.terms[t];
-    if (T.n_taps > kTcMaxTaps) return fail("pinn_create(tc): term %d has %d taps (tcgen05 path: max %d)", t, T.n_taps, kTcMaxTaps);
+    if (T.n_taps > kTcMaxTaps) return fail("pinn_create(tc): term %d has %d taps (tensor-core path: max %d)", t, T.n_taps, kTcMaxTaps);
     n_used_max = std::max(n_used_max, T.n_used);
     for (int s2 = 0; s2 < T.n_used; ++s2) {
       const DevChan& ch = T.chan[s2];
@@ -593,10 +594,10 @@ static int lower_problem(const pinn_problem_desc* d, pinn_engine* e) {
       bool found = false;
       for (int v : ok) found = found || v == key;
       if (wide && (ch.C > kTwMaxC || key == 32))
-        return fail("pinn_create(tc): term %d needs %d channels on a 128-wide network; the tcgen05 path propagates at most "
+        return fail("pinn_create(tc): term %d needs %d channels on a 128-wide network; the tensor-core path propagates at most "
                     "%d there (use PINN_MODE_FFMA)", t, ch.C, kTwMaxC);
       if (!found || ch.C > kTcMaxC)
-        return fail("pinn_create(tc): term %d needs %d first + %d second derivative channels; the tcgen05 path "
+        return fail("pinn_create(tc): term %d needs %d first + %d second derivative channels; the tensor-core path "
                     "propagates at most %d channels per network (use PINN_MODE_FFMA)", t, ch.n1, ch.n2, kTcMaxC);
     }
     for (int i = 0; i < T.n_taps; ++i)
@@ -634,7 +635,7 @@ static int lower_problem(const pinn_problem_desc* d, pinn_engine* e) {
     o2 += tc_misc_bytes(e->tc_mx_dim, e->tc_mx_taps);
     if (o2 + 1024 > (size_t)max_smem)
       return fail("pinn_create(tc): the problem needs %zu bytes of shared memory per CTA (limit %d): too many networks "
-                  "for the 128-wide tcgen05 path", o2, max_smem);
+                  "for the 128-wide tensor-core path", o2, max_smem);
     e->smem = o2;
     // per pass: inputs of the tl_max tensor layers + the last hidden activations (restored for multi-pass terms)
     e->tw_hstash_per_cta = (long long)n_used_max * (tl_max + 1) * kTwMaxC * kTwNB * kTileBytes;
@@ -666,7 +667,7 @@ static int lower_problem(const pinn_problem_desc* d, pinn_engine* e) {
   off += tc_misc_bytes(e->tc_mx_dim, e->tc_mx_taps);
   if (off + 1024 > (size_t)max_smem)   // + the kernel's static shared memory
     return fail("pinn_create(tc): the problem needs %zu bytes of shared memory per CTA (limit %d): too many "
-                "resident weight tiles / channels for the tcgen05 path", off, max_smem);
+                "resident weight tiles / channels for the tensor-core path", off, max_smem);
   e->smem = off;
   e->tc_stash_per_cta = (long long)n_used_max * std::max(tl_max, 1) * kTcMaxC * kTileBytes;
   return 0;
@@ -690,7 +691,7 @@ int pinn_destroy(pinn_handle e) {
   }
   if (e->comm && g_nccl.CommDestroy) g_nccl.CommDestroy(e->comm);
   void* ptrs[] = {e->dprob, e->partial, e->term_sums, e->stash, e->gbufs, e->packed, e->d_state, e->sym,
-                  e->d_theta, e->d_grad, e->d_out, e->adam_m, e->adam_v, e->tw_wpack, e->tw_zstash, e->tw_counter};
+                  e->d_theta, e->d_grad, e->d_out, e->adam_m, e->adam_v, e->tw_wpack, e->tw_zstash, e->tw_counter, e->tc_acc};
   for (void* p : ptrs) if (p) cudaFree(p);
   for (int t = 0; t < PINN_MAX_TERMS; ++t) {
     if (e->own_pts[t]) cudaFree(e->own_pts[t]);
@@ -732,7 +733,7 @@ int pinn_create(const pinn_problem_desc* d, pinn_handle* out) {
   e->n_terms = d->n_terms; e->n_theta = d->n_theta;
   if (lower_problem(d, e)) { pinn_destroy(e); return 1; }
   cudaDeviceGetAttribute(&e->num_sms, cudaDevAttrMultiProcessorCount, e->device);
-  if (e->num_sms <= 0) e->num_sms = 148;
+  if (e->num_sms <= 0) e->num_sms = 132;
 
 #define TRY_OR_DESTROY(x) do { if (x) { pinn_destroy(e); return 1; } } while (0)
   TRY_OR_DESTROY(dev_alloc((void**)&e->dprob, sizeof(DevProblem), e));
@@ -747,6 +748,7 @@ int pinn_create(const pinn_problem_desc* d, pinn_handle* out) {
     if (!e->bufs_smem) TRY_OR_DESTROY(dev_alloc(&e->gbufs, g * 2 * (size_t)e->buf_elems * e->es, e));
   } else {
     TRY_OR_DESTROY(dev_alloc(&e->stash, g * (size_t)e->tc_stash_per_cta, e));
+    TRY_OR_DESTROY(dev_alloc((void**)&e->tc_acc, g * (size_t)kAccCols * kAccRows * sizeof(float), e));
     if (e->tw) {
       TRY_OR_DESTROY(dev_alloc(&e->tw_zstash, g * (size_t)e->tw_zstash_per_cta * sizeof(float), e));
       TRY_OR_DESTROY(dev_alloc(&e->tw_wpack, (size_t)std::max(e->tw_n_images, 1) * kTwImgBytes, e));
@@ -896,7 +898,7 @@ static int launch_fused(pinn_engine* e, const FfmaArgs& a, int grid, cudaStream_
     w.hstash = (uint8_t*)e->stash; w.hstash_per_cta = e->tw_hstash_per_cta;
     w.zstash = (float*)e->tw_zstash; w.zstash_per_cta = e->tw_zstash_per_cta;
     w.wpack = (const uint8_t*)e->tw_wpack; w.tl_max = std::max(e->tc_tl_max, 1);
-    w.tile_begin = a.tile_begin; w.tile_end = a.tile_end; w.mode = a.mode; w.resid_out = (float*)a.resid_out;
+    w.tile_begin = a.tile_begin; w.tile_end = a.tile_end; w.mode = a.mode; w.resid_out = (float*)a.resid_out; w.acc = e->tc_acc;
     w.dbg = e->tc_dbg; w.tile_counter = e->tw_counter;
     w.off_P = e->tw_off_P; w.off_S = e->tw_off_S; w.off_misc = e->tw_off_misc; w.off_ones = e->tw_off_ones; w.off_nets = e->tw_off_nets; w.mx_dim = e->tc_mx_dim; w.mx_taps = e->tc_mx_taps;
     for (int k = 0; k < PINN_MAX_NETS; ++k) {
@@ -917,7 +919,7 @@ static int launch_fused(pinn_engine* e, const FfmaArgs& a, int grid, cudaStream_
   memset(&t, 0, sizeof t);
   t.prob = a.prob; t.theta = (const float*)a.theta; t.partial = (float*)a.partial; t.partial_stride = a.partial_stride; t.term_sums = a.term_sums;
   t.stash = (uint8_t*)e->stash; t.stash_per_cta = e->tc_stash_per_cta; t.split = e->tc_split; t.tl_max = std::max(e->tc_tl_max, 1);
-  t.tile_begin = a.tile_begin; t.tile_end = a.tile_end; t.mode = a.mode; t.resid_out = (float*)a.resid_out;
+  t.tile_begin = a.tile_begin; t.tile_end = a.tile_end; t.mode = a.mode; t.resid_out = (float*)a.resid_out; t.acc = e->tc_acc;
   t.off_P = e->tc_off_P; t.off_Q = e->tc_off_Q; t.off_misc = e->tc_off_misc; t.off_ones = e->tc_off_ones; t.mx_dim = e->tc_mx_dim; t.mx_taps = e->tc_mx_taps;
   t.dbg = e->tc_dbg;
   t.n_nets = e->hprob->n_nets; t.n_terms = e->n_terms; t.n_theta = e->n_theta;
@@ -1432,7 +1434,7 @@ const char* pinn_comm_info(pinn_handle e, int32_t* fused_p2p) {
 }
 
 #ifdef PINN_DEBUG
-// diagnostic (not part of the drop-in ABI): enable phase timestamps of CTA 0 in the tcgen05 kernel and
+// diagnostic (not part of the drop-in ABI): enable phase timestamps of CTA 0 in the tensor-core kernel and
 // read them back (2000 x int64: [0,1000) phase marks id << 48 | clock, [1000,2000) per-CTA
 // {globaltimer start, end, cycles, smid}); host_out == NULL only enables.
 int pinn_debug_tc_timeline(pinn_handle e, long long* host_out) {

@@ -1,6 +1,6 @@
-// tc_common.cuh -- device helpers shared by the tcgen05 kernels (tc_kernel.cu: widths <= 64, all operands resident;
-// tc_wide_kernel.cu: 128-wide layers, streamed weights): packed fp32x2 arithmetic, the forward-mode tap chain rule
-// and its adjoint, TMEM loads, swizzled-tile stores, warp reduce-scatter, MMA issue helpers, dispatch macro.
+// tc_common.cuh -- device helpers shared by the tensor-core kernels (tc_kernel.cu: widths <= 64, all operands resident;
+// tc_wide_kernel.cu: 128-wide layers, streamed weights): fp32x2 arithmetic, the forward-mode tap chain rule
+// and its adjoint, accumulator loads, swizzled-tile stores, warp reduce-scatter, MMA chains, dispatch macro.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -11,7 +11,8 @@
 namespace pinn {
 
 // ---- small helpers ---------------------------------------------------------------------------------
-constexpr int kNH = kTcThreads / 128;   // warps per TMEM lane quadrant: each takes 1/kNH of the columns
+constexpr int kNH = kTcThreads / 128;   // warps per 32-row quadrant of the accumulators: each takes 1/kNH of the columns
+static_assert(kTcThreads == 512, "the MMA chains are spread over four warpgroups");
 #ifndef PINN_TC_GW
 #define PINN_TC_GW 4
 #endif
@@ -84,27 +85,18 @@ __device__ __forceinline__ void store_half(uint32_t tile_hi, uint32_t tile_lo, i
   }
 }
 
-__device__ __forceinline__ void tmem_ld4(uint32_t taddr, float (&v)[4]) {
-#ifdef PINN_EXP_NO_LDTM
-  v[0] = __uint_as_float(taddr & 0x3fffffu) * 1e-9f; v[1] = v[0] + 1e-3f; v[2] = v[0] - 1e-3f; v[3] = v[0] * 0.5f;
-  return;
-#endif
-  uint32_t r[4];
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x4.b32 {%0,%1,%2,%3}, [%4];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3])
-               : "r"(taddr)
-               : "memory");
+// accumulator loads: columns col .. col + n - 1 of row (base + lane), see tc::acc_row
+__device__ __forceinline__ void acc_ld4(uint32_t aaddr, float (&v)[4]) {
+  const float* r = tc::acc_row(aaddr);
 #pragma unroll
-  for (int i = 0; i < 4; ++i) v[i] = __uint_as_float(r[i]);
+  for (int i = 0; i < 4; ++i) v[i] = r[i * kAccRows];
 }
-
-__device__ __forceinline__ void tmem_ld2(uint32_t taddr, float (&v)[2]) {
-  uint32_t r[2];
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x2.b32 {%0,%1}, [%2];" : "=r"(r[0]), "=r"(r[1]) : "r"(taddr) : "memory");
-  v[0] = __uint_as_float(r[0]); v[1] = __uint_as_float(r[1]);
+__device__ __forceinline__ void acc_ld2(uint32_t aaddr, float (&v)[2]) {
+  const float* r = tc::acc_row(aaddr);
+  v[0] = r[0]; v[1] = r[kAccRows];
 }
-__device__ __forceinline__ void tmem_ldg(uint32_t taddr, float (&v)[4]) { tmem_ld4(taddr, v); }
-__device__ __forceinline__ void tmem_ldg(uint32_t taddr, float (&v)[2]) { tmem_ld2(taddr, v); }
+__device__ __forceinline__ void acc_ldg(uint32_t aaddr, float (&v)[4]) { acc_ld4(aaddr, v); }
+__device__ __forceinline__ void acc_ldg(uint32_t aaddr, float (&v)[2]) { acc_ld2(aaddr, v); }
 
 // 2-column variant of store_half
 __device__ __forceinline__ void store_half(uint32_t tile_hi, uint32_t tile_lo, int row, int col0, const float (&v)[2],
@@ -118,13 +110,13 @@ __device__ __forceinline__ void store_half(uint32_t tile_hi, uint32_t tile_lo, i
   }
 }
 
-// ---- packed fp32x2 arithmetic (Blackwell FFMA2 / FMUL2 / FADD2): two columns per instruction ---------------
+// ---- fp32x2 arithmetic: two columns per value (component-wise fp32 instructions) ---------------
 struct P2 { float2 v; };
 __device__ __forceinline__ P2 mk2(float a, float b) { P2 r; r.v = make_float2(a, b); return r; }
 __device__ __forceinline__ P2 splat2(float a) { return mk2(a, a); }
-__device__ __forceinline__ P2 operator*(P2 a, P2 b) { P2 r; r.v = __fmul2_rn(a.v, b.v); return r; }
-__device__ __forceinline__ P2 operator+(P2 a, P2 b) { P2 r; r.v = __fadd2_rn(a.v, b.v); return r; }
-__device__ __forceinline__ P2 vfma(P2 a, P2 b, P2 c) { P2 r; r.v = __ffma2_rn(a.v, b.v, c.v); return r; }
+__device__ __forceinline__ P2 operator*(P2 a, P2 b) { return mk2(__fmul_rn(a.v.x, b.v.x), __fmul_rn(a.v.y, b.v.y)); }
+__device__ __forceinline__ P2 operator+(P2 a, P2 b) { return mk2(__fadd_rn(a.v.x, b.v.x), __fadd_rn(a.v.y, b.v.y)); }
+__device__ __forceinline__ P2 vfma(P2 a, P2 b, P2 c) { return mk2(__fmaf_rn(a.v.x, b.v.x, c.v.x), __fmaf_rn(a.v.y, b.v.y, c.v.y)); }
 __device__ __forceinline__ float vfma(float a, float b, float c) { return fmaf(a, b, c); }
 template <typename T> __device__ __forceinline__ T vsplat(float x);
 template <> __device__ __forceinline__ float vsplat<float>(float x) { return x; }
@@ -274,8 +266,7 @@ __device__ __forceinline__ void dbg_mark(CS* cs, int id) {
 struct Misc {   // carve-up of the misc region
   float *Xs, *taps, *tapbar, *scratch, *qws;
   double* tsum;
-  uint64_t *bar_mma, *bar_ld;
-  uint32_t* tmem_slot;
+  uint64_t* bar_ld;
 };
 // mx_dim / mx_taps: largest point dimension / tap count over the problem's terms (the arrays are sized to them)
 __device__ __forceinline__ Misc misc_of(uint8_t* m, int mx_dim, int mx_taps) {
@@ -286,9 +277,7 @@ __device__ __forceinline__ Misc misc_of(uint8_t* m, int mx_dim, int mx_taps) {
   r.scratch = reinterpret_cast<float*>(m);        m += kTcMaxC * kTcPts * 4;
   r.qws = reinterpret_cast<float*>(m);            m += kTcPts * 4;
   r.tsum = reinterpret_cast<double*>(m);          m += PINN_MAX_TERMS * 8;
-  r.bar_mma = reinterpret_cast<uint64_t*>(m);     m += 8;
-  r.bar_ld = reinterpret_cast<uint64_t*>(m);      m += 8;
-  r.tmem_slot = reinterpret_cast<uint32_t*>(m);
+  r.bar_ld = reinterpret_cast<uint64_t*>(m);
   return r;
 }
 
@@ -313,15 +302,28 @@ __device__ __forceinline__ void wait_bar(uint64_t* bar, uint32_t& phase) {
   phase ^= 1u;
 }
 
-// issue a chain of nk MMAs D (+)= A_k * B_k; descriptors advance by a_step / b_step bytes per k-step
-__device__ __forceinline__ void mma_chain(uint32_t d, uint64_t adesc, uint64_t bdesc, uint32_t a_step, uint32_t b_step, int nk,
+// a chain of nk MMAs D[128 x N] (+)= A_k * B_k into accumulator column d; descriptors advance by a_step / b_step bytes per
+// k-step.  CTA-collective: every thread calls it with the same arguments, and the two 64-row halves of D run on warpgroup
+// pair {0, 1} or {2, 3}, chosen by the parity of the set bits of d / 16.  Chains into the same columns therefore run on one
+// warpgroup in program order (an accumulating chain sees its predecessor's result without a barrier), and chains at any
+// power-of-two column stride (64 per channel in tc_kernel.cu, 128 in tc_wide_kernel.cu) alternate between the two pairs.
+// The second half reads rows 64..127 of a K-major A (+8 KB) or the next 64-column tile of an MN-major A (LBO); an MN-major
+// A with LBO = 0 has 64 rows and only the first half runs.  Results are visible to the CTA after the next __syncthreads.
+static __device__ __noinline__ void mma_chain(uint32_t d, uint64_t adesc, uint64_t bdesc, uint32_t a_step, uint32_t b_step, int nk,
                                           uint32_t idesc, uint32_t acc_first) {
-  const uint64_t da = a_step >> 4, db = b_step >> 4;
+  const int n = (int)(idesc & 0xffu), ta = (int)((idesc >> 8) & 1u), tb = (int)((idesc >> 9) & 1u);
+  const uint32_t dcol = d & 0xffffu, j = dcol >> 4;
+  const uint32_t lbo = (uint32_t)((adesc >> 16) & 0x3fffu) << 4;
+  const int wg = (int)(threadIdx.x >> 7);
 #pragma unroll 1
-  for (int k = 0; k < nk; ++k) {
-    tc::mma_bf16(d, adesc, bdesc, idesc, (k > 0) ? 1u : acc_first);
-    adesc += da;
-    bdesc += db;
+  for (int h = 0; h < 2; ++h) {
+    if (h == 1 && ta && lbo == 0) break;
+    if (wg != 2 * (__popc(j) & 1) + h) continue;
+    const uint64_t a = adesc + ((h ? (ta ? lbo : 8192u) : 0u) >> 4);
+    if (ta == 0 && tb == 0) tc::wg_chain_n<0, 0>(n, dcol, h, a, bdesc, a_step, b_step, nk, acc_first);
+    else if (ta == 0) tc::wg_chain_n<0, 1>(n, dcol, h, a, bdesc, a_step, b_step, nk, acc_first);
+    else if (tb == 0) tc::wg_chain_n<1, 0>(n, dcol, h, a, bdesc, a_step, b_step, nk, acc_first);
+    else tc::wg_chain_n<1, 1>(n, dcol, h, a, bdesc, a_step, b_step, nk, acc_first);
   }
 }
 
@@ -334,7 +336,7 @@ __device__ __forceinline__ Tid tid_of() {
   Tid t;
   t.tid = threadIdx.x; t.warp = t.tid >> 5; t.lane = t.tid & 31; t.q = t.warp & 3; t.hh = t.warp >> 2;
   t.p = t.q * 32 + t.lane;
-  t.lane_addr = (uint32_t)(t.q * 32) << 16;
+  t.lane_addr = (uint32_t)(t.q * 32) << 16;   // accumulator row base of the warp's quadrant
   return t;
 }
 

@@ -1,12 +1,12 @@
-// tc_kernel.cu -- fused PINN loss+gradient kernel, tcgen05 tensor-core path (sm_100a).
+// tc_kernel.cu -- fused PINN loss+gradient kernel, tensor-core path (sm_90a, wgmma).
 //
-// One CTA (512 threads) owns a tile of 128 collocation points; a point is a TMEM lane and a
-// row of every operand tile.  The hidden->hidden Dense layers run on the 5th-generation
-// tensor cores (tcgen05.mma, bf16 operands from 128B-swizzled shared-memory tiles, fp32
-// accumulators in TMEM); every derivative channel (value, d/dx_i, d2/dx_i dx_j) is its own
+// One CTA (512 threads = 4 warpgroups) owns a tile of 128 collocation points; a point is a row
+// of the accumulator region (tc_prims.cuh) and of every operand tile.  The hidden->hidden Dense
+// layers run on the tensor cores (wgmma, bf16 operands from 128B-swizzled shared-memory tiles,
+// fp32 accumulators); every derivative channel (value, d/dx_i, d2/dx_i dx_j) is its own
 // 128-row M block that shares the same weight operand.  The epilogue (bias + activation +
-// forward-mode tap chain rule, or its reverse) runs on the CUDA cores straight out of TMEM
-// and re-packs the result as the next GEMM's bf16 operand tile.
+// forward-mode tap chain rule, or its reverse) runs on the CUDA cores out of the accumulator
+// region and re-packs the result as the next GEMM's bf16 operand tile.
 //
 //   forward, per tensor layer l :  D_c[128 x n_out] = H_c[128 x n_in] * W_l^T        (A, B K-major)
 //   backward, per tensor layer l:  Z_c   (recompute, 32-column groups)  = H_c * W_l^T
@@ -25,7 +25,7 @@
 #include "tail.cuh"
 
 #ifndef PINN_TC_PREFETCH
-#define PINN_TC_PREFETCH 0      // 1: software-pipelined TMEM loads in the tensor-layer epilogues (measurement variant)
+#define PINN_TC_PREFETCH 0      // 1: software-pipelined accumulator loads in the tensor-layer epilogues (measurement variant)
 #endif
 
 namespace pinn {
@@ -33,7 +33,6 @@ namespace pinn {
 // CTA-wide constants kept in shared memory so the per-network passes (separate functions) do not
 // drag a context struct through local memory
 struct CtaShared {
-  uint32_t tmem;
   int split, tl_max, off_P, off_Q, off_misc, off_ones, mx_dim, mx_taps;
   float* partial;
   uint8_t* stash;
@@ -76,7 +75,7 @@ struct LoopCtx {
   uint32_t tQ;            // shared-memory address of the lo operand tiles (forward split)
   float* gb;              // bias gradient of the current layer (CTA partial)
   float* gw;              // weight gradient of the first layer (CTA partial)
-  uint32_t taddr;         // tmem base + lane quadrant
+  uint32_t taddr;         // accumulator address of the warp's row quadrant
   int act, split, p, lane, g0, g1, c0, flag;
 };
 
@@ -116,7 +115,7 @@ __device__ __forceinline__ void l0_fwd_loop(const LoopCtx lc, const PassInfo<N1,
   for (int c = 0; c < C; ++c) up[c] = u[c];
 }
 
-// tensor layer forward epilogue: TMEM accumulators -> bias + activation chain -> next operand tiles
+// tensor layer forward epilogue: accumulators -> bias + activation chain -> next operand tiles
 template <int N1, int N2, bool PURE, int AK>
 __device__ __forceinline__ void tl_fwd_loop(const LoopCtx lc, const Chan<N1, N2> ch, float* up) {
   constexpr int C = 1 + N1 + N2;
@@ -124,28 +123,26 @@ __device__ __forceinline__ void tl_fwd_loop(const LoopCtx lc, const Chan<N1, N2>
 #pragma unroll
   for (int c = 0; c < C; ++c) u[c] = up[c];
 #if PINN_TC_PREFETCH
-  // software pipeline: the TMEM loads of granule g + 1 are in flight while granule g is evaluated
+  // software pipeline: the accumulator loads of granule g + 1 are in flight while granule g is evaluated
   float zn[C][GW];
 #pragma unroll
-  for (int c = 0; c < C; ++c) tmem_ldg(lc.taddr + TM_X + c * 64 + lc.g0 * GW, zn[c]);
+  for (int c = 0; c < C; ++c) acc_ldg(lc.taddr + TM_X + c * 64 + lc.g0 * GW, zn[c]);
 #endif
 #pragma unroll 1
   for (int g = lc.g0; g < lc.g1; ++g) {
     float z[C][GW];
 #if PINN_TC_PREFETCH
-    tc::tmem_ld_wait();
 #pragma unroll
     for (int c = 0; c < C; ++c)
 #pragma unroll
       for (int i = 0; i < GW; ++i) z[c][i] = zn[c][i];
     if (g + 1 < lc.g1) {
 #pragma unroll
-      for (int c = 0; c < C; ++c) tmem_ldg(lc.taddr + TM_X + c * 64 + (g + 1) * GW, zn[c]);
+      for (int c = 0; c < C; ++c) acc_ldg(lc.taddr + TM_X + c * 64 + (g + 1) * GW, zn[c]);
     }
 #else
 #pragma unroll
-    for (int c = 0; c < C; ++c) tmem_ldg(lc.taddr + TM_X + c * 64 + g * GW, z[c]);
-    tc::tmem_ld_wait();
+    for (int c = 0; c < C; ++c) acc_ldg(lc.taddr + TM_X + c * 64 + g * GW, z[c]);
 #endif
 #pragma unroll
     for (int i = 0; i < GW; i += 2) {
@@ -169,8 +166,8 @@ __device__ __forceinline__ void tl_fwd_loop(const LoopCtx lc, const Chan<N1, N2>
   for (int c = 0; c < C; ++c) up[c] = u[c];
 }
 
-// tensor layer backward epilogue for the column group starting at c0: recomputed Z (TMEM Y) and output
-// adjoints (TMEM X, or w_last * ubar for the last hidden layer: flag) -> Zbar tiles (the bias gradient is a
+// tensor layer backward epilogue for the column group starting at c0: recomputed Z (columns Y) and output
+// adjoints (columns X, or w_last * ubar for the last hidden layer: flag) -> Zbar tiles (the bias gradient is a
 // column sum of Zbar_0, taken by one MMA chain against the constant ones atom in net_backward)
 template <int N1, int N2, bool PURE, int AK>
 __device__ __forceinline__ void tl_bwd_loop(const LoopCtx lc, const Chan<N1, N2> ch, const float* ubp) {
@@ -181,10 +178,10 @@ __device__ __forceinline__ void tl_bwd_loop(const LoopCtx lc, const Chan<N1, N2>
 #if PINN_TC_PREFETCH
   float zn[C][GWB], hn[C][GWB];
 #pragma unroll
-  for (int c = 0; c < C; ++c) tmem_ldg(lc.taddr + TM_Y + c * 32 + lc.g0 * GWB, zn[c]);
+  for (int c = 0; c < C; ++c) acc_ldg(lc.taddr + TM_Y + c * 32 + lc.g0 * GWB, zn[c]);
   if (!lc.flag) {
 #pragma unroll
-    for (int c = 0; c < C; ++c) tmem_ldg(lc.taddr + TM_X + c * 64 + lc.c0 + lc.g0 * GWB, hn[c]);
+    for (int c = 0; c < C; ++c) acc_ldg(lc.taddr + TM_X + c * 64 + lc.c0 + lc.g0 * GWB, hn[c]);
   }
 #endif
 #pragma unroll 1
@@ -192,27 +189,25 @@ __device__ __forceinline__ void tl_bwd_loop(const LoopCtx lc, const Chan<N1, N2>
     const int ocol = lc.c0 + g * GWB;
     float z[C][GWB], hb[C][GWB];
 #if PINN_TC_PREFETCH
-    tc::tmem_ld_wait();
 #pragma unroll
     for (int c = 0; c < C; ++c)
 #pragma unroll
       for (int i = 0; i < GWB; ++i) { z[c][i] = zn[c][i]; hb[c][i] = hn[c][i]; }
     if (g + 1 < lc.g1) {
 #pragma unroll
-      for (int c = 0; c < C; ++c) tmem_ldg(lc.taddr + TM_Y + c * 32 + (g + 1) * GWB, zn[c]);
+      for (int c = 0; c < C; ++c) acc_ldg(lc.taddr + TM_Y + c * 32 + (g + 1) * GWB, zn[c]);
       if (!lc.flag) {
 #pragma unroll
-        for (int c = 0; c < C; ++c) tmem_ldg(lc.taddr + TM_X + c * 64 + ocol + GWB, hn[c]);
+        for (int c = 0; c < C; ++c) acc_ldg(lc.taddr + TM_X + c * 64 + ocol + GWB, hn[c]);
       }
     }
 #else
 #pragma unroll
-    for (int c = 0; c < C; ++c) tmem_ldg(lc.taddr + TM_Y + c * 32 + g * GWB, z[c]);
+    for (int c = 0; c < C; ++c) acc_ldg(lc.taddr + TM_Y + c * 32 + g * GWB, z[c]);
     if (!lc.flag) {
 #pragma unroll
-      for (int c = 0; c < C; ++c) tmem_ldg(lc.taddr + TM_X + c * 64 + ocol, hb[c]);
+      for (int c = 0; c < C; ++c) acc_ldg(lc.taddr + TM_X + c * 64 + ocol, hb[c]);
     }
-    tc::tmem_ld_wait();
 #endif
     if (lc.flag) {
 #pragma unroll
@@ -239,7 +234,7 @@ __device__ __forceinline__ void tl_bwd_loop(const LoopCtx lc, const Chan<N1, N2>
   }
 }
 
-// layer 0 backward, tensor-core variant: adjoints of H^0 (TMEM X) -> Zbar^0 tiles (value + first-derivative
+// layer 0 backward, tensor-core variant: adjoints of H^0 (columns X) -> Zbar^0 tiles (value + first-derivative
 // channels; bf16 hi) in P.  The weight / bias gradient is then one small MMA chain against the augmented
 // coordinate tiles (see net_backward), so no cross-lane reductions are needed here.
 template <int N1, int N2, bool PURE, int AK>
@@ -252,8 +247,7 @@ __device__ __forceinline__ void l0_bwd_store_loop(const LoopCtx lc, const PassIn
   for (int g = lc.g0; g < lc.g1; ++g) {
     float hb[C][GWB];
 #pragma unroll
-    for (int c = 0; c < C; ++c) tmem_ldg(lc.taddr + TM_X + c * 64 + g * GWB, hb[c]);
-    tc::tmem_ld_wait();
+    for (int c = 0; c < C; ++c) acc_ldg(lc.taddr + TM_X + c * 64 + g * GWB, hb[c]);
 #pragma unroll
     for (int i = 0; i < GWB; i += 2) {
       float za[C], zb2[C];
@@ -271,7 +265,7 @@ __device__ __forceinline__ void l0_bwd_store_loop(const LoopCtx lc, const PassIn
   }
 }
 
-// layer 0 backward: adjoints of H^0 (TMEM X, or w_last * ubar: flag) -> first-layer weight / bias gradient
+// layer 0 backward: adjoints of H^0 (columns X, or w_last * ubar: flag) -> first-layer weight / bias gradient
 template <int N1, int N2, bool PURE, int AK>
 __device__ __forceinline__ void l0_bwd_loop(const LoopCtx lc, const PassInfo<N1, N2> pi, const float* xp, const float* ubp) {
   constexpr int C = 1 + N1 + N2;
@@ -288,8 +282,7 @@ __device__ __forceinline__ void l0_bwd_loop(const LoopCtx lc, const PassInfo<N1,
     float hb[C][GW];
     if (!lc.flag) {
 #pragma unroll
-      for (int c = 0; c < C; ++c) tmem_ldg(lc.taddr + TM_X + c * 64 + g * GW, hb[c]);
-      tc::tmem_ld_wait();
+      for (int c = 0; c < C; ++c) acc_ldg(lc.taddr + TM_X + c * 64 + g * GW, hb[c]);
     } else {
 #pragma unroll
       for (int i = 0; i < GW; ++i) {
@@ -334,7 +327,7 @@ __device__ __forceinline__ void l0_bwd_loop(const LoopCtx lc, const PassInfo<N1,
 
 // ---------------------------------------------------------------------------------------------------
 // forward of one network for the current tile, channel structure <N1, N2, PURE>.
-// `phase` bit 0 = parity of the MMA barrier, bit 1 = parity of the bulk-load barrier; returned updated.
+// `phase` bit 1 = parity of the bulk-load barrier (bit 0 unused); returned updated.
 template <int N1, int N2, bool PURE, int AK>
 __device__ __noinline__ uint32_t net_forward(CtaShared* cs, const DevProblem* Pp, const DevTerm* tmp, int slot,
                                              int want_grad, uint32_t phase) {
@@ -349,14 +342,13 @@ __device__ __noinline__ uint32_t net_forward(CtaShared* cs, const DevProblem* Pp
   uint8_t* tP = smem + cs->off_P;
   uint8_t* tQ = smem + cs->off_Q;
   const Misc ms = misc_of(smem + cs->off_misc, cs->mx_dim, cs->mx_taps);
-  const uint32_t tmem = cs->tmem;
+  const uint32_t accm = 0;   // accumulator address of row 0, column 0
   const bool split = cs->split != 0;
   PassInfo<N1, N2> pi;
   load_pass<N1, N2>(pi, net, dc);
   const int TL = pi.TL;
   const Tid t = tid_of();
   const int tid = t.tid, hh = t.hh, p = t.p;
-  uint32_t mma_phase = phase & 1u;
   float x[PINN_MAX_IN];
 #pragma unroll
   for (int k = 0; k < PINN_MAX_IN; ++k) x[k] = (k < pi.d_in) ? ms.Xs[dc.rows[k] * kTcPts + p] : 0.f;
@@ -376,7 +368,7 @@ __device__ __noinline__ uint32_t net_forward(CtaShared* cs, const DevProblem* Pp
     const int ng = pi.n1w / GW;
     LoopCtx lc;
     lc.fp = tc::smem_u32(fp); lc.bt = lc.fp; lc.tP = tc::smem_u32(tP); lc.tQ = tc::smem_u32(tQ); lc.gb = nullptr; lc.gw = nullptr;
-    lc.taddr = tmem + t.lane_addr; lc.act = act0; lc.split = split ? 1 : 0; lc.p = p; lc.lane = t.lane; lc.g0 = hh * (ng / kNH); lc.g1 = (hh + 1) * (ng / kNH);
+    lc.taddr = accm + t.lane_addr; lc.act = act0; lc.split = split ? 1 : 0; lc.p = p; lc.lane = t.lane; lc.g0 = hh * (ng / kNH); lc.g1 = (hh + 1) * (ng / kNH);
     lc.c0 = 0; lc.flag = (TL == 0) ? 1 : 0;
     l0_fwd_loop<N1, N2, PURE, AK>(lc, pi, x, u);
   }
@@ -385,55 +377,43 @@ __device__ __noinline__ uint32_t net_forward(CtaShared* cs, const DevProblem* Pp
     const int n_in = net.dims[l], n_out = net.dims[l + 1];
     const int act = net.acts[l];
     tc::fence_async_smem();
-    tc::tc_fence_before();
     __syncthreads();
     dbg_mark(cs, 11);
-    if (tc::uni(t.warp) == 0) {
-      // warp-uniform issue path: every operand is made uniform, one elected lane issues
-      const uint32_t u_tmem = tc::uni(tmem), u_P = tc::uni(tc::smem_u32(tP)), u_Q = tc::uni(tc::smem_u32(tQ));
-      const uint32_t u_whi = tc::uni(tc::smem_u32(smem + ns.w_hi[l - 1])), u_wlo = tc::uni(tc::smem_u32(smem + ns.w_lo[l - 1]));
-      const int u_nk = tc::uni(n_in / 16), u_nout = tc::uni(n_out), u_split = tc::uni(split ? 1 : 0), u_wg = tc::uni(want_grad);
-      const uint64_t u_stash = tc::uni((uint64_t)(stash_slot + (size_t)(l - 1) * kTcMaxC * kTileBytes));
-      if (tc::elect_one()) {
-        tc::tc_fence_after();
-        if (u_wg) {
+    if (want_grad && tid == 0) {
+      // stash this layer's input tiles for the reverse sweep (the bulk copies read P while the MMAs run)
+      for (int c = 0; c < C; ++c)
+        tc::bulk_store(stash_slot + (size_t)(l - 1) * kTcMaxC * kTileBytes + (size_t)c * kTileBytes, tP + c * kTileBytes, kTileBytes);
+      tc::bulk_commit();
+    }
+    {
+      const uint32_t sP = tc::smem_u32(tP), sQ = tc::smem_u32(tQ);
+      const int nk = n_in / 16;
+      const uint32_t idesc = tc::make_idesc(n_out, 0, 0);
+      const uint64_t dwhi = tc::make_desc(tc::smem_u32(smem + ns.w_hi[l - 1]), 0, 1024);
+      const uint64_t dwlo = tc::make_desc(tc::smem_u32(smem + ns.w_lo[l - 1]), 0, 1024);
 #pragma unroll 1
-          for (int c = 0; c < C; ++c)
-            tc::bulk_store_u((void*)(u_stash + (uint64_t)c * kTileBytes), u_P + c * kTileBytes, kTileBytes);
-          tc::bulk_commit();
+      for (int c = 0; c < C; ++c) {
+        const uint64_t dahi = tc::make_desc(sP + c * kTileBytes, 0, 1024);
+        const uint32_t d = accm + TM_X + c * 64;
+        mma_chain(d, dahi, dwhi, 32, 32, nk, idesc, 0);
+        if (split) {
+          const uint64_t dalo = tc::make_desc(sQ + c * kTileBytes, 0, 1024);
+          mma_chain(d, dahi, dwlo, 32, 32, nk, idesc, 1);
+          mma_chain(d, dalo, dwhi, 32, 32, nk, idesc, 1);
         }
-        const uint32_t idesc = tc::make_idesc(128, u_nout, 0, 0);
-        const uint64_t dwhi = tc::make_desc(u_whi, 0, 1024), dwlo = tc::make_desc(u_wlo, 0, 1024);
-#pragma unroll 1
-        for (int c = 0; c < C; ++c) {
-          const uint64_t dahi = tc::make_desc(u_P + c * kTileBytes, 0, 1024);
-          const uint32_t d = u_tmem + TM_X + c * 64;
-          mma_chain(d, dahi, dwhi, 32, 32, u_nk, idesc, 0);
-          if (u_split) {
-            const uint64_t dalo = tc::make_desc(u_Q + c * kTileBytes, 0, 1024);
-            mma_chain(d, dahi, dwlo, 32, 32, u_nk, idesc, 1);
-            mma_chain(d, dalo, dwhi, 32, 32, u_nk, idesc, 1);
-          }
-        }
-        tc::mma_commit(ms.bar_mma);
       }
-      __syncwarp();
     }
     dbg_mark(cs, 12);
-    wait_bar(ms.bar_mma, mma_phase);
-    tc::tc_fence_after();
+    __syncthreads();
     dbg_mark(cs, 13);
-    if (want_grad && tc::uni(t.warp) == 0) {
-      if (tc::elect_one()) tc::bulk_wait_read0();       // stash copies have finished reading P (same lane issued them)
-      __syncwarp();
-    }
+    if (want_grad && tid == 0) tc::bulk_wait_read0();   // stash copies have finished reading P (same thread issued them)
     __syncthreads();
     dbg_mark(cs, 14);
     const int ng = n_out / GW;
     LoopCtx lc;
     lc.fp = tc::smem_u32(fp); lc.bt = lc.fp + (FP_BT + (l - 1) * 64) * 4; lc.tP = tc::smem_u32(tP); lc.tQ = tc::smem_u32(tQ);
     lc.gb = nullptr; lc.gw = nullptr;
-    lc.taddr = tmem + t.lane_addr; lc.act = act; lc.split = split ? 1 : 0; lc.p = p; lc.lane = t.lane;
+    lc.taddr = accm + t.lane_addr; lc.act = act; lc.split = split ? 1 : 0; lc.p = p; lc.lane = t.lane;
     lc.g0 = hh * (ng / kNH); lc.g1 = (hh + 1) * (ng / kNH); lc.c0 = 0; lc.flag = (l == TL) ? 1 : 0;
     tl_fwd_loop<N1, N2, PURE, AK>(lc, pi.ch, u);
   }
@@ -459,7 +439,7 @@ __device__ __noinline__ uint32_t net_forward(CtaShared* cs, const DevProblem* Pp
   }
   __syncthreads();
   dbg_mark(cs, 16);
-  return (phase & 2u) | mma_phase;
+  return phase;
 }
 
 // reverse sweep of one network for the current tile
@@ -477,14 +457,14 @@ __device__ __noinline__ uint32_t net_backward(CtaShared* cs, const DevProblem* P
   uint8_t* tP = smem + cs->off_P;
   uint8_t* tQ = smem + cs->off_Q;
   const Misc ms = misc_of(smem + cs->off_misc, cs->mx_dim, cs->mx_taps);
-  const uint32_t tmem = cs->tmem;
+  const uint32_t accm = 0;   // accumulator address of row 0, column 0
   float* partial = cs->partial;
   PassInfo<N1, N2> pi;
   load_pass<N1, N2>(pi, net, dc);
   const int L = pi.L, TL = pi.TL;
   const Tid t = tid_of();
   const int tid = t.tid, hh = t.hh, p = t.p, lane = t.lane, q = t.q;
-  uint32_t mma_phase = phase & 1u, ld_phase = (phase >> 1) & 1u;
+  uint32_t ld_phase = (phase >> 1) & 1u;
   float x[PINN_MAX_IN];
 #pragma unroll
   for (int k = 0; k < PINN_MAX_IN; ++k) x[k] = (k < pi.d_in) ? ms.Xs[dc.rows[k] * kTcPts + p] : 0.f;
@@ -527,38 +507,28 @@ __device__ __noinline__ uint32_t net_backward(CtaShared* cs, const DevProblem* P
       asm volatile("st.shared.v4.b32 [%0], {%1,%2,%3,%4};" ::"r"(q0 + tc::swz_chunk(p, 1)), "r"(w[4]), "r"(w[5]), "r"(w[6]), "r"(w[7]) : "memory");
     }
     tc::fence_async_smem();
-    tc::tc_fence_before();
     __syncthreads();
-    if (tc::uni(t.warp) == 0) {
-      const uint32_t u_tmem = tc::uni(tmem), u_P = tc::uni(tc::smem_u32(tP)), u_Q = tc::uni(tc::smem_u32(tQ));
-      if (tc::elect_one()) {
-        tc::tc_fence_after();
-        const uint32_t idesc = tc::make_idesc(128, 16, 1, 1);
-        const uint64_t db = tc::make_desc(u_Q, 0, 1024);
+    {
+      const uint32_t sP = tc::smem_u32(tP);
+      const uint32_t idesc = tc::make_idesc(16, 1, 1);
+      const uint64_t db = tc::make_desc(tc::smem_u32(tQ), 0, 1024);
 #pragma unroll 1
-        for (int c = 0; c < C; ++c)
-          mma_chain(u_tmem + TM_Y + 16 * c, tc::make_desc(u_P + c * kTileBytes, 0, 1024), db, 2048, 2048, kTcPts / 16, idesc, 0);
-        tc::mma_commit(ms.bar_mma);
-      }
-      __syncwarp();
+      for (int c = 0; c < C; ++c)
+        mma_chain(accm + TM_Y + 16 * c, tc::make_desc(sP + c * kTileBytes, 0, 1024), db, 2048, 2048, kTcPts / 16, idesc, 0);
     }
-    wait_bar(ms.bar_mma, mma_phase);
-    tc::tc_fence_after();
+    __syncthreads();
     if (q < 2 && hh == 0) {
       const int o = q * 32 + lane;
       float acc = 0.f;
 #pragma unroll
       for (int c = 0; c < C; ++c) {
         float v[2];
-        tmem_ld2(tmem + t.lane_addr + TM_Y + 16 * c + 2 * c, v);
-        tc::tmem_ld_wait();
+        acc_ld2(accm + t.lane_addr + TM_Y + 16 * c + 2 * c, v);
         acc += v[0] + v[1];
       }
       if (o < pi.nL) atomicAdd(gw_last + o, acc);
     }
-    tc::tc_fence_before();
     __syncthreads();
-    tc::tc_fence_after();
   }
 
   // ---- tensor layers, last to first ------------------------------------------------------------------------------------
@@ -570,100 +540,76 @@ __device__ __noinline__ uint32_t net_backward(CtaShared* cs, const DevProblem* P
     const float* bt = fp + FP_BT + (l - 1) * 64;
     const uint32_t whi = tc::smem_u32(smem + ns.w_hi[l - 1]);
     dbg_mark(cs, 21);
-    if (tc::uni(t.warp) == 0) {
+    if (tid == 0) {
       // reload this layer's input tiles H^{l-1} (bf16 hi) from the stash into Q
-      const uint32_t u_Q = tc::uni(tc::smem_u32(tQ)), u_bar = tc::uni(tc::smem_u32(ms.bar_ld));
-      const uint64_t u_stash = tc::uni((uint64_t)(stash_slot + (size_t)(l - 1) * kTcMaxC * kTileBytes));
-      if (tc::elect_one()) {
-        tc::mbar_arrive_expect_tx_u(u_bar, C * kTileBytes);
-#pragma unroll 1
-        for (int c = 0; c < C; ++c)
-          tc::bulk_load_u(u_Q + c * kTileBytes, (const void*)(u_stash + (uint64_t)c * kTileBytes), kTileBytes, u_bar);
-      }
-      __syncwarp();
+      const uint8_t* src = stash_slot + (size_t)(l - 1) * kTcMaxC * kTileBytes;
+      tc::mbar_arrive_expect_tx(ms.bar_ld, C * kTileBytes);
+      for (int c = 0; c < C; ++c) tc::bulk_load(tQ + c * kTileBytes, src + (size_t)c * kTileBytes, kTileBytes, ms.bar_ld);
     }
     wait_bar(ms.bar_ld, ld_phase);
     dbg_mark(cs, 22);
     // recompute pre-activations in groups of <= 32 columns and turn output adjoints into Zbar tiles
     for (int c0 = 0; c0 < n_out; c0 += 32) {
       const int gw_cols = (n_out - c0) < 32 ? (n_out - c0) : 32;     // 32 or 16
-      tc::tc_fence_before();
       __syncthreads();
       dbg_mark(cs, 23);
-      if (tc::uni(t.warp) == 0) {
-        const uint32_t u_tmem = tc::uni(tmem), u_Q = tc::uni(tc::smem_u32(tQ)), u_w = tc::uni(whi + c0 * 128);
-        const int u_nk = tc::uni(n_in / 16), u_gw = tc::uni(gw_cols);
-        if (tc::elect_one()) {
-          tc::tc_fence_after();
-          const uint32_t idesc = tc::make_idesc(128, u_gw, 0, 0);
-          const uint64_t dw = tc::make_desc(u_w, 0, 1024);
+      {
+        const uint32_t sQ = tc::smem_u32(tQ);
+        const uint32_t idesc = tc::make_idesc(gw_cols, 0, 0);
+        const uint64_t dw = tc::make_desc(whi + c0 * 128, 0, 1024);
 #pragma unroll 1
-          for (int c = 0; c < C; ++c)
-            mma_chain(u_tmem + TM_Y + c * 32, tc::make_desc(u_Q + c * kTileBytes, 0, 1024), dw, 32, 32, u_nk, idesc, 0);
-          tc::mma_commit(ms.bar_mma);
-        }
-        __syncwarp();
+        for (int c = 0; c < C; ++c)
+          mma_chain(accm + TM_Y + c * 32, tc::make_desc(sQ + c * kTileBytes, 0, 1024), dw, 32, 32, n_in / 16, idesc, 0);
       }
       dbg_mark(cs, 24);
-      wait_bar(ms.bar_mma, mma_phase);
-      tc::tc_fence_after();
+      __syncthreads();
       dbg_mark(cs, 25);
       const int ng = gw_cols / GWB;
       LoopCtx lc;
       lc.fp = tc::smem_u32(fp); lc.bt = tc::smem_u32(bt); lc.tP = tc::smem_u32(tP); lc.tQ = tc::smem_u32(tQ); lc.gb = gb; lc.gw = nullptr;
-      lc.taddr = tmem + t.lane_addr;
+      lc.taddr = accm + t.lane_addr;
       lc.act = act; lc.split = 0; lc.p = p; lc.lane = lane; lc.g0 = hh * (ng / kNH); lc.g1 = (hh + 1) * (ng / kNH);
       lc.c0 = c0; lc.flag = (l == TL) ? 1 : 0;
       tl_bwd_loop<N1, N2, PURE, AK>(lc, pi.ch, ub);
     }
     tc::fence_async_smem();
-    tc::tc_fence_before();
     __syncthreads();
     dbg_mark(cs, 26);
-    if (tc::uni(t.warp) == 0) {
-      const uint32_t u_tmem = tc::uni(tmem), u_P = tc::uni(tc::smem_u32(tP)), u_Q = tc::uni(tc::smem_u32(tQ)), u_w = tc::uni(whi);
-      const uint32_t u_ones = tc::uni(tc::smem_u32(smem + cs->off_ones));
-      const int u_nin = tc::uni(n_in), u_nko = tc::uni(n_out / 16);
-      if (tc::elect_one()) {
-        tc::tc_fence_after();
-        // dgrad: Hbar_c = Zbar_c * W_l  -> X
-        const uint32_t idg = tc::make_idesc(128, u_nin, 0, 1);
-        const uint64_t dw = tc::make_desc(u_w, 0, 1024);
+    {
+      const uint32_t sP = tc::smem_u32(tP), sQ = tc::smem_u32(tQ);
+      const uint32_t s_ones = tc::smem_u32(smem + cs->off_ones);
+      // dgrad: Hbar_c = Zbar_c * W_l  -> X
+      const uint32_t idg = tc::make_idesc(n_in, 0, 1);
+      const uint64_t dw = tc::make_desc(whi, 0, 1024);
 #pragma unroll 1
-        for (int c = 0; c < C; ++c)
-          mma_chain(u_tmem + TM_X + c * 64, tc::make_desc(u_P + c * kTileBytes, 0, 1024), dw, 32, 2048, u_nko, idg, 0);
-        // wgrad: Wbar_l = sum_c Zbar_c^T * H_c -> Y (rows >= 64 alias rows - 64 through LBO = 0)
-        const uint32_t iwg = tc::make_idesc(128, u_nin, 1, 1);
+      for (int c = 0; c < C; ++c)
+        mma_chain(accm + TM_X + c * 64, tc::make_desc(sP + c * kTileBytes, 0, 1024), dw, 32, 2048, n_out / 16, idg, 0);
+      // wgrad: Wbar_l = sum_c Zbar_c^T * H_c -> Y (rows = output neurons: the 64 columns of the Zbar tiles)
+      const uint32_t iwg = tc::make_idesc(n_in, 1, 1);
 #pragma unroll 1
-        for (int c = 0; c < C; ++c)
-          mma_chain(u_tmem + TM_Y, tc::make_desc(u_P + c * kTileBytes, 0, 1024), tc::make_desc(u_Q + c * kTileBytes, 0, 1024),
-                    2048, 2048, kTcPts / 16, iwg, c > 0 ? 1u : 0u);
-        // bias gradient: bbar_l[o] = sum_p Zbar_0[p][o] -> Y column 64 (B = the constant ones atom, SBO = 0, no k advance)
-        mma_chain(u_tmem + TM_Y + 64, tc::make_desc(u_P, 0, 1024), tc::make_desc(u_ones, 0, 0), 2048, 0, kTcPts / 16,
-                  tc::make_idesc(128, 16, 1, 1), 0);
-        tc::mma_commit(ms.bar_mma);
-      }
-      __syncwarp();
+      for (int c = 0; c < C; ++c)
+        mma_chain(accm + TM_Y, tc::make_desc(sP + c * kTileBytes, 0, 1024), tc::make_desc(sQ + c * kTileBytes, 0, 1024),
+                  2048, 2048, kTcPts / 16, iwg, c > 0 ? 1u : 0u);
+      // bias gradient: bbar_l[o] = sum_p Zbar_0[p][o] -> Y column 64 (B = the constant ones atom, SBO = 0, no k advance)
+      mma_chain(accm + TM_Y + 64, tc::make_desc(sP, 0, 1024), tc::make_desc(s_ones, 0, 0), 2048, 0, kTcPts / 16,
+                tc::make_idesc(16, 1, 1), 0);
     }
     dbg_mark(cs, 27);
-    wait_bar(ms.bar_mma, mma_phase);
-    tc::tc_fence_after();
+    __syncthreads();
     dbg_mark(cs, 28);
-    // flush the weight-gradient tile: TMEM lane = output neuron o, column = input neuron k
+    // flush the weight-gradient tile: accumulator row = output neuron o, column = input neuron k
     if (q < 2) {
       const int o = q * 32 + lane;
       if (hh == 0) {
         float v[2];
-        tmem_ld2(tmem + t.lane_addr + TM_Y + 64, v);
-        tc::tmem_ld_wait();
+        acc_ld2(accm + t.lane_addr + TM_Y + 64, v);
         if (o < n_out) atomicAdd(gb + o, v[0]);
       }
       const int part = n_in / kNH;
 #pragma unroll 1
       for (int k0 = hh * part; k0 < (hh + 1) * part; k0 += 4) {
         float v[4];
-        tmem_ld4(tmem + t.lane_addr + TM_Y + k0, v);
-        tc::tmem_ld_wait();
+        acc_ld4(accm + t.lane_addr + TM_Y + k0, v);
         if (o < n_out) {
 #pragma unroll
           for (int i = 0; i < 4; ++i) atomicAdd(gw + o + (long long)n_out * (k0 + i), v[i]);
@@ -674,16 +620,14 @@ __device__ __noinline__ uint32_t net_backward(CtaShared* cs, const DevProblem* P
 
   // ---- layer 0 backward ---------------------------------------------------------------------------------------------------
   {
-    tc::tc_fence_before();
     __syncthreads();
-    tc::tc_fence_after();
     dbg_mark(cs, 29);
     const int act0 = net.acts[0];
     float* gb0 = partial + net.b_off[0];
     float* gw0 = partial + net.w_off[0];
     LoopCtx lc;
     lc.fp = tc::smem_u32(fp); lc.bt = lc.fp; lc.tP = tc::smem_u32(tP); lc.tQ = tc::smem_u32(tQ); lc.gb = gb0; lc.gw = gw0;
-    lc.taddr = tmem + t.lane_addr; lc.act = act0; lc.split = 0; lc.p = p; lc.lane = lane; lc.c0 = 0; lc.flag = (TL == 0) ? 1 : 0;
+    lc.taddr = accm + t.lane_addr; lc.act = act0; lc.split = 0; lc.p = p; lc.lane = lane; lc.c0 = 0; lc.flag = (TL == 0) ? 1 : 0;
     if (TL == 0) {
       // no tensor layer: everything on the CUDA cores (warp reduce-scatter + atomics)
       const int ng = pi.n1w / GW;
@@ -725,32 +669,24 @@ __device__ __noinline__ uint32_t net_backward(CtaShared* cs, const DevProblem* P
       lc.g0 = hh * (ng / kNH); lc.g1 = (hh + 1) * (ng / kNH);
       l0_bwd_store_loop<N1, N2, PURE, AK>(lc, pi, x);
       tc::fence_async_smem();
-      tc::tc_fence_before();
       __syncthreads();
-      if (tc::uni(t.warp) == 0) {
-        const uint32_t u_tmem = tc::uni(tmem), u_P = tc::uni(tc::smem_u32(tP)), u_Q = tc::uni(tc::smem_u32(tQ));
-        if (tc::elect_one()) {
-          tc::tc_fence_after();
-          const uint32_t idesc = tc::make_idesc(128, 16, 1, 1);
-          const uint64_t a0 = tc::make_desc(u_P, 0, 1024);
-          mma_chain(u_tmem + TM_Y, a0, tc::make_desc(u_Q, 0, 1024), 2048, 2048, kTcPts / 16, idesc, 0);
-          if (N2 > 0)
-            mma_chain(u_tmem + TM_Y, a0, tc::make_desc(u_Q + (1 + N1) * kTileBytes, 0, 1024), 2048, 2048, kTcPts / 16, idesc, 1);
+      {
+        const uint32_t sP = tc::smem_u32(tP), sQ = tc::smem_u32(tQ);
+        const uint32_t idesc = tc::make_idesc(16, 1, 1);
+        const uint64_t a0 = tc::make_desc(sP, 0, 1024);
+        mma_chain(accm + TM_Y, a0, tc::make_desc(sQ, 0, 1024), 2048, 2048, kTcPts / 16, idesc, 0);
+        if (N2 > 0)
+          mma_chain(accm + TM_Y, a0, tc::make_desc(sQ + (1 + N1) * kTileBytes, 0, 1024), 2048, 2048, kTcPts / 16, idesc, 1);
 #pragma unroll 1
-          for (int j = 0; j < N1; ++j)
-            mma_chain(u_tmem + TM_Y, tc::make_desc(u_P + (1 + j) * kTileBytes, 0, 1024),
-                      tc::make_desc(u_Q + (1 + j) * kTileBytes, 0, 1024), 2048, 2048, kTcPts / 16, idesc, 1);
-          tc::mma_commit(ms.bar_mma);
-        }
-        __syncwarp();
+        for (int j = 0; j < N1; ++j)
+          mma_chain(accm + TM_Y, tc::make_desc(sP + (1 + j) * kTileBytes, 0, 1024),
+                    tc::make_desc(sQ + (1 + j) * kTileBytes, 0, 1024), 2048, 2048, kTcPts / 16, idesc, 1);
       }
-      wait_bar(ms.bar_mma, mma_phase);
-      tc::tc_fence_after();
+      __syncthreads();
       if (q < 2 && hh == 0) {
         const int o = q * 32 + lane;
         float v[16];
-        tc::tmem_ld16(tmem + t.lane_addr + TM_Y, v);
-        tc::tmem_ld_wait();
+        tc::acc_ld16(accm + t.lane_addr + TM_Y, v);
         if (o < pi.n1w) {
 #pragma unroll
           for (int k = 0; k < PINN_MAX_IN; ++k)
@@ -762,14 +698,14 @@ __device__ __noinline__ uint32_t net_backward(CtaShared* cs, const DevProblem* P
   }
   __syncthreads();
   dbg_mark(cs, 30);
-  return (ld_phase << 1) | mma_phase;
+  return (ld_phase << 1) | (phase & 1u);
 }
 
 
 __global__ void __launch_bounds__(kTcThreads, 1) tc_loss_grad_kernel(const __grid_constant__ TcArgs args) {
   extern __shared__ __align__(1024) uint8_t smem[];
   __shared__ CtaShared cs;
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int tid = threadIdx.x, lane = tid & 31;
   const DevProblem* Pp = args.prob;
   const DevProblem& P = *Pp;
   const Misc ms = misc_of(smem + args.off_misc, args.mx_dim, args.mx_taps);
@@ -809,7 +745,6 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_loss_grad_kernel(const __gri
     }
   }
   if (tid == 0) {
-    tc::mbar_init(ms.bar_mma, 1);
     tc::mbar_init(ms.bar_ld, 1);
     tc::fence_barrier_init();
     cs.split = args.split; cs.tl_max = args.tl_max; cs.off_P = args.off_P; cs.off_Q = args.off_Q;
@@ -828,7 +763,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_loss_grad_kernel(const __gri
     if (cs.dbg) cs.dbg[cs.dbg_n++] = ((long long)1 << 48) | (clock64() & 0xffffffffffffLL);
 #endif
   }
-  if (warp == 0) tc::tmem_alloc<512>(ms.tmem_slot);
+  if (tid == 0) tc::s_acc = args.acc + (size_t)blockIdx.x * kAccCols * kAccRows;
   if (want_grad) {
     const long long n4 = P.n_theta / 4;
     float4* p4 = reinterpret_cast<float4*>(partial);
@@ -914,10 +849,6 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_loss_grad_kernel(const __gri
     if (tid == 0) fp[FP_BL] = __ldg(&theta[bl]);
   }
   tc::fence_async_smem();
-  tc::tc_fence_before();
-  __syncthreads();
-  tc::tc_fence_after();
-  if (tid == 0) cs.tmem = *ms.tmem_slot;
   __syncthreads();
   dbg_mark(&cs, 2);
   uint32_t phase = 0;
@@ -1040,7 +971,6 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_loss_grad_kernel(const __gri
     }
   }
 
-  tc::tc_fence_before();
   __syncthreads();
   dbg_mark(&cs, 7);
 #ifdef PINN_DEBUG
@@ -1055,7 +985,6 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_loss_grad_kernel(const __gri
   }
 #endif
   if (tid < PINN_MAX_TERMS) args.term_sums[(long long)blockIdx.x * PINN_MAX_TERMS + tid] = ms.tsum[tid];
-  if (warp == 0) tc::tmem_dealloc<512>(cs.tmem);
   // gradient reduction, optimizer step and the multi-GPU sum in the kernel tail (tail.cuh)
   if (args.tail.state)
     fused_tail<float, kTcThreads>(args.tail, args.partial, args.partial_stride, args.term_sums, P.n_theta, P.n_terms, want_grad ? 1 : 0,

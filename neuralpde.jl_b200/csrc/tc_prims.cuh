@@ -1,16 +1,18 @@
-// tc_prims.cuh -- sm_100a primitives used by the tensor-core path: mbarrier, bulk async
-// copies (TMA unit, non-tensor form), tcgen05 alloc / mma / commit / ld, shared-memory
-// matrix descriptors and the 128-byte swizzle used by every operand tile.
+// tc_prims.cuh -- sm_90a primitives used by the tensor-core path: mbarrier, bulk async
+// copies (TMA unit, non-tensor form), warpgroup MMA (wgmma) into the accumulator region,
+// shared-memory matrix descriptors and the 128-byte swizzle used by every operand tile.
 //
 // All operand tiles share ONE physical layout: rows of 64 bf16 (128 bytes), 8-row swizzle
 // atoms (1024 bytes), 16-byte chunk index XORed with (row & 7).  Whether a tile is consumed
 // K-major (rows = M/N index, columns = K) or MN-major (rows = K index, columns = M/N) is
-// chosen per MMA through the descriptor / instruction-descriptor bits, which is what lets
+// chosen per MMA through the descriptor and the wgmma transpose flags, which is what lets
 // the same tile feed the forward GEMM, dgrad and wgrad.
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
+#include "tc_types.h"
+#include "tc_wgmma.cuh"
 
 namespace pinn {
 namespace tc {
@@ -57,119 +59,97 @@ __device__ __forceinline__ void bulk_store(void* gdst, const void* smem_src, uin
                "r"(bytes)
                : "memory");
 }
-__device__ __forceinline__ void bulk_store_u(void* gdst, uint32_t smem_src_addr, uint32_t bytes) {
-  asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(gdst), "r"(smem_src_addr), "r"(bytes)
-               : "memory");
-}
 __device__ __forceinline__ void bulk_load_u(uint32_t smem_dst_addr, const void* gsrc, uint32_t bytes, uint32_t bar_addr) {
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(smem_dst_addr),
                "l"(gsrc), "r"(bytes), "r"(bar_addr)
                : "memory");
 }
-__device__ __forceinline__ void mbar_arrive_expect_tx_u(uint32_t bar_addr, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar_addr), "r"(bytes) : "memory");
-}
 __device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
 __device__ __forceinline__ void bulk_wait_read0() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
 __device__ __forceinline__ void bulk_wait0() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
-// generic-proxy writes to shared memory -> visible to the async proxy (tcgen05.mma, bulk copies)
+// generic-proxy writes to shared memory -> visible to the async proxy (wgmma, bulk copies)
 __device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
-// ---- tensor memory ------------------------------------------------------------------------------------
-template <uint32_t COLS>
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_result) {   // warp-wide
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_result)),
-               "n"(COLS)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-template <uint32_t COLS>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr) {        // warp-wide
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(COLS) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
+// ---- accumulator region ------------------------------------------------------------------------------
+// The MMA results of a CTA live in an fp32 region of global memory, [kAccCols columns][128 rows] (256 KB per CTA,
+// L2-resident: 132 CTAs take 33 MB of the 50 MB L2).  An "accumulator address" packs a row base in the high 16 bits
+// and a column in the low 16 bits; acc_ld* read consecutive columns of row (base + lane), so a warp reads whole
+// 128-byte lines.  The region pointer of the CTA is kept in shared memory (set once by the kernel).
+static __shared__ float* s_acc;
 
-// D[tmem] (+)= A[smem desc] * B[smem desc], bf16 x bf16 -> fp32, issued by ONE thread
-__device__ __forceinline__ void mma_bf16(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                                         uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}\n" ::"r"(d_tmem),
-      "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
+__device__ __forceinline__ const float* acc_row(uint32_t aaddr) {
+  return s_acc + (aaddr & 0xffffu) * kAccRows + (aaddr >> 16) + (threadIdx.x & 31);
 }
-// all previously issued MMAs of this thread arrive on the mbarrier when complete
-__device__ __forceinline__ void mma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-
-// 32 lanes x 32 bit, 8 consecutive columns: thread i of the warp gets lane (quadrant base + i)
-__device__ __forceinline__ void tmem_ld8(uint32_t taddr, float (&v)[8]) {
-  uint32_t r[8];
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-               : "r"(taddr)
-               : "memory");
+__device__ __forceinline__ void acc_ld16(uint32_t aaddr, float (&v)[16]) {
+  const float* r = acc_row(aaddr);
 #pragma unroll
-  for (int i = 0; i < 8; ++i) v[i] = __uint_as_float(r[i]);
+  for (int i = 0; i < 16; ++i) v[i] = r[i * kAccRows];
 }
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, float (&v)[16]) {
-  uint32_t r[16];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-#pragma unroll
-  for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
 
-// one lane of a fully active warp (warp-uniform code): lets the compiler keep the operands of
-// tcgen05.mma / cp.async.bulk in uniform registers instead of emitting a per-lane waterfall loop
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred;
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "elect.sync _|p, 0xffffffff;\n\t"
-      "selp.u32 %0, 1, 0, p;\n\t"
-      "}\n"
-      : "=r"(pred));
-  return pred != 0;
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait0() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+
+// One warpgroup computes rows [64 h, 64 h + 64) of D (+)= A * B over nk k-steps of 16 and stores them to the
+// accumulator region at column dcol.  Fragment layout of m64nNk16: d[i] is row 16 w + lane/4 + 8 ((i >> 1) & 1),
+// column 8 (i >> 2) + 2 (lane & 3) + (i & 1).
+template <int N, int TA, int TB>
+__device__ __forceinline__ void wg_chain(uint32_t dcol, int h, uint64_t adesc, uint64_t bdesc, uint32_t a_step, uint32_t b_step,
+                                         int nk, uint32_t acc_first) {
+  float d[N / 2];
+  const int w = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
+  float* base = s_acc + dcol * kAccRows + 64 * h + 16 * w + (lane >> 2) + (size_t)(2 * (lane & 3)) * kAccRows;
+#pragma unroll
+  for (int i = 0; i < N / 2; ++i)
+    d[i] = acc_first ? base[((i >> 2) * 8 + (i & 1)) * kAccRows + 8 * ((i >> 1) & 1)] : 0.f;
+  wgmma_fence();
+  const uint64_t da = a_step >> 4, db = b_step >> 4;
+#pragma unroll 1
+  for (int k = 0; k < nk; ++k) {
+    const uint32_t sc = (k > 0) ? 1u : acc_first;
+    if (N == 16) wgmma_n16<TA, TB>(*reinterpret_cast<float(*)[8]>(d), adesc, bdesc, sc);
+    if (N == 32) wgmma_n32<TA, TB>(*reinterpret_cast<float(*)[16]>(d), adesc, bdesc, sc);
+    if (N == 48) wgmma_n48<TA, TB>(*reinterpret_cast<float(*)[24]>(d), adesc, bdesc, sc);
+    if (N == 64) wgmma_n64<TA, TB>(*reinterpret_cast<float(*)[32]>(d), adesc, bdesc, sc);
+    if (N == 128) wgmma_n128<TA, TB>(*reinterpret_cast<float(*)[64]>(d), adesc, bdesc, sc);
+    adesc += da;
+    bdesc += db;
+  }
+  wgmma_commit();
+  wgmma_wait0();
+#pragma unroll
+  for (int i = 0; i < N / 2; ++i) base[((i >> 2) * 8 + (i & 1)) * kAccRows + 8 * ((i >> 1) & 1)] = d[i];
 }
-__device__ __forceinline__ uint32_t uni(uint32_t v) { return __shfl_sync(0xffffffffu, v, 0); }
-__device__ __forceinline__ int uni(int v) { return __shfl_sync(0xffffffffu, v, 0); }
-__device__ __forceinline__ uint64_t uni(uint64_t v) { return __shfl_sync(0xffffffffu, (unsigned long long)v, 0); }
+
+template <int TA, int TB>
+__device__ __forceinline__ void wg_chain_n(int n, uint32_t dcol, int h, uint64_t adesc, uint64_t bdesc, uint32_t a_step,
+                                           uint32_t b_step, int nk, uint32_t acc_first) {
+  switch (n) {
+    case 16: wg_chain<16, TA, TB>(dcol, h, adesc, bdesc, a_step, b_step, nk, acc_first); break;
+    case 32: wg_chain<32, TA, TB>(dcol, h, adesc, bdesc, a_step, b_step, nk, acc_first); break;
+    case 48: wg_chain<48, TA, TB>(dcol, h, adesc, bdesc, a_step, b_step, nk, acc_first); break;
+    case 64: wg_chain<64, TA, TB>(dcol, h, adesc, bdesc, a_step, b_step, nk, acc_first); break;
+    case 128: wg_chain<128, TA, TB>(dcol, h, adesc, bdesc, a_step, b_step, nk, acc_first); break;
+    default: __trap();   // pinn_create admits only layer widths that give these N
+  }
+}
+
 __device__ __forceinline__ void prefetch_l1(const void* p) { asm volatile("prefetch.global.L1 [%0];" ::"l"(p)); }
 __device__ __forceinline__ void prefetch_l2(const void* p) { asm volatile("prefetch.global.L2 [%0];" ::"l"(p)); }
 
 // ---- descriptors ---------------------------------------------------------------------------------------
-// shared-memory matrix descriptor, 128-byte swizzle, sm_100 version field = 1
+// shared-memory matrix descriptor (wgmma), 128-byte swizzle
 __device__ __forceinline__ uint64_t make_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
   uint64_t d = 0;
   d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);
   d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
   d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= 1ull << 46;   // descriptor version (Blackwell)
-  d |= 2ull << 61;   // SWIZZLE_128B
+  d |= 1ull << 62;   // SWIZZLE_128B
   return d;
 }
-// instruction descriptor, kind::f16: D = f32, A = B = bf16, dense
-__host__ __device__ constexpr uint32_t make_idesc(uint32_t m, uint32_t n, uint32_t a_mn_major, uint32_t b_mn_major) {
-  return (1u << 4)                 // D format: f32
-         | (1u << 7)               // A format: bf16
-         | (1u << 10)              // B format: bf16
-         | (a_mn_major << 15)      // A major: 0 = K-major, 1 = MN-major
-         | (b_mn_major << 16)      // B major
-         | ((n >> 3) << 17)        // N / 8
-         | ((m >> 4) << 24);       // M / 16
+// shape of an MMA chain (M = 128): N (16, 32, 48, 64 or 128) and the operand majors (0 = K-major, 1 = MN-major)
+__host__ __device__ constexpr uint32_t make_idesc(uint32_t n, uint32_t a_mn_major, uint32_t b_mn_major) {
+  return n | (a_mn_major << 8) | (b_mn_major << 9);
 }
 
 // byte offset of element (row, col) inside a [rows x 64] bf16 tile with the 128-byte swizzle

@@ -1,4 +1,4 @@
-// tc_types.h -- constants and launch arguments of the tcgen05 path, shared by the kernel and
+// tc_types.h -- constants and launch arguments of the tensor-core path, shared by the kernel and
 // the host ABI layer.
 #pragma once
 #include <stdint.h>
@@ -15,6 +15,8 @@ constexpr int kTcMaxC = 5;
 constexpr int kTcMaxTaps = 6;
 constexpr int kTcMaxTL = 6;            // tensor (hidden->hidden) layers per network
 constexpr int kTileBytes = 16384;      // 128 rows x 128 bytes
+constexpr int kAccRows = 128;          // accumulator region of a CTA: [kAccCols][kAccRows] fp32 (tc_prims.cuh)
+constexpr int kAccCols = 512;
 // fp32 parameter block per network (floats)
 constexpr int FP_W1 = 0;               // [64][8] first-layer weight, W1[o*8 + k]
 constexpr int FP_B1 = 512;             // [64]
@@ -22,7 +24,7 @@ constexpr int FP_BT = 576;             // [kTcMaxTL][64] tensor-layer biases
 constexpr int FP_WL = FP_BT + kTcMaxTL * 64;   // [64] last-layer weight
 constexpr int FP_BL = FP_WL + 64;      // [1]
 constexpr int FP_SIZE = FP_BL + 4;
-// TMEM columns
+// accumulator-region columns (tc_prims.cuh)
 constexpr uint32_t TM_X = 0;           // [c][64]: forward accumulators / adjoints of layer outputs
 constexpr uint32_t TM_Y = 320;         // [c][32] recompute group, or [64] weight-gradient accumulator
 
@@ -45,6 +47,7 @@ struct TcArgs {
   int tile_begin, tile_end;
   int mode;               // 0 loss+grad, 1 loss only, 2 residual out
   float* resid_out;
+  float* acc;             // [grid][kAccCols * kAccRows] fp32 accumulator regions
   long long* dbg;         // optional: 1000 x int64 phase timestamps of CTA 0 (pinn_debug_tc_timeline)
   int off_P, off_Q, off_misc;   // byte offsets into dynamic shared memory
   int off_Q_bytes;              // size of the Q tile region
@@ -62,8 +65,8 @@ struct TcArgs {
 
 
 // ---- wide path (tc_wide_kernel.cu): hidden widths 64 / 128, bf16 operands, weights streamed per layer ---------------
-constexpr int kTwMaxC = 4;             // channels per network: C x 128 TMEM columns
-constexpr int kTwW = 128;              // TMEM column stride of a channel = widest supported layer
+constexpr int kTwMaxC = 4;             // channels per network: C x 128 accumulator columns
+constexpr int kTwW = 128;              // accumulator column stride of a channel = widest supported layer
 constexpr int kTwNB = 2;               // 64-column operand tiles per channel
 constexpr int kTwImgBytes = kTwNB * kTileBytes;   // packed bf16 image of one tensor layer's weight: [kb][128 rows o][64 k]
 // fp32 parameter block per network (floats)
@@ -91,6 +94,7 @@ struct TwArgs {
   int tile_begin, tile_end;
   int mode;                // 0 loss+grad, 1 loss only, 2 residual out
   float* resid_out;
+  float* acc;              // [grid][kAccCols * kAccRows] fp32 accumulator regions
   long long* dbg;
   int off_P, off_S, off_misc;       // byte offsets into dynamic shared memory (P: C x 2 tiles, S: 2 x 32 KB)
   int off_ones;                     // 1 KB constant atom (bias gradient by MMA)

@@ -1,20 +1,20 @@
-// tc_wide_kernel.cu -- fused PINN loss+gradient kernel, tcgen05 path for 128-wide layers (sm_100a, bf16 operands).
+// tc_wide_kernel.cu -- fused PINN loss+gradient kernel, tensor-core path for 128-wide layers (sm_90a wgmma, bf16 operands).
 //
-// Same decomposition as tc_kernel.cu (one CTA of 512 threads per 128-point tile, a point is a TMEM lane and a row
-// of every operand tile, derivative channels share the weight operand), re-planned for hidden widths 64 / 128 where
+// Same decomposition as tc_kernel.cu (one CTA of 512 threads per 128-point tile, a point is a row of the accumulator
+// region and of every operand tile, derivative channels share the weight operand), re-planned for hidden widths 64 / 128 where
 // neither the weights of all layers nor two generations of activations fit in shared memory:
 //
 //   * an activation set is C channels x 2 tiles (128 points x 64 bf16, 128-byte swizzle) = C x 32 KB in region P;
-//     TMEM holds C x 128 accumulator columns (C <= 4), so the epilogue of a layer overwrites its own input in place;
+//     the accumulator region holds C x 128 columns (C <= 4), so the epilogue of a layer overwrites its own input in place;
 //   * weights are packed once per step by tw_pack_kernel into bf16 swizzled images (32 KB per layer) and streamed
 //     through two 32 KB buffers S0 / S1 with cp.async.bulk + mbarrier, prefetched one layer ahead;
 //   * the forward sweep stashes every tensor layer's input tiles (bf16, for wgrad) and biased pre-activations
 //     (fp32, point-fastest so that a warp writes / reads 256 contiguous bytes) to a per-CTA global buffer (L2);
-//     the reverse sweep reads the pre-activations straight into registers -- no recompute, no TMEM for it;
+//     the reverse sweep reads the pre-activations straight into registers -- no recompute, no accumulator columns for it;
 //   * reverse, per tensor layer:  Zbar tiles -> P;  wgrad  Wbar_l = sum_c Zbar_c^T H_c  with H_c streamed through
 //     S0 / S1 per channel;  then dgrad  Hbar_c = Zbar_c W_l  with W_l in the buffer wgrad released first.
 //     MN-major operands whose M / N extent is 128 span two tiles through the descriptor's leading-dimension byte
-//     offset (pinned on hardware by scripts/tc_probe_wide.py).
+//     offset.
 //
 // Replaces the same reference functions as the other paths (Phi src/pinn_types.jl:79-90, numeric_derivative
 // :445-482, the generated residual and mean(abs2) src/training_strategies.jl:215-221, Zygote gradient
@@ -30,7 +30,6 @@ namespace pinn {
 constexpr uint32_t TB = kTileBytes;
 
 struct TwShared {
-  uint32_t tmem;
   int tl_max, off_P, off_S, off_misc, off_ones, off_nets, mx_dim, mx_taps;
   float* partial;
   uint8_t* hstash;
@@ -41,8 +40,8 @@ struct TwShared {
   int dbg_n;
   int off_fp[PINN_MAX_NETS], wimg[PINN_MAX_NETS];
   int next_tile;                     // dynamic scheduler: tile claimed for the next iteration
-  uint32_t ph_ld[2], ph_free[2];     // phases of the streaming barriers, owned by the issuing lane of warp 0
-  uint64_t bar_ld[2], bar_free[2];   // S0 / S1: bytes landed, MMAs that read the buffer retired
+  uint32_t ph_ld[2];                 // phases of the streaming barriers (flipped by thread 0 after a CTA-wide wait)
+  uint64_t bar_ld[2];                // S0 / S1: bytes landed
 };
 
 // first-layer pre-activations of neuron o (channel vector zz); fpa = shared-memory address of the fp32 block
@@ -72,7 +71,7 @@ struct LoopW {
   uint32_t bt;            // shared-memory address of the current tensor layer's bias
   uint32_t tP;            // shared-memory address of the operand tiles (channel c, column block kb: (c*2+kb)*TB)
   float* gb;              // bias gradient of the current layer (CTA partial)
-  uint32_t taddr;         // tmem base + lane quadrant
+  uint32_t taddr;         // accumulator address of the warp's row quadrant
   int act, p, lane, g0, g1, flag;
 };
 
@@ -106,7 +105,7 @@ __device__ __forceinline__ void tw_l0_fwd_loop(const LoopW lc, const PassInfo<N1
   }
 }
 
-// tensor layer forward epilogue: TMEM accumulators -> bias + activation chain -> next operand tiles (in place),
+// tensor layer forward epilogue: accumulators -> bias + activation chain -> next operand tiles (in place),
 // biased pre-activations -> fp32 stash (zst != nullptr), last-layer dot products (flag)
 template <int N1, int N2, bool PURE, int AK>
 __device__ __forceinline__ void tw_fwd_loop(const LoopW lc, const Chan<N1, N2> ch, float* up, float2* zst) {
@@ -118,8 +117,7 @@ __device__ __forceinline__ void tw_fwd_loop(const LoopW lc, const Chan<N1, N2> c
   for (int g = lc.g0; g < lc.g1; ++g) {
     float z[C][4];
 #pragma unroll
-    for (int c = 0; c < C; ++c) tmem_ld4(lc.taddr + c * kTwW + g * 4, z[c]);
-    tc::tmem_ld_wait();
+    for (int c = 0; c < C; ++c) acc_ld4(lc.taddr + c * kTwW + g * 4, z[c]);
     const int col = g * 4;
 #pragma unroll
     for (int i = 0; i < 4; i += 2) {
@@ -147,12 +145,10 @@ __device__ __forceinline__ void tw_fwd_loop(const LoopW lc, const Chan<N1, N2> c
   for (int c = 0; c < C; ++c) up[c] = u[c];
 }
 
-// tensor layer reverse epilogue: stashed pre-activations and output adjoints (TMEM X, or w_last * ubar for the last
+// tensor layer reverse epilogue: stashed pre-activations and output adjoints (columns X, or w_last * ubar for the last
 // hidden layer: flag) -> Zbar tiles in P (the bias gradient is a column sum of Zbar_0, taken by an MMA chain against
-// the ones atom).  The stash is read from HBM more often than from L2 (148 CTAs x 1.5 MB in flight > L2); the next
-// granule's loads are in flight while the current one is processed.  Measured on the same box (profiles/
-// r01_wide_timeline.md): no prefetch 0.652 ms, this 0.648 ms, two granules ahead 0.737 ms (spills), bf16 stash of the
-// derivative channels 0.669 ms and 4x the gradient error -- the phase is bound by the burst of HBM reads, not by latency.
+// the ones atom).  The stash is read from HBM more often than from L2 (132 CTAs x 1.5 MB in flight > the 50 MB L2); the
+// next granule's loads are in flight while the current one is processed.
 template <int N1, int N2, bool PURE, int AK>
 __device__ __forceinline__ void tw_bwd_loop(const LoopW lc, const Chan<N1, N2> ch, const float* ubp, const float2* zst) {
   constexpr int C = 1 + N1 + N2;
@@ -172,8 +168,7 @@ __device__ __forceinline__ void tw_bwd_loop(const LoopW lc, const Chan<N1, N2> c
     float hb[C][4];
     if (!lc.flag) {
 #pragma unroll
-      for (int c = 0; c < C; ++c) tmem_ld4(lc.taddr + c * kTwW + ocol, hb[c]);
-      tc::tmem_ld_wait();
+      for (int c = 0; c < C; ++c) acc_ld4(lc.taddr + c * kTwW + ocol, hb[c]);
     } else {
 #pragma unroll
       for (int i = 0; i < 4; ++i) {
@@ -204,7 +199,7 @@ __device__ __forceinline__ void tw_bwd_loop(const LoopW lc, const Chan<N1, N2> c
   }
 }
 
-// layer 0 reverse: adjoints of H^0 (TMEM X) -> Zbar^0 tiles of the value + first-derivative channels in P
+// layer 0 reverse: adjoints of H^0 (columns X) -> Zbar^0 tiles of the value + first-derivative channels in P
 template <int N1, int N2, bool PURE, int AK>
 __device__ __forceinline__ void tw_l0_bwd_store_loop(const LoopW lc, const PassInfo<N1, N2> pi, const float* xp) {
   constexpr int C = 1 + N1 + N2;
@@ -216,8 +211,7 @@ __device__ __forceinline__ void tw_l0_bwd_store_loop(const LoopW lc, const PassI
     const int col = g * 2;
     float hb[C][2];
 #pragma unroll
-    for (int c = 0; c < C; ++c) tmem_ld2(lc.taddr + c * kTwW + col, hb[c]);
-    tc::tmem_ld_wait();
+    for (int c = 0; c < C; ++c) acc_ld2(lc.taddr + c * kTwW + col, hb[c]);
     float za[C], zb2[C];
     first_layer_elem_w<N1, N2>(lc.fp, pi, x, col, za);
     first_layer_elem_w<N1, N2>(lc.fp, pi, x, col + 1, zb2);
@@ -233,26 +227,24 @@ __device__ __forceinline__ void tw_l0_bwd_store_loop(const LoopW lc, const PassI
   }
 }
 
-// ---- issuing-lane helpers (one elected lane of warp 0; phases live in shared memory) --------------------------------
+// ---- streaming helpers: thread 0 issues the bulk loads, every thread waits for them -----------------------------------
 __device__ __forceinline__ void tw_load(TwShared* cs, int b, uint32_t dst, const uint8_t* src, int n_tiles) {
   tc::mbar_arrive_expect_tx(&cs->bar_ld[b], (uint32_t)n_tiles * TB);
   for (int i = 0; i < n_tiles; ++i)
     tc::bulk_load_u(dst + (uint32_t)i * TB, src + (size_t)i * TB, TB, tc::smem_u32(&cs->bar_ld[b]));
 }
+// CTA-wide: the next read of cs->ph_ld[b] must follow another __syncthreads
 __device__ __forceinline__ void tw_wait_ld(TwShared* cs, int b) {
-  tc::mbar_wait(&cs->bar_ld[b], cs->ph_ld[b]);
-  cs->ph_ld[b] ^= 1u;
-}
-__device__ __forceinline__ void tw_wait_free(TwShared* cs, int b) {
-  tc::mbar_wait(&cs->bar_free[b], cs->ph_free[b]);
-  cs->ph_free[b] ^= 1u;
+  const uint32_t ph = cs->ph_ld[b];
+  tc::mbar_wait(&cs->bar_ld[b], ph);
+  __syncthreads();
+  if (threadIdx.x == 0) cs->ph_ld[b] = ph ^ 1u;
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
-// forward of one network for the current tile.  Returns the updated parity of the MMA barrier.
+// forward of one network for the current tile
 template <int N1, int N2, bool PURE, int AK>
-__device__ __noinline__ uint32_t tw_net_forward(TwShared* cs, const DevProblem* Pp, const DevTerm* tmp, int slot,
-                                                int want_grad, uint32_t mma_phase) {
+__device__ __noinline__ void tw_net_forward(TwShared* cs, const DevProblem* Pp, const DevTerm* tmp, int slot, int want_grad) {
   extern __shared__ __align__(1024) uint8_t smem[];
   constexpr int C = 1 + N1 + N2;
   const DevTerm& tm = *tmp;
@@ -263,7 +255,7 @@ __device__ __noinline__ uint32_t tw_net_forward(TwShared* cs, const DevProblem* 
   uint8_t* tP = smem + cs->off_P;
   uint8_t* tS = smem + cs->off_S;
   const Misc ms = misc_of(smem + cs->off_misc, cs->mx_dim, cs->mx_taps);
-  const uint32_t tmem = cs->tmem;
+  const uint32_t accm = 0;   // accumulator address of row 0, column 0
   PassInfo<N1, N2> pi;
   load_pass<N1, N2>(pi, net, dc);
   const int TL = pi.TL;
@@ -282,80 +274,59 @@ __device__ __noinline__ uint32_t tw_net_forward(TwShared* cs, const DevProblem* 
   for (int c = 0; c < C; ++c) u[c] = 0.f;
   if (tid < C * kTcPts / 4) reinterpret_cast<float4*>(ms.scratch)[tid] = make_float4(0.f, 0.f, 0.f, 0.f);
   // first tensor layer's weights stream in behind the layer-0 epilogue (buffer S[1])
-  if (tc::uni(t.warp) == 0) {
-    const uint32_t u_S = tc::uni(tc::smem_u32(tS));
-    const uint64_t u_w = tc::uni((uint64_t)wimg);
-    const int u_nb = tc::uni((net.dims[1] + 63) >> 6);
-    if (tc::elect_one()) {
-      tc::fence_async_smem();
-      tw_load(cs, 1, u_S + kTwImgBytes, (const uint8_t*)u_w, u_nb);
-    }
-    __syncwarp();
+  if (tid == 0) {
+    tc::fence_async_smem();
+    tw_load(cs, 1, tc::smem_u32(tS) + kTwImgBytes, wimg, (net.dims[1] + 63) >> 6);
   }
   {
     const int ng = pi.n1w / 4;
     LoopW lc;
     lc.fp = tc::smem_u32(fp); lc.bt = lc.fp; lc.tP = tc::smem_u32(tP); lc.gb = nullptr;
-    lc.taddr = tmem + t.lane_addr; lc.act = net.acts[0]; lc.p = p; lc.lane = t.lane;
+    lc.taddr = accm + t.lane_addr; lc.act = net.acts[0]; lc.p = p; lc.lane = t.lane;
     lc.g0 = hh * (ng / kNH); lc.g1 = (hh + 1) * (ng / kNH); lc.flag = 0;
     tw_l0_fwd_loop<N1, N2, PURE, AK>(lc, pi, x);
   }
   for (int l = 1; l <= TL; ++l) {
     const int n_in = net.dims[l], n_out = net.dims[l + 1];
     tc::fence_async_smem();
-    tc::tc_fence_before();
     __syncthreads();
     dbg_mark(cs, 11);
-    if (tc::uni(t.warp) == 0) {
-      const uint32_t u_tmem = tc::uni(tmem), u_P = tc::uni(tc::smem_u32(tP)), u_S = tc::uni(tc::smem_u32(tS));
-      const int u_nin = tc::uni(n_in), u_nout = tc::uni(n_out), u_wg = tc::uni(want_grad), u_l = tc::uni(l), u_TL = tc::uni(TL);
-      const int u_nnext = tc::uni(l < TL ? net.dims[l + 1] : 0);
-      const uint64_t u_hst = tc::uni((uint64_t)(hst + (size_t)(l - 1) * kTwMaxC * 2 * TB));
-      const uint64_t u_w = tc::uni((uint64_t)wimg);
-      if (tc::elect_one()) {
-        tc::tc_fence_after();
-        const int nb_in = (u_nin + 63) >> 6;
-        if (u_wg) {
-#pragma unroll 1
-          for (int c = 0; c < C; ++c)
-            for (int kb = 0; kb < nb_in; ++kb)
-              tc::bulk_store_u((void*)(u_hst + (uint64_t)(c * 2 + kb) * TB), u_P + (c * 2 + kb) * TB, TB);
-          tc::bulk_commit();
-        }
-        if (u_l < u_TL)     // next layer's weights -> the other buffer (its last readers, layer l-1's MMAs, have retired)
-          tw_load(cs, (u_l + 1) & 1, u_S + ((u_l + 1) & 1) * kTwImgBytes, (const uint8_t*)u_w + (size_t)u_l * kTwImgBytes,
-                  (u_nnext + 63) >> 6);
-        tw_wait_ld(cs, u_l & 1);
-        const uint32_t idesc = tc::make_idesc(128, u_nout, 0, 0);
-        const uint32_t wbuf = u_S + (u_l & 1) * kTwImgBytes;
-#pragma unroll 1
-        for (int c = 0; c < C; ++c) {
-          const uint32_t d = u_tmem + c * kTwW;
-#pragma unroll 1
-          for (int kb = 0; kb < nb_in; ++kb) {
-            const int nk = ((u_nin - kb * 64) < 64 ? (u_nin - kb * 64) : 64) >> 4;
-            mma_chain(d, tc::make_desc(u_P + (c * 2 + kb) * TB, 0, 1024), tc::make_desc(wbuf + kb * TB, 0, 1024), 32, 32, nk,
-                      idesc, kb > 0 ? 1u : 0u);
-          }
-        }
-        tc::mma_commit(ms.bar_mma);
+    const uint32_t sP = tc::smem_u32(tP), sS = tc::smem_u32(tS);
+    const int nb_in = (n_in + 63) >> 6;
+    if (tid == 0) {
+      if (want_grad) {
+        uint8_t* h = hst + (size_t)(l - 1) * kTwMaxC * 2 * TB;
+        for (int c = 0; c < C; ++c)
+          for (int kb = 0; kb < nb_in; ++kb) tc::bulk_store(h + (size_t)(c * 2 + kb) * TB, tP + (c * 2 + kb) * TB, TB);
+        tc::bulk_commit();
       }
-      __syncwarp();
+      if (l < TL)     // next layer's weights -> the other buffer (its last readers, layer l-1's MMAs, have retired)
+        tw_load(cs, (l + 1) & 1, sS + ((l + 1) & 1) * kTwImgBytes, wimg + (size_t)l * kTwImgBytes, (net.dims[l + 1] + 63) >> 6);
+    }
+    tw_wait_ld(cs, l & 1);
+    {
+      const uint32_t idesc = tc::make_idesc(n_out, 0, 0);
+      const uint32_t wbuf = sS + (l & 1) * kTwImgBytes;
+#pragma unroll 1
+      for (int c = 0; c < C; ++c) {
+#pragma unroll 1
+        for (int kb = 0; kb < nb_in; ++kb) {
+          const int nk = ((n_in - kb * 64) < 64 ? (n_in - kb * 64) : 64) >> 4;
+          mma_chain(accm + c * kTwW, tc::make_desc(sP + (c * 2 + kb) * TB, 0, 1024), tc::make_desc(wbuf + kb * TB, 0, 1024), 32, 32,
+                    nk, idesc, kb > 0 ? 1u : 0u);
+        }
+      }
     }
     dbg_mark(cs, 12);
-    wait_bar(ms.bar_mma, mma_phase);
-    tc::tc_fence_after();
+    __syncthreads();
     dbg_mark(cs, 13);
-    if (want_grad && tc::uni(t.warp) == 0) {
-      if (tc::elect_one()) tc::bulk_wait_read0();       // stash copies have finished reading P
-      __syncwarp();
-    }
+    if (want_grad && tid == 0) tc::bulk_wait_read0();   // stash copies have finished reading P
     __syncthreads();
     dbg_mark(cs, 14);
     const int ng = n_out / 4;
     LoopW lc;
     lc.fp = tc::smem_u32(fp); lc.bt = lc.fp + (FW_BT + (l - 1) * 128) * 4; lc.tP = tc::smem_u32(tP); lc.gb = nullptr;
-    lc.taddr = tmem + t.lane_addr; lc.act = net.acts[l]; lc.p = p; lc.lane = t.lane;
+    lc.taddr = accm + t.lane_addr; lc.act = net.acts[l]; lc.p = p; lc.lane = t.lane;
     lc.g0 = hh * (ng / kNH); lc.g1 = (hh + 1) * (ng / kNH); lc.flag = (l == TL) ? 1 : 0;
     float2* zl = want_grad ? reinterpret_cast<float2*>(zst + (size_t)(l - 1) * kTwMaxC * 64 * kTcPts * 2) + p : nullptr;
     tw_fwd_loop<N1, N2, PURE, AK>(lc, pi.ch, u, zl);
@@ -365,19 +336,13 @@ __device__ __noinline__ uint32_t tw_net_forward(TwShared* cs, const DevProblem* 
     // several passes share P: keep this pass's last hidden activations for its reverse sweep
     tc::fence_async_smem();
     __syncthreads();
-    if (tc::uni(t.warp) == 0) {
-      const uint32_t u_P = tc::uni(tc::smem_u32(tP));
-      const uint64_t u_hst = tc::uni((uint64_t)(hst + (size_t)TL * kTwMaxC * 2 * TB));
-      const int u_nb = tc::uni((pi.nL + 63) >> 6);
-      if (tc::elect_one()) {
-#pragma unroll 1
-        for (int c = 0; c < C; ++c)
-          for (int kb = 0; kb < u_nb; ++kb)
-            tc::bulk_store_u((void*)(u_hst + (uint64_t)(c * 2 + kb) * TB), u_P + (c * 2 + kb) * TB, TB);
-        tc::bulk_commit();
-        tc::bulk_wait_read0();
-      }
-      __syncwarp();
+    if (tid == 0) {
+      uint8_t* h = hst + (size_t)TL * kTwMaxC * 2 * TB;
+      const int nb = (pi.nL + 63) >> 6;
+      for (int c = 0; c < C; ++c)
+        for (int kb = 0; kb < nb; ++kb) tc::bulk_store(h + (size_t)(c * 2 + kb) * TB, tP + (c * 2 + kb) * TB, TB);
+      tc::bulk_commit();
+      tc::bulk_wait_read0();
     }
   }
   __syncthreads();
@@ -401,18 +366,16 @@ __device__ __noinline__ uint32_t tw_net_forward(TwShared* cs, const DevProblem* 
   }
   __syncthreads();
   dbg_mark(cs, 16);
-  return mma_phase;
 }
 
 // reverse sweep of one network for the current tile (P still holds the last hidden activations)
 template <int N1, int N2, bool PURE, int AK>
-__device__ __noinline__ uint32_t tw_net_backward(TwShared* cs, const DevProblem* Pp, const DevTerm* tmp, int slot,
-                                                 uint32_t mma_phase) {
+__device__ __noinline__ void tw_net_backward(TwShared* cs, const DevProblem* Pp, const DevTerm* tmp, int slot) {
   extern __shared__ __align__(1024) uint8_t smem[];
   constexpr int C = 1 + N1 + N2;
-  constexpr uint32_t WG = (C <= 3) ? 384u : 0u;       // TMEM column of the weight-gradient accumulator
-  constexpr uint32_t BC = (C <= 2) ? 256u : 128u;     // TMEM column of the bias-gradient column sums (16 columns)
-  // dgrad channels whose TMEM columns hold the weight / bias gradient until it is flushed: issued after the flush
+  constexpr uint32_t WG = (C <= 3) ? 384u : 0u;       // accumulator column of the weight gradient
+  constexpr uint32_t BC = (C <= 2) ? 256u : 128u;     // accumulator column of the bias-gradient column sums (16 columns)
+  // dgrad channels whose accumulator columns hold the weight / bias gradient until it is flushed: issued after the flush
   constexpr uint32_t DEFER = (C == 4) ? 0x3u : ((C == 3) ? 0x2u : 0x0u);
   const DevTerm& tm = *tmp;
   const int net_id = tm.used_net[slot];
@@ -422,7 +385,7 @@ __device__ __noinline__ uint32_t tw_net_backward(TwShared* cs, const DevProblem*
   uint8_t* tP = smem + cs->off_P;
   uint8_t* tS = smem + cs->off_S;
   const Misc ms = misc_of(smem + cs->off_misc, cs->mx_dim, cs->mx_taps);
-  const uint32_t tmem = cs->tmem;
+  const uint32_t accm = 0;   // accumulator address of row 0, column 0
   float* partial = cs->partial;
   PassInfo<N1, N2> pi;
   load_pass<N1, N2>(pi, net, dc);
@@ -439,21 +402,15 @@ __device__ __noinline__ uint32_t tw_net_backward(TwShared* cs, const DevProblem*
   dbg_mark(cs, 20);
   if (tm.n_used > 1) {
     // restore this pass's last hidden activations into P
-    if (tc::uni(t.warp) == 0) {
-      const uint32_t u_P = tc::uni(tc::smem_u32(tP));
-      const uint64_t u_hst = tc::uni((uint64_t)(hst + (size_t)TL * kTwMaxC * 2 * TB));
-      const int u_nb = tc::uni((pi.nL + 63) >> 6);
-      if (tc::elect_one()) {
-        tc::fence_async_smem();
-        tc::mbar_arrive_expect_tx(&cs->bar_ld[0], (uint32_t)(C * u_nb) * TB);
-#pragma unroll 1
-        for (int c = 0; c < C; ++c)
-          for (int kb = 0; kb < u_nb; ++kb)
-            tc::bulk_load_u(u_P + (c * 2 + kb) * TB, (const void*)(u_hst + (uint64_t)(c * 2 + kb) * TB), TB, tc::smem_u32(&cs->bar_ld[0]));
-        tw_wait_ld(cs, 0);
-      }
-      __syncwarp();
+    if (tid == 0) {
+      const uint8_t* h = hst + (size_t)TL * kTwMaxC * 2 * TB;
+      const int nb = (pi.nL + 63) >> 6;
+      tc::fence_async_smem();
+      tc::mbar_arrive_expect_tx(&cs->bar_ld[0], (uint32_t)(C * nb) * TB);
+      for (int c = 0; c < C; ++c)
+        for (int kb = 0; kb < nb; ++kb) tc::bulk_load(tP + (c * 2 + kb) * TB, h + (size_t)(c * 2 + kb) * TB, TB, &cs->bar_ld[0]);
     }
+    tw_wait_ld(cs, 0);
     __syncthreads();
   }
   float ub[C];
@@ -491,40 +448,29 @@ __device__ __noinline__ uint32_t tw_net_backward(TwShared* cs, const DevProblem*
       asm volatile("st.shared.v4.b32 [%0], {%1,%2,%3,%4};" ::"r"(q0 + tc::swz_chunk(p, 1)), "r"(0u), "r"(0u), "r"(0u), "r"(0u) : "memory");
     }
     tc::fence_async_smem();
-    tc::tc_fence_before();
     __syncthreads();
-    if (tc::uni(t.warp) == 0) {
-      const uint32_t u_tmem = tc::uni(tmem), u_P = tc::uni(tc::smem_u32(tP)), u_S = tc::uni(tc::smem_u32(tS));
-      const int u_nL = tc::uni(pi.nL);
-      if (tc::elect_one()) {
-        tc::tc_fence_after();
-        const uint32_t idesc = tc::make_idesc(128, 16, 1, 1);
-        const uint32_t a_lbo = (u_nL > 64) ? TB : 0u;
-        const uint64_t db = tc::make_desc(u_S, 0, 1024);
+    {
+      const uint32_t sP = tc::smem_u32(tP);
+      const uint32_t idesc = tc::make_idesc(16, 1, 1);
+      const uint32_t a_lbo = (pi.nL > 64) ? TB : 0u;
+      const uint64_t db = tc::make_desc(tc::smem_u32(tS), 0, 1024);
 #pragma unroll 1
-        for (int c = 0; c < C; ++c)
-          mma_chain(u_tmem + 16 * c, tc::make_desc(u_P + c * 2 * TB, a_lbo, 1024), db, 2048, 2048, kTcPts / 16, idesc, 0);
-        tc::mma_commit(ms.bar_mma);
-      }
-      __syncwarp();
+      for (int c = 0; c < C; ++c)
+        mma_chain(accm + 16 * c, tc::make_desc(sP + c * 2 * TB, a_lbo, 1024), db, 2048, 2048, kTcPts / 16, idesc, 0);
     }
-    wait_bar(ms.bar_mma, mma_phase);
-    tc::tc_fence_after();
+    __syncthreads();
     if (hh == 0) {
       const int o = q * 32 + lane;
       float acc = 0.f;
 #pragma unroll
       for (int c = 0; c < C; ++c) {
         float v[2];
-        tmem_ld2(tmem + t.lane_addr + 16 * c + 2 * c, v);
-        tc::tmem_ld_wait();
+        acc_ld2(accm + t.lane_addr + 16 * c + 2 * c, v);
         acc += v[0] + v[1];
       }
       if (o < pi.nL) atomicAdd(gw_last + o, acc);
     }
-    tc::tc_fence_before();
     __syncthreads();
-    tc::tc_fence_after();
   }
 
   // ---- tensor layers, last to first ------------------------------------------------------------------------------------
@@ -534,115 +480,82 @@ __device__ __noinline__ uint32_t tw_net_backward(TwShared* cs, const DevProblem*
     float* gw = partial + net.w_off[l];
     dbg_mark(cs, 21);
     // this layer's input tiles of channels 0 and 1 stream into S0 / S1 behind the epilogue
-    if (tc::uni(t.warp) == 0) {
-      const uint32_t u_S = tc::uni(tc::smem_u32(tS));
-      const uint64_t u_hst = tc::uni((uint64_t)(hst + (size_t)(l - 1) * kTwMaxC * 2 * TB));
-      const int u_nb = tc::uni((n_in + 63) >> 6);
-      if (tc::elect_one()) {
-        tc::fence_async_smem();
-        tw_load(cs, 0, u_S, (const uint8_t*)u_hst, u_nb);
-        if (C > 1) tw_load(cs, 1, u_S + kTwImgBytes, (const uint8_t*)u_hst + 2 * TB, u_nb);
-      }
-      __syncwarp();
+    if (tid == 0) {
+      const uint8_t* h = hst + (size_t)(l - 1) * kTwMaxC * 2 * TB;
+      const int nb = (n_in + 63) >> 6;
+      tc::fence_async_smem();
+      tw_load(cs, 0, tc::smem_u32(tS), h, nb);
+      if (C > 1) tw_load(cs, 1, tc::smem_u32(tS) + kTwImgBytes, h + 2 * TB, nb);
     }
     {
       const int ng = n_out / 4;
       LoopW lc;
       lc.fp = tc::smem_u32(fp); lc.bt = lc.fp; lc.tP = tc::smem_u32(tP); lc.gb = gb;
-      lc.taddr = tmem + t.lane_addr; lc.act = net.acts[l]; lc.p = p; lc.lane = lane;
+      lc.taddr = accm + t.lane_addr; lc.act = net.acts[l]; lc.p = p; lc.lane = lane;
       lc.g0 = hh * (ng / kNH); lc.g1 = (hh + 1) * (ng / kNH); lc.flag = (l == TL) ? 1 : 0;
       const float2* zl = reinterpret_cast<const float2*>(zst + (size_t)(l - 1) * kTwMaxC * 64 * kTcPts * 2) + p;
       tw_bwd_loop<N1, N2, PURE, AK>(lc, pi.ch, ub, zl);
     }
     tc::fence_async_smem();
-    tc::tc_fence_before();
     __syncthreads();
     dbg_mark(cs, 26);
-    // wgrad: Wbar_l[o][k] = sum_c sum_p Zbar_c[p][o] H_c[p][k]  -> TMEM columns WG .. WG + n_in (lane = o)
-    if (tc::uni(t.warp) == 0) {
-      const uint32_t u_tmem = tc::uni(tmem), u_P = tc::uni(tc::smem_u32(tP)), u_S = tc::uni(tc::smem_u32(tS));
-      const int u_nin = tc::uni(n_in), u_nout = tc::uni(n_out), u_l = tc::uni(l);
-      const uint32_t u_ones = tc::uni(tc::smem_u32(smem + cs->off_ones));
-      const uint64_t u_hst = tc::uni((uint64_t)(hst + (size_t)(l - 1) * kTwMaxC * 2 * TB));
-      const uint64_t u_w = tc::uni((uint64_t)wimg);
-      if (tc::elect_one()) {
-        tc::tc_fence_after();
-        const int nb_in = (u_nin + 63) >> 6;
-        const uint32_t iwg = tc::make_idesc(128, u_nin, 1, 1);
-        const uint32_t a_lbo = (u_nout > 64) ? TB : 0u;      // rows >= 64 of M: next tile, or alias rows - 64 when n_out <= 64
-        if (C == 1) tw_load(cs, 1, u_S + kTwImgBytes, (const uint8_t*)u_w + (size_t)(u_l - 1) * kTwImgBytes, nb_in);
-        int pend0 = 0, pend1 = 0;
+    // wgrad: Wbar_l[o][k] = sum_c sum_p Zbar_c[p][o] H_c[p][k]  -> accumulator columns WG .. WG + n_in (row = o)
+    const uint32_t sP = tc::smem_u32(tP), sS = tc::smem_u32(tS);
+    {
+      const int nb_in = (n_in + 63) >> 6;
+      const uint32_t iwg = tc::make_idesc(n_in, 1, 1);
+      const uint32_t a_lbo = (n_out > 64) ? TB : 0u;      // rows >= 64 of M: the next tile (n_out = 128)
+      const uint8_t* h = hst + (size_t)(l - 1) * kTwMaxC * 2 * TB;
+      if (C == 1 && tid == 0) tw_load(cs, 1, sS + kTwImgBytes, wimg + (size_t)(l - 1) * kTwImgBytes, nb_in);
 #pragma unroll 1
-        for (int c = 0; c < C; ++c) {
-          const int b = c & 1;
-          tw_wait_ld(cs, b);
-          mma_chain(u_tmem + WG, tc::make_desc(u_P + (c * 2) * TB, a_lbo, 1024), tc::make_desc(u_S + b * kTwImgBytes, TB, 1024),
-                    2048, 2048, kTcPts / 16, iwg, c > 0 ? 1u : 0u);
-          tc::mma_commit(&cs->bar_free[b]);
-          if (b) pend1 = 1; else pend0 = 1;
-          if (c + 2 < C) {
-            tw_wait_free(cs, b);
-            if (b) pend1 = 0; else pend0 = 0;
-            tw_load(cs, b, u_S + b * kTwImgBytes, (const uint8_t*)u_hst + (size_t)(c + 2) * 2 * TB, nb_in);
-          } else if (c == C - 2) {
-            // W_l for dgrad goes into the buffer wgrad releases first
-            tw_wait_free(cs, b);
-            if (b) pend1 = 0; else pend0 = 0;
-            tw_load(cs, b, u_S + b * kTwImgBytes, (const uint8_t*)u_w + (size_t)(u_l - 1) * kTwImgBytes, nb_in);
-          }
+      for (int c = 0; c < C; ++c) {
+        const int b = c & 1;
+        tw_wait_ld(cs, b);
+        mma_chain(accm + WG, tc::make_desc(sP + (c * 2) * TB, a_lbo, 1024), tc::make_desc(sS + b * kTwImgBytes, TB, 1024),
+                  2048, 2048, kTcPts / 16, iwg, c > 0 ? 1u : 0u);
+        __syncthreads();      // S[b] has been read
+        if (tid == 0) {
+          if (c + 2 < C) tw_load(cs, b, sS + b * kTwImgBytes, h + (size_t)(c + 2) * 2 * TB, nb_in);
+          else if (c == C - 2)   // W_l for dgrad goes into the buffer wgrad releases first
+            tw_load(cs, b, sS + b * kTwImgBytes, wimg + (size_t)(l - 1) * kTwImgBytes, nb_in);
         }
-        // bias gradient: bbar_l[o] = sum_p Zbar_0[p][o]  (B = the constant ones atom: SBO = 0, no k advance)
-        mma_chain(u_tmem + BC, tc::make_desc(u_P, a_lbo, 1024), tc::make_desc(u_ones, 0, 0), 2048, 0, kTcPts / 16,
-                  tc::make_idesc(128, 16, 1, 1), 0);
-        if (pend0) tw_wait_free(cs, 0);
-        if (pend1) tw_wait_free(cs, 1);
-        tc::mma_commit(ms.bar_mma);
       }
-      __syncwarp();
+      // bias gradient: bbar_l[o] = sum_p Zbar_0[p][o]  (B = the constant ones atom: SBO = 0, no k advance)
+      mma_chain(accm + BC, tc::make_desc(sP, a_lbo, 1024), tc::make_desc(tc::smem_u32(smem + cs->off_ones), 0, 0), 2048, 0,
+                kTcPts / 16, tc::make_idesc(16, 1, 1), 0);
     }
     dbg_mark(cs, 27);
-    wait_bar(ms.bar_mma, mma_phase);
-    tc::tc_fence_after();
+    __syncthreads();
     dbg_mark(cs, 28);
     // dgrad: Hbar_c[p][k] = sum_o Zbar_c[p][o] W_l[o][k] -> X (channel c at column c*128); W_l sits in S[C & 1]
     const int wb = C & 1;
-    if (tc::uni(t.warp) == 0) {
-      const uint32_t u_tmem = tc::uni(tmem), u_P = tc::uni(tc::smem_u32(tP)), u_S = tc::uni(tc::smem_u32(tS));
-      const int u_nin = tc::uni(n_in), u_nout = tc::uni(n_out);
-      if (tc::elect_one()) {
-        tw_wait_ld(cs, wb);
-        const int nb_out = (u_nout + 63) >> 6;
-        const uint32_t idg = tc::make_idesc(128, u_nin, 0, 1);
-        const uint32_t wbuf = u_S + wb * kTwImgBytes;
+    tw_wait_ld(cs, wb);
+    const int nb_out = (n_out + 63) >> 6;
+    const uint32_t idg = tc::make_idesc(n_in, 0, 1);
+    const uint32_t wbuf = sS + wb * kTwImgBytes;
 #pragma unroll 1
-        for (int c = C - 1; c >= 0; --c) {
-          if ((DEFER >> c) & 1u) continue;
+    for (int c = C - 1; c >= 0; --c) {
+      if ((DEFER >> c) & 1u) continue;
 #pragma unroll 1
-          for (int ob = 0; ob < nb_out; ++ob) {
-            const int nk = ((u_nout - ob * 64) < 64 ? (u_nout - ob * 64) : 64) >> 4;
-            mma_chain(u_tmem + c * kTwW, tc::make_desc(u_P + (c * 2 + ob) * TB, 0, 1024), tc::make_desc(wbuf + ob * 8192, TB, 1024),
-                      32, 2048, nk, idg, ob > 0 ? 1u : 0u);
-          }
-        }
-        if (DEFER == 0) tc::mma_commit(ms.bar_mma);
+      for (int ob = 0; ob < nb_out; ++ob) {
+        const int nk = ((n_out - ob * 64) < 64 ? (n_out - ob * 64) : 64) >> 4;
+        mma_chain(accm + c * kTwW, tc::make_desc(sP + (c * 2 + ob) * TB, 0, 1024), tc::make_desc(wbuf + ob * 8192, TB, 1024),
+                  32, 2048, nk, idg, ob > 0 ? 1u : 0u);
       }
-      __syncwarp();
     }
-    // flush the weight-gradient accumulator: TMEM lane = output neuron o, column = input neuron k
+    // flush the weight-gradient accumulator: accumulator row = output neuron o, column = input neuron k
     {
       const int o = q * 32 + lane;
       if (hh == 0) {
         float v[2];
-        tmem_ld2(tmem + t.lane_addr + BC, v);
-        tc::tmem_ld_wait();
+        acc_ld2(accm + t.lane_addr + BC, v);
         if (o < n_out) atomicAdd(gb + o, v[0]);
       }
       const int part = n_in / kNH;
 #pragma unroll 1
       for (int k0 = hh * part; k0 < (hh + 1) * part; k0 += 4) {
         float v[4];
-        tmem_ld4(tmem + t.lane_addr + WG + k0, v);
-        tc::tmem_ld_wait();
+        acc_ld4(accm + t.lane_addr + WG + k0, v);
         if (o < n_out) {
 #pragma unroll
           for (int i = 0; i < 4; ++i) atomicAdd(gw + o + (long long)n_out * (k0 + i), v[i]);
@@ -651,33 +564,19 @@ __device__ __noinline__ uint32_t tw_net_backward(TwShared* cs, const DevProblem*
     }
     if (DEFER != 0) {
       // the remaining channels' adjoints land on the columns the weight / bias gradient just left
-      tc::tc_fence_before();
       __syncthreads();
-      if (tc::uni(t.warp) == 0) {
-        const uint32_t u_tmem = tc::uni(tmem), u_P = tc::uni(tc::smem_u32(tP)), u_S = tc::uni(tc::smem_u32(tS));
-        const int u_nin = tc::uni(n_in), u_nout = tc::uni(n_out);
-        if (tc::elect_one()) {
-          tc::tc_fence_after();
-          const int nb_out = (u_nout + 63) >> 6;
-          const uint32_t idg = tc::make_idesc(128, u_nin, 0, 1);
-          const uint32_t wbuf = u_S + wb * kTwImgBytes;
 #pragma unroll 1
-          for (int c = C - 1; c >= 0; --c) {
-            if (!((DEFER >> c) & 1u)) continue;
+      for (int c = C - 1; c >= 0; --c) {
+        if (!((DEFER >> c) & 1u)) continue;
 #pragma unroll 1
-            for (int ob = 0; ob < nb_out; ++ob) {
-              const int nk = ((u_nout - ob * 64) < 64 ? (u_nout - ob * 64) : 64) >> 4;
-              mma_chain(u_tmem + c * kTwW, tc::make_desc(u_P + (c * 2 + ob) * TB, 0, 1024),
-                        tc::make_desc(wbuf + ob * 8192, TB, 1024), 32, 2048, nk, idg, ob > 0 ? 1u : 0u);
-            }
-          }
-          tc::mma_commit(ms.bar_mma);
+        for (int ob = 0; ob < nb_out; ++ob) {
+          const int nk = ((n_out - ob * 64) < 64 ? (n_out - ob * 64) : 64) >> 4;
+          mma_chain(accm + c * kTwW, tc::make_desc(sP + (c * 2 + ob) * TB, 0, 1024), tc::make_desc(wbuf + ob * 8192, TB, 1024),
+                    32, 2048, nk, idg, ob > 0 ? 1u : 0u);
         }
-        __syncwarp();
       }
     }
-    wait_bar(ms.bar_mma, mma_phase);
-    tc::tc_fence_after();
+    __syncthreads();
     dbg_mark(cs, 29);
   }
 
@@ -716,38 +615,29 @@ __device__ __noinline__ uint32_t tw_net_backward(TwShared* cs, const DevProblem*
       const int ng = pi.n1w / 2;
       LoopW lc;
       lc.fp = tc::smem_u32(fp); lc.bt = lc.fp; lc.tP = tc::smem_u32(tP); lc.gb = gb0;
-      lc.taddr = tmem + t.lane_addr; lc.act = net.acts[0]; lc.p = p; lc.lane = lane;
+      lc.taddr = accm + t.lane_addr; lc.act = net.acts[0]; lc.p = p; lc.lane = lane;
       lc.g0 = hh * (ng / kNH); lc.g1 = (hh + 1) * (ng / kNH); lc.flag = 0;
       tw_l0_bwd_store_loop<N1, N2, PURE, AK>(lc, pi, x);
     }
     tc::fence_async_smem();
-    tc::tc_fence_before();
     __syncthreads();
-    if (tc::uni(t.warp) == 0) {
-      const uint32_t u_tmem = tc::uni(tmem), u_P = tc::uni(tc::smem_u32(tP)), u_S = tc::uni(tc::smem_u32(tS));
-      const int u_n1w = tc::uni(pi.n1w);
-      if (tc::elect_one()) {
-        tc::tc_fence_after();
-        const uint32_t idesc = tc::make_idesc(128, 16, 1, 1);
-        const uint32_t a_lbo = (u_n1w > 64) ? TB : 0u;
-        const uint64_t a0 = tc::make_desc(u_P, a_lbo, 1024);
-        mma_chain(u_tmem + WG, a0, tc::make_desc(u_S, 0, 1024), 2048, 2048, kTcPts / 16, idesc, 0);
-        if (kLo) mma_chain(u_tmem + WG, a0, tc::make_desc(u_S + (1 + N1) * TB, 0, 1024), 2048, 2048, kTcPts / 16, idesc, 1);
+    {
+      const uint32_t sP = tc::smem_u32(tP), sS = tc::smem_u32(tS);
+      const uint32_t idesc = tc::make_idesc(16, 1, 1);
+      const uint32_t a_lbo = (pi.n1w > 64) ? TB : 0u;
+      const uint64_t a0 = tc::make_desc(sP, a_lbo, 1024);
+      mma_chain(accm + WG, a0, tc::make_desc(sS, 0, 1024), 2048, 2048, kTcPts / 16, idesc, 0);
+      if (kLo) mma_chain(accm + WG, a0, tc::make_desc(sS + (1 + N1) * TB, 0, 1024), 2048, 2048, kTcPts / 16, idesc, 1);
 #pragma unroll 1
-        for (int j = 0; j < N1; ++j)
-          mma_chain(u_tmem + WG, tc::make_desc(u_P + (1 + j) * 2 * TB, a_lbo, 1024), tc::make_desc(u_S + (1 + j) * TB, 0, 1024),
-                    2048, 2048, kTcPts / 16, idesc, 1);
-        tc::mma_commit(ms.bar_mma);
-      }
-      __syncwarp();
+      for (int j = 0; j < N1; ++j)
+        mma_chain(accm + WG, tc::make_desc(sP + (1 + j) * 2 * TB, a_lbo, 1024), tc::make_desc(sS + (1 + j) * TB, 0, 1024),
+                  2048, 2048, kTcPts / 16, idesc, 1);
     }
-    wait_bar(ms.bar_mma, mma_phase);
-    tc::tc_fence_after();
+    __syncthreads();
     if (hh == 0) {
       const int o = q * 32 + lane;
       float v[16];
-      tc::tmem_ld16(tmem + t.lane_addr + WG, v);
-      tc::tmem_ld_wait();
+      tc::acc_ld16(accm + t.lane_addr + WG, v);
       if (o < pi.n1w) {
 #pragma unroll
         for (int k = 0; k < PINN_MAX_IN; ++k)
@@ -756,10 +646,8 @@ __device__ __noinline__ uint32_t tw_net_backward(TwShared* cs, const DevProblem*
       }
     }
   }
-  tc::tc_fence_before();
   __syncthreads();
   dbg_mark(cs, 30);
-  return mma_phase;
 }
 
 
@@ -806,7 +694,7 @@ __global__ void __launch_bounds__(256) tw_pack_kernel(const TwPackArgs a) {
 __global__ void __launch_bounds__(kTcThreads, 1) tw_loss_grad_kernel(const __grid_constant__ TwArgs args) {
   extern __shared__ __align__(1024) uint8_t smem[];
   __shared__ TwShared cs;
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int tid = threadIdx.x, lane = tid & 31;
   const DevProblem* Pp = args.prob;
   const DevProblem& P = *Pp;
   const Misc ms = misc_of(smem + args.off_misc, args.mx_dim, args.mx_taps);
@@ -824,12 +712,10 @@ __global__ void __launch_bounds__(kTcThreads, 1) tw_loss_grad_kernel(const __gri
 
   // ---- per-CTA setup --------------------------------------------------------------------------------------------------------
   if (tid == 0) {
-    tc::mbar_init(ms.bar_mma, 1);
     tc::mbar_init(ms.bar_ld, 1);            // collocation-tile bulk loads (own barrier: the weight stream uses cs.bar_ld[])
     for (int b = 0; b < 2; ++b) {
       tc::mbar_init(&cs.bar_ld[b], 1);
-      tc::mbar_init(&cs.bar_free[b], 1);
-      cs.ph_ld[b] = 0; cs.ph_free[b] = 0;
+      cs.ph_ld[b] = 0;
     }
     tc::fence_barrier_init();
     cs.tl_max = args.tl_max; cs.off_P = args.off_P; cs.off_S = args.off_S; cs.off_misc = args.off_misc; cs.off_ones = args.off_ones; cs.off_nets = args.off_nets; cs.mx_dim = args.mx_dim; cs.mx_taps = args.mx_taps;
@@ -848,7 +734,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) tw_loss_grad_kernel(const __gri
     if (cs.dbg) cs.dbg[cs.dbg_n++] = ((long long)1 << 48) | (clock64() & 0xffffffffffffLL);
 #endif
   }
-  if (warp == 0) tc::tmem_alloc<512>(ms.tmem_slot);
+  if (tid == 0) tc::s_acc = args.acc + (size_t)blockIdx.x * kAccCols * kAccRows;
   if (want_grad) {
     const long long n4 = P.n_theta / 4;
     float4* p4 = reinterpret_cast<float4*>(partial);
@@ -895,13 +781,8 @@ __global__ void __launch_bounds__(kTcThreads, 1) tw_loss_grad_kernel(const __gri
     if (tid == 0) fp[FW_BL] = __ldg(&theta[bl]);
   }
   tc::fence_async_smem();
-  tc::tc_fence_before();
-  __syncthreads();
-  tc::tc_fence_after();
-  if (tid == 0) cs.tmem = *ms.tmem_slot;
   __syncthreads();
   dbg_mark(&cs, 2);
-  uint32_t phase = 0;
   uint32_t tile_ld_phase = 0;      // parity of the collocation-tile barrier (ms.bar_ld)
 
   // tiles are claimed dynamically after the first one (heavy PDE tiles come first in the enumeration, cheap boundary
@@ -950,7 +831,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) tw_loss_grad_kernel(const __gri
     for (int slot = 0; slot < n_used; ++slot) {
       const int k1 = tm.chan[slot].n1, k2 = tm.chan[slot].n2, pu = tm.chan[slot].pure;
       const int ak = args.net_ak[tm.used_net[slot]];
-      PINN_TW_DISPATCH(k1, k2, pu, ak, (phase = tw_net_forward<A1, A2, PU, AK>(&cs, Pp, tmp, slot, want_grad ? 1 : 0, phase)));
+      PINN_TW_DISPATCH(k1, k2, pu, ak, (tw_net_forward<A1, A2, PU, AK>(&cs, Pp, tmp, slot, want_grad ? 1 : 0)));
     }
 
     dbg_mark(&cs, 4);
@@ -1006,7 +887,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) tw_loss_grad_kernel(const __gri
       for (int slot = n_used - 1; slot >= 0; --slot) {
         const int k1 = tm.chan[slot].n1, k2 = tm.chan[slot].n2, pu = tm.chan[slot].pure;
         const int ak = args.net_ak[tm.used_net[slot]];
-        PINN_TW_DISPATCH(k1, k2, pu, ak, (phase = tw_net_backward<A1, A2, PU, AK>(&cs, Pp, tmp, slot, phase)));
+        PINN_TW_DISPATCH(k1, k2, pu, ak, (tw_net_backward<A1, A2, PU, AK>(&cs, Pp, tmp, slot)));
       }
     }
     // claim the next tile only now: claiming a tile ahead would hand the last cheap tiles to CTAs that still owe a heavy one
@@ -1015,7 +896,6 @@ __global__ void __launch_bounds__(kTcThreads, 1) tw_loss_grad_kernel(const __gri
     tile = cs.next_tile;
   }
 
-  tc::tc_fence_before();
   __syncthreads();
   dbg_mark(&cs, 7);
 #ifdef PINN_DEBUG
@@ -1030,7 +910,6 @@ __global__ void __launch_bounds__(kTcThreads, 1) tw_loss_grad_kernel(const __gri
   }
 #endif
   if (tid < PINN_MAX_TERMS) args.term_sums[(long long)blockIdx.x * PINN_MAX_TERMS + tid] = ms.tsum[tid];
-  if (warp == 0) tc::tmem_dealloc<512>(cs.tmem);
   // gradient reduction, optimizer step and the multi-GPU sum in the kernel tail (tail.cuh)
   if (args.tail.state)
     fused_tail<float, kTcThreads>(args.tail, args.partial, args.partial_stride, args.term_sums, P.n_theta, P.n_terms, want_grad ? 1 : 0,

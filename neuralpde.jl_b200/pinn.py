@@ -311,7 +311,7 @@ class PhysicsInformedNN(AbstractPINN):
             raise ValueError("a custom `derivative` cannot be injected: derivatives are exact forward-mode "
                              "taps evaluated inside the CUDA kernel")
         if self.phi is not None:
-            raise ValueError("a custom trial solution `phi` is not supported by the B200 engine (MLP chains only)")
+            raise ValueError("a custom trial solution `phi` is not supported by the engine (MLP chains only)")
         self.multioutput = isinstance(self.chain, (list, tuple))
         if self.iteration is None:
             self.iteration = [0]

@@ -1,4 +1,4 @@
-"""Device-resident loss+grad timing of the BASELINE configs on the parity (FFMA) path (and tcgen05 where the
+"""Device-resident loss+grad timing of the BASELINE configs on the parity (FFMA) path (and tensor-core where the
 shape is supported).  Development aid; the contract bench is bench.py."""
 import sys, time
 import numpy as np

@@ -1,4 +1,4 @@
-"""Phase timeline of one tile of the tcgen05 kernel (CTA 0), from in-kernel clock64() marks."""
+"""Phase timeline of one tile of the tensor-core kernel (CTA 0), from in-kernel clock64() marks."""
 import os
 os.environ.setdefault("PINN_B200_LIB", os.path.join("neuralpde.jl_b200", "lib", "libpinn_b200_debug.so"))   # build.py --debug
 import ctypes as C, sys

@@ -35,7 +35,7 @@ TC_CASES = ["cfg1", "cfg2_small", "cfg3_small", "neumann_sin"]
 
 @pytest.mark.parametrize("name", TC_CASES)
 def test_tc_split_loss_rtol_1e5(name):
-    """tcgen05 path, forward operands split hi+lo (3 MMAs per product): loss rtol 1e-5 (north star); the reverse
+    """tensor-core path, forward operands split hi+lo (3 MMAs per product): loss rtol 1e-5 (north star); the reverse
     sweep uses bf16 operands, gradient relative L2 error stated at 1e-2."""
     g, sets, qw = load_golden(name)
     rep, total, terms, grad = engine_eval_sets(CASES[name](), np.float32, sets, qw, mode="tc_split", theta=g["theta"])
@@ -57,7 +57,7 @@ WIDE_CASES = ["burgers_wide", "poisson1d_wide", "cfg5_wide"]     # cfg5_wide: 6 
 
 @pytest.mark.parametrize("name", WIDE_CASES)
 def test_tc_wide_bf16_loss_rtol_1e2(name):
-    """128-wide layers on the tcgen05 path (bf16 operands, streamed weights, fp32 pre-activation stash; BASELINE config 3
+    """128-wide layers on the tensor-core path (bf16 operands, streamed weights, fp32 pre-activation stash; BASELINE config 3
     names this mode): same stated tolerance as the narrow bf16 mode, loss 1e-2 / gradient 2e-2."""
     g, sets, qw = load_golden(name)
     rep, total, terms, grad = engine_eval_sets(CASES[name](), np.float32, sets, qw, mode="tc_bf16", theta=g["theta"])
@@ -87,7 +87,7 @@ def test_tc_split_rejects_wide_layers_loudly():
 
 @pytest.mark.parametrize("name", ["mixed", "cfg4_tiny", "cfg5_small"])
 def test_tc_rejects_unsupported_shapes_loudly(name):
-    """More than 5 propagated channels per network: the tcgen05 path refuses (no silent fallback)."""
+    """More than 5 propagated channels per network: the tensor-core path refuses (no silent fallback)."""
     g, sets, qw = load_golden(name)
     with pytest.raises(npde.EngineError, match="channels|taps"):
         engine_eval_sets(CASES[name](), np.float32, sets, qw, mode="tc_split", theta=g["theta"])

@@ -164,7 +164,7 @@ def test_in_kernel_tail_matches_separate_reduce_kernel(monkeypatch, mode, dtype,
         t2, _, g2 = rep.engine.loss_grad_host(th, None, True)
     if mode == "ffma":        # the FFMA kernel's partials have one writer per entry: bitwise reproducible
         assert t2 == t1 and np.array_equal(g2, g1)
-    else:                     # the tcgen05 kernels combine a few warps' sums per entry with atomics inside a CTA
+    else:                     # the tensor-core kernels combine a few warps' sums per entry with atomics inside a CTA
         assert abs(t2 - t1) <= 1e-6 * abs(t1) and rel(g2, g1) < 1e-6
 
 
