@@ -57,17 +57,15 @@ def _extra_units():
     return [(f[:-3] + ".o", f, []) for f in sorted(os.listdir(CSRC)) if f.startswith("tc_") and f.endswith(".cu")]
 
 
-def build(verbose: bool = False, force: bool = False, defines=(), debug: bool = False) -> str:
+def build(verbose: bool = False, force: bool = False, debug: bool = False) -> str:
     """Default: the product library lib/libpinn_b200.so (no instrumentation).
-    debug=True: lib/libpinn_b200_debug.so with -DPINN_DEBUG (phase timestamps for scripts/tc_timeline.py and
-    scripts/tail_timeline.py).  defines=("NAME=VAL", ...): a measurement variant
-    lib/libpinn_b200_<tag>.so built in build_<tag>/ (select it with PINN_B200_LIB)."""
+    debug=True: lib/libpinn_b200_debug.so built in build_debug/ with -DPINN_DEBUG (phase timestamps for
+    scripts/tc_timeline.py and scripts/tail_timeline.py; select it with PINN_B200_LIB)."""
     objdir, lib, flags = OBJDIR, LIB, list(NVCC_FLAGS)
-    tag = ("debug" if debug else "") + "".join(d.replace("=", "") for d in defines)
-    if tag:
-        objdir = os.path.join(HERE, "build_" + tag)
-        lib = os.path.join(LIBDIR, "libpinn_b200_%s.so" % tag)
-        flags += ["-D" + d for d in defines] + (["-DPINN_DEBUG"] if debug else [])
+    if debug:
+        objdir = os.path.join(HERE, "build_debug")
+        lib = os.path.join(LIBDIR, "libpinn_b200_debug.so")
+        flags.append("-DPINN_DEBUG")
     os.makedirs(LIBDIR, exist_ok=True)
     os.makedirs(objdir, exist_ok=True)
     nvcc = _nvcc()
@@ -101,5 +99,4 @@ def build(verbose: bool = False, force: bool = False, defines=(), debug: bool = 
 
 
 if __name__ == "__main__":
-    print(build(verbose="-v" in sys.argv, force="-f" in sys.argv, debug="--debug" in sys.argv,
-                defines=tuple(a[2:] for a in sys.argv if a.startswith("-D"))))
+    print(build(verbose="-v" in sys.argv, force="-f" in sys.argv, debug="--debug" in sys.argv))

@@ -15,11 +15,7 @@ namespace pinn {
 #define PINN_LAUNCH_NAME PINN_CAT(PINN_CAT(PINN_CAT(ffma_launch_, PINN_INST_REAL), _), PINN_BUFS_NAME)
 
 cudaError_t PINN_LAUNCH_NAME(const FfmaArgs& a, int grid, size_t smem, cudaStream_t st) {
-  auto k = ffma_loss_grad_kernel<PINN_INST_REAL, (PINN_INST_BUFS != 0)>;
-  static size_t granted[64] = {0};
-  cudaError_t e = ensure_dynamic_smem(k, smem, granted);
-  if (e != cudaSuccess) return e;
-  return launch_fused_kernel(k, a, grid, kThreads, smem, st, a.tail.state != nullptr);
+  return launch_fused_kernel<ffma_loss_grad_kernel<PINN_INST_REAL, (PINN_INST_BUFS != 0)>>(a, grid, kThreads, smem, st);
 }
 
 }  // namespace pinn

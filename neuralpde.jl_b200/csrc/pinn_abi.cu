@@ -110,17 +110,19 @@ struct pinn_engine {
   long long buf_elems = 0, stash_per_cta = 0;
   // tensor-core path geometry
   int tile_pts = kTilePts;
+  // (tc_off_P / _misc / _ones, tc_mx_*, tc_stash_per_cta and tc_net_ak serve both tensor-core kernels)
   int tc_split = 0, tc_tl_max = 0, tc_off_P = 0, tc_off_Q = 0, tc_off_misc = 0, tc_off_ones = 0, tc_mx_dim = 1, tc_mx_taps = 1;
+  int tc_net_ak[PINN_MAX_NETS];  // 1: every hidden activation of the network is tanh (fast path), 0: generic
   TcNetSmem tc_nets[PINN_MAX_NETS];
   long long tc_stash_per_cta = 0;
   long long* tc_dbg = nullptr;   // device buffer for pinn_debug_tc_timeline
   long long* tail_dbg = nullptr; // device buffer for pinn_debug_tail_marks (PINN_DEBUG builds)
   // wide tensor path (128-wide layers): streamed weights, fp32 pre-activation stash
   bool tw = false;
-  int tw_off_P = 0, tw_off_S = 0, tw_off_misc = 0, tw_off_ones = 0, tw_off_nets = 0, tw_off_fp[PINN_MAX_NETS], tw_wimg[PINN_MAX_NETS];
+  int tw_off_S = 0, tw_off_nets = 0, tw_off_fp[PINN_MAX_NETS], tw_wimg[PINN_MAX_NETS];
   int tw_n_images = 0;
   unsigned char tw_img_net[kTwMaxImages], tw_img_layer[kTwMaxImages];
-  long long tw_hstash_per_cta = 0, tw_zstash_per_cta = 0;
+  long long tw_zstash_per_cta = 0;
   void* tw_wpack = nullptr;
   int* tw_counter = nullptr;
   void* tw_zstash = nullptr;
@@ -491,8 +493,11 @@ static int lower_problem(const pinn_problem_desc* d, pinn_engine* e) {
   e->tile_pts = kTcPts;
   int tl_max = 0;
   bool wide = false;
+  for (int k = 0; k < PINN_MAX_NETS; ++k) e->tc_net_ak[k] = 1;
   for (int k = 0; k < d->n_nets; ++k) {
     const DevNet& n = P.nets[k];
+    for (int l = 0; l + 1 < n.n_layers; ++l)
+      if (n.acts[l] != PINN_ACT_TANH) e->tc_net_ak[k] = 0;
     if (n.n_layers < 2) return fail("pinn_create(tc): net %d needs at least 2 Dense layers", k);
     if (n.dims[n.n_layers] != 1) return fail("pinn_create(tc): net %d must have a 1-dimensional output", k);
     if (n.acts[n.n_layers - 1] != PINN_ACT_IDENTITY)
@@ -614,14 +619,14 @@ static int lower_problem(const pinn_problem_desc* d, pinn_engine* e) {
     for (int t = 0; t < d->n_terms; ++t)
       for (int s2 = 0; s2 < P.terms[t].n_used; ++s2) maxCw = std::max(maxCw, (int)P.terms[t].chan[s2].C);
     size_t o2 = 0;
-    e->tw_off_P = (int)o2; o2 += (size_t)maxCw * kTwNB * kTileBytes;
+    e->tc_off_P = (int)o2; o2 += (size_t)maxCw * kTwNB * kTileBytes;
     e->tw_off_S = (int)o2; o2 += (size_t)2 * kTwImgBytes;
-    e->tw_off_ones = (int)o2; o2 += 1024;
+    e->tc_off_ones = (int)o2; o2 += 1024;
     e->tw_n_images = 0;
     for (int k = 0; k < PINN_MAX_NETS; ++k) { e->tw_off_fp[k] = -1; e->tw_wimg[k] = 0; }
     for (int k = 0; k < d->n_nets; ++k) {
       e->tw_off_fp[k] = (int)o2;
-      o2 += ((size_t)FW_SIZE * 4 + 15) & ~size_t(15);
+      o2 += ((size_t)FpBlock<kTwW>::SIZE * 4 + 15) & ~size_t(15);
       e->tw_wimg[k] = e->tw_n_images;
       for (int l = 1; l <= P.nets[k].n_layers - 2; ++l) {
         e->tw_img_net[e->tw_n_images] = (unsigned char)k;
@@ -631,16 +636,15 @@ static int lower_problem(const pinn_problem_desc* d, pinn_engine* e) {
     }
     e->tw_off_nets = (int)o2;
     o2 += ((size_t)d->n_nets * sizeof(DevNet) + 15) & ~size_t(15);
-    e->tw_off_misc = (int)o2;
+    e->tc_off_misc = (int)o2;
     o2 += tc_misc_bytes(e->tc_mx_dim, e->tc_mx_taps);
     if (o2 + 1024 > (size_t)max_smem)
       return fail("pinn_create(tc): the problem needs %zu bytes of shared memory per CTA (limit %d): too many networks "
                   "for the 128-wide tensor-core path", o2, max_smem);
     e->smem = o2;
     // per pass: inputs of the tl_max tensor layers + the last hidden activations (restored for multi-pass terms)
-    e->tw_hstash_per_cta = (long long)n_used_max * (tl_max + 1) * kTwMaxC * kTwNB * kTileBytes;
+    e->tc_stash_per_cta = (long long)n_used_max * (tl_max + 1) * kTwMaxC * kTwNB * kTileBytes;
     e->tw_zstash_per_cta = (long long)n_used_max * tl_max * kTwMaxC * 64 * kTcPts * 2;      // floats
-    e->tc_stash_per_cta = e->tw_hstash_per_cta;
     return 0;
   }
   size_t off = 0;
@@ -661,7 +665,7 @@ static int lower_problem(const pinn_problem_desc* d, pinn_engine* e) {
   e->tc_off_ones = (int)off; off += 1024;      // 1024-aligned: P, Q and the weight tiles are multiples of 8 KB
   for (int k = 0; k < d->n_nets; ++k) {
     e->tc_nets[k].fp = (int)off;
-    off += ((size_t)FP_SIZE * 4 + 15) & ~size_t(15);
+    off += ((size_t)FpBlock<kTcW>::SIZE * 4 + 15) & ~size_t(15);
   }
   e->tc_off_misc = (int)off;
   off += tc_misc_bytes(e->tc_mx_dim, e->tc_mx_taps);
@@ -883,6 +887,16 @@ static int launch_fused(pinn_engine* e, const FfmaArgs& a, int grid, cudaStream_
     CUDA_TRY(ffma_launch(e->dtype, e->bufs_smem, a, grid, e->smem, st));
     return 0;
   }
+  TcCommonArgs c;
+  memset(&c, 0, sizeof c);
+  c.prob = a.prob; c.theta = (const float*)a.theta; c.partial = (float*)a.partial; c.partial_stride = a.partial_stride; c.term_sums = a.term_sums;
+  c.tl_max = std::max(e->tc_tl_max, 1);
+  c.tile_begin = a.tile_begin; c.tile_end = a.tile_end; c.mode = a.mode; c.resid_out = (float*)a.resid_out; c.acc = e->tc_acc;
+  c.dbg = e->tc_dbg;
+  c.off_P = e->tc_off_P; c.off_misc = e->tc_off_misc; c.off_ones = e->tc_off_ones; c.mx_dim = e->tc_mx_dim; c.mx_taps = e->tc_mx_taps;
+  memcpy(c.net_ak, e->tc_net_ak, sizeof c.net_ak);
+  for (int k = 0; k < PINN_MAX_TERMS; ++k) { c.seed[k] = a.seed[k]; c.dyn[k] = a.dyn[k]; }
+  c.tail = a.tail;
   if (e->tw) {
     TwPackArgs pk;
     memset(&pk, 0, sizeof pk);
@@ -894,48 +908,25 @@ static int launch_fused(pinn_engine* e, const FfmaArgs& a, int grid, cudaStream_
     e->launches += 1;
     TwArgs w;
     memset(&w, 0, sizeof w);
-    w.prob = a.prob; w.theta = (const float*)a.theta; w.partial = (float*)a.partial; w.partial_stride = a.partial_stride; w.term_sums = a.term_sums;
-    w.hstash = (uint8_t*)e->stash; w.hstash_per_cta = e->tw_hstash_per_cta;
+    static_cast<TcCommonArgs&>(w) = c;
+    w.hstash = (uint8_t*)e->stash; w.hstash_per_cta = e->tc_stash_per_cta;
     w.zstash = (float*)e->tw_zstash; w.zstash_per_cta = e->tw_zstash_per_cta;
-    w.wpack = (const uint8_t*)e->tw_wpack; w.tl_max = std::max(e->tc_tl_max, 1);
-    w.tile_begin = a.tile_begin; w.tile_end = a.tile_end; w.mode = a.mode; w.resid_out = (float*)a.resid_out; w.acc = e->tc_acc;
-    w.dbg = e->tc_dbg; w.tile_counter = e->tw_counter;
-    w.off_P = e->tw_off_P; w.off_S = e->tw_off_S; w.off_misc = e->tw_off_misc; w.off_ones = e->tw_off_ones; w.off_nets = e->tw_off_nets; w.mx_dim = e->tc_mx_dim; w.mx_taps = e->tc_mx_taps;
-    for (int k = 0; k < PINN_MAX_NETS; ++k) {
-      w.off_fp[k] = e->tw_off_fp[k]; w.wimg[k] = e->tw_wimg[k];
-      int ak = 1;
-      if (k < e->hprob->n_nets) {
-        const DevNet& n = e->hprob->nets[k];
-        for (int l = 0; l + 1 < n.n_layers; ++l) if (n.acts[l] != PINN_ACT_TANH) ak = 0;
-      }
-      w.net_ak[k] = ak;
-    }
-    for (int k = 0; k < PINN_MAX_TERMS; ++k) { w.seed[k] = a.seed[k]; w.dyn[k] = a.dyn[k]; }
-    w.tail = a.tail;
+    w.wpack = (const uint8_t*)e->tw_wpack; w.tile_counter = e->tw_counter;
+    w.off_S = e->tw_off_S; w.off_nets = e->tw_off_nets;
+    memcpy(w.off_fp, e->tw_off_fp, sizeof w.off_fp);
+    memcpy(w.wimg, e->tw_wimg, sizeof w.wimg);
     CUDA_TRY(tw_launch(w, grid, e->smem, st));
     return 0;
   }
   TcArgs t;
   memset(&t, 0, sizeof t);
-  t.prob = a.prob; t.theta = (const float*)a.theta; t.partial = (float*)a.partial; t.partial_stride = a.partial_stride; t.term_sums = a.term_sums;
-  t.stash = (uint8_t*)e->stash; t.stash_per_cta = e->tc_stash_per_cta; t.split = e->tc_split; t.tl_max = std::max(e->tc_tl_max, 1);
-  t.tile_begin = a.tile_begin; t.tile_end = a.tile_end; t.mode = a.mode; t.resid_out = (float*)a.resid_out; t.acc = e->tc_acc;
-  t.off_P = e->tc_off_P; t.off_Q = e->tc_off_Q; t.off_misc = e->tc_off_misc; t.off_ones = e->tc_off_ones; t.mx_dim = e->tc_mx_dim; t.mx_taps = e->tc_mx_taps;
-  t.dbg = e->tc_dbg;
+  static_cast<TcCommonArgs&>(t) = c;
+  t.stash = (uint8_t*)e->stash; t.stash_per_cta = e->tc_stash_per_cta; t.split = e->tc_split;
+  t.off_Q = e->tc_off_Q;
+  t.off_Q_bytes = e->tc_off_Q - e->tc_off_P;   // P and Q regions have the same size
   t.n_nets = e->hprob->n_nets; t.n_terms = e->n_terms; t.n_theta = e->n_theta;
   for (int k = 0; k < e->n_terms; ++k) t.term_dim[k] = (unsigned char)e->hprob->terms[k].dim;
-  t.off_Q_bytes = e->tc_off_Q - e->tc_off_P;   // P and Q regions have the same size
-  for (int k = 0; k < PINN_MAX_NETS; ++k) {
-    t.nets[k] = e->tc_nets[k];
-    int ak = 1;
-    if (k < e->hprob->n_nets) {
-      const DevNet& n = e->hprob->nets[k];
-      for (int l = 0; l + 1 < n.n_layers; ++l) if (n.acts[l] != PINN_ACT_TANH) ak = 0;
-    }
-    t.net_ak[k] = ak;
-  }
-  for (int k = 0; k < PINN_MAX_TERMS; ++k) { t.seed[k] = a.seed[k]; t.dyn[k] = a.dyn[k]; }
-  t.tail = a.tail;
+  memcpy(t.nets, e->tc_nets, sizeof t.nets);
   CUDA_TRY(tc_launch(t, grid, e->smem, st));
   return 0;
 }

@@ -22,29 +22,27 @@
 
 namespace pinn {
 
-// cudaFuncSetAttribute(MaxDynamicSharedMemorySize) once per device and size instead of on every launch (host time of the
-// per-step call path); cache: bytes already granted on device d
-template <typename K>
-static cudaError_t ensure_dynamic_smem(K kernel, size_t smem, size_t (&granted)[64]) {
+// launch `kernel` with the cooperative attribute when it ends with the grid-wide tail (a.tail.state set: all CTAs must be
+// co-resident).  The dynamic shared-memory limit is raised once per kernel, device and size instead of on every launch
+// (host time of the per-step call path): each kernel has its own instantiation and so its own cache.
+template <auto kernel, typename A>
+static cudaError_t launch_fused_kernel(const A& a, int grid, int threads, size_t smem, cudaStream_t st) {
+  static size_t granted[64] = {0};   // bytes already granted on device d
   int dev = 0;
   cudaError_t e = cudaGetDevice(&dev);
   if (e != cudaSuccess) return e;
-  if (dev >= 0 && dev < 64 && granted[dev] >= smem) return cudaSuccess;
-  e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-  if (e == cudaSuccess && dev >= 0 && dev < 64) granted[dev] = smem;
-  return e;
-}
-
-// launch with the cooperative attribute when the kernel ends with the grid-wide tail (all CTAs must be co-resident)
-template <typename K, typename A>
-static cudaError_t launch_fused_kernel(K kernel, const A& a, int grid, int threads, size_t smem, cudaStream_t st, bool coop) {
+  if (dev < 0 || dev >= 64 || granted[dev] < smem) {
+    e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return e;
+    if (dev >= 0 && dev < 64) granted[dev] = smem;
+  }
   cudaLaunchConfig_t cfg;
   memset(&cfg, 0, sizeof cfg);
   cfg.gridDim = dim3((unsigned)grid); cfg.blockDim = dim3((unsigned)threads); cfg.dynamicSmemBytes = smem; cfg.stream = st;
   cudaLaunchAttribute at[1];
   at[0].id = cudaLaunchAttributeCooperative;
   static const bool no_coop = [] { const char* v = getenv("PINN_B200_COOP"); return v && v[0] == '0'; }();   // measurement aid
-  at[0].val.cooperative = (coop && !no_coop) ? 1 : 0;
+  at[0].val.cooperative = (a.tail.state != nullptr && !no_coop) ? 1 : 0;
   cfg.attrs = at; cfg.numAttrs = 1;
   return cudaLaunchKernelEx(&cfg, kernel, a);
 }

@@ -1,26 +1,22 @@
 // tc_common.cuh -- device helpers shared by the tensor-core kernels (tc_kernel.cu: widths <= 64, all operands resident;
 // tc_wide_kernel.cu: 128-wide layers, streamed weights): fp32x2 arithmetic, the forward-mode tap chain rule
-// and its adjoint, accumulator loads, swizzled-tile stores, warp reduce-scatter, MMA chains, dispatch macro.
+// and its adjoint, accumulator loads, swizzled-tile stores, warp reduce-scatter, MMA chains, the steps of the tile
+// driver both kernels share (CTA setup, parameter and point-tile staging, residual program, kernel end), dispatch macro.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include "tc_types.h"
 #include "ffma_kernel.cuh"   // act_eval, run_program, warp_sum
 #include "tc_prims.cuh"
+#include "tail.cuh"
 
 namespace pinn {
 
 // ---- small helpers ---------------------------------------------------------------------------------
 constexpr int kNH = kTcThreads / 128;   // warps per 32-row quadrant of the accumulators: each takes 1/kNH of the columns
 static_assert(kTcThreads == 512, "the MMA chains are spread over four warpgroups");
-#ifndef PINN_TC_GW
-#define PINN_TC_GW 4
-#endif
-constexpr int GW = PINN_TC_GW;          // columns per epilogue granule (4 or 2)
-#ifndef PINN_TC_GWB
-#define PINN_TC_GWB 2
-#endif
-constexpr int GWB = PINN_TC_GWB;        // granule of the tensor-layer reverse epilogue (register-heaviest loop)
+constexpr int GW = 4;                   // columns per epilogue granule
+constexpr int GWB = 2;                  // granule of the tensor-layer reverse epilogue (register-heaviest loop)
 
 template <int N>
 __device__ __forceinline__ float pick(const float* v, int idx) {
@@ -40,9 +36,6 @@ __device__ __forceinline__ void add_at(float* v, int idx, float x) {
 // AK = 0: any activation through the accurate generic evaluator.
 template <int AK>
 __device__ __forceinline__ void act_eval_tc(int act, float z, float& a, float& d1, float& d2, float& d3) {
-#ifdef PINN_EXP_NO_ACT
-  a = z; d1 = 1.f; d2 = 0.5f; d3 = 0.25f; return;
-#endif
   if (AK == 1) {
     const float e = __expf(2.f * z);
     const float t = 1.f - __fdividef(2.f, e + 1.f);
@@ -71,10 +64,6 @@ __device__ __forceinline__ void sts_v2(uint32_t addr, uint32_t x, uint32_t y) {
 // also the bf16 residual v - bf16(v) into the lo tile
 __device__ __forceinline__ void store_half(uint32_t tile_hi, uint32_t tile_lo, int row, int col0, const float (&v)[4],
                                            bool split) {
-#ifdef PINN_EXP_NO_STS
-  asm volatile("" ::"f"(v[0]), "f"(v[1]), "f"(v[2]), "f"(v[3]));
-  return;
-#endif
   const uint32_t off = tc::swz_chunk(row, col0 >> 3) + ((col0 & 4) << 1);
   const uint32_t hx = tc::pack_bf16(v[0], v[1]), hy = tc::pack_bf16(v[2], v[3]);
   sts_v2(tile_hi + off, hx, hy);
@@ -220,12 +209,9 @@ __device__ __forceinline__ void chain_bwd(int act, const Chan<N1, N2>& ch, const
   zb[0] = acc0;
 }
 
-// sum over the 32 lanes of 4 per-lane values with 6 shuffles.  Every lane receives the total of
-// element e = ((lane>>4)&1)*2 + ((lane>>3)&1); lanes with (lane & 7) == 0 act on it.
-__device__ __forceinline__ float warp_reduce4(const float (&v)[4], int lane) {
-#ifdef PINN_EXP_NO_RED
-  return v[0] + v[1] + v[2] + v[3];
-#endif
+// sum over the 32 lanes of the GW = 4 per-lane values of a granule with 6 shuffles.  Every lane receives the total of
+// element reduceg_elem(lane); the lanes with reduceg_lead(lane) act on it.
+__device__ __forceinline__ float warp_reduceg(const float (&v)[GW], int lane) {
   const bool up16 = (lane & 16) != 0;
   float a0 = (up16 ? v[2] : v[0]) + __shfl_xor_sync(0xffffffffu, up16 ? v[0] : v[2], 16);
   float a1 = (up16 ? v[3] : v[1]) + __shfl_xor_sync(0xffffffffu, up16 ? v[1] : v[3], 16);
@@ -236,21 +222,8 @@ __device__ __forceinline__ float warp_reduce4(const float (&v)[4], int lane) {
   r += __shfl_xor_sync(0xffffffffu, r, 1);
   return r;
 }
-__device__ __forceinline__ int reduce4_elem(int lane) { return ((lane >> 4) & 1) * 2 + ((lane >> 3) & 1); }
-// 2 values: 5 shuffles; every lane gets the total of element e = (lane >> 4) & 1; lanes with (lane & 15) == 0 act
-__device__ __forceinline__ float warp_reduce2(const float (&v)[2], int lane) {
-  const bool up16 = (lane & 16) != 0;
-  float r = (up16 ? v[1] : v[0]) + __shfl_xor_sync(0xffffffffu, up16 ? v[0] : v[1], 16);
-  r += __shfl_xor_sync(0xffffffffu, r, 8);
-  r += __shfl_xor_sync(0xffffffffu, r, 4);
-  r += __shfl_xor_sync(0xffffffffu, r, 2);
-  r += __shfl_xor_sync(0xffffffffu, r, 1);
-  return r;
-}
-__device__ __forceinline__ float warp_reduceg(const float (&v)[4], int lane) { return warp_reduce4(v, lane); }
-__device__ __forceinline__ float warp_reduceg(const float (&v)[2], int lane) { return warp_reduce2(v, lane); }
-__device__ __forceinline__ int reduceg_elem(int lane) { return GW == 4 ? reduce4_elem(lane) : ((lane >> 4) & 1); }
-__device__ __forceinline__ bool reduceg_lead(int lane) { return GW == 4 ? ((lane & 7) == 0) : ((lane & 15) == 0); }
+__device__ __forceinline__ int reduceg_elem(int lane) { return ((lane >> 4) & 1) * 2 + ((lane >> 3) & 1); }
+__device__ __forceinline__ bool reduceg_lead(int lane) { return (lane & 7) == 0; }
 
 // phase timestamps for the timeline tool (scripts/tc_timeline.py): id in the high bits, clock in the low
 // (only in -DPINN_DEBUG builds: libpinn_b200_debug.so; the product library carries no instrumentation)
@@ -297,6 +270,29 @@ __device__ __forceinline__ void load_pass(PassInfo<N1, N2>& pi, const DevNet& ne
   for (int s = 0; s < N2; ++s) { pi.ch.sa[s] = dc.s_a[s]; pi.ch.sb[s] = dc.s_b[s]; }
 }
 
+// first-layer pre-activations of neuron o (channel vector zz); fpa = shared-memory address of the FpBlock<W>
+template <int W, int N1, int N2>
+__device__ __forceinline__ void first_layer_elem(uint32_t fpa, const PassInfo<N1, N2>& pi, const float (&x)[PINN_MAX_IN],
+                                                 int o, float* zz) {
+  using F = FpBlock<W>;
+  float s = lds_f32(fpa + (F::B1 + o) * 4);
+  const uint32_t wa = fpa + (F::W1 + o * 8) * 4;
+  if (pi.d_in <= 3) {            // common 1-D / 2-D / 3-D problems: no predicated tail
+    s = fmaf(lds_f32(wa), x[0], s);
+    if (pi.d_in >= 2) s = fmaf(lds_f32(wa + 4), x[1], s);
+    if (pi.d_in == 3) s = fmaf(lds_f32(wa + 8), x[2], s);
+  } else {
+#pragma unroll
+    for (int k = 0; k < PINN_MAX_IN; ++k)
+      if (k < pi.d_in) s = fmaf(lds_f32(wa + k * 4), x[k], s);
+  }
+  zz[0] = s;
+#pragma unroll
+  for (int j = 0; j < N1; ++j) zz[1 + j] = lds_f32(fpa + (F::W1 + o * 8 + pi.dir1[j]) * 4);
+#pragma unroll
+  for (int j = 0; j < N2; ++j) zz[1 + N1 + j] = 0.f;
+}
+
 __device__ __forceinline__ void wait_bar(uint64_t* bar, uint32_t& phase) {
   tc::mbar_wait(bar, phase);
   phase ^= 1u;
@@ -340,33 +336,230 @@ __device__ __forceinline__ Tid tid_of() {
   return t;
 }
 
-#define PINN_TC_CASE(a1, a2, pu, CALL)                                                    \
-  {                                                                                       \
-    constexpr int A1 = a1, A2 = a2;                                                       \
-    constexpr bool PU = pu;                                                               \
-    if (_ak == 1) { constexpr int AK = 1; CALL; } else { constexpr int AK = 0; CALL; }   \
-  }                                                                                       \
+// ---- steps of the tile driver that both tensor-core kernels share ----------------------------------------------------------
+// (plain helpers: each kernel body keeps its own setup, tile loop and sweeps, and calls these where the steps coincide)
+
+// zero the CTA's gradient partial (want_grad) and term sums, write the ones atom
+__device__ __forceinline__ void cta_setup(const TcCommonArgs& a, const Misc& ms, float* partial, long long n_theta, bool want_grad) {
+  extern __shared__ __align__(1024) uint8_t smem[];
+  const int tid = threadIdx.x;
+  if (want_grad) {
+    const long long n4 = n_theta / 4;
+    float4* p4 = reinterpret_cast<float4*>(partial);
+    if ((reinterpret_cast<uintptr_t>(partial) & 15) == 0) {
+      for (long long i = tid; i < n4; i += kTcThreads) p4[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+      for (long long i = n4 * 4 + tid; i < n_theta; i += kTcThreads) partial[i] = 0.f;
+    } else {
+      for (long long i = tid; i < n_theta; i += kTcThreads) partial[i] = 0.f;
+    }
+  }
+  if (tid < PINN_MAX_TERMS) ms.tsum[tid] = 0.0;
+  if (tid < 64) {      // ones atom: row r (128 B) holds bf16 1.0 in logical column 0 = 16-byte chunk (0 ^ r)
+    const int r = tid >> 3, ch = tid & 7;
+    *reinterpret_cast<uint4*>(smem + a.off_ones + r * 128 + ch * 16) = make_uint4(ch == r ? 0x00003f80u : 0u, 0u, 0u, 0u);
+  }
+}
+
+// fp32 parameter block FpBlock<W> of one network: first layer, tensor-layer biases, last layer (CTA-wide: has a barrier)
+template <int W>
+__device__ __forceinline__ void stage_fp_block(float* fp, const DevNet& net, const float* theta) {
+  using F = FpBlock<W>;
+  const int tid = threadIdx.x, L = net.n_layers;
+  for (int i = tid; i < F::SIZE; i += kTcThreads) fp[i] = 0.f;
+  __syncthreads();
+  const int n1w = net.dims[1], d_in = net.dims[0];
+  const long long w0 = net.w_off[0], b0 = net.b_off[0];
+  for (int i = tid; i < n1w * d_in; i += kTcThreads) {
+    const int o = i % n1w, k = i / n1w;
+    fp[F::W1 + o * 8 + k] = __ldg(&theta[w0 + i]);
+  }
+  for (int i = tid; i < n1w; i += kTcThreads) fp[F::B1 + i] = __ldg(&theta[b0 + i]);
+  for (int i = tid; i < (L - 2) * W; i += kTcThreads) {
+    const int l = 1 + i / W, o = i & (W - 1);
+    if (o < net.dims[l + 1]) fp[F::BT + (l - 1) * W + o] = __ldg(&theta[net.b_off[l] + o]);
+  }
+  const int nL = net.dims[L - 1];
+  const long long wl = net.w_off[L - 1], bl = net.b_off[L - 1];
+  for (int i = tid; i < nL; i += kTcThreads) fp[F::WL + i] = __ldg(&theta[wl + i]);
+  if (tid == 0) fp[F::BL] = __ldg(&theta[bl]);
+}
+
+// a point tile: its term, the index of its first point in the term, the term's point count
+struct TileRef {
+  int ti;
+  long long p0, n_pts;
+};
+
+// find the term of `tile`, stage its points into ms.Xs ([row][point]) and quadrature weights into ms.qws, clear the tap
+// adjoints.  ld_phase: parity of the collocation-tile barrier ms.bar_ld.  CTA-wide, ends with a barrier.
+__device__ __forceinline__ TileRef stage_tile(const TcCommonArgs& a, const DevProblem& P, const Misc& ms, int tile,
+                                              uint32_t& ld_phase) {
+  const int tid = threadIdx.x;
+  int ti = 0;
+  while (ti + 1 < P.n_terms && tile >= a.dyn[ti + 1].tile0) ++ti;
+  const DevTerm& tm = P.terms[ti];
+  const long long p0 = (long long)(tile - a.dyn[ti].tile0) * kTcPts;
+  const long long n_pts = a.dyn[ti].n;
+  const float* pts = reinterpret_cast<const float*>(a.dyn[ti].pts);
+  const float* qw = reinterpret_cast<const float*>(a.dyn[ti].qw);
+  // warm L1 with the term header + residual program (read by every phase)
+  if (tid < (int)((sizeof(DevTerm) + 127) / 128)) tc::prefetch_l1(reinterpret_cast<const char*>(&tm) + tid * 128);
+  const int dim = tm.dim, n_taps = tm.n_taps, weighted = tm.weighted;
+  // Collocation tile: one point = dim contiguous scalars (the reference's d x N train-set layout), so a full 128-point
+  // tile is ONE contiguous block of dim x 512 bytes.  The TMA unit copies it into shared memory in a single bulk transfer
+  // (cp.async.bulk + mbarrier transaction count; staged in the scratch array, free between tiles, kTcMaxC rows) and 128
+  // threads transpose it to [row][point].  Partial last tiles (clamped rows) and callers' buffers that are not 16-byte
+  // aligned take the per-element path.
+  const float* tile_src = pts + p0 * dim;
+  const bool bulk_tile = (p0 + kTcPts <= n_pts) && dim <= kTcMaxC && ((reinterpret_cast<uintptr_t>(tile_src) & 15) == 0);
+  if (bulk_tile) {
+    if (tid == 0) {
+      tc::mbar_arrive_expect_tx(ms.bar_ld, (uint32_t)(dim * kTcPts * 4));
+      tc::bulk_load(ms.scratch, tile_src, (uint32_t)(dim * kTcPts * 4), ms.bar_ld);
+    }
+    wait_bar(ms.bar_ld, ld_phase);
+    if (tid < kTcPts)
+      for (int r = 0; r < dim; ++r) ms.Xs[r * kTcPts + tid] = ms.scratch[tid * dim + r];
+  } else {
+    for (int i = tid; i < dim * kTcPts; i += kTcThreads) {
+      int pp = i / dim, r = i - pp * dim;
+      long long gp = p0 + pp;
+      if (gp >= n_pts) gp = n_pts - 1;
+      ms.Xs[r * kTcPts + pp] = pts[gp * dim + r];
+    }
+  }
+  if (tid < kTcPts) {
+    long long gp = p0 + tid;
+    float w = 0.f;
+    if (gp < n_pts) w = weighted ? qw[gp] : 1.f;
+    ms.qws[tid] = w;
+  }
+  for (int i = tid; i < n_taps * kTcPts; i += kTcThreads) ms.tapbar[i] = 0.f;
+  __syncthreads();
+  return TileRef{ti, p0, n_pts};
+}
+
+// residual program of the tile (threads 0..127: one point each): loss partial into ms.tsum, the residual probe (mode 2)
+// and, for a gradient, the tap adjoints scaled by the loss seed and the theta.p gradient.  The program text and the
+// per-point value / adjoint arrays go to the idle shared memory [region, region + region_bytes) when they fit.
+// CTA-wide, ends with a barrier.
+__device__ __forceinline__ void residual_step(const TcCommonArgs& a, const DevProblem& P, const DevTerm& tm, const Misc& ms,
+                                              const TileRef& tr, uint8_t* region, size_t region_bytes, float* partial,
+                                              bool want_grad) {
+  const int tid = threadIdx.x, lane = tid & 31;
+  const int n_instr = tm.n_instr, n_taps = tm.n_taps;
+  DevInstr* sprog = reinterpret_cast<DevInstr*>(region);
+  float* sval = reinterpret_cast<float*>(region + 8192);
+  const bool prog_sm = (size_t)8192 + (size_t)2 * n_instr * kTcPts * 4 <= region_bytes;
+  if (prog_sm) {
+    const int nw = n_instr * (int)(sizeof(DevInstr) / 4);
+    const int* src = reinterpret_cast<const int*>(tm.prog);
+    for (int i = tid; i < nw; i += kTcThreads) reinterpret_cast<int*>(sprog)[i] = __ldg(src + i);
+    __syncthreads();
+  }
+  if (tid < kTcPts) {
+    float pbar[PINN_MAX_PARAMS];
+#pragma unroll
+    for (int j = 0; j < PINN_MAX_PARAMS; ++j) pbar[j] = 0.f;
+    float r;
+    if (prog_sm) {
+      r = run_program_t<float, kTcPts, true>(sprog, n_instr, a.theta + P.param_off, ms.Xs, ms.taps, ms.tapbar, pbar, tid,
+                                             want_grad, sval, sval + n_instr * kTcPts);
+    } else {
+      r = run_program<float, kTcPts>(tm, a.theta + P.param_off, ms.Xs, ms.taps, ms.tapbar, pbar, tid, want_grad);
+    }
+    const float w = ms.qws[tid];
+    double s = (double)w * (double)r * (double)r;
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+    if (lane == 0) atomicAdd(&ms.tsum[tr.ti], s);
+    if (a.mode == 2) {
+      long long gp = tr.p0 + tid;
+      if (gp < tr.n_pts) a.resid_out[gp] = r;
+    }
+    if (want_grad) {
+      const float g = (float)a.seed[tr.ti] * w * 2.f * r;
+      for (int tt = 0; tt < n_taps; ++tt) ms.tapbar[tt * kTcPts + tid] *= g;
+      const int n_params = P.n_params;
+      for (int j = 0; j < n_params; ++j) {
+        float v = warp_sum<float>(pbar[j] * g);
+        if (lane == 0) atomicAdd(&partial[P.param_off + j], v);
+      }
+    }
+  }
+  __syncthreads();
+}
+
+// start clocks of the CTA's span record (PINN_DEBUG builds, written by cta_finish)
+struct DbgSpan {
+  long long c0;
+  unsigned long long g0;
+};
+__device__ __forceinline__ DbgSpan dbg_span_begin(const long long* dbg) {
+  DbgSpan s{0, 0};
+#ifdef PINN_DEBUG
+  if (dbg && threadIdx.x == 0) {
+    s.c0 = clock64();
+    asm volatile("mov.u64 %0, %globaltimer;" : "=l"(s.g0));
+  }
+#endif
+  return s;
+}
+
+// end of the kernel: span record (PINN_DEBUG), per-CTA term sums, and the kernel tail (tail.cuh: gradient reduction,
+// optimizer step, multi-GPU sum)
+template <typename CS>
+__device__ __forceinline__ void cta_finish(const TcCommonArgs& a, const CS& cs, const DbgSpan& span, const Misc& ms,
+                                           const DevProblem& P, bool want_grad) {
+  extern __shared__ __align__(1024) uint8_t smem[];
+  const int tid = threadIdx.x;
+#ifdef PINN_DEBUG
+  if (tid == 0 && cs.dbg) cs.dbg[999] = cs.dbg_n;
+  if (a.dbg && tid == 0 && blockIdx.x < 250) {
+    unsigned long long g1;
+    unsigned int smid;
+    asm volatile("mov.u64 %0, %globaltimer;" : "=l"(g1));
+    asm volatile("mov.u32 %0, %smid;" : "=r"(smid));
+    long long* rec = a.dbg + 1000 + 4 * blockIdx.x;
+    rec[0] = (long long)span.g0; rec[1] = (long long)g1; rec[2] = clock64() - span.c0; rec[3] = smid;
+  }
+#endif
+  if (tid < PINN_MAX_TERMS) a.term_sums[(long long)blockIdx.x * PINN_MAX_TERMS + tid] = ms.tsum[tid];
+  if (a.tail.state)
+    fused_tail<float, kTcThreads>(a.tail, a.partial, a.partial_stride, a.term_sums, P.n_theta, P.n_terms, want_grad ? 1 : 0,
+                                  reinterpret_cast<float*>(smem + a.off_P));
+}
+
+// channel structure <A1, A2, PU> of PINN_TC_DISPATCH; not instantiated when it has more than maxc channels
+#define PINN_TC_CASE(maxc, a1, a2, pu, CALL)                                                  \
+  {                                                                                           \
+    constexpr int A1 = a1, A2 = a2;                                                           \
+    constexpr bool PU = pu;                                                                   \
+    if constexpr (1 + A1 + A2 <= (maxc)) {                                                    \
+      if (_ak == 1) { constexpr int AK = 1; CALL; } else { constexpr int AK = 0; CALL; }     \
+    }                                                                                         \
+  }                                                                                           \
   break
-// ak = 1 when every hidden layer of the network is tanh (fast branch-free activation), else 0
-#define PINN_TC_DISPATCH(n1, n2, pure, ak, CALL)                              \
-  do {                                                                        \
-    const int _ak = (ak);                                                     \
-    const int _key = ((n1) * 8 + (n2)) * 2 + ((pure) ? 1 : 0);                \
-    switch (_key) {                                                           \
-      case (0 * 8 + 0) * 2: case (0 * 8 + 0) * 2 + 1: PINN_TC_CASE(0, 0, true, CALL);   \
-      case (1 * 8 + 0) * 2: case (1 * 8 + 0) * 2 + 1: PINN_TC_CASE(1, 0, true, CALL);   \
-      case (2 * 8 + 0) * 2: case (2 * 8 + 0) * 2 + 1: PINN_TC_CASE(2, 0, true, CALL);   \
-      case (3 * 8 + 0) * 2: case (3 * 8 + 0) * 2 + 1: PINN_TC_CASE(3, 0, true, CALL);   \
-      case (4 * 8 + 0) * 2: case (4 * 8 + 0) * 2 + 1: PINN_TC_CASE(4, 0, true, CALL);   \
-      case (1 * 8 + 1) * 2: case (1 * 8 + 1) * 2 + 1: PINN_TC_CASE(1, 1, true, CALL);   \
-      case (2 * 8 + 1) * 2 + 1: PINN_TC_CASE(2, 1, true, CALL);               \
-      case (2 * 8 + 1) * 2: PINN_TC_CASE(2, 1, false, CALL);                  \
-      case (3 * 8 + 1) * 2 + 1: PINN_TC_CASE(3, 1, true, CALL);               \
-      case (3 * 8 + 1) * 2: PINN_TC_CASE(3, 1, false, CALL);                  \
-      case (2 * 8 + 2) * 2 + 1: PINN_TC_CASE(2, 2, true, CALL);               \
-      case (2 * 8 + 2) * 2: PINN_TC_CASE(2, 2, false, CALL);                  \
-      default: break;                                                         \
-    }                                                                         \
+// maxc: the kernel's channel limit; ak = 1 when every hidden layer of the network is tanh (fast branch-free activation), else 0
+#define PINN_TC_DISPATCH(maxc, n1, n2, pure, ak, CALL)                                        \
+  do {                                                                                        \
+    const int _ak = (ak);                                                                     \
+    const int _key = ((n1) * 8 + (n2)) * 2 + ((pure) ? 1 : 0);                                \
+    switch (_key) {                                                                           \
+      case (0 * 8 + 0) * 2: case (0 * 8 + 0) * 2 + 1: PINN_TC_CASE(maxc, 0, 0, true, CALL);   \
+      case (1 * 8 + 0) * 2: case (1 * 8 + 0) * 2 + 1: PINN_TC_CASE(maxc, 1, 0, true, CALL);   \
+      case (2 * 8 + 0) * 2: case (2 * 8 + 0) * 2 + 1: PINN_TC_CASE(maxc, 2, 0, true, CALL);   \
+      case (3 * 8 + 0) * 2: case (3 * 8 + 0) * 2 + 1: PINN_TC_CASE(maxc, 3, 0, true, CALL);   \
+      case (4 * 8 + 0) * 2: case (4 * 8 + 0) * 2 + 1: PINN_TC_CASE(maxc, 4, 0, true, CALL);   \
+      case (1 * 8 + 1) * 2: case (1 * 8 + 1) * 2 + 1: PINN_TC_CASE(maxc, 1, 1, true, CALL);   \
+      case (2 * 8 + 1) * 2 + 1: PINN_TC_CASE(maxc, 2, 1, true, CALL);                         \
+      case (2 * 8 + 1) * 2: PINN_TC_CASE(maxc, 2, 1, false, CALL);                            \
+      case (3 * 8 + 1) * 2 + 1: PINN_TC_CASE(maxc, 3, 1, true, CALL);                         \
+      case (3 * 8 + 1) * 2: PINN_TC_CASE(maxc, 3, 1, false, CALL);                            \
+      case (2 * 8 + 2) * 2 + 1: PINN_TC_CASE(maxc, 2, 2, true, CALL);                         \
+      case (2 * 8 + 2) * 2: PINN_TC_CASE(maxc, 2, 2, false, CALL);                            \
+      default: break;                                                                         \
+    }                                                                                         \
   } while (0)
 
 }  // namespace pinn

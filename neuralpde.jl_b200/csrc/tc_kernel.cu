@@ -22,13 +22,10 @@
 //
 // Replaces the same reference functions as the FFMA path (see ffma_kernel.cuh).
 #include "tc_common.cuh"
-#include "tail.cuh"
-
-#ifndef PINN_TC_PREFETCH
-#define PINN_TC_PREFETCH 0      // 1: software-pipelined accumulator loads in the tensor-layer epilogues (measurement variant)
-#endif
 
 namespace pinn {
+
+using Fp = FpBlock<kTcW>;   // fp32 parameter block of a network
 
 // CTA-wide constants kept in shared memory so the per-network passes (separate functions) do not
 // drag a context struct through local memory
@@ -41,29 +38,6 @@ struct CtaShared {
   int dbg_n;
   TcNetSmem nets[PINN_MAX_NETS];
 };
-
-
-// first-layer pre-activations of neuron o (channel vector zz); fpa = shared-memory address of the fp32 block
-template <int N1, int N2>
-__device__ __forceinline__ void first_layer_elem(uint32_t fpa, const PassInfo<N1, N2>& pi, const float (&x)[PINN_MAX_IN],
-                                                 int o, float* zz) {
-  float s = lds_f32(fpa + (FP_B1 + o) * 4);
-  const uint32_t wa = fpa + (FP_W1 + o * 8) * 4;
-  if (pi.d_in <= 3) {            // common 1-D / 2-D / 3-D problems: no predicated tail
-    s = fmaf(lds_f32(wa), x[0], s);
-    if (pi.d_in >= 2) s = fmaf(lds_f32(wa + 4), x[1], s);
-    if (pi.d_in == 3) s = fmaf(lds_f32(wa + 8), x[2], s);
-  } else {
-#pragma unroll
-    for (int k = 0; k < PINN_MAX_IN; ++k)
-      if (k < pi.d_in) s = fmaf(lds_f32(wa + k * 4), x[k], s);
-  }
-  zz[0] = s;
-#pragma unroll
-  for (int j = 0; j < N1; ++j) zz[1 + j] = lds_f32(fpa + (FP_W1 + o * 8 + pi.dir1[j]) * 4);
-#pragma unroll
-  for (int j = 0; j < N2; ++j) zz[1 + N1 + j] = 0.f;
-}
 
 
 // ---- granule loops (4 columns x all channels per step), specialised on the activation kind -------------
@@ -94,8 +68,8 @@ __device__ __forceinline__ void l0_fwd_loop(const LoopCtx lc, const PassInfo<N1,
 #pragma unroll
     for (int i = 0; i < GW; i += 2) {
       float za[C], zb2[C];
-      first_layer_elem<N1, N2>(lc.fp, pi, x, g * GW + i, za);
-      first_layer_elem<N1, N2>(lc.fp, pi, x, g * GW + i + 1, zb2);
+      first_layer_elem<kTcW>(lc.fp, pi, x, g * GW + i, za);
+      first_layer_elem<kTcW>(lc.fp, pi, x, g * GW + i + 1, zb2);
       P2 zz[C], hv[C];
 #pragma unroll
       for (int c = 0; c < C; ++c) zz[c] = mk2(za[c], zb2[c]);
@@ -103,7 +77,7 @@ __device__ __forceinline__ void l0_fwd_loop(const LoopCtx lc, const PassInfo<N1,
 #pragma unroll
       for (int c = 0; c < C; ++c) { h[c][i] = hv[c].v.x; h[c][i + 1] = hv[c].v.y; }
       if (lc.flag) {
-        const float w0 = lds_f32(lc.fp + (FP_WL + g * GW + i) * 4), w1 = lds_f32(lc.fp + (FP_WL + g * GW + i + 1) * 4);
+        const float w0 = lds_f32(lc.fp + (Fp::WL + g * GW + i) * 4), w1 = lds_f32(lc.fp + (Fp::WL + g * GW + i + 1) * 4);
 #pragma unroll
         for (int c = 0; c < C; ++c) u[c] = fmaf(w1, hv[c].v.y, fmaf(w0, hv[c].v.x, u[c]));
       }
@@ -122,28 +96,11 @@ __device__ __forceinline__ void tl_fwd_loop(const LoopCtx lc, const Chan<N1, N2>
   float u[C];
 #pragma unroll
   for (int c = 0; c < C; ++c) u[c] = up[c];
-#if PINN_TC_PREFETCH
-  // software pipeline: the accumulator loads of granule g + 1 are in flight while granule g is evaluated
-  float zn[C][GW];
-#pragma unroll
-  for (int c = 0; c < C; ++c) acc_ldg(lc.taddr + TM_X + c * 64 + lc.g0 * GW, zn[c]);
-#endif
 #pragma unroll 1
   for (int g = lc.g0; g < lc.g1; ++g) {
     float z[C][GW];
-#if PINN_TC_PREFETCH
-#pragma unroll
-    for (int c = 0; c < C; ++c)
-#pragma unroll
-      for (int i = 0; i < GW; ++i) z[c][i] = zn[c][i];
-    if (g + 1 < lc.g1) {
-#pragma unroll
-      for (int c = 0; c < C; ++c) acc_ldg(lc.taddr + TM_X + c * 64 + (g + 1) * GW, zn[c]);
-    }
-#else
 #pragma unroll
     for (int c = 0; c < C; ++c) acc_ldg(lc.taddr + TM_X + c * 64 + g * GW, z[c]);
-#endif
 #pragma unroll
     for (int i = 0; i < GW; i += 2) {
       P2 zz[C], hv[C];
@@ -154,7 +111,7 @@ __device__ __forceinline__ void tl_fwd_loop(const LoopCtx lc, const Chan<N1, N2>
 #pragma unroll
       for (int c = 0; c < C; ++c) { z[c][i] = hv[c].v.x; z[c][i + 1] = hv[c].v.y; }
       if (lc.flag) {
-        const float w0 = lds_f32(lc.fp + (FP_WL + g * GW + i) * 4), w1 = lds_f32(lc.fp + (FP_WL + g * GW + i + 1) * 4);
+        const float w0 = lds_f32(lc.fp + (Fp::WL + g * GW + i) * 4), w1 = lds_f32(lc.fp + (Fp::WL + g * GW + i + 1) * 4);
 #pragma unroll
         for (int c = 0; c < C; ++c) u[c] = fmaf(w1, hv[c].v.y, fmaf(w0, hv[c].v.x, u[c]));
       }
@@ -175,44 +132,20 @@ __device__ __forceinline__ void tl_bwd_loop(const LoopCtx lc, const Chan<N1, N2>
   float ub[C];
 #pragma unroll
   for (int c = 0; c < C; ++c) ub[c] = ubp[c];
-#if PINN_TC_PREFETCH
-  float zn[C][GWB], hn[C][GWB];
-#pragma unroll
-  for (int c = 0; c < C; ++c) acc_ldg(lc.taddr + TM_Y + c * 32 + lc.g0 * GWB, zn[c]);
-  if (!lc.flag) {
-#pragma unroll
-    for (int c = 0; c < C; ++c) acc_ldg(lc.taddr + TM_X + c * 64 + lc.c0 + lc.g0 * GWB, hn[c]);
-  }
-#endif
 #pragma unroll 1
   for (int g = lc.g0; g < lc.g1; ++g) {
     const int ocol = lc.c0 + g * GWB;
     float z[C][GWB], hb[C][GWB];
-#if PINN_TC_PREFETCH
-#pragma unroll
-    for (int c = 0; c < C; ++c)
-#pragma unroll
-      for (int i = 0; i < GWB; ++i) { z[c][i] = zn[c][i]; hb[c][i] = hn[c][i]; }
-    if (g + 1 < lc.g1) {
-#pragma unroll
-      for (int c = 0; c < C; ++c) acc_ldg(lc.taddr + TM_Y + c * 32 + (g + 1) * GWB, zn[c]);
-      if (!lc.flag) {
-#pragma unroll
-        for (int c = 0; c < C; ++c) acc_ldg(lc.taddr + TM_X + c * 64 + ocol + GWB, hn[c]);
-      }
-    }
-#else
 #pragma unroll
     for (int c = 0; c < C; ++c) acc_ldg(lc.taddr + TM_Y + c * 32 + g * GWB, z[c]);
     if (!lc.flag) {
 #pragma unroll
       for (int c = 0; c < C; ++c) acc_ldg(lc.taddr + TM_X + c * 64 + ocol, hb[c]);
     }
-#endif
     if (lc.flag) {
 #pragma unroll
       for (int i = 0; i < GWB; ++i) {
-        const float wl = lds_f32(lc.fp + (FP_WL + ocol + i) * 4);
+        const float wl = lds_f32(lc.fp + (Fp::WL + ocol + i) * 4);
 #pragma unroll
         for (int c = 0; c < C; ++c) hb[c][i] = wl * ub[c];
       }
@@ -251,8 +184,8 @@ __device__ __forceinline__ void l0_bwd_store_loop(const LoopCtx lc, const PassIn
 #pragma unroll
     for (int i = 0; i < GWB; i += 2) {
       float za[C], zb2[C];
-      first_layer_elem<N1, N2>(lc.fp, pi, x, g * GWB + i, za);
-      first_layer_elem<N1, N2>(lc.fp, pi, x, g * GWB + i + 1, zb2);
+      first_layer_elem<kTcW>(lc.fp, pi, x, g * GWB + i, za);
+      first_layer_elem<kTcW>(lc.fp, pi, x, g * GWB + i + 1, zb2);
       P2 zz[C], hv[C], zv[C];
 #pragma unroll
       for (int c = 0; c < C; ++c) { zz[c] = mk2(za[c], zb2[c]); hv[c] = mk2(hb[c][i], hb[c][i + 1]); }
@@ -286,7 +219,7 @@ __device__ __forceinline__ void l0_bwd_loop(const LoopCtx lc, const PassInfo<N1,
     } else {
 #pragma unroll
       for (int i = 0; i < GW; ++i) {
-        const float wl = lds_f32(lc.fp + (FP_WL + g * GW + i) * 4);
+        const float wl = lds_f32(lc.fp + (Fp::WL + g * GW + i) * 4);
 #pragma unroll
         for (int c = 0; c < C; ++c) hb[c][i] = wl * ub[c];
       }
@@ -296,7 +229,7 @@ __device__ __forceinline__ void l0_bwd_loop(const LoopCtx lc, const PassInfo<N1,
     for (int i = 0; i < GW; ++i) {
       // scalar here: the packed form raises the register pressure of this loop past the 128-register budget
       float zz[C], hv[C], zv[C];
-      first_layer_elem<N1, N2>(lc.fp, pi, x, g * GW + i, zz);
+      first_layer_elem<kTcW>(lc.fp, pi, x, g * GW + i, zz);
 #pragma unroll
       for (int c = 0; c < C; ++c) hv[c] = hb[c][i];
       chain_bwd<N1, N2, PURE, AK, float>(lc.act, pi.ch, zz, hv, zv);
@@ -411,7 +344,7 @@ __device__ __noinline__ uint32_t net_forward(CtaShared* cs, const DevProblem* Pp
     dbg_mark(cs, 14);
     const int ng = n_out / GW;
     LoopCtx lc;
-    lc.fp = tc::smem_u32(fp); lc.bt = lc.fp + (FP_BT + (l - 1) * 64) * 4; lc.tP = tc::smem_u32(tP); lc.tQ = tc::smem_u32(tQ);
+    lc.fp = tc::smem_u32(fp); lc.bt = lc.fp + (Fp::BT + (l - 1) * 64) * 4; lc.tP = tc::smem_u32(tP); lc.tQ = tc::smem_u32(tQ);
     lc.gb = nullptr; lc.gw = nullptr;
     lc.taddr = accm + t.lane_addr; lc.act = act; lc.split = split ? 1 : 0; lc.p = p; lc.lane = t.lane;
     lc.g0 = hh * (ng / kNH); lc.g1 = (hh + 1) * (ng / kNH); lc.c0 = 0; lc.flag = (l == TL) ? 1 : 0;
@@ -426,7 +359,7 @@ __device__ __noinline__ uint32_t net_forward(CtaShared* cs, const DevProblem* Pp
   if (hh == 0) {
 #pragma unroll
     for (int c = 0; c < C; ++c) u[c] = ms.scratch[c * kTcPts + p];
-    u[0] += fp[FP_BL];
+    u[0] += fp[Fp::BL];
     const int n_taps = tm.n_taps;
     for (int tt = 0; tt < n_taps; ++tt)
       if (tm.tap_slot[tt] == slot) {
@@ -537,7 +470,7 @@ __device__ __noinline__ uint32_t net_backward(CtaShared* cs, const DevProblem* P
     const int act = net.acts[l];
     float* gb = partial + net.b_off[l];
     float* gw = partial + net.w_off[l];
-    const float* bt = fp + FP_BT + (l - 1) * 64;
+    const float* bt = fp + Fp::BT + (l - 1) * 64;
     const uint32_t whi = tc::smem_u32(smem + ns.w_hi[l - 1]);
     dbg_mark(cs, 21);
     if (tid == 0) {
@@ -705,21 +638,14 @@ __device__ __noinline__ uint32_t net_backward(CtaShared* cs, const DevProblem* P
 __global__ void __launch_bounds__(kTcThreads, 1) tc_loss_grad_kernel(const __grid_constant__ TcArgs args) {
   extern __shared__ __align__(1024) uint8_t smem[];
   __shared__ CtaShared cs;
-  const int tid = threadIdx.x, lane = tid & 31;
+  const int tid = threadIdx.x;
   const DevProblem* Pp = args.prob;
   const DevProblem& P = *Pp;
   const Misc ms = misc_of(smem + args.off_misc, args.mx_dim, args.mx_taps);
   float* partial = args.partial + (long long)blockIdx.x * args.partial_stride;
   const bool want_grad = (args.mode == 0);
   const float* theta = args.theta;
-#ifdef PINN_DEBUG
-  long long span_c0 = 0;
-  unsigned long long span_g0 = 0;
-  if (args.dbg && tid == 0) {
-    span_c0 = clock64();
-    asm volatile("mov.u64 %0, %globaltimer;" : "=l"(span_g0));
-  }
-#endif
+  const DbgSpan span = dbg_span_begin(args.dbg);
 
   // ---- per-CTA setup --------------------------------------------------------------------------------------------------------
   // The step usually starts with everything cold in L2 (the caller's other work evicted it).  Pull what the serial setup
@@ -764,37 +690,14 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_loss_grad_kernel(const __gri
 #endif
   }
   if (tid == 0) tc::s_acc = args.acc + (size_t)blockIdx.x * kAccCols * kAccRows;
-  if (want_grad) {
-    const long long n4 = P.n_theta / 4;
-    float4* p4 = reinterpret_cast<float4*>(partial);
-    if ((reinterpret_cast<uintptr_t>(partial) & 15) == 0) {
-      for (long long i = tid; i < n4; i += kTcThreads) p4[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-      for (long long i = n4 * 4 + tid; i < P.n_theta; i += kTcThreads) partial[i] = 0.f;
-    } else {
-      for (long long i = tid; i < P.n_theta; i += kTcThreads) partial[i] = 0.f;
-    }
-  }
-  if (tid < PINN_MAX_TERMS) ms.tsum[tid] = 0.0;
-  if (tid < 64) {      // ones atom: row r (128 B) holds bf16 1.0 in logical column 0 = 16-byte chunk (0 ^ r)
-    const int r = tid >> 3, ch = tid & 7;
-    *reinterpret_cast<uint4*>(smem + args.off_ones + r * 128 + ch * 16) = make_uint4(ch == r ? 0x00003f80u : 0u, 0u, 0u, 0u);
-  }
-  // stage weights: bf16 hi / lo operand tiles of the tensor layers, fp32 blocks of the first / last layers
+  cta_setup(args, ms, partial, P.n_theta, want_grad);
+  // stage weights: fp32 blocks of the first / last layers, bf16 hi / lo operand tiles of the tensor layers
   for (int kn = 0; kn < P.n_nets; ++kn) {
     const DevNet& net = P.nets[kn];
     const TcNetSmem& ns = args.nets[kn];
     if (ns.fp < 0) continue;
-    float* fp = reinterpret_cast<float*>(smem + ns.fp);
+    stage_fp_block<kTcW>(reinterpret_cast<float*>(smem + ns.fp), net, theta);
     const int L = net.n_layers;
-    for (int i = tid; i < FP_SIZE; i += kTcThreads) fp[i] = 0.f;
-    __syncthreads();
-    const int n1w = net.dims[1], d_in = net.dims[0];
-    const long long w0 = net.w_off[0], b0 = net.b_off[0];
-    for (int i = tid; i < n1w * d_in; i += kTcThreads) {
-      const int o = i % n1w, k = i / n1w;
-      fp[FP_W1 + o * 8 + k] = __ldg(&theta[w0 + i]);
-    }
-    for (int i = tid; i < n1w; i += kTcThreads) fp[FP_B1 + i] = __ldg(&theta[b0 + i]);
     // thread <-> (layer, row o, chunk of 8 k).  All global loads of all layers are issued before the first conversion
     // (fully unrolled, predicated on the layer count): one memory round trip instead of one per layer -- the step
     // starts with theta cold in L2 when the caller's other work has evicted it
@@ -839,14 +742,6 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_loss_grad_kernel(const __gri
         }
       }
     }
-    for (int i = tid; i < (L - 2) * 64; i += kTcThreads) {
-      const int l = 1 + i / 64, o = i & 63;
-      if (o < net.dims[l + 1]) fp[FP_BT + (l - 1) * 64 + o] = __ldg(&theta[net.b_off[l] + o]);
-    }
-    const int nL = net.dims[L - 1];
-    const long long wl = net.w_off[L - 1], bl = net.b_off[L - 1];
-    for (int i = tid; i < nL; i += kTcThreads) fp[FP_WL + i] = __ldg(&theta[wl + i]);
-    if (tid == 0) fp[FP_BL] = __ldg(&theta[bl]);
   }
   tc::fence_async_smem();
   __syncthreads();
@@ -854,105 +749,26 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_loss_grad_kernel(const __gri
   uint32_t phase = 0;
 
   for (int tile = args.tile_begin + blockIdx.x; tile < args.tile_end; tile += gridDim.x) {
-    int ti = 0;
-    while (ti + 1 < P.n_terms && tile >= args.dyn[ti + 1].tile0) ++ti;
-    const DevTerm* tmp = &P.terms[ti];
-    const DevTerm& tm = *tmp;
-    const long long p0 = (long long)(tile - args.dyn[ti].tile0) * kTcPts;
-    const long long n_pts = args.dyn[ti].n;
-    const float* pts = reinterpret_cast<const float*>(args.dyn[ti].pts);
-    const float* qw = reinterpret_cast<const float*>(args.dyn[ti].qw);
-    // warm L1 with the term header + residual program and the network descriptors (read by every phase)
-    if (tid < (int)((sizeof(DevTerm) + 127) / 128)) tc::prefetch_l1(reinterpret_cast<const char*>(tmp) + tid * 128);
+    // warm L1 with the network descriptors (read by every phase)
     if (tid >= 128 && tid < 128 + (int)((sizeof(DevNet) * PINN_MAX_NETS + 127) / 128))
       tc::prefetch_l1(reinterpret_cast<const char*>(&P.nets[0]) + (tid - 128) * 128);
-    const int dim = tm.dim, n_taps = tm.n_taps, n_used = tm.n_used, weighted = tm.weighted;
-    // Collocation tile: one point = dim contiguous scalars (the reference's d x N train-set layout), so a full 128-point
-    // tile is ONE contiguous block of dim x 512 bytes.  The TMA unit copies it into shared memory in a single bulk transfer
-    // (cp.async.bulk + mbarrier transaction count; staged in the scratch array, free between tiles) and 128 threads
-    // transpose it to [row][point].  Partial last tiles (clamped rows) and callers' buffers that are not 16-byte aligned
-    // take the per-element path.
-    const float* tile_src = pts + p0 * dim;
-    const bool bulk_tile = (p0 + kTcPts <= n_pts) && dim <= kTcMaxC && ((reinterpret_cast<uintptr_t>(tile_src) & 15) == 0);
-    if (bulk_tile) {
-      uint32_t ldp = (phase >> 1) & 1u;
-      if (tid == 0) {
-        tc::mbar_arrive_expect_tx(ms.bar_ld, (uint32_t)(dim * kTcPts * 4));
-        tc::bulk_load(ms.scratch, tile_src, (uint32_t)(dim * kTcPts * 4), ms.bar_ld);
-      }
-      wait_bar(ms.bar_ld, ldp);
-      phase = (phase & 1u) | (ldp << 1);
-      if (tid < kTcPts)
-        for (int r = 0; r < dim; ++r) ms.Xs[r * kTcPts + tid] = ms.scratch[tid * dim + r];
-    } else {
-      for (int i = tid; i < dim * kTcPts; i += kTcThreads) {
-        int pp = i / dim, r = i - pp * dim;
-        long long gp = p0 + pp;
-        if (gp >= n_pts) gp = n_pts - 1;
-        ms.Xs[r * kTcPts + pp] = pts[gp * dim + r];
-      }
-    }
-    if (tid < kTcPts) {
-      long long gp = p0 + tid;
-      float w = 0.f;
-      if (gp < n_pts) w = weighted ? qw[gp] : 1.f;
-      ms.qws[tid] = w;
-    }
-    for (int i = tid; i < n_taps * kTcPts; i += kTcThreads) ms.tapbar[i] = 0.f;
-    __syncthreads();
+    uint32_t ldp = (phase >> 1) & 1u;
+    const TileRef tr = stage_tile(args, P, ms, tile, ldp);
+    phase = (phase & 1u) | (ldp << 1);
+    const DevTerm* tmp = &P.terms[tr.ti];
+    const DevTerm& tm = *tmp;
+    const int n_used = tm.n_used;
     dbg_mark(&cs, 3);
 
     for (int slot = 0; slot < n_used; ++slot) {
       const int k1 = tm.chan[slot].n1, k2 = tm.chan[slot].n2, pu = tm.chan[slot].pure;
       const int ak = args.net_ak[tm.used_net[slot]];
-      PINN_TC_DISPATCH(k1, k2, pu, ak, (phase = net_forward<A1, A2, PU, AK>(&cs, Pp, tmp, slot, want_grad ? 1 : 0, phase)));
+      PINN_TC_DISPATCH(kTcMaxC, k1, k2, pu, ak, (phase = net_forward<A1, A2, PU, AK>(&cs, Pp, tmp, slot, want_grad ? 1 : 0, phase)));
     }
 
     dbg_mark(&cs, 4);
-    // the lo-tile region Q is free between the forward and the reverse sweep: stage the program text and the
-    // per-point value / adjoint arrays there (shared memory instead of global + local memory)
-    const int n_instr = tm.n_instr;
-    DevInstr* sprog = reinterpret_cast<DevInstr*>(smem + args.off_Q);
-    float* sval = reinterpret_cast<float*>(smem + args.off_Q + 8192);
-    const bool prog_sm = (size_t)8192 + (size_t)2 * n_instr * kTcPts * 4 <= (size_t)(args.off_Q_bytes);
-    if (prog_sm) {
-      const int nw = n_instr * (int)(sizeof(DevInstr) / 4);
-      const int* src = reinterpret_cast<const int*>(tm.prog);
-      for (int i = tid; i < nw; i += kTcThreads) reinterpret_cast<int*>(sprog)[i] = __ldg(src + i);
-      __syncthreads();
-    }
-    // ---- residual program, loss partial, tap adjoints (threads 0..127: one point each) -----------------------------------------
-    if (tid < kTcPts) {
-      float pbar[PINN_MAX_PARAMS];
-#pragma unroll
-      for (int j = 0; j < PINN_MAX_PARAMS; ++j) pbar[j] = 0.f;
-      float r;
-      if (prog_sm) {
-        r = run_program_t<float, kTcPts, true>(sprog, n_instr, theta + P.param_off, ms.Xs, ms.taps, ms.tapbar, pbar, tid,
-                                               want_grad, sval, sval + n_instr * kTcPts);
-      } else {
-        r = run_program<float, kTcPts>(tm, theta + P.param_off, ms.Xs, ms.taps, ms.tapbar, pbar, tid, want_grad);
-      }
-      const float w = ms.qws[tid];
-      double s = (double)w * (double)r * (double)r;
-#pragma unroll
-      for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-      if (lane == 0) atomicAdd(&ms.tsum[ti], s);
-      if (args.mode == 2) {
-        long long gp = p0 + tid;
-        if (gp < n_pts) args.resid_out[gp] = r;
-      }
-      if (want_grad) {
-        const float g = (float)args.seed[ti] * w * 2.f * r;
-        for (int tt = 0; tt < n_taps; ++tt) ms.tapbar[tt * kTcPts + tid] *= g;
-        const int n_params = P.n_params;
-        for (int j = 0; j < n_params; ++j) {
-          float v = warp_sum<float>(pbar[j] * g);
-          if (lane == 0) atomicAdd(&partial[P.param_off + j], v);
-        }
-      }
-    }
-    __syncthreads();
+    // the lo-tile region Q is free between the forward and the reverse sweep
+    residual_step(args, P, tm, ms, tr, smem + args.off_Q, (size_t)args.off_Q_bytes, partial, want_grad);
 
     dbg_mark(&cs, 5);
     if (want_grad) {
@@ -964,31 +780,16 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_loss_grad_kernel(const __gri
         const int ak = args.net_ak[tm.used_net[slot]];
         if (n_used > 1) {
           // P must hold this slot's last hidden activations again: recompute its forward
-          PINN_TC_DISPATCH(k1, k2, pu, ak, (phase = net_forward<A1, A2, PU, AK>(&cs, Pp, tmp, slot, 0, phase)));
+          PINN_TC_DISPATCH(kTcMaxC, k1, k2, pu, ak, (phase = net_forward<A1, A2, PU, AK>(&cs, Pp, tmp, slot, 0, phase)));
         }
-        PINN_TC_DISPATCH(k1, k2, pu, ak, (phase = net_backward<A1, A2, PU, AK>(&cs, Pp, tmp, slot, phase)));
+        PINN_TC_DISPATCH(kTcMaxC, k1, k2, pu, ak, (phase = net_backward<A1, A2, PU, AK>(&cs, Pp, tmp, slot, phase)));
       }
     }
   }
 
   __syncthreads();
   dbg_mark(&cs, 7);
-#ifdef PINN_DEBUG
-  if (tid == 0 && cs.dbg) cs.dbg[999] = cs.dbg_n;
-  if (args.dbg && tid == 0 && blockIdx.x < 250) {
-    unsigned long long g1;
-    unsigned int smid;
-    asm volatile("mov.u64 %0, %globaltimer;" : "=l"(g1));
-    asm volatile("mov.u32 %0, %smid;" : "=r"(smid));
-    long long* rec = args.dbg + 1000 + 4 * blockIdx.x;
-    rec[0] = (long long)span_g0; rec[1] = (long long)g1; rec[2] = clock64() - span_c0; rec[3] = smid;
-  }
-#endif
-  if (tid < PINN_MAX_TERMS) args.term_sums[(long long)blockIdx.x * PINN_MAX_TERMS + tid] = ms.tsum[tid];
-  // gradient reduction, optimizer step and the multi-GPU sum in the kernel tail (tail.cuh)
-  if (args.tail.state)
-    fused_tail<float, kTcThreads>(args.tail, args.partial, args.partial_stride, args.term_sums, P.n_theta, P.n_terms, want_grad ? 1 : 0,
-                                  reinterpret_cast<float*>(smem + args.off_P));
+  cta_finish(args, cs, span, ms, P, want_grad);
 }
 
 // ---- host side ------------------------------------------------------------------------------------------------------------------
@@ -998,10 +799,7 @@ size_t tc_misc_bytes(int mx_dim, int mx_taps) {
 }
 
 cudaError_t tc_launch(const TcArgs& a, int grid, size_t smem, cudaStream_t st) {
-  static size_t granted[64] = {0};
-  cudaError_t e = ensure_dynamic_smem(tc_loss_grad_kernel, smem, granted);
-  if (e != cudaSuccess) return e;
-  return launch_fused_kernel(tc_loss_grad_kernel, a, grid, kTcThreads, smem, st, a.tail.state != nullptr);
+  return launch_fused_kernel<tc_loss_grad_kernel>(a, grid, kTcThreads, smem, st);
 }
 
 }  // namespace pinn

@@ -23,11 +23,11 @@
 #include <stdint.h>
 #include <string.h>
 #include "tc_common.cuh"
-#include "tail.cuh"
 
 namespace pinn {
 
 constexpr uint32_t TB = kTileBytes;
+using Fp = FpBlock<kTwW>;   // fp32 parameter block of a network
 
 struct TwShared {
   int tl_max, off_P, off_S, off_misc, off_ones, off_nets, mx_dim, mx_taps;
@@ -43,28 +43,6 @@ struct TwShared {
   uint32_t ph_ld[2];                 // phases of the streaming barriers (flipped by thread 0 after a CTA-wide wait)
   uint64_t bar_ld[2];                // S0 / S1: bytes landed
 };
-
-// first-layer pre-activations of neuron o (channel vector zz); fpa = shared-memory address of the fp32 block
-template <int N1, int N2>
-__device__ __forceinline__ void first_layer_elem_w(uint32_t fpa, const PassInfo<N1, N2>& pi, const float (&x)[PINN_MAX_IN],
-                                                   int o, float* zz) {
-  float s = lds_f32(fpa + (FW_B1 + o) * 4);
-  const uint32_t wa = fpa + (FW_W1 + o * 8) * 4;
-  if (pi.d_in <= 3) {
-    s = fmaf(lds_f32(wa), x[0], s);
-    if (pi.d_in >= 2) s = fmaf(lds_f32(wa + 4), x[1], s);
-    if (pi.d_in == 3) s = fmaf(lds_f32(wa + 8), x[2], s);
-  } else {
-#pragma unroll
-    for (int k = 0; k < PINN_MAX_IN; ++k)
-      if (k < pi.d_in) s = fmaf(lds_f32(wa + k * 4), x[k], s);
-  }
-  zz[0] = s;
-#pragma unroll
-  for (int j = 0; j < N1; ++j) zz[1 + j] = lds_f32(fpa + (FW_W1 + o * 8 + pi.dir1[j]) * 4);
-#pragma unroll
-  for (int j = 0; j < N2; ++j) zz[1 + N1 + j] = 0.f;
-}
 
 struct LoopW {
   uint32_t fp;            // shared-memory address of the network's fp32 parameter block
@@ -90,8 +68,8 @@ __device__ __forceinline__ void tw_l0_fwd_loop(const LoopW lc, const PassInfo<N1
 #pragma unroll
     for (int i = 0; i < 4; i += 2) {
       float za[C], zb2[C];
-      first_layer_elem_w<N1, N2>(lc.fp, pi, x, g * 4 + i, za);
-      first_layer_elem_w<N1, N2>(lc.fp, pi, x, g * 4 + i + 1, zb2);
+      first_layer_elem<kTwW>(lc.fp, pi, x, g * 4 + i, za);
+      first_layer_elem<kTwW>(lc.fp, pi, x, g * 4 + i + 1, zb2);
       P2 zz[C], hv[C];
 #pragma unroll
       for (int c = 0; c < C; ++c) zz[c] = mk2(za[c], zb2[c]);
@@ -133,7 +111,7 @@ __device__ __forceinline__ void tw_fwd_loop(const LoopW lc, const Chan<N1, N2> c
 #pragma unroll
       for (int c = 0; c < C; ++c) { z[c][i] = hv[c].v.x; z[c][i + 1] = hv[c].v.y; }
       if (lc.flag) {
-        const float w0 = lds_f32(lc.fp + (FW_WL + col + i) * 4), w1 = lds_f32(lc.fp + (FW_WL + col + i + 1) * 4);
+        const float w0 = lds_f32(lc.fp + (Fp::WL + col + i) * 4), w1 = lds_f32(lc.fp + (Fp::WL + col + i + 1) * 4);
 #pragma unroll
         for (int c = 0; c < C; ++c) u[c] = fmaf(w1, hv[c].v.y, fmaf(w0, hv[c].v.x, u[c]));
       }
@@ -172,7 +150,7 @@ __device__ __forceinline__ void tw_bwd_loop(const LoopW lc, const Chan<N1, N2> c
     } else {
 #pragma unroll
       for (int i = 0; i < 4; ++i) {
-        const float wl = lds_f32(lc.fp + (FW_WL + ocol + i) * 4);
+        const float wl = lds_f32(lc.fp + (Fp::WL + ocol + i) * 4);
 #pragma unroll
         for (int c = 0; c < C; ++c) hb[c][i] = wl * ub[c];
       }
@@ -213,8 +191,8 @@ __device__ __forceinline__ void tw_l0_bwd_store_loop(const LoopW lc, const PassI
 #pragma unroll
     for (int c = 0; c < C; ++c) acc_ld2(lc.taddr + c * kTwW + col, hb[c]);
     float za[C], zb2[C];
-    first_layer_elem_w<N1, N2>(lc.fp, pi, x, col, za);
-    first_layer_elem_w<N1, N2>(lc.fp, pi, x, col + 1, zb2);
+    first_layer_elem<kTwW>(lc.fp, pi, x, col, za);
+    first_layer_elem<kTwW>(lc.fp, pi, x, col + 1, zb2);
     P2 zz[C], hv[C], zv[C];
 #pragma unroll
     for (int c = 0; c < C; ++c) { zz[c] = mk2(za[c], zb2[c]); hv[c] = mk2(hb[c][0], hb[c][1]); }
@@ -325,7 +303,7 @@ __device__ __noinline__ void tw_net_forward(TwShared* cs, const DevProblem* Pp, 
     dbg_mark(cs, 14);
     const int ng = n_out / 4;
     LoopW lc;
-    lc.fp = tc::smem_u32(fp); lc.bt = lc.fp + (FW_BT + (l - 1) * 128) * 4; lc.tP = tc::smem_u32(tP); lc.gb = nullptr;
+    lc.fp = tc::smem_u32(fp); lc.bt = lc.fp + (Fp::BT + (l - 1) * 128) * 4; lc.tP = tc::smem_u32(tP); lc.gb = nullptr;
     lc.taddr = accm + t.lane_addr; lc.act = net.acts[l]; lc.p = p; lc.lane = t.lane;
     lc.g0 = hh * (ng / kNH); lc.g1 = (hh + 1) * (ng / kNH); lc.flag = (l == TL) ? 1 : 0;
     float2* zl = want_grad ? reinterpret_cast<float2*>(zst + (size_t)(l - 1) * kTwMaxC * 64 * kTcPts * 2) + p : nullptr;
@@ -353,7 +331,7 @@ __device__ __noinline__ void tw_net_forward(TwShared* cs, const DevProblem* Pp, 
   if (hh == 0) {
 #pragma unroll
     for (int c = 0; c < C; ++c) u[c] = ms.scratch[c * kTcPts + p];
-    u[0] += fp[FW_BL];
+    u[0] += fp[Fp::BL];
     const int n_taps = tm.n_taps;
     for (int tt = 0; tt < n_taps; ++tt)
       if (tm.tap_slot[tt] == slot) {
@@ -651,23 +629,6 @@ __device__ __noinline__ void tw_net_backward(TwShared* cs, const DevProblem* Pp,
 }
 
 
-// channel structures the wide path instantiates (C <= 4)
-#define PINN_TW_DISPATCH(n1, n2, pure, ak, CALL)                              \
-  do {                                                                        \
-    const int _ak = (ak);                                                     \
-    const int _key = ((n1) * 8 + (n2)) * 2 + ((pure) ? 1 : 0);                \
-    switch (_key) {                                                           \
-      case (0 * 8 + 0) * 2: case (0 * 8 + 0) * 2 + 1: PINN_TC_CASE(0, 0, true, CALL);   \
-      case (1 * 8 + 0) * 2: case (1 * 8 + 0) * 2 + 1: PINN_TC_CASE(1, 0, true, CALL);   \
-      case (2 * 8 + 0) * 2: case (2 * 8 + 0) * 2 + 1: PINN_TC_CASE(2, 0, true, CALL);   \
-      case (3 * 8 + 0) * 2: case (3 * 8 + 0) * 2 + 1: PINN_TC_CASE(3, 0, true, CALL);   \
-      case (1 * 8 + 1) * 2: case (1 * 8 + 1) * 2 + 1: PINN_TC_CASE(1, 1, true, CALL);   \
-      case (2 * 8 + 1) * 2 + 1: PINN_TC_CASE(2, 1, true, CALL);               \
-      case (2 * 8 + 1) * 2: PINN_TC_CASE(2, 1, false, CALL);                  \
-      default: break;                                                         \
-    }                                                                         \
-  } while (0)
-
 // ---- weight packing: theta (fp32, out x in column-major) -> bf16 swizzled images [kb][128 rows o][64 k] ---------------
 __global__ void __launch_bounds__(256) tw_pack_kernel(const TwPackArgs a) {
   const int img = blockIdx.x >> 3;
@@ -694,21 +655,14 @@ __global__ void __launch_bounds__(256) tw_pack_kernel(const TwPackArgs a) {
 __global__ void __launch_bounds__(kTcThreads, 1) tw_loss_grad_kernel(const __grid_constant__ TwArgs args) {
   extern __shared__ __align__(1024) uint8_t smem[];
   __shared__ TwShared cs;
-  const int tid = threadIdx.x, lane = tid & 31;
+  const int tid = threadIdx.x;
   const DevProblem* Pp = args.prob;
   const DevProblem& P = *Pp;
   const Misc ms = misc_of(smem + args.off_misc, args.mx_dim, args.mx_taps);
   float* partial = args.partial + (long long)blockIdx.x * args.partial_stride;
   const bool want_grad = (args.mode == 0);
   const float* theta = args.theta;
-#ifdef PINN_DEBUG
-  long long span_c0 = 0;
-  unsigned long long span_g0 = 0;
-  if (args.dbg && tid == 0) {
-    span_c0 = clock64();
-    asm volatile("mov.u64 %0, %globaltimer;" : "=l"(span_g0));
-  }
-#endif
+  const DbgSpan span = dbg_span_begin(args.dbg);
 
   // ---- per-CTA setup --------------------------------------------------------------------------------------------------------
   if (tid == 0) {
@@ -735,51 +689,16 @@ __global__ void __launch_bounds__(kTcThreads, 1) tw_loss_grad_kernel(const __gri
 #endif
   }
   if (tid == 0) tc::s_acc = args.acc + (size_t)blockIdx.x * kAccCols * kAccRows;
-  if (want_grad) {
-    const long long n4 = P.n_theta / 4;
-    float4* p4 = reinterpret_cast<float4*>(partial);
-    if ((reinterpret_cast<uintptr_t>(partial) & 15) == 0) {
-      for (long long i = tid; i < n4; i += kTcThreads) p4[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-      for (long long i = n4 * 4 + tid; i < P.n_theta; i += kTcThreads) partial[i] = 0.f;
-    } else {
-      for (long long i = tid; i < P.n_theta; i += kTcThreads) partial[i] = 0.f;
-    }
-  }
-  if (tid < PINN_MAX_TERMS) ms.tsum[tid] = 0.0;
+  cta_setup(args, ms, partial, P.n_theta, want_grad);
   {      // network descriptors: every layer of every sweep reads widths / offsets / activations
     const int nw = P.n_nets * (int)(sizeof(DevNet) / 4);
     const int* src = reinterpret_cast<const int*>(&P.nets[0]);
     int* dst = reinterpret_cast<int*>(smem + args.off_nets);
     for (int i = tid; i < nw; i += kTcThreads) dst[i] = __ldg(src + i);
   }
-  if (tid < 64) {      // ones atom: row r (128 B) holds bf16 1.0 in logical column 0 = 16-byte chunk (0 ^ r)
-    const int r = tid >> 3, ch = tid & 7;
-    *reinterpret_cast<uint4*>(smem + args.off_ones + r * 128 + ch * 16) = make_uint4(ch == r ? 0x00003f80u : 0u, 0u, 0u, 0u);
-  }
   // fp32 blocks of the first / last layers and the tensor-layer biases
-  for (int kn = 0; kn < P.n_nets; ++kn) {
-    if (args.off_fp[kn] < 0) continue;
-    const DevNet& net = P.nets[kn];
-    float* fp = reinterpret_cast<float*>(smem + args.off_fp[kn]);
-    const int L = net.n_layers;
-    for (int i = tid; i < FW_SIZE; i += kTcThreads) fp[i] = 0.f;
-    __syncthreads();
-    const int n1w = net.dims[1], d_in = net.dims[0];
-    const long long w0 = net.w_off[0], b0 = net.b_off[0];
-    for (int i = tid; i < n1w * d_in; i += kTcThreads) {
-      const int o = i % n1w, k = i / n1w;
-      fp[FW_W1 + o * 8 + k] = __ldg(&theta[w0 + i]);
-    }
-    for (int i = tid; i < n1w; i += kTcThreads) fp[FW_B1 + i] = __ldg(&theta[b0 + i]);
-    for (int i = tid; i < (L - 2) * 128; i += kTcThreads) {
-      const int l = 1 + i / 128, o = i & 127;
-      if (o < net.dims[l + 1]) fp[FW_BT + (l - 1) * 128 + o] = __ldg(&theta[net.b_off[l] + o]);
-    }
-    const int nL = net.dims[L - 1];
-    const long long wl = net.w_off[L - 1], bl = net.b_off[L - 1];
-    for (int i = tid; i < nL; i += kTcThreads) fp[FW_WL + i] = __ldg(&theta[wl + i]);
-    if (tid == 0) fp[FW_BL] = __ldg(&theta[bl]);
-  }
+  for (int kn = 0; kn < P.n_nets; ++kn)
+    if (args.off_fp[kn] >= 0) stage_fp_block<kTwW>(reinterpret_cast<float*>(smem + args.off_fp[kn]), P.nets[kn], theta);
   tc::fence_async_smem();
   __syncthreads();
   dbg_mark(&cs, 2);
@@ -788,95 +707,21 @@ __global__ void __launch_bounds__(kTcThreads, 1) tw_loss_grad_kernel(const __gri
   // tiles are claimed dynamically after the first one (heavy PDE tiles come first in the enumeration, cheap boundary
   // tiles last): a static round-robin leaves the CTAs that drew an extra PDE tile 20 % behind the rest
   for (int tile = args.tile_begin + blockIdx.x; tile < args.tile_end;) {
-    int ti = 0;
-    while (ti + 1 < P.n_terms && tile >= args.dyn[ti + 1].tile0) ++ti;
-    const DevTerm* tmp = &P.terms[ti];
+    const TileRef tr = stage_tile(args, P, ms, tile, tile_ld_phase);
+    const DevTerm* tmp = &P.terms[tr.ti];
     const DevTerm& tm = *tmp;
-    const long long p0 = (long long)(tile - args.dyn[ti].tile0) * kTcPts;
-    const long long n_pts = args.dyn[ti].n;
-    const float* pts = reinterpret_cast<const float*>(args.dyn[ti].pts);
-    const float* qw = reinterpret_cast<const float*>(args.dyn[ti].qw);
-    if (tid < (int)((sizeof(DevTerm) + 127) / 128)) tc::prefetch_l1(reinterpret_cast<const char*>(tmp) + tid * 128);
-    const int dim = tm.dim, n_taps = tm.n_taps, n_used = tm.n_used, weighted = tm.weighted;
-    // collocation tile = one contiguous block of dim x 512 bytes: one bulk transfer of the TMA unit into the scratch array,
-    // transposed to [row][point] by 128 threads (see tc_kernel.cu); partial / unaligned tiles take the per-element path
-    const float* tile_src = pts + p0 * dim;
-    const bool bulk_tile = (p0 + kTcPts <= n_pts) && dim <= kTwMaxC && ((reinterpret_cast<uintptr_t>(tile_src) & 15) == 0);
-    if (bulk_tile) {
-      if (tid == 0) {
-        tc::mbar_arrive_expect_tx(ms.bar_ld, (uint32_t)(dim * kTcPts * 4));
-        tc::bulk_load(ms.scratch, tile_src, (uint32_t)(dim * kTcPts * 4), ms.bar_ld);
-      }
-      wait_bar(ms.bar_ld, tile_ld_phase);
-      if (tid < kTcPts)
-        for (int r = 0; r < dim; ++r) ms.Xs[r * kTcPts + tid] = ms.scratch[tid * dim + r];
-    } else {
-      for (int i = tid; i < dim * kTcPts; i += kTcThreads) {
-        int pp = i / dim, r = i - pp * dim;
-        long long gp = p0 + pp;
-        if (gp >= n_pts) gp = n_pts - 1;
-        ms.Xs[r * kTcPts + pp] = pts[gp * dim + r];
-      }
-    }
-    if (tid < kTcPts) {
-      long long gp = p0 + tid;
-      float w = 0.f;
-      if (gp < n_pts) w = weighted ? qw[gp] : 1.f;
-      ms.qws[tid] = w;
-    }
-    for (int i = tid; i < n_taps * kTcPts; i += kTcThreads) ms.tapbar[i] = 0.f;
-    __syncthreads();
+    const int n_used = tm.n_used;
     dbg_mark(&cs, 3);
 
     for (int slot = 0; slot < n_used; ++slot) {
       const int k1 = tm.chan[slot].n1, k2 = tm.chan[slot].n2, pu = tm.chan[slot].pure;
       const int ak = args.net_ak[tm.used_net[slot]];
-      PINN_TW_DISPATCH(k1, k2, pu, ak, (tw_net_forward<A1, A2, PU, AK>(&cs, Pp, tmp, slot, want_grad ? 1 : 0)));
+      PINN_TC_DISPATCH(kTwMaxC, k1, k2, pu, ak, (tw_net_forward<A1, A2, PU, AK>(&cs, Pp, tmp, slot, want_grad ? 1 : 0)));
     }
 
     dbg_mark(&cs, 4);
-    // S0 / S1 are idle between the sweeps: stage the program text and the per-point value / adjoint arrays there
-    const int n_instr = tm.n_instr;
-    DevInstr* sprog = reinterpret_cast<DevInstr*>(smem + args.off_S);
-    float* sval = reinterpret_cast<float*>(smem + args.off_S + 8192);
-    const bool prog_sm = (size_t)8192 + (size_t)2 * n_instr * kTcPts * 4 <= (size_t)(2 * kTwImgBytes);
-    if (prog_sm) {
-      const int nw = n_instr * (int)(sizeof(DevInstr) / 4);
-      const int* src = reinterpret_cast<const int*>(tm.prog);
-      for (int i = tid; i < nw; i += kTcThreads) reinterpret_cast<int*>(sprog)[i] = __ldg(src + i);
-      __syncthreads();
-    }
-    if (tid < kTcPts) {
-      float pbar[PINN_MAX_PARAMS];
-#pragma unroll
-      for (int j = 0; j < PINN_MAX_PARAMS; ++j) pbar[j] = 0.f;
-      float r;
-      if (prog_sm) {
-        r = run_program_t<float, kTcPts, true>(sprog, n_instr, theta + P.param_off, ms.Xs, ms.taps, ms.tapbar, pbar, tid,
-                                               want_grad, sval, sval + n_instr * kTcPts);
-      } else {
-        r = run_program<float, kTcPts>(tm, theta + P.param_off, ms.Xs, ms.taps, ms.tapbar, pbar, tid, want_grad);
-      }
-      const float w = ms.qws[tid];
-      double s = (double)w * (double)r * (double)r;
-#pragma unroll
-      for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-      if (lane == 0) atomicAdd(&ms.tsum[ti], s);
-      if (args.mode == 2) {
-        long long gp = p0 + tid;
-        if (gp < n_pts) args.resid_out[gp] = r;
-      }
-      if (want_grad) {
-        const float g = (float)args.seed[ti] * w * 2.f * r;
-        for (int tt = 0; tt < n_taps; ++tt) ms.tapbar[tt * kTcPts + tid] *= g;
-        const int n_params = P.n_params;
-        for (int j = 0; j < n_params; ++j) {
-          float v = warp_sum<float>(pbar[j] * g);
-          if (lane == 0) atomicAdd(&partial[P.param_off + j], v);
-        }
-      }
-    }
-    __syncthreads();
+    // S0 / S1 are idle between the sweeps
+    residual_step(args, P, tm, ms, tr, smem + args.off_S, (size_t)(2 * kTwImgBytes), partial, want_grad);
 
     dbg_mark(&cs, 5);
     if (want_grad) {
@@ -887,7 +732,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) tw_loss_grad_kernel(const __gri
       for (int slot = n_used - 1; slot >= 0; --slot) {
         const int k1 = tm.chan[slot].n1, k2 = tm.chan[slot].n2, pu = tm.chan[slot].pure;
         const int ak = args.net_ak[tm.used_net[slot]];
-        PINN_TW_DISPATCH(k1, k2, pu, ak, (tw_net_backward<A1, A2, PU, AK>(&cs, Pp, tmp, slot)));
+        PINN_TC_DISPATCH(kTwMaxC, k1, k2, pu, ak, (tw_net_backward<A1, A2, PU, AK>(&cs, Pp, tmp, slot)));
       }
     }
     // claim the next tile only now: claiming a tile ahead would hand the last cheap tiles to CTAs that still owe a heavy one
@@ -898,22 +743,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) tw_loss_grad_kernel(const __gri
 
   __syncthreads();
   dbg_mark(&cs, 7);
-#ifdef PINN_DEBUG
-  if (tid == 0 && cs.dbg) cs.dbg[999] = cs.dbg_n;
-  if (args.dbg && tid == 0 && blockIdx.x < 250) {
-    unsigned long long g1;
-    unsigned int smid;
-    asm volatile("mov.u64 %0, %globaltimer;" : "=l"(g1));
-    asm volatile("mov.u32 %0, %smid;" : "=r"(smid));
-    long long* rec = args.dbg + 1000 + 4 * blockIdx.x;
-    rec[0] = (long long)span_g0; rec[1] = (long long)g1; rec[2] = clock64() - span_c0; rec[3] = smid;
-  }
-#endif
-  if (tid < PINN_MAX_TERMS) args.term_sums[(long long)blockIdx.x * PINN_MAX_TERMS + tid] = ms.tsum[tid];
-  // gradient reduction, optimizer step and the multi-GPU sum in the kernel tail (tail.cuh)
-  if (args.tail.state)
-    fused_tail<float, kTcThreads>(args.tail, args.partial, args.partial_stride, args.term_sums, P.n_theta, P.n_terms, want_grad ? 1 : 0,
-                                  reinterpret_cast<float*>(smem + args.off_P));
+  cta_finish(args, cs, span, ms, P, want_grad);
 }
 
 // ---- host side ------------------------------------------------------------------------------------------------------------------
@@ -923,10 +753,7 @@ cudaError_t tw_pack_launch(const TwPackArgs& a, cudaStream_t st) {
 }
 
 cudaError_t tw_launch(const TwArgs& a, int grid, size_t smem, cudaStream_t st) {
-  static size_t granted[64] = {0};
-  cudaError_t e = ensure_dynamic_smem(tw_loss_grad_kernel, smem, granted);
-  if (e != cudaSuccess) return e;
-  return launch_fused_kernel(tw_loss_grad_kernel, a, grid, kTcThreads, smem, st, a.tail.state != nullptr);
+  return launch_fused_kernel<tw_loss_grad_kernel>(a, grid, kTcThreads, smem, st);
 }
 
 }  // namespace pinn

@@ -1,6 +1,6 @@
 """Device-resident step time of one BASELINE config / mode: K steps, each bracketed by CUDA events on the launching
 stream, L2 flushed (256 MiB memset) between steps; prints median / min ms and launches per step.  Development aid
-(A/B of PINN_B200_TAIL / PINN_B200_COOP and kernel variants via PINN_B200_LIB); the contract bench is bench.py.
+(A/B of PINN_B200_TAIL / PINN_B200_COOP and of two library builds via PINN_B200_LIB); the contract bench is bench.py.
 usage: step_time.py [cfg2|cfg3|cfg1] [mode] [steps] [n (cfg2 grid size)]"""
 import os, sys
 import numpy as np
