@@ -10,8 +10,8 @@
 //      -- replaces the RuntimeGeneratedFunction body (src/discretize.jl:28-175);
 //   3. sum_p qw_p r_p^2 (mean(abs2, .), src/training_strategies.jl:220);
 //   4. the reverse sweep through every network, accumulating d(total)/d(theta) into a
-//      per-CTA partial (no atomics; reduced in fixed order by reduce_kernel, so the
-//      gradient is deterministic) -- replaces the Zygote pullback (src/discretize.jl:778).
+//      per-CTA partial (no atomics; reduced in fixed order by the kernel tail, tail.cuh,
+//      so the gradient is deterministic) -- replaces the Zygote pullback (src/discretize.jl:778).
 //
 // Data layout: activation buffers are [channel][neuron][point] with the point index
 // fastest and a row stride of TP = 32 + 16/sizeof(real) scalars, which makes both the

@@ -1,97 +1,9 @@
-// ffma_launch.cu -- gradient/loss reduction kernels and the host-callable launchers of the
-// FFMA path.
+// ffma_launch.cu -- host-callable launchers of the FFMA path, finish_kernel (unpacks the NCCL fallback's
+// allreduced [grad | term losses]), the gradient statistics kernel and the device-side point samplers.
 #include <cuda_runtime.h>
 #include "dev_types.h"
 
 namespace pinn {
-
-// ------------------------------------------------------------------------------------------
-// Fixed-order reduction of the per-CTA partials; also turns the per-term sums into losses.
-//   out_grad[i]      = sum_b partial[b][i]
-//   out_terms[k]     = scale_k * sum_b term_sums[b][k]          (unweighted L_k)
-//   out_total        = sum_k w_k * out_terms[k]
-// When `packed` is non-null (multi-GPU), grad and the term losses are written contiguously
-// into packed[0..n_theta+n_terms) for a single allreduce and finish_kernel unpacks.
-template <typename real>
-__global__ void reduce_kernel(const real* __restrict__ partial, long long stride, const double* __restrict__ term_sums, int nb,
-                              long long n_theta, int n_terms, const ScaleW sw,
-                              real* out_grad, real* out_terms, real* out_total, int want_grad) {
-  // block = 32 gradient entries x 8 slices of the CTA partials; fixed summation order (slice-major)
-  __shared__ real red[8][33];
-  const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
-  const long long i = (long long)blockIdx.x * 32 + tx;
-  if (want_grad) {
-    real s = real(0);
-    if (i < n_theta) {
-      const int chunk = (nb + 7) / 8;
-      const int b0 = ty * chunk, b1 = (b0 + chunk < nb) ? b0 + chunk : nb;
-      for (int b = b0; b < b1; ++b) s += partial[(long long)b * stride + i];
-    }
-    red[ty][tx] = s;
-    __syncthreads();
-    if (ty == 0 && i < n_theta) {
-      real t = red[0][tx];
-#pragma unroll
-      for (int k = 1; k < 8; ++k) t += red[k][tx];
-      out_grad[i] = t;
-    }
-  }
-  if (blockIdx.x == 0 && threadIdx.x < 32) {
-    double tot = 0.0;
-    for (int k = 0; k < n_terms; ++k) {
-      double s = 0.0;
-      for (int b = threadIdx.x; b < nb; b += 32) s += term_sums[(long long)b * PINN_MAX_TERMS + k];
-#pragma unroll
-      for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-      double Lk = s * sw.scale[k];
-      tot += Lk * sw.w[k];
-      if (threadIdx.x == 0) out_terms[k] = real(Lk);
-    }
-    if (threadIdx.x == 0 && out_total) *out_total = real(tot);
-  }
-}
-
-// gradient reduction fused with the Adam update: theta, m, v updated in place (single-GPU path)
-template <typename real>
-__global__ void reduce_adam_kernel(const real* __restrict__ partial, long long stride, const double* __restrict__ term_sums, int nb,
-                                   long long n_theta, int n_terms, const ScaleW sw, real* theta, real* m, real* v,
-                                   double lr_t, double beta1, double beta2, double eps_t, real* out_terms, real* out_total) {
-  __shared__ real red[8][33];
-  const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
-  const long long i = (long long)blockIdx.x * 32 + tx;
-  real s = real(0);
-  if (i < n_theta) {
-    const int chunk = (nb + 7) / 8;
-    const int b0 = ty * chunk, b1 = (b0 + chunk < nb) ? b0 + chunk : nb;
-    for (int b = b0; b < b1; ++b) s += partial[(long long)b * stride + i];
-  }
-  red[ty][tx] = s;
-  __syncthreads();
-  if (ty == 0 && i < n_theta) {
-    real g = red[0][tx];
-#pragma unroll
-    for (int k = 1; k < 8; ++k) g += red[k][tx];
-    const double gd = (double)g;
-    const double mi = beta1 * (double)m[i] + (1.0 - beta1) * gd;
-    const double vi = beta2 * (double)v[i] + (1.0 - beta2) * gd * gd;
-    m[i] = real(mi); v[i] = real(vi);
-    // lr_t = lr * sqrt(1 - beta2^t) / (1 - beta1^t), eps_t = eps * sqrt(1 - beta2^t)
-    theta[i] = real((double)theta[i] - lr_t * mi / (sqrt(vi) + eps_t));
-  }
-  if (blockIdx.x == 0 && threadIdx.x < 32) {
-    double tot = 0.0;
-    for (int k = 0; k < n_terms; ++k) {
-      double t = 0.0;
-      for (int b = threadIdx.x; b < nb; b += 32) t += term_sums[(long long)b * PINN_MAX_TERMS + k];
-#pragma unroll
-      for (int o = 16; o > 0; o >>= 1) t += __shfl_xor_sync(0xffffffffu, t, o);
-      double Lk = t * sw.scale[k];
-      tot += Lk * sw.w[k];
-      if (threadIdx.x == 0) out_terms[k] = real(Lk);
-    }
-    if (threadIdx.x == 0) *out_total = real(tot);
-  }
-}
 
 // after the allreduce of packed = [grad | term losses]: copy the gradient out and form total = sum_k w_k L_k
 template <typename real>
@@ -131,37 +43,6 @@ cudaError_t ffma_launch(int dtype, bool bufs_smem, const FfmaArgs& a, int grid, 
   if (dtype == PINN_F64)
     return bufs_smem ? ffma_launch_double_smem(a, grid, smem, st) : ffma_launch_double_gmem(a, grid, smem, st);
   return bufs_smem ? ffma_launch_float_smem(a, grid, smem, st) : ffma_launch_float_gmem(a, grid, smem, st);
-}
-
-cudaError_t reduce_launch(int dtype, const void* partial, long long stride, const double* term_sums, int nb, long long n_theta,
-                          int n_terms, const ScaleW& scale_w, void* out_grad, void* out_terms, void* out_total,
-                          int want_grad, cudaStream_t st) {
-  long long n = want_grad ? n_theta : 1;
-  int blocks = (int)((n + 31) / 32);
-  if (blocks < 1) blocks = 1;
-  if (dtype == PINN_F64)
-    reduce_kernel<double><<<blocks, 256, 0, st>>>((const double*)partial, stride, term_sums, nb, n_theta, n_terms, scale_w,
-                                                   (double*)out_grad, (double*)out_terms, (double*)out_total,
-                                                   want_grad);
-  else
-    reduce_kernel<float><<<blocks, 256, 0, st>>>((const float*)partial, stride, term_sums, nb, n_theta, n_terms, scale_w,
-                                                  (float*)out_grad, (float*)out_terms, (float*)out_total, want_grad);
-  return cudaGetLastError();
-}
-
-cudaError_t reduce_adam_launch(int dtype, const void* partial, long long stride, const double* term_sums, int nb, long long n_theta,
-                               int n_terms, const ScaleW& sw, void* theta, void* m, void* v, double lr_t, double beta1,
-                               double beta2, double eps_t, void* out_terms, void* out_total, cudaStream_t st) {
-  int blocks = (int)((n_theta + 31) / 32);
-  if (dtype == PINN_F64)
-    reduce_adam_kernel<double><<<blocks, 256, 0, st>>>((const double*)partial, stride, term_sums, nb, n_theta, n_terms, sw,
-                                                        (double*)theta, (double*)m, (double*)v, lr_t, beta1, beta2, eps_t,
-                                                        (double*)out_terms, (double*)out_total);
-  else
-    reduce_adam_kernel<float><<<blocks, 256, 0, st>>>((const float*)partial, stride, term_sums, nb, n_theta, n_terms, sw,
-                                                       (float*)theta, (float*)m, (float*)v, lr_t, beta1, beta2, eps_t,
-                                                       (float*)out_terms, (float*)out_total);
-  return cudaGetLastError();
 }
 
 cudaError_t finish_launch(int dtype, const void* packed, long long n_grad, int n_terms, const ScaleW& scale_w, void* out_grad,

@@ -19,9 +19,6 @@
 namespace pinn {
 size_t ffma_smem_bytes(int dtype, long long buf_elems, int w_area, bool bufs_smem);
 cudaError_t ffma_launch(int dtype, bool bufs_smem, const FfmaArgs& a, int grid, size_t smem, cudaStream_t st);
-cudaError_t reduce_launch(int dtype, const void* partial, long long stride, const double* term_sums, int nb, long long n_theta,
-                          int n_terms, const ScaleW& scale_w, void* out_grad, void* out_terms, void* out_total,
-                          int want_grad, cudaStream_t st);
 cudaError_t grad_stats_launch(int dtype, const void* grad, long long n, double* out2, cudaStream_t st);
 cudaError_t sample_uniform_launch(int dtype, void* pts, long long n, int dim, const double* lb, const double* ub,
                                   unsigned long long seed, unsigned long long draw, const unsigned long long* draw_dev,
@@ -31,9 +28,6 @@ cudaError_t sample_lhs_launch(int dtype, void* pts, long long n, int dim, const 
                               cudaStream_t st);
 cudaError_t finish_launch(int dtype, const void* packed, long long n_grad, int n_terms, const ScaleW& scale_w, void* out_grad,
                           void* out_terms, void* out_total, cudaStream_t st);
-cudaError_t reduce_adam_launch(int dtype, const void* partial, long long stride, const double* term_sums, int nb, long long n_theta,
-                               int n_terms, const ScaleW& sw, void* theta, void* m, void* v, double lr_t, double beta1,
-                               double beta2, double eps_t, void* out_terms, void* out_total, cudaStream_t st);
 }  // namespace pinn
 
 using namespace pinn;
@@ -146,13 +140,11 @@ struct pinn_engine {
   void* h_pin_in = nullptr;      // pinned theta
   void* h_pin_out = nullptr;     // pinned grad + losses
   cudaStream_t own_stream = nullptr;
-  bool h2d_direct = false;       // PINN_B200_H2D_DIRECT=1: small theta copied from the caller's (pageable) buffer directly
   bool zero_copy_out = false;    // h_pin_out is addressable from the device (kernel tail writes results to the host directly)
   // device-resident Adam state
   void* adam_m = nullptr;
   void* adam_v = nullptr;
   double adam_lr = 1e-3, adam_b1 = 0.9, adam_b2 = 0.999, adam_eps = 1e-8;
-  long long adam_t = 0;
   bool adam_ready = false;
   // device-side samplers (StochasticTraining): per term box, seed, point count; draw counter shared by all terms
   bool sampler_on[PINN_MAX_TERMS];
@@ -161,9 +153,8 @@ struct pinn_engine {
   unsigned long long sampler_seed[PINN_MAX_TERMS];
   long long sampler_n[PINN_MAX_TERMS];
   unsigned long long sampler_draw = 0;
-  // fused kernel tail (tail.cuh): device-resident barrier / step state; PINN_B200_TAIL=0 selects the separate reduce kernel
+  // fused kernel tail (tail.cuh): device-resident barrier / step state
   TailState* d_state = nullptr;
-  bool tail_on = true;
   unsigned long long tail_timeout_ns = 20ull * 1000000000ull;
   // captured iteration graph of the device-resident Adam loop
   cudaGraphExec_t adam_graph = nullptr;
@@ -764,8 +755,6 @@ int pinn_create(const pinn_problem_desc* d, pinn_handle* out) {
   err = cudaMemset(e->d_state, 0, sizeof(TailState));
   if (err != cudaSuccess) { fail("pinn_create: state init failed: %s", cudaGetErrorString(err)); pinn_destroy(e); return 1; }
   {
-    const char* tv = getenv("PINN_B200_TAIL");
-    e->tail_on = !(tv && tv[0] == '0');
     const char* to = getenv("PINN_B200_TAIL_TIMEOUT_S");
     if (to && atof(to) > 0) e->tail_timeout_ns = (unsigned long long)(atof(to) * 1e9);
   }
@@ -776,10 +765,7 @@ int pinn_create(const pinn_problem_desc* d, pinn_handle* out) {
   if (err == cudaSuccess) err = cudaHostAlloc(&e->h_pin_out, ((size_t)e->n_theta + PINN_MAX_TERMS + 1) * e->es, cudaHostAllocMapped);
   if (err == cudaSuccess) {
     void* dptr = nullptr;
-    const char* hd = getenv("PINN_B200_H2D_DIRECT");
-    e->h2d_direct = hd && hd[0] == '1';
-    const char* zc = getenv("PINN_B200_ZERO_COPY");
-    e->zero_copy_out = !(zc && zc[0] == '0') && cudaHostGetDevicePointer(&dptr, e->h_pin_out, 0) == cudaSuccess && dptr == e->h_pin_out;
+    e->zero_copy_out = cudaHostGetDevicePointer(&dptr, e->h_pin_out, 0) == cudaSuccess && dptr == e->h_pin_out;
     cudaGetLastError();
   }
   // a BLOCKING stream: the *_host entry points run here and must order after uploads / sampler draws that callers
@@ -958,10 +944,9 @@ static void fill_tail(pinn_engine* e, TailArgs& t, const ScaleW& sw, void* out_g
   t.sw = sw;
 }
 
-// One evaluation of the hot path on stream st: fused kernel (+ tail) and whatever follows it on this configuration.
+// One evaluation of the hot path on stream st: fused kernel + tail and whatever follows it on this configuration.
 //   single GPU, or peer memory mapped:  ONE launch (tail reduces, sums over the peers, writes / applies Adam)
 //   multi-GPU without peer memory:      fused kernel (tail reduces into `packed`) -> ncclAllReduce -> finish_kernel
-//   PINN_B200_TAIL=0:                   fused kernel -> reduce_kernel [-> ncclAllReduce -> finish_kernel]   (round-1 sequence)
 static int eval_step(pinn_engine* e, const void* theta, const double* host_weights, void* out_grad, void* out_terms,
                      void* out_total, bool adam, cudaStream_t st) {
   const bool want_grad = adam || out_grad != nullptr;
@@ -978,50 +963,27 @@ static int eval_step(pinn_engine* e, const void* theta, const double* host_weigh
   if (grid > kTailSlots) return fail("pinn_loss_grad: %d CTAs exceed the %d tail slots", grid, kTailSlots);
   if (e->timing) CUDA_TRY(cudaEventRecord(e->ev0, st));
   const long long ng = want_grad ? e->n_theta : 0;
-  char* pk = (char*)e->packed;
-  void* pk_terms = pk + (size_t)ng * e->es;
-  if (e->tail_on && (!multi || e->p2p)) {
+  const bool nccl = multi && !e->p2p;
+  if (!nccl) {
     fill_tail(e, a.tail, sw, out_grad, out_terms, out_total, adam, multi);
-    if (launch_fused(e, a, grid, st)) return 1;
-    if (e->timing) CUDA_TRY(cudaEventRecord(e->ev1, st));
-    e->launches += 1;
   } else {
-    if (adam && multi)
+    if (adam)
       return fail("pinn_adam_iterate: the multi-GPU device loop needs the peer-memory allreduce (%s)",
                   e->p2p_why[0] ? e->p2p_why : "not available");
-    if (e->tail_on) {
-      fill_tail(e, a.tail, sw, want_grad ? e->packed : nullptr, pk_terms, nullptr, false, false);
-      if (launch_fused(e, a, grid, st)) return 1;
-      if (e->timing) CUDA_TRY(cudaEventRecord(e->ev1, st));
-      e->launches += 1;
-    } else {
-      if (launch_fused(e, a, grid, st)) return 1;
-      if (e->timing) CUDA_TRY(cudaEventRecord(e->ev1, st));
-      e->launches += 1;
-      if (adam) {
-        e->adam_t += 1;
-        const double c1 = 1.0 - pow(e->adam_b1, (double)e->adam_t), c2 = sqrt(1.0 - pow(e->adam_b2, (double)e->adam_t));
-        CUDA_TRY(reduce_adam_launch(e->dtype, e->partial, e->partial_stride, e->term_sums, grid, e->n_theta, e->n_terms, sw, e->d_theta, e->adam_m,
-                                    e->adam_v, e->adam_lr * c2 / c1, e->adam_b1, e->adam_b2, e->adam_eps * c2, out_terms,
-                                    out_total, st));
-      } else if (multi) {
-        CUDA_TRY(reduce_launch(e->dtype, e->partial, e->partial_stride, e->term_sums, grid, e->n_theta, e->n_terms, sw, e->packed, pk_terms,
-                               nullptr, want_grad ? 1 : 0, st));
-      } else {
-        CUDA_TRY(reduce_launch(e->dtype, e->partial, e->partial_stride, e->term_sums, grid, e->n_theta, e->n_terms, sw, out_grad, out_terms,
-                               out_total, want_grad ? 1 : 0, st));
-      }
-      e->launches += 1;
-    }
-    if (multi) {
-      // packed = [grad (n_theta, zero-length when no gradient is wanted) | term losses]: one allreduce
-      ncclResult_t r = g_nccl.AllReduce(e->packed, e->packed, (size_t)ng + (size_t)e->n_terms,
-                                        e->dtype == PINN_F64 ? ncclFloat64 : ncclFloat32, ncclSumOp, e->comm, st);
-      if (r != 0) return fail("ncclAllReduce failed: %s", g_nccl.GetErrorString ? g_nccl.GetErrorString(r) : "?");
-      e->launches += 1;
-      CUDA_TRY(finish_launch(e->dtype, e->packed, ng, e->n_terms, sw, out_grad, out_terms, out_total, st));
-      e->launches += 1;
-    }
+    void* pk_terms = (char*)e->packed + (size_t)ng * e->es;
+    fill_tail(e, a.tail, sw, want_grad ? e->packed : nullptr, pk_terms, nullptr, false, false);
+  }
+  if (launch_fused(e, a, grid, st)) return 1;
+  if (e->timing) CUDA_TRY(cudaEventRecord(e->ev1, st));
+  e->launches += 1;
+  if (nccl) {
+    // packed = [grad (n_theta, zero-length when no gradient is wanted) | term losses]: one allreduce
+    ncclResult_t r = g_nccl.AllReduce(e->packed, e->packed, (size_t)ng + (size_t)e->n_terms,
+                                      e->dtype == PINN_F64 ? ncclFloat64 : ncclFloat32, ncclSumOp, e->comm, st);
+    if (r != 0) return fail("ncclAllReduce failed: %s", g_nccl.GetErrorString ? g_nccl.GetErrorString(r) : "?");
+    e->launches += 1;
+    CUDA_TRY(finish_launch(e->dtype, e->packed, ng, e->n_terms, sw, out_grad, out_terms, out_total, st));
+    e->launches += 1;
   }
   if (e->timing) {
     CUDA_TRY(cudaEventSynchronize(e->ev1));
@@ -1049,16 +1011,10 @@ int pinn_loss_grad_host(pinn_handle e, const void* host_theta, const double* hos
   CUDA_TRY(cudaSetDevice(e->device));
   cudaStream_t st = e->own_stream;
   const size_t tb = (size_t)e->n_theta * e->es;
-  if (e->h2d_direct && tb <= 65536) {
-    // small theta: the driver inlines a pageable copy of <= 64 KB into the command stream (and returns once it is staged),
-    // which is cheaper than staging it ourselves in pinned memory and programming a DMA
-    CUDA_TRY(cudaMemcpyAsync(e->d_theta, host_theta, tb, cudaMemcpyHostToDevice, st));
-  } else {
-    memcpy(e->h_pin_in, host_theta, tb);
-    CUDA_TRY(cudaMemcpyAsync(e->d_theta, e->h_pin_in, tb, cudaMemcpyHostToDevice, st));
-  }
+  memcpy(e->h_pin_in, host_theta, tb);
+  CUDA_TRY(cudaMemcpyAsync(e->d_theta, e->h_pin_in, tb, cudaMemcpyHostToDevice, st));
   char* hout = (char*)e->h_pin_out;
-  if (e->zero_copy_out && e->tail_on && (e->nranks <= 1 || e->p2p)) {
+  if (e->zero_copy_out && (e->nranks <= 1 || e->p2p)) {
     // the kernel tail writes the gradient and the losses straight into the pinned host buffer (mapped into the device
     // address space): no device-to-host copies after the launch, just the stream synchronisation
     if (pinn_loss_grad(e, e->d_theta, host_weights, host_grad ? (void*)hout : nullptr, hout + tb,
@@ -1090,7 +1046,7 @@ int pinn_adam_begin(pinn_handle e, const void* host_theta0, double lr, double be
   CUDA_TRY(cudaMemsetAsync(&e->d_state->adam_t, 0, sizeof(unsigned long long), e->own_stream));
   CUDA_TRY(cudaMemcpyAsync(e->d_theta, host_theta0, tb, cudaMemcpyHostToDevice, e->own_stream));
   CUDA_TRY(cudaStreamSynchronize(e->own_stream));
-  e->adam_lr = lr; e->adam_b1 = beta1; e->adam_b2 = beta2; e->adam_eps = eps; e->adam_t = 0; e->adam_ready = true;
+  e->adam_lr = lr; e->adam_b1 = beta1; e->adam_b2 = beta2; e->adam_eps = eps; e->adam_ready = true;
   return 0;
 }
 
@@ -1099,15 +1055,9 @@ static int draw_term(pinn_engine* e, int term, unsigned long long draw, const un
 // one iteration of the device-resident loop: fresh points for the sampled terms, then the fused step with Adam in its tail
 static int enqueue_adam_iteration(pinn_engine* e, const double* host_weights, cudaStream_t st) {
   char* dout = (char*)e->d_out;
-  if (any_sampler(e)) {
-    if (e->tail_on) {
-      // draw = host counter + 1 + device counter; the tail advances the device counter, so graph replays resample
-      for (int t = 0; t < e->n_terms; ++t)
-        if (e->sampler_on[t] && draw_term(e, t, e->sampler_draw + 1, &e->d_state->draw, st)) return 1;
-    } else if (pinn_resample(e, st)) {
-      return 1;
-    }
-  }
+  // draw = host counter + 1 + device counter; the tail advances the device counter, so graph replays resample
+  for (int t = 0; t < e->n_terms; ++t)
+    if (e->sampler_on[t] && draw_term(e, t, e->sampler_draw + 1, &e->d_state->draw, st)) return 1;
   return eval_step(e, e->d_theta, host_weights, nullptr, dout, dout + (size_t)e->n_terms * e->es, true, st);
 }
 
@@ -1125,7 +1075,7 @@ int pinn_adam_iterate(pinn_handle e, int32_t n_steps, const double* host_weights
   if (e->total_tiles <= 0 && e->nranks <= 1) return fail("pinn_adam_iterate: no collocation points");
   cudaStream_t st = e->own_stream;
   const char* ng = getenv("PINN_B200_NO_GRAPH");
-  const bool use_graph = e->tail_on && (e->nranks <= 1 || e->p2p) && !e->timing && !(ng && ng[0] == '1');
+  const bool use_graph = (e->nranks <= 1 || e->p2p) && !e->timing && !(ng && ng[0] == '1');
   if (use_graph) {
     // the n_steps iterations are captured once into a CUDA graph (sampler draws + ONE fused launch per iteration) and
     // replayed while the launch arguments stay the same: step counter, bias correction and draw counter live on the device
@@ -1338,7 +1288,6 @@ static int setup_p2p(pinn_engine* e) {
   if (!g_nccl.AllGather) { why("ncclAllGather not found"); return 0; }        // same library on every rank: uniform exit
   const char* no = getenv("PINN_B200_NO_P2P");
   if (no && no[0] == '1') why("disabled by PINN_B200_NO_P2P=1");
-  if (!e->tail_on) why("PINN_B200_TAIL=0");
   if (e->nranks > kMaxRanks) why("more ranks than one NVSwitch domain (8)");
   if (e->num_sms > kTailSlots) why("more SMs than tail slots");
   e->recv_words = e->n_theta * (long long)(e->es / 4) + 2 * PINN_MAX_TERMS;

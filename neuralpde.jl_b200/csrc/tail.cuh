@@ -16,7 +16,6 @@
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
-#include <stdlib.h>
 #include <string.h>
 #include "dev_types.h"
 
@@ -41,8 +40,7 @@ static cudaError_t launch_fused_kernel(const A& a, int grid, int threads, size_t
   cfg.gridDim = dim3((unsigned)grid); cfg.blockDim = dim3((unsigned)threads); cfg.dynamicSmemBytes = smem; cfg.stream = st;
   cudaLaunchAttribute at[1];
   at[0].id = cudaLaunchAttributeCooperative;
-  static const bool no_coop = [] { const char* v = getenv("PINN_B200_COOP"); return v && v[0] == '0'; }();   // measurement aid
-  at[0].val.cooperative = (a.tail.state != nullptr && !no_coop) ? 1 : 0;
+  at[0].val.cooperative = a.tail.state != nullptr ? 1 : 0;
   cfg.attrs = at; cfg.numAttrs = 1;
   return cudaLaunchKernelEx(&cfg, kernel, a);
 }

@@ -1,6 +1,6 @@
 """Device-resident step time of one BASELINE config / mode: K steps, each bracketed by CUDA events on the launching
 stream, L2 flushed (256 MiB memset) between steps; prints median / min ms and launches per step.  Development aid
-(A/B of PINN_B200_TAIL / PINN_B200_COOP and of two library builds via PINN_B200_LIB); the contract bench is bench.py.
+(A/B of two library builds via PINN_B200_LIB); the contract bench is bench.py.
 usage: step_time.py [cfg2|cfg3|cfg1] [mode] [steps] [n (cfg2 grid size)]"""
 import os, sys
 import numpy as np
@@ -31,7 +31,6 @@ for a, b in ev:
     flush.zero_(); a.record(); eng.loss_grad_device(th, g, terms, tot, None, st); b.record()
 torch.cuda.synchronize()
 ms = np.array([a.elapsed_time(b) for a, b in ev])
-print("%s %s %s TAIL=%s COOP=%s lib=%s: median %.4f ms min %.4f ms launches/step %.1f loss %.8g pts/s %.4g" % (
-    which, mode, kw, os.environ.get("PINN_B200_TAIL", "1"), os.environ.get("PINN_B200_COOP", "1"),
-    os.path.basename(os.environ.get("PINN_B200_LIB", "default")), np.median(ms), ms.min(), (eng.launch_count() - l0) / K,
+print("%s %s %s lib=%s: median %.4f ms min %.4f ms launches/step %.1f loss %.8g pts/s %.4g" % (
+    which, mode, kw, os.path.basename(os.environ.get("PINN_B200_LIB", "default")), np.median(ms), ms.min(), (eng.launch_count() - l0) / K,
     float(tot.item()), cfg.n_pde_points / (np.median(ms) * 1e-3)), flush=True)

@@ -142,21 +142,24 @@ def test_device_sampler_bounds_determinism_and_oracle_parity():
 
 
 @pytest.mark.parametrize("mode,dtype,tol", [("ffma", np.float64, 1e-13), ("tc_split", np.float32, 2e-6), ("tc_bf16", np.float32, 2e-6)])
-def test_in_kernel_tail_matches_separate_reduce_kernel(monkeypatch, mode, dtype, tol):
-    """The gradient reduction in the fused kernel's tail (one launch per step) gives the round-1 sequence's result
-    (fused kernel -> reduce_kernel, selected with PINN_B200_TAIL=0) up to summation order, and launches once."""
+def test_in_kernel_tail_matches_sum_of_shards(mode, dtype, tol):
+    """The gradient reduction in the fused kernel's tail (one launch per step) over the full point sets equals the sum of
+    two half-size shards with n_global set up to summation order.  The shards launch on smaller grids than the full
+    problem, so a tail that drops or double-counts a CTA's partial row or a slice boundary fails this."""
     cfg = configs.config2(n=48, width=32, hidden=3)
     rep = npde.symbolic_discretize(cfg.pde_system, cfg.discretization(dtype=dtype, mode=mode))
     th = rep.flat_init_params
     n0 = rep.engine.launch_count()
     t1, terms1, g1 = rep.engine.loss_grad_host(th, None, True)
     assert rep.engine.launch_count() - n0 == 1
-    monkeypatch.setenv("PINN_B200_TAIL", "0")
-    rep0 = npde.symbolic_discretize(cfg.pde_system, cfg.discretization(dtype=dtype, mode=mode))
-    monkeypatch.delenv("PINN_B200_TAIL")
-    n0 = rep0.engine.launch_count()
-    t0, terms0, g0 = rep0.engine.loss_grad_host(th, None, True)
-    assert rep0.engine.launch_count() - n0 == 2
+    t0, terms0, g0 = 0.0, np.zeros(terms1.shape), np.zeros(g1.shape)
+    for r in range(2):
+        rr = npde.symbolic_discretize(cfg.pde_system, cfg.discretization(dtype=dtype, mode=mode))
+        for i, s in enumerate(rep.point_sets):
+            lo, hi = shard_range(s.shape[1], r, 2)
+            rr.set_points(i, s[:, lo:hi], n_global=s.shape[1])
+        t_r, terms_r, g_r = rr.engine.loss_grad_host(th, None, True)
+        t0 += float(t_r); terms0 += terms_r; g0 += g_r
     assert abs(t1 - t0) <= tol * abs(t0) and rel(g1, g0) < 10 * tol
     np.testing.assert_allclose(terms1, terms0, rtol=10 * tol)
     # many steps through one handle: the self-resetting grid barrier and the step counter stay consistent
