@@ -28,6 +28,7 @@ NVCC_FLAGS = [
 # (object name, source, extra defines)
 UNITS = [
     ("pinn_abi.o", "pinn_abi.cu", []),
+    ("plan.o", "plan.cu", []),
     ("ffma_launch.o", "ffma_launch.cu", []),
     ("ffma_f32_smem.o", "ffma_inst.cu", ["-DPINN_INST_REAL=float", "-DPINN_INST_BUFS=1"]),
     ("ffma_f32_gmem.o", "ffma_inst.cu", ["-DPINN_INST_REAL=float", "-DPINN_INST_BUFS=0"]),

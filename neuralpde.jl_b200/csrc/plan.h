@@ -1,0 +1,29 @@
+// plan.h -- host planner: validates a pinn_problem_desc and lowers it to what a handle keeps fixed for its lifetime.
+#pragma once
+#include "dev_types.h"
+#include "tc_types.h"
+
+namespace pinn {
+int fail(const char* fmt, ...);    // sets the message pinn_last_error returns; returns 1
+const char* last_error();
+
+struct TermPlan {
+  int reduction;                   // PINN_REDUCE_MEAN or PINN_REDUCE_WSUM
+  double scale;                    // WSUM scale (MEAN: 1/n_global, formed at launch time)
+  double flops_per_point;          // algorithmic: 6 * sum over the term's networks of C * sum_l dims[l] * dims[l+1]
+};
+
+struct Plan {
+  DevProblem prob;                 // uploaded once by pinn_create
+  TermPlan term[PINN_MAX_TERMS];
+  int tile_pts;                    // points per tile of the mode's kernels
+  size_t smem;                     // dynamic shared memory per CTA
+  bool bufs_smem;                  // FFMA: the two activation buffers live in shared memory (else in gbufs)
+  bool wide;                       // tensor-core modes: tw_pack + the 128-wide kernel run instead of the narrow one
+  // launch-argument templates: the planner fills the layout, pinn_create the buffers, a launch the per-call fields
+  FfmaArgs ffma; TcArgs tc; TwArgs tw; TwPackArgs pack;
+};
+
+// Pure host code (no CUDA runtime call); max_smem: the device's opt-in shared memory per block in bytes.
+int plan_problem(const pinn_problem_desc* d, int max_smem, Plan& p);
+}  // namespace pinn
