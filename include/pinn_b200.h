@@ -259,6 +259,49 @@ int pinn_adam_iterate(pinn_handle h, int32_t n_steps, const double* host_weights
                       void* host_term_losses);
 int pinn_adam_theta(pinn_handle h, void* host_theta_out);
 
+/* ---- device-resident quasi-Newton (BFGS / L-BFGS) ------------------------------------------------------------------
+ * The reference's users finish most PINNs with Optim's quasi-Newton methods through OptimizationOptimJL, e.g.
+ *   BFGS()                               test/NNPDE1/nnpde__pde_iii_3rd_order_ode.jl:126, every IntegroDiff/ test
+ *   BFGS(linesearch = BackTracking())    test/NNPDE1/nnpde__pde_ii_2d_poisson.jl:85 (polish after Adam)
+ *   BFGS(initial_stepnorm = 0.01)        test/NNPDE2/direct_function__approximation_of_function_1d.jl:36
+ *   LBFGS()                              test/NNPDE2/additional_loss__fokker_planck.jl:71
+ * The options restate Optim's documented defaults: alphaguess = InitialStatic (the first trial step of every line search
+ * is alpha = 1), LBFGS m = 10 with scaleinvH0 (H0 = gamma I, gamma = s'y / y'y of the newest pair; the first step is
+ * along -g), BFGS H0 = I or I * initial_stepnorm / ||g0||_inf, convergence at ||g||_inf <= 1e-8 (g_abstol).
+ * Line searches (LineSearches.jl defaults): HagerZhang delta 0.1, sigma 0.9, epsilon 1e-6, midpoint bisection, gamma 0.66,
+ * rho 5, psi3 0.1, 50 iterations; BackTracking c_1 1e-4, rho_hi 0.5, rho_lo 0.1, order 3, 1000 iterations.
+ * A pair with s'y <= 0 is not stored (L-BFGS) / does not update H (BFGS); a direction that is not a descent direction
+ * resets the history / H to the identity and steps along -g.
+ *
+ * theta, g, the direction, the L-BFGS pairs ([m+1][n_theta] ring) and BFGS's dense H (n_theta x n_theta) are float64 on
+ * the device for both engine dtypes; the fused kernel sees theta rounded to the engine dtype.  The line search runs on
+ * the host: each evaluation copies {phi, phi'} (16 bytes) back and synchronises once.  Every reduction has a fixed
+ * order and a grid that depends on n_theta only, so two runs -- and all ranks of a multi-GPU handle -- are bit-identical.
+ * With device samplers registered every evaluation draws fresh points first (as pinn_resample).  BFGS is refused for
+ * n_theta > 16384 (H would exceed 2 GiB). */
+enum { PINN_QN_LBFGS = 0, PINN_QN_BFGS = 1 };
+enum { PINN_LS_HAGERZHANG = 0, PINN_LS_BACKTRACKING = 1 };
+/* status after pinn_qn_iterate: still iterating, converged (||g||_inf <= 1e-8, or an accepted step left theta
+ * unchanged), or the line search failed (theta stays at the last accepted point) */
+enum { PINN_QN_RUNNING = 0, PINN_QN_CONVERGED = 1, PINN_QN_LS_FAILED = 2 };
+typedef struct {
+  int32_t kind;              /* PINN_QN_*                                                  */
+  int32_t m;                 /* L-BFGS history length (Optim default 10), 1..32            */
+  int32_t linesearch;        /* PINN_LS_*                                                  */
+  int32_t _pad;
+  double initial_stepnorm;   /* BFGS: H0 = I * initial_stepnorm / ||g0||_inf; <= 0: H0 = I */
+} pinn_qn_options;
+/* Start from host theta0 (engine dtype): allocates the state and evaluates loss and gradient at theta0.
+ * host_weights [n_terms] (nullable) stay fixed for the whole run.  Synchronises. */
+int pinn_qn_begin(pinn_handle h, const void* host_theta0, const pinn_qn_options* opts, const double* host_weights);
+/* Run up to n_iters iterations (accepted steps); the state persists across calls, so callers may iterate one step at a
+ * time.  Outputs (each nullable): loss at the current theta, ||g||_inf there, PINN_QN_* status, iterations and loss /
+ * gradient evaluations since pinn_qn_begin (the one at theta0 included).  Once stopped, further calls do nothing. */
+int pinn_qn_iterate(pinn_handle h, int32_t n_iters, double* host_f, double* host_gnorm_inf, int32_t* host_status,
+                    int64_t* host_iters, int64_t* host_evals);
+/* current theta rounded to the engine dtype */
+int pinn_qn_theta(pinn_handle h, void* host_theta_out);
+
 /* ---- multi-GPU -------------------------------------------------------------------- */
 /* Attach an NCCL communicator built from a 128-byte ncclUniqueId that the caller
  * distributed (rank 0 obtains it from pinn_comm_unique_id). */

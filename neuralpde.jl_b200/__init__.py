@@ -11,9 +11,9 @@ from .symbolic import (Differential, Eq, Equation, In, Interval, PDESystem, VarD
 from .lowering import LoweringError, lower_equation
 from .strategies import (AbstractTrainingStrategy, GridTraining, QuadratureTraining, QuasiRandomTraining,
                          StochasticTraining, generate_training_sets, get_bounds, shard_range)
-from .pinn import (AbstractPINN, Adam, BayesianPINN, Chain, DataLoss, Dense, Descent, GradientScaleAdaptiveLoss, LogOptions, MiniMaxAdaptiveLoss,
+from .pinn import (AbstractPINN, Adam, BFGS, BackTracking, BayesianPINN, Chain, DataLoss, Dense, Descent, GradientScaleAdaptiveLoss, HagerZhang, LBFGS, LogOptions, MiniMaxAdaptiveLoss,
                    NonAdaptiveLoss, ReLoBRaLoAdaptiveLoss, SoftAdaptAdaptiveLoss,
-                   OptimizationFunction, OptimizationProblem, Phi, PhysicsInformedNN, PINNRepresentation,
+                   OptimizationFunction, OptimizationProblem, Phi, PhysicsInformedNN, PINNRepresentation, Solution,
                    discretize, initialparameters, logscalar, logvector, solve, symbolic_discretize)
 
 __all__ = [n for n in dir() if not n.startswith("_")]

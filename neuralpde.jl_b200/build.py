@@ -29,6 +29,7 @@ NVCC_FLAGS = [
 UNITS = [
     ("pinn_abi.o", "pinn_abi.cu", []),
     ("plan.o", "plan.cu", []),
+    ("qn.o", "qn.cu", []),
     ("ffma_launch.o", "ffma_launch.cu", []),
     ("ffma_f32_smem.o", "ffma_inst.cu", ["-DPINN_INST_REAL=float", "-DPINN_INST_BUFS=1"]),
     ("ffma_f32_gmem.o", "ffma_inst.cu", ["-DPINN_INST_REAL=float", "-DPINN_INST_BUFS=0"]),

@@ -1,6 +1,6 @@
 // pinn_abi.cu -- host side of the C ABI declared in include/pinn_b200.h: workspace ownership, kernel
 // launch sequencing, host-buffer staging and the optional NCCL gradient allreduce.  Descriptor
-// validation and lowering live in the planner (plan.cu).
+// validation and lowering live in the planner (plan.cu), the handle struct in engine.h, the quasi-Newton driver in qn.cu.
 #include <cuda_runtime.h>
 #include <dlfcn.h>
 #include <math.h>
@@ -11,7 +11,7 @@
 #include <algorithm>
 #include <vector>
 
-#include "plan.h"
+#include "engine.h"
 
 namespace pinn {
 cudaError_t ffma_launch(int dtype, bool bufs_smem, const FfmaArgs& a, int grid, size_t smem, cudaStream_t st);
@@ -29,7 +29,6 @@ cudaError_t finish_launch(int dtype, const void* packed, long long n_grad, int n
 using namespace pinn;
 
 // ---- minimal NCCL binding (resolved at run time so single-GPU use has no dependency) ----
-typedef struct ncclComm* ncclComm_t;
 typedef struct { char internal[128]; } ncclUniqueId;
 typedef int ncclResult_t;
 enum { ncclInt8 = 0, ncclInt32 = 2, ncclFloat32 = 7, ncclFloat64 = 8, ncclSumOp = 0, ncclMinOp = 3 };
@@ -43,12 +42,6 @@ struct NcclApi {
   const char* (*GetErrorString)(ncclResult_t) = nullptr;
 };
 static NcclApi g_nccl;
-
-#define CUDA_TRY(expr)                                                                  \
-  do {                                                                                  \
-    cudaError_t _e = (expr);                                                            \
-    if (_e != cudaSuccess) return fail("%s failed: %s", #expr, cudaGetErrorString(_e)); \
-  } while (0)
 
 static bool load_nccl() {
   if (g_nccl.lib) return true;
@@ -67,77 +60,7 @@ static bool load_nccl() {
   return g_nccl.GetUniqueId && g_nccl.CommInitRank && g_nccl.CommDestroy && g_nccl.AllReduce;
 }
 
-// per-term host state that changes after pinn_create
-struct TermState {
-  long long n_global = 0; bool n_global_set = false;   // pinn_set_global_count: points over all ranks (MEAN scale)
-  // device-side sampler (StochasticTraining): box, seed, point count; the draw counter is shared by all terms
-  bool sampler_on = false; int sampler_kind = 0;
-  double sampler_lb[PINN_MAX_DIM] = {}, sampler_ub[PINN_MAX_DIM] = {};
-  unsigned long long sampler_seed = 0; long long sampler_n = 0;
-  void *own_pts = nullptr, *own_qw = nullptr;   // engine-owned point copies
-  size_t own_pts_cap = 0, own_qw_cap = 0;
-};
-
-struct pinn_engine {
-  int dtype = 0, mode = 0, device = 0;
-  size_t es = 4;
-  Plan plan;                     // what the handle keeps fixed: problem image, term values, launch-argument templates
-  DevProblem* dprob = nullptr;   // device copy of plan.prob
-  int n_terms = 0;
-  long long n_theta = 0, partial_stride = 0;
-  TermState term[PINN_MAX_TERMS];
-  TermDyn dyn[PINN_MAX_TERMS] = {};
-  int total_tiles = 0, num_sms = 0;
-  long long *tc_dbg = nullptr, *tail_dbg = nullptr;   // pinn_debug_tc_timeline / pinn_debug_tail_marks buffers
-  // wide tensor path (128-wide layers): streamed weights, fp32 pre-activation stash
-  void *tw_wpack = nullptr, *tw_zstash = nullptr;
-  int* tw_counter = nullptr;
-  float* tc_acc = nullptr;       // tensor-core paths: per-CTA fp32 accumulator regions (tc_prims.cuh)
-  // workspaces (device)
-  void* partial = nullptr;
-  double* term_sums = nullptr;
-  void* stash = nullptr;
-  void* gbufs = nullptr;
-  void* packed = nullptr;        // [n_theta + n_terms] allreduce buffer
-  long long ws_bytes = 0;
-  // host staging for the *_host entry points
-  void* d_theta = nullptr;
-  void* d_grad = nullptr;
-  void* d_out = nullptr;         // [n_terms + 1] term losses then total
-  void* h_pin_in = nullptr;      // pinned theta
-  void* h_pin_out = nullptr;     // pinned grad + losses
-  cudaStream_t own_stream = nullptr;
-  bool zero_copy_out = false;    // h_pin_out is addressable from the device (kernel tail writes results to the host directly)
-  // device-resident Adam state
-  void* adam_m = nullptr;
-  void* adam_v = nullptr;
-  double adam_lr = 1e-3, adam_b1 = 0.9, adam_b2 = 0.999, adam_eps = 1e-8;
-  bool adam_ready = false;
-  unsigned long long sampler_draw = 0;
-  // fused kernel tail (tail.cuh): device-resident barrier / step state
-  TailState* d_state = nullptr;
-  unsigned long long tail_timeout_ns = 20ull * 1000000000ull;
-  // captured iteration graph of the device-resident Adam loop
-  cudaGraphExec_t adam_graph = nullptr;
-  unsigned long long adam_graph_key = 0;
-  // comm
-  ncclComm_t comm = nullptr;
-  int rank = 0, nranks = 1;
-  // peer-memory allreduce (NVLink): receive region [2 parities][nranks][recv_words] of 8-byte {word, flag} slots,
-  // mapped from every rank
-  bool p2p = false;
-  void* sym = nullptr;
-  long long recv_words = 0;
-  void* peer_base[kMaxRanks] = {};
-  char p2p_why[160] = {};
-  // introspection
-  long long launches = 0;
-  bool timing = false;
-  cudaEvent_t ev0 = nullptr, ev1 = nullptr;
-  float last_ms = 0.f;
-};
-
-static int dev_alloc(void** p, size_t bytes, pinn_engine* e) {
+int pinn::dev_alloc(void** p, size_t bytes, pinn_engine* e) {
   if (bytes == 0) bytes = 16;
   cudaError_t err = cudaMalloc(p, bytes);
   if (err != cudaSuccess) return fail("cudaMalloc(%zu bytes) failed: %s", bytes, cudaGetErrorString(err));
@@ -198,6 +121,7 @@ int pinn_destroy(pinn_handle e) {
   if (!e) return 0;
   cudaSetDevice(e->device);
   if (e->adam_graph) cudaGraphExecDestroy(e->adam_graph);
+  qn_release(e);
   if (e->p2p) {
     // peers may still be reading this rank's symmetric buffers inside their last step: callers synchronise the ranks
     // (any collective / barrier) before destroying handles; here only this device is drained
@@ -397,8 +321,9 @@ static int launch_fused(pinn_engine* e, const LaunchCall& c, int grid, cudaStrea
   return 0;
 }
 
+}  // extern "C"
 
-static bool any_sampler(const pinn_engine* e) {
+bool pinn::any_sampler(const pinn_engine* e) {
   for (int t = 0; t < e->n_terms; ++t) if (e->term[t].sampler_on) return true;
   return false;
 }
@@ -427,7 +352,7 @@ static void fill_tail(pinn_engine* e, TailArgs& t, const ScaleW& sw, void* out_g
 // One evaluation of the hot path on stream st: fused kernel + tail and whatever follows it on this configuration.
 //   single GPU, or peer memory mapped:  ONE launch (tail reduces, sums over the peers, writes / applies Adam)
 //   multi-GPU without peer memory:      fused kernel (tail reduces into `packed`) -> ncclAllReduce -> finish_kernel
-static int eval_step(pinn_engine* e, const void* theta, const double* host_weights, void* out_grad, void* out_terms,
+int pinn::eval_step(pinn_engine* e, const void* theta, const double* host_weights, void* out_grad, void* out_terms,
                      void* out_total, bool adam, cudaStream_t st) {
   const bool want_grad = adam || out_grad != nullptr;
   LaunchCall c = {};
@@ -469,6 +394,8 @@ static int eval_step(pinn_engine* e, const void* theta, const double* host_weigh
   }
   return 0;
 }
+
+extern "C" {
 
 int pinn_loss_grad(pinn_handle e, const void* dev_theta, const double* host_weights, void* dev_grad,
                    void* dev_term_losses, void* dev_total, void* stream) {

@@ -37,8 +37,13 @@ EXPORTS = [
     "pinn_launch_count", "pinn_set_timing", "pinn_last_kernel_ms", "pinn_workspace_bytes",
     "pinn_flops_per_eval", "pinn_adam_begin", "pinn_adam_iterate", "pinn_adam_theta",
     "pinn_term_grad_stats", "pinn_term_grad_stats_host", "pinn_set_sampler", "pinn_resample", "pinn_get_points_host",
-    "pinn_comm_info", "pinn_set_sampler_ex",
+    "pinn_comm_info", "pinn_set_sampler_ex", "pinn_qn_begin", "pinn_qn_iterate", "pinn_qn_theta",
 ]
+
+# quasi-Newton optimizer / line search kinds and run states (pinn_qn_options, pinn_qn_iterate)
+QN_LBFGS, QN_BFGS = 0, 1
+LS_HAGERZHANG, LS_BACKTRACKING = 0, 1
+QN_RUNNING, QN_CONVERGED, QN_LS_FAILED = 0, 1, 2
 
 
 class EngineError(RuntimeError):
@@ -47,6 +52,11 @@ class EngineError(RuntimeError):
 
 class _Instr(C.Structure):
     _fields_ = [("op", C.c_int32), ("a", C.c_int32), ("b", C.c_int32), ("_pad", C.c_int32), ("imm", C.c_double)]
+
+
+class _QnOptions(C.Structure):
+    _fields_ = [("kind", C.c_int32), ("m", C.c_int32), ("linesearch", C.c_int32), ("_pad", C.c_int32),
+                ("initial_stepnorm", C.c_double)]
 
 
 class _NetDesc(C.Structure):
@@ -184,6 +194,12 @@ def load_library():
     lib.pinn_adam_iterate.restype = C.c_int
     lib.pinn_adam_theta.argtypes = [vp, vp]
     lib.pinn_adam_theta.restype = C.c_int
+    lib.pinn_qn_begin.argtypes = [vp, vp, C.POINTER(_QnOptions), C.POINTER(dbl)]
+    lib.pinn_qn_begin.restype = C.c_int
+    lib.pinn_qn_iterate.argtypes = [vp, i32, C.POINTER(dbl), C.POINTER(dbl), C.POINTER(i32), C.POINTER(i64), C.POINTER(i64)]
+    lib.pinn_qn_iterate.restype = C.c_int
+    lib.pinn_qn_theta.argtypes = [vp, vp]
+    lib.pinn_qn_theta.restype = C.c_int
     _lib = lib
     return lib
 
@@ -395,6 +411,32 @@ class Engine:
     def adam_theta(self) -> np.ndarray:
         th = np.empty(self.n_theta, dtype=self.np_dtype)
         _check(self.lib.pinn_adam_theta(self._h, _ptr(th)))
+        return th
+
+    # -- device-resident quasi-Newton (BFGS / L-BFGS) ---------------------------------------------------------
+    def qn_begin(self, theta0: np.ndarray, kind: int = QN_LBFGS, m: int = 10, linesearch: int = LS_HAGERZHANG,
+                 initial_stepnorm: Optional[float] = None, weights=None):
+        """Start a quasi-Newton run at theta0 (one loss / gradient evaluation); weights stay fixed for the run."""
+        th = np.ascontiguousarray(theta0, dtype=self.np_dtype)
+        if th.shape != (self.n_theta,):
+            raise ValueError("theta must have length %d" % self.n_theta)
+        opt = _QnOptions(int(kind), int(m), int(linesearch), 0, float(initial_stepnorm or 0.0))
+        w = self._weights(weights)
+        wp = w.ctypes.data_as(C.POINTER(C.c_double)) if w is not None else None
+        _check(self.lib.pinn_qn_begin(self._h, _ptr(th), C.byref(opt), wp))
+
+    def qn_iterate(self, n_iters: int):
+        """Up to n_iters iterations; returns (loss, ||g||_inf, status, iterations, evaluations), the counts since
+        qn_begin.  status: QN_RUNNING, QN_CONVERGED or QN_LS_FAILED."""
+        f, gn = C.c_double(0.0), C.c_double(0.0)
+        st, it, ev = C.c_int32(0), C.c_int64(0), C.c_int64(0)
+        _check(self.lib.pinn_qn_iterate(self._h, int(n_iters), C.byref(f), C.byref(gn), C.byref(st), C.byref(it),
+                                        C.byref(ev)))
+        return float(f.value), float(gn.value), int(st.value), int(it.value), int(ev.value)
+
+    def qn_theta(self) -> np.ndarray:
+        th = np.empty(self.n_theta, dtype=self.np_dtype)
+        _check(self.lib.pinn_qn_theta(self._h, _ptr(th)))
         return th
 
     # -- multi-GPU --------------------------------------------------------------------------------

@@ -118,6 +118,48 @@ class Adam:
 
 
 @dataclass
+class HagerZhang:
+    """``LineSearches.HagerZhang()`` with its defaults (Hager & Zhang 2006): Wolfe / approximate-Wolfe parameters δ, σ,
+    ε; bisection weight θ; interval shrink γ; bracket expansion ρ; step shrink ψ₃ after a non-finite value; iteration
+    cap.  The device driver implements these values only."""
+    delta: float = 0.1
+    sigma: float = 0.9
+    epsilon: float = 1e-6
+    theta: float = 0.5
+    gamma: float = 0.66
+    rho: float = 5.0
+    psi3: float = 0.1
+    linesearchmax: int = 50
+
+
+@dataclass
+class BackTracking:
+    """``LineSearches.BackTracking()`` with its defaults: Armijo constant c₁, step clamp [ρ_lo, ρ_hi], cubic
+    interpolation (order 3), iteration cap.  The device driver implements these values only."""
+    c_1: float = 1e-4
+    rho_hi: float = 0.5
+    rho_lo: float = 0.1
+    iterations: int = 1000
+    order: int = 3
+
+
+@dataclass
+class LBFGS:
+    """``Optim.LBFGS(m = 10, linesearch = HagerZhang())``: α₀ = 1 every iteration (InitialStatic), initial inverse
+    Hessian γI with γ = sᵀy / yᵀy of the newest pair (scaleinvH0); the first step is along -g."""
+    m: int = 10
+    linesearch: object = field(default_factory=HagerZhang)
+
+
+@dataclass
+class BFGS:
+    """``Optim.BFGS(linesearch = HagerZhang(), initial_stepnorm = nothing)``: dense inverse Hessian,
+    H₀ = I or I · initial_stepnorm / ‖g₀‖∞."""
+    linesearch: object = field(default_factory=HagerZhang)
+    initial_stepnorm: Optional[float] = None
+
+
+@dataclass
 class Descent:
     """``Optimisers.Descent(η)``."""
     lr: float = 0.1
@@ -703,6 +745,7 @@ def symbolic_discretize(pde_system: PDESystem, discretization: PhysicsInformedNN
         term_names=["pde_%d" % (i + 1) for i in range(n_pde)] + ["bc_%d" % (j + 1) for j in range(n_bc)]
         + (["additional"] if isinstance(add, DataLoss) else []))
     rep.point_sets = point_sets
+    rep.resample = resample
     rep.quad_weights = quad_w
     rep.weights = weights
 
@@ -785,24 +828,79 @@ class Solution:
     u: np.ndarray
     objective: float
     iterations: int
+    retcode: str = "Default"     # quasi-Newton runs: "Success", "MaxIters", "Failure" or "Terminated" (by the callback)
 
 
-def solve(prob: OptimizationProblem, opt: Adam, maxiters: int = 100, callback: Optional[Callable] = None,
+def _host_resampled(rep) -> bool:
+    return (isinstance(rep.strategy, StochasticTraining) and not rep.strategy.device_sampler) or \
+           (isinstance(rep.strategy, QuasiRandomTraining) and rep.strategy.resampling and
+            not rep.strategy.device_sampler) if rep is not None else True
+
+
+_DEVICE_LOOP_SETS = ("point sets that live on the device: Grid, Quadrature, non-resampled QuasiRandom, or "
+                     "StochasticTraining(..., device_sampler=True)")
+
+
+def _solve_quasi_newton(prob: OptimizationProblem, opt, maxiters: int, callback: Optional[Callable]) -> Solution:
+    """BFGS / L-BFGS with theta, the gradient and the curvature history on the device (pinn_qn_*); the line search runs
+    on the host with one 16-byte read-back per evaluation."""
+    rep = prob.representation
+    if _host_resampled(rep):
+        raise ValueError("BFGS / LBFGS need " + _DEVICE_LOOP_SETS)
+    if not isinstance(rep.adaloss, NonAdaptiveLoss):
+        raise ValueError("BFGS / LBFGS need fixed loss weights (NonAdaptiveLoss): an adaptive loss would change the "
+                         "objective between the line search's trial points")
+    ls = opt.linesearch
+    if isinstance(ls, HagerZhang) and ls == HagerZhang():
+        ls_kind = _eng.LS_HAGERZHANG
+    elif isinstance(ls, BackTracking) and ls == BackTracking():
+        ls_kind = _eng.LS_BACKTRACKING
+    else:
+        raise ValueError("linesearch must be HagerZhang() or BackTracking() with their default parameters, got %r" % (ls,))
+    if isinstance(rep.strategy, QuasiRandomTraining) and not rep.strategy.device_sampler:
+        rep.resample()                               # non-resampled QuasiRandom places its points at the first loss call
+    eng = rep.engine
+    w = rep.weights
+    term_w = np.concatenate([w["pde"], w["bc"]] + ([w["add"]] if rep.additional_loss is not None else []))
+    if isinstance(opt, LBFGS):
+        eng.qn_begin(prob.u0, _eng.QN_LBFGS, m=opt.m, linesearch=ls_kind, weights=term_w)
+    else:
+        eng.qn_begin(prob.u0, _eng.QN_BFGS, linesearch=ls_kind, initial_stepnorm=opt.initial_stepnorm, weights=term_w)
+    f, _, status, iters, evals = eng.qn_iterate(0)
+    retcode = None
+    if callback is None:
+        f, _, status, iters, evals = eng.qn_iterate(maxiters)
+    else:
+        while status == _eng.QN_RUNNING and iters < maxiters:
+            f, _, status, iters, evals = eng.qn_iterate(1)
+            if callback({"iter": iters, "u": eng.qn_theta()}, f):
+                retcode = "Terminated"
+                break
+    rep.iteration[0] += evals                        # one loss call per evaluation, as the reference counts them
+    if retcode is None:
+        retcode = {_eng.QN_CONVERGED: "Success", _eng.QN_LS_FAILED: "Failure"}.get(status, "MaxIters")
+    return Solution(eng.qn_theta().astype(prob.u0.dtype), f, iters, retcode)
+
+
+def solve(prob: OptimizationProblem, opt: Union[Adam, LBFGS, BFGS], maxiters: int = 100, callback: Optional[Callable] = None,
           device_loop: bool = False, chunk: int = 50) -> Solution:
-    """Minimal stand-in for ``Optimization.solve(prob, Adam(lr); maxiters, callback)``.
+    """Minimal stand-in for ``Optimization.solve(prob, opt; maxiters, callback)``.
+
+    ``LBFGS()`` / ``BFGS()``: the device-resident quasi-Newton driver (pinn_qn_*), whatever ``device_loop`` says; one
+    ``maxiters`` call without a callback, one iteration per call with one (the callback sees θ and the loss after every
+    accepted step, and returning True halts the run).  Point sets as for ``device_loop=True``; the loss weights must be
+    fixed (NonAdaptiveLoss).
 
     Default: a host Adam loop that calls the engine's loss+gradient once per iteration.
     ``device_loop=True`` (fixed point sets, or StochasticTraining with the device-side sampler, which then draws fresh
     points before every step): theta, m, v stay on the device and the Adam update is fused into the gradient reduction
     (pinn_adam_iterate); the callback sees the loss every `chunk` steps."""
+    if isinstance(opt, (LBFGS, BFGS)):
+        return _solve_quasi_newton(prob, opt, maxiters, callback)
     rep = prob.representation
     if device_loop:
-        host_resampled = (isinstance(rep.strategy, StochasticTraining) and not rep.strategy.device_sampler) or \
-                         (isinstance(rep.strategy, QuasiRandomTraining) and rep.strategy.resampling and
-                          not rep.strategy.device_sampler) if rep is not None else True
-        if host_resampled:
-            raise ValueError("device_loop needs point sets that live on the device: Grid, Quadrature, non-resampled "
-                             "QuasiRandom, or StochasticTraining(..., device_sampler=True)")
+        if _host_resampled(rep):
+            raise ValueError("device_loop needs " + _DEVICE_LOOP_SETS)
         eng = rep.engine
         eng.adam_begin(prob.u0, opt.lr, opt.beta1, opt.beta2, opt.eps)
         done, obj = 0, float("nan")
