@@ -1,7 +1,9 @@
 // tc_common.cuh -- device helpers shared by the tensor-core kernels (tc_kernel.cu: widths <= 64, all operands resident;
 // tc_wide_kernel.cu: 128-wide layers, streamed weights): fp32x2 arithmetic, the forward-mode tap chain rule
-// and its adjoint, accumulator loads, swizzled-tile stores, warp reduce-scatter, MMA chains, the steps of the tile
-// driver both kernels share (CTA setup, parameter and point-tile staging, residual program, kernel end), dispatch macro.
+// and its adjoint, accumulator loads, swizzled-tile stores and bf16 hi / lo splits, warp reduce-scatter, MMA chains, the
+// common part of the CTA's shared constants, the steps of the tile driver both kernels share (CTA setup, parameter and
+// point-tile staging, residual program, kernel end), the steps of the per-network passes they share (end of the forward,
+// ubar gather, last-layer gradient, tensor-layer gradient flush, layer-0 gradient), dispatch macro.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -59,6 +61,15 @@ __device__ __forceinline__ float lds_f32(uint32_t addr) {
 __device__ __forceinline__ void sts_v2(uint32_t addr, uint32_t x, uint32_t y) {
   asm volatile("st.shared.v2.b32 [%0], {%1, %2};" ::"r"(addr), "r"(x), "r"(y) : "memory");
 }
+__device__ __forceinline__ void sts_v4(uint32_t addr, uint32_t x, uint32_t y, uint32_t z, uint32_t w) {
+  asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(x), "r"(y), "r"(z), "r"(w) : "memory");
+}
+
+// bf16 (hi, lo) split of the pair (a, b): hi = tc::pack_bf16(a, b), lo = bf16x2_lo(a, b, hi) = bf16x2 of the residuals
+// (a, b) - hi.  lo is a call of its own so that a lo that only one branch stores is computed on that branch alone.
+__device__ __forceinline__ uint32_t bf16x2_lo(float a, float b, uint32_t hi) {
+  return tc::pack_bf16(a - __uint_as_float(hi << 16), b - __uint_as_float(hi & 0xffff0000u));
+}
 
 // store 4 consecutive columns (half of a 16-byte chunk) of a row into a swizzled tile; with `split`
 // also the bf16 residual v - bf16(v) into the lo tile
@@ -67,11 +78,7 @@ __device__ __forceinline__ void store_half(uint32_t tile_hi, uint32_t tile_lo, i
   const uint32_t off = tc::swz_chunk(row, col0 >> 3) + ((col0 & 4) << 1);
   const uint32_t hx = tc::pack_bf16(v[0], v[1]), hy = tc::pack_bf16(v[2], v[3]);
   sts_v2(tile_hi + off, hx, hy);
-  if (split) {
-    const uint32_t lx = tc::pack_bf16(v[0] - __uint_as_float(hx << 16), v[1] - __uint_as_float(hx & 0xffff0000u));
-    const uint32_t ly = tc::pack_bf16(v[2] - __uint_as_float(hy << 16), v[3] - __uint_as_float(hy & 0xffff0000u));
-    sts_v2(tile_lo + off, lx, ly);
-  }
+  if (split) sts_v2(tile_lo + off, bf16x2_lo(v[0], v[1], hx), bf16x2_lo(v[2], v[3], hy));
 }
 
 // accumulator loads: columns col .. col + n - 1 of row (base + lane), see tc::acc_row
@@ -93,10 +100,7 @@ __device__ __forceinline__ void store_half(uint32_t tile_hi, uint32_t tile_lo, i
   const uint32_t off = tc::swz_chunk(row, col0 >> 3) + ((col0 & 6) << 1);
   const uint32_t hx = tc::pack_bf16(v[0], v[1]);
   asm volatile("st.shared.b32 [%0], %1;" ::"r"(tile_hi + off), "r"(hx) : "memory");
-  if (split) {
-    const uint32_t lx = tc::pack_bf16(v[0] - __uint_as_float(hx << 16), v[1] - __uint_as_float(hx & 0xffff0000u));
-    asm volatile("st.shared.b32 [%0], %1;" ::"r"(tile_lo + off), "r"(lx) : "memory");
-  }
+  if (split) asm volatile("st.shared.b32 [%0], %1;" ::"r"(tile_lo + off), "r"(bf16x2_lo(v[0], v[1], hx)) : "memory");
 }
 
 // ---- fp32x2 arithmetic: two columns per value (component-wise fp32 instructions) ---------------
@@ -234,6 +238,28 @@ __device__ __forceinline__ void dbg_mark(CS* cs, int id) {
     cs->dbg[cs->dbg_n++] = ((long long)id << 48) | (clock64() & 0xffffffffffffLL);
   }
 #endif
+}
+
+// CTA-wide constants kept in shared memory so that the per-network passes (separate functions) do not drag a context
+// struct through local memory: the fields both kernels use (each kernel's CtaShared / TwShared adds its own)
+struct CtaBase {
+  float* partial;          // this CTA's gradient partial
+  long long* dbg;          // optional phase-timestamp buffer (CTA 0, thread 0)
+  int dbg_n;
+  int tl_max, off_P, off_misc, off_ones, mx_dim, mx_taps;
+};
+// thread 0: fill the common fields and write the start record of the phase timeline
+__device__ __forceinline__ void cta_base_init(CtaBase& cs, const TcCommonArgs& a, float* partial) {
+  cs.partial = partial;
+  cs.tl_max = a.tl_max; cs.off_P = a.off_P; cs.off_misc = a.off_misc; cs.off_ones = a.off_ones;
+  cs.mx_dim = a.mx_dim; cs.mx_taps = a.mx_taps;
+#ifdef PINN_DEBUG
+  cs.dbg = (blockIdx.x == 0) ? a.dbg : nullptr;
+#else
+  cs.dbg = nullptr;
+#endif
+  cs.dbg_n = 0;
+  dbg_mark(&cs, 1);
 }
 
 struct Misc {   // carve-up of the misc region
@@ -528,6 +554,186 @@ __device__ __forceinline__ void cta_finish(const TcCommonArgs& a, const CS& cs, 
   if (a.tail.state)
     fused_tail<float, kTcThreads>(a.tail, a.partial, a.partial_stride, a.term_sums, P.n_theta, P.n_terms, want_grad ? 1 : 0,
                                   reinterpret_cast<float*>(smem + a.off_P));
+}
+
+// ---- steps of the per-network passes that both tensor-core kernels share --------------------------------------------------
+// (what differs between the kernels comes in as arguments: shared-memory tile addresses and strides, descriptor LBOs,
+// accumulator columns, and `rows`, the accumulator rows a flush reads = the kernel's widest layer)
+
+// end of the forward: combine the per-warp last-layer dots u of every point through ms.scratch (zeroed when the pass
+// began), add b_L (*bl) and write the taps the term reads from network slot `slot`.  CTA-wide.
+template <int C, typename CS>
+__device__ __forceinline__ void finish_forward(CS* cs, const DevTerm& tm, int slot, const Misc& ms, const float* bl, const Tid& t,
+                                               const float (&u)[C]) {
+  __syncthreads();
+  dbg_mark(cs, 15);
+#pragma unroll
+  for (int c = 0; c < C; ++c) atomicAdd(&ms.scratch[c * kTcPts + t.p], u[c]);
+  __syncthreads();
+  if (t.hh == 0) {
+    float s[C];
+#pragma unroll
+    for (int c = 0; c < C; ++c) s[c] = ms.scratch[c * kTcPts + t.p];
+    s[0] += *bl;
+    const int n_taps = tm.n_taps;
+    for (int tt = 0; tt < n_taps; ++tt)
+      if (tm.tap_slot[tt] == slot) {
+        const int tch = tm.tap_ch[tt];
+        float v = s[0];
+#pragma unroll
+        for (int c = 1; c < C; ++c) v = (tch == c) ? s[c] : v;
+        ms.taps[tt * kTcPts + t.p] = v;
+      }
+  }
+  __syncthreads();
+  dbg_mark(cs, 16);
+}
+
+// adjoints of the network outputs per channel at point p (every thread of the point needs them)
+template <int C>
+__device__ __forceinline__ void gather_ubar(const DevTerm& tm, int slot, const Misc& ms, int p, float (&ub)[C]) {
+#pragma unroll
+  for (int c = 0; c < C; ++c) ub[c] = 0.f;
+  const int n_taps = tm.n_taps;
+  for (int tt = 0; tt < n_taps; ++tt)
+    if (tm.tap_slot[tt] == slot) {
+      const float g = ms.tapbar[tt * kTcPts + p];
+      const int tch = tm.tap_ch[tt];
+#pragma unroll
+      for (int c = 0; c < C; ++c) ub[c] += (tch == c) ? g : 0.f;
+    }
+}
+
+// last layer: bias gradient by warp sums; weight gradient  wbar_L[o] = sum_{c,p} ubar_c[p] H_c[p][o]  on the tensor core:
+// D_c[o][0..15] = H_c^T U into accumulator columns acol + 16c, with U[p] = (hi, lo) bf16 pairs of ubar_0..ubar_(C-1)
+// (columns 2c, 2c+1) written to the tile at u_tile.  H_c is the tile at h_tile + c * h_stride, read MN-major (h_lbo: the
+// next 64 rows of M when the last hidden layer is wider than 64).  CTA-wide.
+template <int C>
+__device__ __forceinline__ void last_layer_grad(const Tid& t, const float (&ub)[C], int nL, float* gw, float* gb, uint32_t u_tile,
+                                                uint32_t h_tile, uint32_t h_stride, uint32_t h_lbo, uint32_t acol, int rows) {
+  if (t.hh == 0) {
+    const float s = warp_sum<float>(ub[0]);
+    if (t.lane == 0) atomicAdd(gb, s);
+    uint32_t w[8];
+#pragma unroll
+    for (int c = 0; c < 8; ++c) w[c] = 0u;
+#pragma unroll
+    for (int c = 0; c < C; ++c) {
+      const uint32_t hi = tc::pack_bf16(ub[c], 0.f);   // upper halves bf16(0): hi | lo << 16 = (bf16 hi, bf16 lo) of ubar_c
+      w[c] = hi | (bf16x2_lo(ub[c], 0.f, hi) << 16);
+    }
+    sts_v4(u_tile + tc::swz_chunk(t.p, 0), w[0], w[1], w[2], w[3]);
+    sts_v4(u_tile + tc::swz_chunk(t.p, 1), w[4], w[5], w[6], w[7]);
+  }
+  tc::fence_async_smem();
+  __syncthreads();
+  {
+    const uint32_t idesc = tc::make_idesc(16, 1, 1);
+    const uint64_t db = tc::make_desc(u_tile, 0, 1024);
+#pragma unroll 1
+    for (int c = 0; c < C; ++c)
+      mma_chain(acol + 16 * c, tc::make_desc(h_tile + c * h_stride, h_lbo, 1024), db, 2048, 2048, kTcPts / 16, idesc, 0);
+  }
+  __syncthreads();
+  if (t.hh == 0 && t.q * 32 < rows) {
+    const int o = t.q * 32 + t.lane;
+    float acc = 0.f;
+#pragma unroll
+    for (int c = 0; c < C; ++c) {
+      float v[2];
+      acc_ld2(t.lane_addr + acol + 16 * c + 2 * c, v);
+      acc += v[0] + v[1];
+    }
+    if (o < nL) atomicAdd(gw + o, acc);
+  }
+  __syncthreads();
+}
+
+// flush a tensor layer's gradient tile: accumulator row = output neuron o, columns wcol .. wcol + n_in - 1 = input
+// neuron k of the weight gradient, column bcol = the bias gradient
+__device__ __forceinline__ void flush_wgrad(const Tid& t, uint32_t wcol, uint32_t bcol, int rows, int n_in, int n_out, float* gw,
+                                            float* gb) {
+  if (t.q * 32 < rows) {
+    const int o = t.q * 32 + t.lane;
+    if (t.hh == 0) {
+      float v[2];
+      acc_ld2(t.lane_addr + bcol, v);
+      if (o < n_out) atomicAdd(gb + o, v[0]);
+    }
+    const int part = n_in / kNH;
+#pragma unroll 1
+    for (int k0 = t.hh * part; k0 < (t.hh + 1) * part; k0 += 4) {
+      float v[4];
+      acc_ld4(t.lane_addr + wcol + k0, v);
+      if (o < n_out) {
+#pragma unroll
+        for (int i = 0; i < 4; ++i) atomicAdd(gw + o + (long long)n_out * (k0 + i), v[i]);
+      }
+    }
+  }
+}
+
+// layer-0 weight / bias gradient as one MMA chain over K = the 128 points:
+//   D[o][0..15] = Zbar_0^T [x | 1] + sum_j Zbar_(1+j)^T E_(dir1[j]),  Wbar_0[o][k] = D[o][k],  bbar_0[o] = D[o][8].
+// coord_tiles writes the B tiles (rows = points, 16 columns used), kTileBytes apart from b_tile (threads 0..127):
+//   tile 0: bf16 hi of (x_0..x_7) in columns 0..7, 1.0 in column 8;  tile 1+j: 1.0 in column dir1[j];
+//   tile 1+N1: bf16 lo of x (x_lo: when the kernel has a spare tile for it)
+template <int N1>
+__device__ __forceinline__ void coord_tiles(const Tid& t, uint32_t b_tile, const float (&x)[PINN_MAX_IN],
+                                            const int (&dir1)[N1 > 0 ? N1 : 1], bool x_lo) {
+  if (t.tid >= kTcPts) return;
+  uint32_t hi[4], lo[4];
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {
+    hi[k] = tc::pack_bf16(x[2 * k], x[2 * k + 1]);
+    lo[k] = bf16x2_lo(x[2 * k], x[2 * k + 1], hi[k]);
+  }
+  const uint32_t c0a = b_tile + tc::swz_chunk(t.p, 0), c1a = b_tile + tc::swz_chunk(t.p, 1);
+  sts_v4(c0a, hi[0], hi[1], hi[2], hi[3]);
+  sts_v4(c1a, 0x00003f80u, 0u, 0u, 0u);
+  if (x_lo) {
+    sts_v4(c0a + (1 + N1) * kTileBytes, lo[0], lo[1], lo[2], lo[3]);
+    sts_v4(c1a + (1 + N1) * kTileBytes, 0u, 0u, 0u, 0u);
+  }
+#pragma unroll
+  for (int j = 0; j < N1; ++j) {
+    const int d = dir1[j];
+    uint32_t w[4];
+#pragma unroll
+    for (int k = 0; k < 4; ++k) w[k] = (d == 2 * k) ? 0x00003f80u : ((d == 2 * k + 1) ? 0x3f800000u : 0u);
+    sts_v4(c0a + (1 + j) * kTileBytes, w[0], w[1], w[2], w[3]);
+    sts_v4(c1a + (1 + j) * kTileBytes, 0u, 0u, 0u, 0u);
+  }
+}
+// the MMA chains against the coord_tiles at b_tile and the flush into W_0 / b_0.  Zbar_c is the tile at z_tile + c * z_stride,
+// read MN-major (z_lbo: the next 64 rows of M when the first layer is wider than 64).  Publishes the tiles itself; CTA-wide.
+template <int N1>
+__device__ __forceinline__ void layer0_grad(const Tid& t, uint32_t z_tile, uint32_t z_stride, uint32_t z_lbo, uint32_t b_tile,
+                                            bool x_lo, uint32_t acol, int rows, int n1w, int d_in, float* gw0, float* gb0) {
+  tc::fence_async_smem();
+  __syncthreads();
+  {
+    const uint32_t idesc = tc::make_idesc(16, 1, 1);
+    const uint64_t a0 = tc::make_desc(z_tile, z_lbo, 1024);
+    mma_chain(acol, a0, tc::make_desc(b_tile, 0, 1024), 2048, 2048, kTcPts / 16, idesc, 0);
+    if (x_lo) mma_chain(acol, a0, tc::make_desc(b_tile + (1 + N1) * kTileBytes, 0, 1024), 2048, 2048, kTcPts / 16, idesc, 1);
+#pragma unroll 1
+    for (int j = 0; j < N1; ++j)
+      mma_chain(acol, tc::make_desc(z_tile + (1 + j) * z_stride, z_lbo, 1024), tc::make_desc(b_tile + (1 + j) * kTileBytes, 0, 1024),
+                2048, 2048, kTcPts / 16, idesc, 1);
+  }
+  __syncthreads();
+  if (t.hh == 0 && t.q * 32 < rows) {
+    const int o = t.q * 32 + t.lane;
+    float v[16];
+    tc::acc_ld16(t.lane_addr + acol, v);
+    if (o < n1w) {
+#pragma unroll
+      for (int k = 0; k < PINN_MAX_IN; ++k)
+        if (k < d_in) atomicAdd(gw0 + o + (long long)n1w * k, v[k]);
+      atomicAdd(gb0 + o, v[8]);
+    }
+  }
 }
 
 // channel structure <A1, A2, PU> of PINN_TC_DISPATCH; not instantiated when it has more than maxc channels

@@ -27,18 +27,11 @@ namespace pinn {
 
 using Fp = FpBlock<kTcW>;   // fp32 parameter block of a network
 
-// CTA-wide constants kept in shared memory so the per-network passes (separate functions) do not
-// drag a context struct through local memory
-struct CtaShared {
-  int split, tl_max, off_P, off_Q, off_misc, off_ones, mx_dim, mx_taps;
-  float* partial;
+struct CtaShared : CtaBase {
+  int split, off_Q;
   uint8_t* stash;
-  const float* theta;
-  long long* dbg;          // optional phase-timestamp buffer (CTA 0, thread 0)
-  int dbg_n;
   TcNetSmem nets[PINN_MAX_NETS];
 };
-
 
 // ---- granule loops (4 columns x all channels per step), specialised on the activation kind -------------
 // (inlined into the per-network passes; a noinline callee only gets the ABI scratch registers and spills)
@@ -51,6 +44,11 @@ struct LoopCtx {
   float* gw;              // weight gradient of the first layer (CTA partial)
   uint32_t taddr;         // accumulator address of the warp's row quadrant
   int act, split, p, lane, g0, g1, c0, flag;
+  // ng granules of the layer, spread over the kNH warps of the thread's row quadrant
+  __device__ __forceinline__ LoopCtx(uint32_t fp_, uint32_t bt_, uint32_t tP_, uint32_t tQ_, const Tid& t, int act_, int ng,
+                                     int flag_, int split_ = 0, int c0_ = 0, float* gb_ = nullptr, float* gw_ = nullptr)
+      : fp(fp_), bt(bt_), tP(tP_), tQ(tQ_), gb(gb_), gw(gw_), taddr(t.lane_addr), act(act_), split(split_), p(t.p), lane(t.lane),
+        g0(t.hh * (ng / kNH)), g1((t.hh + 1) * (ng / kNH)), c0(c0_), flag(flag_) {}
 };
 
 // layer 0 forward: coordinates -> H^0 tiles (+ last-layer dot when there is no tensor layer: flag)
@@ -281,7 +279,7 @@ __device__ __noinline__ uint32_t net_forward(CtaShared* cs, const DevProblem* Pp
   load_pass<N1, N2>(pi, net, dc);
   const int TL = pi.TL;
   const Tid t = tid_of();
-  const int tid = t.tid, hh = t.hh, p = t.p;
+  const int tid = t.tid, p = t.p;
   float x[PINN_MAX_IN];
 #pragma unroll
   for (int k = 0; k < PINN_MAX_IN; ++k) x[k] = (k < pi.d_in) ? ms.Xs[dc.rows[k] * kTcPts + p] : 0.f;
@@ -291,18 +289,11 @@ __device__ __noinline__ uint32_t net_forward(CtaShared* cs, const DevProblem* Pp
   float u[C];                                   // last-layer partial dot products of this thread
 #pragma unroll
   for (int c = 0; c < C; ++c) u[c] = 0.f;
-  // the cross-warp combination of u goes through shared-memory atomics
+  // the cross-warp combination of u goes through shared-memory atomics (finish_forward)
   if (tid < C * kTcPts / 4) reinterpret_cast<float4*>(ms.scratch)[tid] = make_float4(0.f, 0.f, 0.f, 0.f);
-  if (kTcThreads < C * kTcPts / 4 && tid + kTcThreads < C * kTcPts / 4)
-    reinterpret_cast<float4*>(ms.scratch)[tid + kTcThreads] = make_float4(0.f, 0.f, 0.f, 0.f);
   {
     // ---- layer 0 on the CUDA cores ------------------------------------------------------------------
-    const int act0 = net.acts[0];
-    const int ng = pi.n1w / GW;
-    LoopCtx lc;
-    lc.fp = tc::smem_u32(fp); lc.bt = lc.fp; lc.tP = tc::smem_u32(tP); lc.tQ = tc::smem_u32(tQ); lc.gb = nullptr; lc.gw = nullptr;
-    lc.taddr = accm + t.lane_addr; lc.act = act0; lc.split = split ? 1 : 0; lc.p = p; lc.lane = t.lane; lc.g0 = hh * (ng / kNH); lc.g1 = (hh + 1) * (ng / kNH);
-    lc.c0 = 0; lc.flag = (TL == 0) ? 1 : 0;
+    const LoopCtx lc(tc::smem_u32(fp), tc::smem_u32(fp), tc::smem_u32(tP), tc::smem_u32(tQ), t, net.acts[0], pi.n1w / GW, TL == 0, split);
     l0_fwd_loop<N1, N2, PURE, AK>(lc, pi, x, u);
   }
   // ---- tensor layers -------------------------------------------------------------------------------------
@@ -342,36 +333,11 @@ __device__ __noinline__ uint32_t net_forward(CtaShared* cs, const DevProblem* Pp
     if (want_grad && tid == 0) tc::bulk_wait_read0();   // stash copies have finished reading P (same thread issued them)
     __syncthreads();
     dbg_mark(cs, 14);
-    const int ng = n_out / GW;
-    LoopCtx lc;
-    lc.fp = tc::smem_u32(fp); lc.bt = lc.fp + (Fp::BT + (l - 1) * 64) * 4; lc.tP = tc::smem_u32(tP); lc.tQ = tc::smem_u32(tQ);
-    lc.gb = nullptr; lc.gw = nullptr;
-    lc.taddr = accm + t.lane_addr; lc.act = act; lc.split = split ? 1 : 0; lc.p = p; lc.lane = t.lane;
-    lc.g0 = hh * (ng / kNH); lc.g1 = (hh + 1) * (ng / kNH); lc.c0 = 0; lc.flag = (l == TL) ? 1 : 0;
+    const LoopCtx lc(tc::smem_u32(fp), tc::smem_u32(fp) + (Fp::BT + (l - 1) * 64) * 4, tc::smem_u32(tP), tc::smem_u32(tQ), t, act, n_out / GW, l == TL, split);
     tl_fwd_loop<N1, N2, PURE, AK>(lc, pi.ch, u);
   }
   // ---- last layer (n -> 1, identity): combine the column parts of every point ---------------------------------
-  __syncthreads();   // scratch zeroed
-  dbg_mark(cs, 15);
-#pragma unroll
-  for (int c = 0; c < C; ++c) atomicAdd(&ms.scratch[c * kTcPts + p], u[c]);
-  __syncthreads();
-  if (hh == 0) {
-#pragma unroll
-    for (int c = 0; c < C; ++c) u[c] = ms.scratch[c * kTcPts + p];
-    u[0] += fp[Fp::BL];
-    const int n_taps = tm.n_taps;
-    for (int tt = 0; tt < n_taps; ++tt)
-      if (tm.tap_slot[tt] == slot) {
-        const int tch = tm.tap_ch[tt];
-        float v = u[0];
-#pragma unroll
-        for (int c = 1; c < C; ++c) v = (tch == c) ? u[c] : v;
-        ms.taps[tt * kTcPts + p] = v;
-      }
-  }
-  __syncthreads();
-  dbg_mark(cs, 16);
+  finish_forward<C>(cs, tm, slot, ms, fp + Fp::BL, t, u);
   return phase;
 }
 
@@ -396,7 +362,7 @@ __device__ __noinline__ uint32_t net_backward(CtaShared* cs, const DevProblem* P
   load_pass<N1, N2>(pi, net, dc);
   const int L = pi.L, TL = pi.TL;
   const Tid t = tid_of();
-  const int tid = t.tid, hh = t.hh, p = t.p, lane = t.lane, q = t.q;
+  const int tid = t.tid, p = t.p;
   uint32_t ld_phase = (phase >> 1) & 1u;
   float x[PINN_MAX_IN];
 #pragma unroll
@@ -404,65 +370,11 @@ __device__ __noinline__ uint32_t net_backward(CtaShared* cs, const DevProblem* P
   uint8_t* stash_slot = cs->stash + (size_t)slot * cs->tl_max * kTcMaxC * kTileBytes;
 
   dbg_mark(cs, 20);
-  // adjoint of the network outputs per channel (every thread of the point needs it)
   float ub[C];
-#pragma unroll
-  for (int c = 0; c < C; ++c) ub[c] = 0.f;
-  {
-    const int n_taps = tm.n_taps;
-    for (int tt = 0; tt < n_taps; ++tt)
-      if (tm.tap_slot[tt] == slot) {
-        const float g = ms.tapbar[tt * kTcPts + p];
-        const int tch = tm.tap_ch[tt];
-#pragma unroll
-        for (int c = 0; c < C; ++c) ub[c] += (tch == c) ? g : 0.f;
-      }
-  }
-  // ---- last layer: bias gradient by warp sums; weight gradient  wbar_last[o] = sum_{c,p} ubar_c[p] H_c^{L-2}[p][o]  on the
-  // tensor core: D_c[o][0..15] = H_c^T U with U[p] = (hi, lo) bf16 pairs of ubar_0..ubar_(C-1) (columns 2c, 2c+1) ------------
-  {
-    float* gb_last = partial + net.b_off[L - 1];
-    float* gw_last = partial + net.w_off[L - 1];
-    if (hh == 0) {
-      const float s = warp_sum<float>(ub[0]);
-      if (lane == 0) atomicAdd(gb_last, s);
-      uint32_t w[8];
-#pragma unroll
-      for (int c = 0; c < 8; ++c) w[c] = 0u;
-#pragma unroll
-      for (int c = 0; c < C; ++c) {
-        const uint32_t hi = tc::pack_bf16(ub[c], 0.f) & 0xffffu;
-        const float r = ub[c] - __uint_as_float(hi << 16);
-        w[c] = hi | (tc::pack_bf16(r, 0.f) << 16);
-      }
-      const uint32_t q0 = tc::smem_u32(tQ);
-      asm volatile("st.shared.v4.b32 [%0], {%1,%2,%3,%4};" ::"r"(q0 + tc::swz_chunk(p, 0)), "r"(w[0]), "r"(w[1]), "r"(w[2]), "r"(w[3]) : "memory");
-      asm volatile("st.shared.v4.b32 [%0], {%1,%2,%3,%4};" ::"r"(q0 + tc::swz_chunk(p, 1)), "r"(w[4]), "r"(w[5]), "r"(w[6]), "r"(w[7]) : "memory");
-    }
-    tc::fence_async_smem();
-    __syncthreads();
-    {
-      const uint32_t sP = tc::smem_u32(tP);
-      const uint32_t idesc = tc::make_idesc(16, 1, 1);
-      const uint64_t db = tc::make_desc(tc::smem_u32(tQ), 0, 1024);
-#pragma unroll 1
-      for (int c = 0; c < C; ++c)
-        mma_chain(accm + TM_Y + 16 * c, tc::make_desc(sP + c * kTileBytes, 0, 1024), db, 2048, 2048, kTcPts / 16, idesc, 0);
-    }
-    __syncthreads();
-    if (q < 2 && hh == 0) {
-      const int o = q * 32 + lane;
-      float acc = 0.f;
-#pragma unroll
-      for (int c = 0; c < C; ++c) {
-        float v[2];
-        acc_ld2(accm + t.lane_addr + TM_Y + 16 * c + 2 * c, v);
-        acc += v[0] + v[1];
-      }
-      if (o < pi.nL) atomicAdd(gw_last + o, acc);
-    }
-    __syncthreads();
-  }
+  gather_ubar<C>(tm, slot, ms, p, ub);
+  // ---- last layer: the ubar tile goes to Q, the products into accumulator columns Y ----------------------------------------
+  last_layer_grad<C>(t, ub, pi.nL, partial + net.w_off[L - 1], partial + net.b_off[L - 1], tc::smem_u32(tQ), tc::smem_u32(tP),
+                     kTileBytes, 0u, accm + TM_Y, kTcW);
 
   // ---- tensor layers, last to first ------------------------------------------------------------------------------------
   for (int l = TL; l >= 1; --l) {
@@ -497,12 +409,7 @@ __device__ __noinline__ uint32_t net_backward(CtaShared* cs, const DevProblem* P
       dbg_mark(cs, 24);
       __syncthreads();
       dbg_mark(cs, 25);
-      const int ng = gw_cols / GWB;
-      LoopCtx lc;
-      lc.fp = tc::smem_u32(fp); lc.bt = tc::smem_u32(bt); lc.tP = tc::smem_u32(tP); lc.tQ = tc::smem_u32(tQ); lc.gb = gb; lc.gw = nullptr;
-      lc.taddr = accm + t.lane_addr;
-      lc.act = act; lc.split = 0; lc.p = p; lc.lane = lane; lc.g0 = hh * (ng / kNH); lc.g1 = (hh + 1) * (ng / kNH);
-      lc.c0 = c0; lc.flag = (l == TL) ? 1 : 0;
+      const LoopCtx lc(tc::smem_u32(fp), tc::smem_u32(bt), tc::smem_u32(tP), tc::smem_u32(tQ), t, act, gw_cols / GWB, l == TL, 0, c0);
       tl_bwd_loop<N1, N2, PURE, AK>(lc, pi.ch, ub);
     }
     tc::fence_async_smem();
@@ -530,25 +437,7 @@ __device__ __noinline__ uint32_t net_backward(CtaShared* cs, const DevProblem* P
     dbg_mark(cs, 27);
     __syncthreads();
     dbg_mark(cs, 28);
-    // flush the weight-gradient tile: accumulator row = output neuron o, column = input neuron k
-    if (q < 2) {
-      const int o = q * 32 + lane;
-      if (hh == 0) {
-        float v[2];
-        acc_ld2(accm + t.lane_addr + TM_Y + 64, v);
-        if (o < n_out) atomicAdd(gb + o, v[0]);
-      }
-      const int part = n_in / kNH;
-#pragma unroll 1
-      for (int k0 = hh * part; k0 < (hh + 1) * part; k0 += 4) {
-        float v[4];
-        acc_ld4(accm + t.lane_addr + TM_Y + k0, v);
-        if (o < n_out) {
-#pragma unroll
-          for (int i = 0; i < 4; ++i) atomicAdd(gw + o + (long long)n_out * (k0 + i), v[i]);
-        }
-      }
-    }
+    flush_wgrad(t, accm + TM_Y, accm + TM_Y + 64, kTcW, n_in, n_out, gw, gb);
   }
 
   // ---- layer 0 backward ---------------------------------------------------------------------------------------------------
@@ -558,75 +447,18 @@ __device__ __noinline__ uint32_t net_backward(CtaShared* cs, const DevProblem* P
     const int act0 = net.acts[0];
     float* gb0 = partial + net.b_off[0];
     float* gw0 = partial + net.w_off[0];
-    LoopCtx lc;
-    lc.fp = tc::smem_u32(fp); lc.bt = lc.fp; lc.tP = tc::smem_u32(tP); lc.tQ = tc::smem_u32(tQ); lc.gb = gb0; lc.gw = gw0;
-    lc.taddr = accm + t.lane_addr; lc.act = act0; lc.split = 0; lc.p = p; lc.lane = lane; lc.c0 = 0; lc.flag = (TL == 0) ? 1 : 0;
+    const uint32_t sP = tc::smem_u32(tP), sQ = tc::smem_u32(tQ);
     if (TL == 0) {
       // no tensor layer: everything on the CUDA cores (warp reduce-scatter + atomics)
-      const int ng = pi.n1w / GW;
-      lc.g0 = hh * (ng / kNH); lc.g1 = (hh + 1) * (ng / kNH);
+      const LoopCtx lc(tc::smem_u32(fp), tc::smem_u32(fp), sP, sQ, t, act0, pi.n1w / GW, 1, 0, 0, gb0, gw0);
       l0_bwd_loop<N1, N2, PURE, AK>(lc, pi, x, ub);
     } else {
-      // Wbar_0[o][k] = sum_p zbar_0[p][o] x_k[p] + zbar_(1+j)[p][o] [dir1[j] == k],  bbar_0[o] = sum_p zbar_0[p][o]:
-      // one MMA chain  D[o][0..15] = Zbar_0^T [x | 1] + sum_j Zbar_(1+j)^T E_(dir1[j])  with K = the 128 points.
-      // B tiles (rows = points, 16 columns used) live in Q, which is free after the last tensor layer:
-      //   tile 0: bf16 hi of (x_0..x_7) in columns 0..7, 1.0 in column 8;  tile 1+j: 1.0 in column dir1[j];
-      //   tile 1+N1: bf16 lo of x (only when the channel count leaves a spare tile, i.e. N2 > 0)
-      if (tid < kTcPts) {
-        uint32_t hi[4], lo[4];
-#pragma unroll
-        for (int k = 0; k < 4; ++k) {
-          hi[k] = tc::pack_bf16(x[2 * k], x[2 * k + 1]);
-          lo[k] = tc::pack_bf16(x[2 * k] - __uint_as_float(hi[k] << 16), x[2 * k + 1] - __uint_as_float(hi[k] & 0xffff0000u));
-        }
-        const uint32_t q0 = tc::smem_u32(tQ);
-        const uint32_t c0a = tc::swz_chunk(p, 0), c1a = tc::swz_chunk(p, 1);
-        asm volatile("st.shared.v4.b32 [%0], {%1,%2,%3,%4};" ::"r"(q0 + c0a), "r"(hi[0]), "r"(hi[1]), "r"(hi[2]), "r"(hi[3]) : "memory");
-        asm volatile("st.shared.v4.b32 [%0], {%1,%2,%3,%4};" ::"r"(q0 + c1a), "r"(0x00003f80u), "r"(0u), "r"(0u), "r"(0u) : "memory");
-        if (N2 > 0) {
-          asm volatile("st.shared.v4.b32 [%0], {%1,%2,%3,%4};" ::"r"(q0 + (1 + N1) * kTileBytes + c0a), "r"(lo[0]), "r"(lo[1]), "r"(lo[2]), "r"(lo[3]) : "memory");
-          asm volatile("st.shared.v4.b32 [%0], {%1,%2,%3,%4};" ::"r"(q0 + (1 + N1) * kTileBytes + c1a), "r"(0u), "r"(0u), "r"(0u), "r"(0u) : "memory");
-        }
-#pragma unroll
-        for (int j = 0; j < N1; ++j) {
-          const int d = pi.dir1[j];
-          uint32_t w[4] = {0u, 0u, 0u, 0u};
-#pragma unroll
-          for (int k = 0; k < 4; ++k) w[k] = (d == 2 * k) ? 0x00003f80u : ((d == 2 * k + 1) ? 0x3f800000u : 0u);
-          const uint32_t qb = q0 + (1 + j) * kTileBytes;
-          asm volatile("st.shared.v4.b32 [%0], {%1,%2,%3,%4};" ::"r"(qb + c0a), "r"(w[0]), "r"(w[1]), "r"(w[2]), "r"(w[3]) : "memory");
-          asm volatile("st.shared.v4.b32 [%0], {%1,%2,%3,%4};" ::"r"(qb + c1a), "r"(0u), "r"(0u), "r"(0u), "r"(0u) : "memory");
-        }
-      }
-      const int ng = pi.n1w / GWB;
-      lc.g0 = hh * (ng / kNH); lc.g1 = (hh + 1) * (ng / kNH);
+      // the weight / bias gradient by MMA (layer0_grad); the coordinate tiles live in Q, which is free after the last
+      // tensor layer, and the channel count leaves a spare tile for the lo of x when N2 > 0
+      coord_tiles<N1>(t, sQ, x, pi.dir1, N2 > 0);
+      const LoopCtx lc(tc::smem_u32(fp), tc::smem_u32(fp), sP, sQ, t, act0, pi.n1w / GWB, 0);
       l0_bwd_store_loop<N1, N2, PURE, AK>(lc, pi, x);
-      tc::fence_async_smem();
-      __syncthreads();
-      {
-        const uint32_t sP = tc::smem_u32(tP), sQ = tc::smem_u32(tQ);
-        const uint32_t idesc = tc::make_idesc(16, 1, 1);
-        const uint64_t a0 = tc::make_desc(sP, 0, 1024);
-        mma_chain(accm + TM_Y, a0, tc::make_desc(sQ, 0, 1024), 2048, 2048, kTcPts / 16, idesc, 0);
-        if (N2 > 0)
-          mma_chain(accm + TM_Y, a0, tc::make_desc(sQ + (1 + N1) * kTileBytes, 0, 1024), 2048, 2048, kTcPts / 16, idesc, 1);
-#pragma unroll 1
-        for (int j = 0; j < N1; ++j)
-          mma_chain(accm + TM_Y, tc::make_desc(sP + (1 + j) * kTileBytes, 0, 1024),
-                    tc::make_desc(sQ + (1 + j) * kTileBytes, 0, 1024), 2048, 2048, kTcPts / 16, idesc, 1);
-      }
-      __syncthreads();
-      if (q < 2 && hh == 0) {
-        const int o = q * 32 + lane;
-        float v[16];
-        tc::acc_ld16(accm + t.lane_addr + TM_Y, v);
-        if (o < pi.n1w) {
-#pragma unroll
-          for (int k = 0; k < PINN_MAX_IN; ++k)
-            if (k < pi.d_in) atomicAdd(gw0 + o + (long long)pi.n1w * k, v[k]);
-          atomicAdd(gb0 + o, v[8]);
-        }
-      }
+      layer0_grad<N1>(t, sP, kTileBytes, 0u, sQ, N2 > 0, accm + TM_Y, kTcW, pi.n1w, pi.d_in, gw0, gb0);
     }
   }
   __syncthreads();
@@ -673,21 +505,10 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_loss_grad_kernel(const __gri
   if (tid == 0) {
     tc::mbar_init(ms.bar_ld, 1);
     tc::fence_barrier_init();
-    cs.split = args.split; cs.tl_max = args.tl_max; cs.off_P = args.off_P; cs.off_Q = args.off_Q;
-    cs.off_misc = args.off_misc; cs.off_ones = args.off_ones; cs.mx_dim = args.mx_dim; cs.mx_taps = args.mx_taps;
-    cs.partial = partial;
+    cs.split = args.split; cs.off_Q = args.off_Q;
     cs.stash = args.stash + (long long)blockIdx.x * args.stash_per_cta;
-    cs.theta = theta;
-#ifdef PINN_DEBUG
-    cs.dbg = (blockIdx.x == 0) ? args.dbg : nullptr;
-#else
-    cs.dbg = nullptr;
-#endif
-    cs.dbg_n = 0;
     for (int k = 0; k < PINN_MAX_NETS; ++k) cs.nets[k] = args.nets[k];
-#ifdef PINN_DEBUG
-    if (cs.dbg) cs.dbg[cs.dbg_n++] = ((long long)1 << 48) | (clock64() & 0xffffffffffffLL);
-#endif
+    cta_base_init(cs, args, partial);
   }
   if (tid == 0) tc::s_acc = args.acc + (size_t)blockIdx.x * kAccCols * kAccRows;
   cta_setup(args, ms, partial, P.n_theta, want_grad);
@@ -728,17 +549,14 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_loss_grad_kernel(const __gri
           const int o = r & 63, kc = r >> 6;
           uint8_t* thi = smem + ns.w_hi[l - 1];
           uint8_t* tlo = smem + ns.w_lo[l - 1];
-          uint4 h, lo4;
-          h.x = tc::pack_bf16(w[it][0], w[it][1]); h.y = tc::pack_bf16(w[it][2], w[it][3]);
-          h.z = tc::pack_bf16(w[it][4], w[it][5]); h.w = tc::pack_bf16(w[it][6], w[it][7]);
-          *reinterpret_cast<uint4*>(thi + tc::swz_chunk(o, kc)) = h;
-          if (args.split) {
-            lo4.x = tc::pack_bf16(w[it][0] - __uint_as_float(h.x << 16), w[it][1] - __uint_as_float(h.x & 0xffff0000u));
-            lo4.y = tc::pack_bf16(w[it][2] - __uint_as_float(h.y << 16), w[it][3] - __uint_as_float(h.y & 0xffff0000u));
-            lo4.z = tc::pack_bf16(w[it][4] - __uint_as_float(h.z << 16), w[it][5] - __uint_as_float(h.z & 0xffff0000u));
-            lo4.w = tc::pack_bf16(w[it][6] - __uint_as_float(h.w << 16), w[it][7] - __uint_as_float(h.w & 0xffff0000u));
-            *reinterpret_cast<uint4*>(tlo + tc::swz_chunk(o, kc)) = lo4;
-          }
+          const float* v = w[it];
+          uint32_t h[4];
+#pragma unroll
+          for (int e = 0; e < 4; ++e) h[e] = tc::pack_bf16(v[2 * e], v[2 * e + 1]);
+          *reinterpret_cast<uint4*>(thi + tc::swz_chunk(o, kc)) = make_uint4(h[0], h[1], h[2], h[3]);
+          if (args.split)
+            *reinterpret_cast<uint4*>(tlo + tc::swz_chunk(o, kc)) = make_uint4(
+                bf16x2_lo(v[0], v[1], h[0]), bf16x2_lo(v[2], v[3], h[1]), bf16x2_lo(v[4], v[5], h[2]), bf16x2_lo(v[6], v[7], h[3]));
         }
       }
     }

@@ -29,15 +29,11 @@ namespace pinn {
 constexpr uint32_t TB = kTileBytes;
 using Fp = FpBlock<kTwW>;   // fp32 parameter block of a network
 
-struct TwShared {
-  int tl_max, off_P, off_S, off_misc, off_ones, off_nets, mx_dim, mx_taps;
-  float* partial;
+struct TwShared : CtaBase {
+  int off_S, off_nets;
   uint8_t* hstash;
   float* zstash;
-  const float* theta;
   const uint8_t* wpack;
-  long long* dbg;
-  int dbg_n;
   int off_fp[PINN_MAX_NETS], wimg[PINN_MAX_NETS];
   int next_tile;                     // dynamic scheduler: tile claimed for the next iteration
   uint32_t ph_ld[2];                 // phases of the streaming barriers (flipped by thread 0 after a CTA-wide wait)
@@ -48,9 +44,12 @@ struct LoopW {
   uint32_t fp;            // shared-memory address of the network's fp32 parameter block
   uint32_t bt;            // shared-memory address of the current tensor layer's bias
   uint32_t tP;            // shared-memory address of the operand tiles (channel c, column block kb: (c*2+kb)*TB)
-  float* gb;              // bias gradient of the current layer (CTA partial)
   uint32_t taddr;         // accumulator address of the warp's row quadrant
-  int act, p, lane, g0, g1, flag;
+  int act, p, g0, g1, flag;
+  // ng granules of the layer, spread over the kNH warps of the thread's row quadrant
+  __device__ __forceinline__ LoopW(uint32_t fp_, uint32_t bt_, uint32_t tP_, const Tid& t, int act_, int ng, int flag_)
+      : fp(fp_), bt(bt_), tP(tP_), taddr(t.lane_addr), act(act_), p(t.p), g0(t.hh * (ng / kNH)), g1((t.hh + 1) * (ng / kNH)),
+        flag(flag_) {}
 };
 
 __device__ __forceinline__ uint32_t tile_of(uint32_t tP, int c, int col) { return tP + (uint32_t)(c * 2 + (col >> 6)) * TB; }
@@ -238,7 +237,7 @@ __device__ __noinline__ void tw_net_forward(TwShared* cs, const DevProblem* Pp, 
   load_pass<N1, N2>(pi, net, dc);
   const int TL = pi.TL;
   const Tid t = tid_of();
-  const int tid = t.tid, hh = t.hh, p = t.p;
+  const int tid = t.tid, p = t.p;
   float x[PINN_MAX_IN];
 #pragma unroll
   for (int k = 0; k < PINN_MAX_IN; ++k) x[k] = (k < pi.d_in) ? ms.Xs[dc.rows[k] * kTcPts + p] : 0.f;
@@ -256,14 +255,8 @@ __device__ __noinline__ void tw_net_forward(TwShared* cs, const DevProblem* Pp, 
     tc::fence_async_smem();
     tw_load(cs, 1, tc::smem_u32(tS) + kTwImgBytes, wimg, (net.dims[1] + 63) >> 6);
   }
-  {
-    const int ng = pi.n1w / 4;
-    LoopW lc;
-    lc.fp = tc::smem_u32(fp); lc.bt = lc.fp; lc.tP = tc::smem_u32(tP); lc.gb = nullptr;
-    lc.taddr = accm + t.lane_addr; lc.act = net.acts[0]; lc.p = p; lc.lane = t.lane;
-    lc.g0 = hh * (ng / kNH); lc.g1 = (hh + 1) * (ng / kNH); lc.flag = 0;
-    tw_l0_fwd_loop<N1, N2, PURE, AK>(lc, pi, x);
-  }
+  const uint32_t sfp = tc::smem_u32(fp);
+  tw_l0_fwd_loop<N1, N2, PURE, AK>(LoopW(sfp, sfp, tc::smem_u32(tP), t, net.acts[0], pi.n1w / 4, 0), pi, x);
   for (int l = 1; l <= TL; ++l) {
     const int n_in = net.dims[l], n_out = net.dims[l + 1];
     tc::fence_async_smem();
@@ -301,11 +294,7 @@ __device__ __noinline__ void tw_net_forward(TwShared* cs, const DevProblem* Pp, 
     if (want_grad && tid == 0) tc::bulk_wait_read0();   // stash copies have finished reading P
     __syncthreads();
     dbg_mark(cs, 14);
-    const int ng = n_out / 4;
-    LoopW lc;
-    lc.fp = tc::smem_u32(fp); lc.bt = lc.fp + (Fp::BT + (l - 1) * 128) * 4; lc.tP = tc::smem_u32(tP); lc.gb = nullptr;
-    lc.taddr = accm + t.lane_addr; lc.act = net.acts[l]; lc.p = p; lc.lane = t.lane;
-    lc.g0 = hh * (ng / kNH); lc.g1 = (hh + 1) * (ng / kNH); lc.flag = (l == TL) ? 1 : 0;
+    const LoopW lc(sfp, sfp + (Fp::BT + (l - 1) * 128) * 4, sP, t, net.acts[l], n_out / 4, l == TL);
     float2* zl = want_grad ? reinterpret_cast<float2*>(zst + (size_t)(l - 1) * kTwMaxC * 64 * kTcPts * 2) + p : nullptr;
     tw_fwd_loop<N1, N2, PURE, AK>(lc, pi.ch, u, zl);
   }
@@ -323,27 +312,7 @@ __device__ __noinline__ void tw_net_forward(TwShared* cs, const DevProblem* Pp, 
       tc::bulk_wait_read0();
     }
   }
-  __syncthreads();
-  dbg_mark(cs, 15);
-#pragma unroll
-  for (int c = 0; c < C; ++c) atomicAdd(&ms.scratch[c * kTcPts + p], u[c]);
-  __syncthreads();
-  if (hh == 0) {
-#pragma unroll
-    for (int c = 0; c < C; ++c) u[c] = ms.scratch[c * kTcPts + p];
-    u[0] += fp[Fp::BL];
-    const int n_taps = tm.n_taps;
-    for (int tt = 0; tt < n_taps; ++tt)
-      if (tm.tap_slot[tt] == slot) {
-        const int tch = tm.tap_ch[tt];
-        float v = u[0];
-#pragma unroll
-        for (int c = 1; c < C; ++c) v = (tch == c) ? u[c] : v;
-        ms.taps[tt * kTcPts + p] = v;
-      }
-  }
-  __syncthreads();
-  dbg_mark(cs, 16);
+  finish_forward<C>(cs, tm, slot, ms, fp + Fp::BL, t, u);
 }
 
 // reverse sweep of one network for the current tile (P still holds the last hidden activations)
@@ -369,13 +338,14 @@ __device__ __noinline__ void tw_net_backward(TwShared* cs, const DevProblem* Pp,
   load_pass<N1, N2>(pi, net, dc);
   const int L = pi.L, TL = pi.TL;
   const Tid t = tid_of();
-  const int tid = t.tid, hh = t.hh, p = t.p, lane = t.lane, q = t.q;
+  const int tid = t.tid, p = t.p;
   float x[PINN_MAX_IN];
 #pragma unroll
   for (int k = 0; k < PINN_MAX_IN; ++k) x[k] = (k < pi.d_in) ? ms.Xs[dc.rows[k] * kTcPts + p] : 0.f;
   uint8_t* hst = cs->hstash + (size_t)slot * (cs->tl_max + 1) * kTwMaxC * 2 * TB;
   const float* zst = cs->zstash + (size_t)slot * cs->tl_max * kTwMaxC * 64 * kTcPts * 2;
   const uint8_t* wimg = cs->wpack + (size_t)cs->wimg[net_id] * kTwImgBytes;
+  const uint32_t sfp = tc::smem_u32(fp);
 
   dbg_mark(cs, 20);
   if (tm.n_used > 1) {
@@ -392,64 +362,10 @@ __device__ __noinline__ void tw_net_backward(TwShared* cs, const DevProblem* Pp,
     __syncthreads();
   }
   float ub[C];
-#pragma unroll
-  for (int c = 0; c < C; ++c) ub[c] = 0.f;
-  {
-    const int n_taps = tm.n_taps;
-    for (int tt = 0; tt < n_taps; ++tt)
-      if (tm.tap_slot[tt] == slot) {
-        const float g = ms.tapbar[tt * kTcPts + p];
-        const int tch = tm.tap_ch[tt];
-#pragma unroll
-        for (int c = 0; c < C; ++c) ub[c] += (tch == c) ? g : 0.f;
-      }
-  }
-  // ---- last layer: bias gradient by warp sums; weight gradient  wbar_last[o] = sum_{c,p} ubar_c[p] H_c^{TL}[p][o]  on the
-  // tensor core: D_c[o][0..15] = H_c^T U with U[p] = (hi, lo) bf16 pairs of ubar_0..ubar_(C-1) (columns 2c, 2c+1) ------------
-  {
-    float* gb_last = partial + net.b_off[L - 1];
-    float* gw_last = partial + net.w_off[L - 1];
-    if (hh == 0) {
-      const float s = warp_sum<float>(ub[0]);
-      if (lane == 0) atomicAdd(gb_last, s);
-      uint32_t w[4];
-#pragma unroll
-      for (int c = 0; c < 4; ++c) w[c] = 0u;
-#pragma unroll
-      for (int c = 0; c < C; ++c) {
-        const uint32_t hi = tc::pack_bf16(ub[c], 0.f) & 0xffffu;
-        const float r = ub[c] - __uint_as_float(hi << 16);
-        w[c] = hi | (tc::pack_bf16(r, 0.f) << 16);
-      }
-      const uint32_t q0 = tc::smem_u32(tS);
-      asm volatile("st.shared.v4.b32 [%0], {%1,%2,%3,%4};" ::"r"(q0 + tc::swz_chunk(p, 0)), "r"(w[0]), "r"(w[1]), "r"(w[2]), "r"(w[3]) : "memory");
-      asm volatile("st.shared.v4.b32 [%0], {%1,%2,%3,%4};" ::"r"(q0 + tc::swz_chunk(p, 1)), "r"(0u), "r"(0u), "r"(0u), "r"(0u) : "memory");
-    }
-    tc::fence_async_smem();
-    __syncthreads();
-    {
-      const uint32_t sP = tc::smem_u32(tP);
-      const uint32_t idesc = tc::make_idesc(16, 1, 1);
-      const uint32_t a_lbo = (pi.nL > 64) ? TB : 0u;
-      const uint64_t db = tc::make_desc(tc::smem_u32(tS), 0, 1024);
-#pragma unroll 1
-      for (int c = 0; c < C; ++c)
-        mma_chain(accm + 16 * c, tc::make_desc(sP + c * 2 * TB, a_lbo, 1024), db, 2048, 2048, kTcPts / 16, idesc, 0);
-    }
-    __syncthreads();
-    if (hh == 0) {
-      const int o = q * 32 + lane;
-      float acc = 0.f;
-#pragma unroll
-      for (int c = 0; c < C; ++c) {
-        float v[2];
-        acc_ld2(accm + t.lane_addr + 16 * c + 2 * c, v);
-        acc += v[0] + v[1];
-      }
-      if (o < pi.nL) atomicAdd(gw_last + o, acc);
-    }
-    __syncthreads();
-  }
+  gather_ubar<C>(tm, slot, ms, p, ub);
+  // ---- last layer: the ubar tile goes to S0, the products into accumulator columns 0 .. 16C ---------------------------------
+  last_layer_grad<C>(t, ub, pi.nL, partial + net.w_off[L - 1], partial + net.b_off[L - 1], tc::smem_u32(tS), tc::smem_u32(tP),
+                     2 * TB, pi.nL > 64 ? TB : 0u, accm, kTwW);
 
   // ---- tensor layers, last to first ------------------------------------------------------------------------------------
   for (int l = TL; l >= 1; --l) {
@@ -466,11 +382,7 @@ __device__ __noinline__ void tw_net_backward(TwShared* cs, const DevProblem* Pp,
       if (C > 1) tw_load(cs, 1, tc::smem_u32(tS) + kTwImgBytes, h + 2 * TB, nb);
     }
     {
-      const int ng = n_out / 4;
-      LoopW lc;
-      lc.fp = tc::smem_u32(fp); lc.bt = lc.fp; lc.tP = tc::smem_u32(tP); lc.gb = gb;
-      lc.taddr = accm + t.lane_addr; lc.act = net.acts[l]; lc.p = p; lc.lane = lane;
-      lc.g0 = hh * (ng / kNH); lc.g1 = (hh + 1) * (ng / kNH); lc.flag = (l == TL) ? 1 : 0;
+      const LoopW lc(sfp, sfp, tc::smem_u32(tP), t, net.acts[l], n_out / 4, l == TL);
       const float2* zl = reinterpret_cast<const float2*>(zst + (size_t)(l - 1) * kTwMaxC * 64 * kTcPts * 2) + p;
       tw_bwd_loop<N1, N2, PURE, AK>(lc, pi.ch, ub, zl);
     }
@@ -521,25 +433,7 @@ __device__ __noinline__ void tw_net_backward(TwShared* cs, const DevProblem* Pp,
                   32, 2048, nk, idg, ob > 0 ? 1u : 0u);
       }
     }
-    // flush the weight-gradient accumulator: accumulator row = output neuron o, column = input neuron k
-    {
-      const int o = q * 32 + lane;
-      if (hh == 0) {
-        float v[2];
-        acc_ld2(accm + t.lane_addr + BC, v);
-        if (o < n_out) atomicAdd(gb + o, v[0]);
-      }
-      const int part = n_in / kNH;
-#pragma unroll 1
-      for (int k0 = hh * part; k0 < (hh + 1) * part; k0 += 4) {
-        float v[4];
-        acc_ld4(accm + t.lane_addr + WG + k0, v);
-        if (o < n_out) {
-#pragma unroll
-          for (int i = 0; i < 4; ++i) atomicAdd(gw + o + (long long)n_out * (k0 + i), v[i]);
-        }
-      }
-    }
+    flush_wgrad(t, accm + WG, accm + BC, kTwW, n_in, n_out, gw, gb);
     if (DEFER != 0) {
       // the remaining channels' adjoints land on the columns the weight / bias gradient just left
       __syncthreads();
@@ -563,66 +457,10 @@ __device__ __noinline__ void tw_net_backward(TwShared* cs, const DevProblem* Pp,
     float* gb0 = partial + net.b_off[0];
     float* gw0 = partial + net.w_off[0];
     constexpr bool kLo = (2 + N1) <= 4;         // a spare tile for the bf16 residual of the coordinates
-    if (tid < kTcPts) {
-      uint32_t hi[4], lo[4];
-#pragma unroll
-      for (int k = 0; k < 4; ++k) {
-        hi[k] = tc::pack_bf16(x[2 * k], x[2 * k + 1]);
-        lo[k] = tc::pack_bf16(x[2 * k] - __uint_as_float(hi[k] << 16), x[2 * k + 1] - __uint_as_float(hi[k] & 0xffff0000u));
-      }
-      const uint32_t q0 = tc::smem_u32(tS);
-      const uint32_t c0a = tc::swz_chunk(p, 0), c1a = tc::swz_chunk(p, 1);
-      asm volatile("st.shared.v4.b32 [%0], {%1,%2,%3,%4};" ::"r"(q0 + c0a), "r"(hi[0]), "r"(hi[1]), "r"(hi[2]), "r"(hi[3]) : "memory");
-      asm volatile("st.shared.v4.b32 [%0], {%1,%2,%3,%4};" ::"r"(q0 + c1a), "r"(0x00003f80u), "r"(0u), "r"(0u), "r"(0u) : "memory");
-      if (kLo) {
-        asm volatile("st.shared.v4.b32 [%0], {%1,%2,%3,%4};" ::"r"(q0 + (1 + N1) * TB + c0a), "r"(lo[0]), "r"(lo[1]), "r"(lo[2]), "r"(lo[3]) : "memory");
-        asm volatile("st.shared.v4.b32 [%0], {%1,%2,%3,%4};" ::"r"(q0 + (1 + N1) * TB + c1a), "r"(0u), "r"(0u), "r"(0u), "r"(0u) : "memory");
-      }
-#pragma unroll
-      for (int j = 0; j < N1; ++j) {
-        const int d = pi.dir1[j];
-        uint32_t w[4] = {0u, 0u, 0u, 0u};
-#pragma unroll
-        for (int k = 0; k < 4; ++k) w[k] = (d == 2 * k) ? 0x00003f80u : ((d == 2 * k + 1) ? 0x3f800000u : 0u);
-        const uint32_t qb = q0 + (1 + j) * TB;
-        asm volatile("st.shared.v4.b32 [%0], {%1,%2,%3,%4};" ::"r"(qb + c0a), "r"(w[0]), "r"(w[1]), "r"(w[2]), "r"(w[3]) : "memory");
-        asm volatile("st.shared.v4.b32 [%0], {%1,%2,%3,%4};" ::"r"(qb + c1a), "r"(0u), "r"(0u), "r"(0u), "r"(0u) : "memory");
-      }
-    }
-    {
-      const int ng = pi.n1w / 2;
-      LoopW lc;
-      lc.fp = tc::smem_u32(fp); lc.bt = lc.fp; lc.tP = tc::smem_u32(tP); lc.gb = gb0;
-      lc.taddr = accm + t.lane_addr; lc.act = net.acts[0]; lc.p = p; lc.lane = lane;
-      lc.g0 = hh * (ng / kNH); lc.g1 = (hh + 1) * (ng / kNH); lc.flag = 0;
-      tw_l0_bwd_store_loop<N1, N2, PURE, AK>(lc, pi, x);
-    }
-    tc::fence_async_smem();
-    __syncthreads();
-    {
-      const uint32_t sP = tc::smem_u32(tP), sS = tc::smem_u32(tS);
-      const uint32_t idesc = tc::make_idesc(16, 1, 1);
-      const uint32_t a_lbo = (pi.n1w > 64) ? TB : 0u;
-      const uint64_t a0 = tc::make_desc(sP, a_lbo, 1024);
-      mma_chain(accm + WG, a0, tc::make_desc(sS, 0, 1024), 2048, 2048, kTcPts / 16, idesc, 0);
-      if (kLo) mma_chain(accm + WG, a0, tc::make_desc(sS + (1 + N1) * TB, 0, 1024), 2048, 2048, kTcPts / 16, idesc, 1);
-#pragma unroll 1
-      for (int j = 0; j < N1; ++j)
-        mma_chain(accm + WG, tc::make_desc(sP + (1 + j) * 2 * TB, a_lbo, 1024), tc::make_desc(sS + (1 + j) * TB, 0, 1024),
-                  2048, 2048, kTcPts / 16, idesc, 1);
-    }
-    __syncthreads();
-    if (hh == 0) {
-      const int o = q * 32 + lane;
-      float v[16];
-      tc::acc_ld16(accm + t.lane_addr + WG, v);
-      if (o < pi.n1w) {
-#pragma unroll
-        for (int k = 0; k < PINN_MAX_IN; ++k)
-          if (k < pi.d_in) atomicAdd(gw0 + o + (long long)pi.n1w * k, v[k]);
-        atomicAdd(gb0 + o, v[8]);
-      }
-    }
+    const uint32_t sP = tc::smem_u32(tP), sS = tc::smem_u32(tS);
+    coord_tiles<N1>(t, sS, x, pi.dir1, kLo);
+    tw_l0_bwd_store_loop<N1, N2, PURE, AK>(LoopW(sfp, sfp, sP, t, net.acts[0], pi.n1w / 2, 0), pi, x);
+    layer0_grad<N1>(t, sP, 2 * TB, pi.n1w > 64 ? TB : 0u, sS, kLo, accm + WG, kTwW, pi.n1w, pi.d_in, gw0, gb0);
   }
   __syncthreads();
   dbg_mark(cs, 30);
@@ -672,21 +510,12 @@ __global__ void __launch_bounds__(kTcThreads, 1) tw_loss_grad_kernel(const __gri
       cs.ph_ld[b] = 0;
     }
     tc::fence_barrier_init();
-    cs.tl_max = args.tl_max; cs.off_P = args.off_P; cs.off_S = args.off_S; cs.off_misc = args.off_misc; cs.off_ones = args.off_ones; cs.off_nets = args.off_nets; cs.mx_dim = args.mx_dim; cs.mx_taps = args.mx_taps;
-    cs.partial = partial;
+    cs.off_S = args.off_S; cs.off_nets = args.off_nets;
     cs.hstash = args.hstash + (long long)blockIdx.x * args.hstash_per_cta;
     cs.zstash = args.zstash + (long long)blockIdx.x * args.zstash_per_cta;
-    cs.theta = theta; cs.wpack = args.wpack;
-#ifdef PINN_DEBUG
-    cs.dbg = (blockIdx.x == 0) ? args.dbg : nullptr;
-#else
-    cs.dbg = nullptr;
-#endif
-    cs.dbg_n = 0;
+    cs.wpack = args.wpack;
     for (int k = 0; k < PINN_MAX_NETS; ++k) { cs.off_fp[k] = args.off_fp[k]; cs.wimg[k] = args.wimg[k]; }
-#ifdef PINN_DEBUG
-    if (cs.dbg) cs.dbg[cs.dbg_n++] = ((long long)1 << 48) | (clock64() & 0xffffffffffffLL);
-#endif
+    cta_base_init(cs, args, partial);
   }
   if (tid == 0) tc::s_acc = args.acc + (size_t)blockIdx.x * kAccCols * kAccRows;
   cta_setup(args, ms, partial, P.n_theta, want_grad);
