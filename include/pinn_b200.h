@@ -302,6 +302,47 @@ int pinn_qn_iterate(pinn_handle h, int32_t n_iters, double* host_f, double* host
 /* current theta rounded to the engine dtype */
 int pinn_qn_theta(pinn_handle h, void* host_theta_out);
 
+/* ---- device-resident HMC sampler (BayesianPINN posteriors) --------------------------------------------------------
+ * Samples the log density l(theta) = sum_k w_k L_k(theta) + ll_const + log N(theta; prior_mean, prior_std^2 I), where
+ * L_k are the engine's term losses and w_k the host weights (for a BayesianPINN: w_k = -W n_k / (2 sigma_k^2) and
+ * ll_const the Gaussian normalisation, so that the first two parts are full_loss_function(theta, allstd)).
+ * Hamiltonian Monte Carlo with a fixed number of leapfrog steps and end-point Metropolis acceptance, with AdvancedHMC's
+ * defaults: find_good_stepsize for the initial step size, Nesterov dual averaging of the step size (gamma 0.05, t0 10,
+ * kappa 0.75) and Stan's windowed diagonal mass-matrix adaptation (buffers 75 / 25 / 50) over the first n_adapts
+ * transitions.  theta, the momentum, the gradient, M^-1 and the adaptation state are float64 on the device for both
+ * engine dtypes; the fused kernel sees theta rounded to the engine dtype.  One transition is a fixed launch sequence with
+ * no host decision, captured once into a CUDA graph (PINN_B200_NO_GRAPH=1: enqueued directly).  Random numbers are
+ * Philox4x32-10 draws keyed by (seed, transition, index, stream), so two runs with one seed are bit-identical.
+ * Single-GPU handles with fixed point sets only (no device sampler, nranks == 1). */
+enum { PINN_HMC_ADAPT_NONE = 0, PINN_HMC_ADAPT_STAN = 1 };
+enum { PINN_HMC_METRIC_UNIT = 0, PINN_HMC_METRIC_DIAG = 1 };
+/* columns of one statistics row of pinn_hmc_iterate */
+enum {
+  PINN_HMC_STAT_STEP_SIZE = 0, PINN_HMC_STAT_ACCEPTANCE_RATE = 1, PINN_HMC_STAT_IS_ACCEPT = 2,
+  PINN_HMC_STAT_LOG_DENSITY = 3, PINN_HMC_STAT_HAMILTONIAN_ENERGY = 4, PINN_HMC_STAT_HAMILTONIAN_ENERGY_ERROR = 5,
+  PINN_HMC_STAT_NUMERICAL_ERROR = 6, PINN_HMC_STAT_IS_ADAPT = 7, PINN_HMC_N_STATS = 8
+};
+typedef struct {
+  int32_t n_leapfrog;        /* leapfrog steps per transition (HMC(0.1, 30): 30), >= 1                     */
+  int32_t adaptor;           /* PINN_HMC_ADAPT_*                                                          */
+  int32_t metric;            /* PINN_HMC_METRIC_*                                                         */
+  int32_t n_adapts;          /* transitions 1..n_adapts adapt (AdvancedHMC: min(draws / 10, 1000)), >= 0  */
+  double target_accept;      /* dual-averaging target acceptance rate delta, in (0, 1)                    */
+  double step_size;          /* initial step size; <= 0: find_good_stepsize                               */
+  double prior_mean, prior_std;   /* Normal prior of every parameter; prior_std > 0                       */
+  uint64_t seed;
+} pinn_hmc_options;
+/* Start a chain at host_theta0 (float64 [n_theta]): allocates the state, evaluates l and its gradient there and, when
+ * opts->step_size <= 0, runs find_good_stepsize (one synchronisation per trial).  host_weights [n_terms] (nullable:
+ * all 1) and ll_const stay fixed for the chain.  *step_size_out (nullable): the initial step size. */
+int pinn_hmc_begin(pinn_handle h, const double* host_theta0, const pinn_hmc_options* opts, const double* host_weights,
+                   double ll_const, double* step_size_out);
+/* Run n transitions: host_samples [n][n_theta] float64 (theta after each transition) and host_stats
+ * [n][PINN_HMC_N_STATS] (each nullable).  The chain continues across calls. */
+int pinn_hmc_iterate(pinn_handle h, int32_t n, double* host_samples, double* host_stats);
+/* the chain's current theta (float64 [n_theta]) */
+int pinn_hmc_theta(pinn_handle h, double* host_theta_out);
+
 /* ---- multi-GPU -------------------------------------------------------------------- */
 /* Attach an NCCL communicator built from a 128-byte ncclUniqueId that the caller
  * distributed (rank 0 obtains it from pinn_comm_unique_id). */

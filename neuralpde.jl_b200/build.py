@@ -30,6 +30,7 @@ UNITS = [
     ("pinn_abi.o", "pinn_abi.cu", []),
     ("plan.o", "plan.cu", []),
     ("qn.o", "qn.cu", []),
+    ("hmc.o", "hmc.cu", []),
     ("ffma_launch.o", "ffma_launch.cu", []),
     ("ffma_f32_smem.o", "ffma_inst.cu", ["-DPINN_INST_REAL=float", "-DPINN_INST_BUFS=1"]),
     ("ffma_f32_gmem.o", "ffma_inst.cu", ["-DPINN_INST_REAL=float", "-DPINN_INST_BUFS=0"]),

@@ -1,4 +1,5 @@
-// engine.h -- the handle behind pinn_handle and the host helpers the C-ABI translation units share (pinn_abi.cu, qn.cu).
+// engine.h -- the handle behind pinn_handle and the host helpers the C-ABI translation units share (pinn_abi.cu, qn.cu,
+// hmc.cu).
 #pragma once
 #include <cuda_runtime.h>
 
@@ -26,6 +27,7 @@ struct TermState {
 };
 
 struct QnState;   // quasi-Newton driver state (qn.cu)
+struct HmcState;  // HMC sampler state (hmc.cu)
 
 }  // namespace pinn
 
@@ -67,6 +69,8 @@ struct pinn_engine {
   unsigned long long sampler_draw = 0;
   // device-resident quasi-Newton state (pinn_qn_begin)
   pinn::QnState* qn = nullptr;
+  // device-resident HMC sampler state (pinn_hmc_begin)
+  pinn::HmcState* hmc = nullptr;
   // fused kernel tail (tail.cuh): device-resident barrier / step state
   pinn::TailState* d_state = nullptr;
   unsigned long long tail_timeout_ns = 20ull * 1000000000ull;
@@ -99,4 +103,6 @@ int eval_step(pinn_engine* e, const void* theta, const double* host_weights, voi
               void* out_total, bool adam, cudaStream_t st);
 // frees the quasi-Newton state (qn.cu); called by pinn_destroy and by a repeated pinn_qn_begin
 void qn_release(pinn_engine* e);
+// frees the HMC sampler state and its graph (hmc.cu); called by pinn_destroy and by a repeated pinn_hmc_begin
+void hmc_release(pinn_engine* e);
 }  // namespace pinn

@@ -2,6 +2,7 @@
 // allreduced [grad | term losses]), the gradient statistics kernel and the device-side point samplers.
 #include <cuda_runtime.h>
 #include "dev_types.h"
+#include "philox.cuh"
 
 namespace pinn {
 
@@ -84,18 +85,8 @@ __global__ void __launch_bounds__(1024) grad_stats_kernel(const real* g, long lo
 }
 
 // ---- device-side StochasticTraining sampler ---------------------------------------------------------------------------
-// Philox4x32-10 (Salmon et al., SC'11): counter = (point index, group of 4 rows, draw), key = seed.  One thread per point
+// Philox4x32-10 (philox.cuh): counter = (point index, group of 4 rows, draw), key = seed.  One thread per point
 // writes its `dim` coordinates lb_r + (ub_r - lb_r) * u, u uniform in [0, 1) from the high 24 (float) / 53 (double) bits.
-__device__ __forceinline__ void philox4x32_10(uint32_t (&c)[4], uint32_t k0, uint32_t k1) {
-#pragma unroll
-  for (int r = 0; r < 10; ++r) {
-    const uint32_t hi0 = __umulhi(0xD2511F53u, c[0]), lo0 = 0xD2511F53u * c[0];
-    const uint32_t hi1 = __umulhi(0xCD9E8D57u, c[2]), lo1 = 0xCD9E8D57u * c[2];
-    const uint32_t n0 = hi1 ^ c[1] ^ k0, n1 = lo1, n2 = hi0 ^ c[3] ^ k1, n3 = lo0;
-    c[0] = n0; c[1] = n1; c[2] = n2; c[3] = n3;
-    k0 += 0x9E3779B9u; k1 += 0xBB67AE85u;
-  }
-}
 
 struct SampleBox { double lb[PINN_MAX_DIM], ub[PINN_MAX_DIM]; };
 

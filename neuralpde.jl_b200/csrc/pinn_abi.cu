@@ -1,6 +1,7 @@
 // pinn_abi.cu -- host side of the C ABI declared in include/pinn_b200.h: workspace ownership, kernel
 // launch sequencing, host-buffer staging and the optional NCCL gradient allreduce.  Descriptor
-// validation and lowering live in the planner (plan.cu), the handle struct in engine.h, the quasi-Newton driver in qn.cu.
+// validation and lowering live in the planner (plan.cu), the handle struct in engine.h, the quasi-Newton driver in qn.cu, the HMC sampler in
+// hmc.cu.
 #include <cuda_runtime.h>
 #include <dlfcn.h>
 #include <math.h>
@@ -122,6 +123,7 @@ int pinn_destroy(pinn_handle e) {
   cudaSetDevice(e->device);
   if (e->adam_graph) cudaGraphExecDestroy(e->adam_graph);
   qn_release(e);
+  hmc_release(e);
   if (e->p2p) {
     // peers may still be reading this rank's symmetric buffers inside their last step: callers synchronise the ranks
     // (any collective / barrier) before destroying handles; here only this device is drained

@@ -14,6 +14,7 @@
 
 #include "engine.h"
 #include "linesearch.h"
+#include "reduce.cuh"
 
 namespace pinn {
 namespace {
@@ -44,24 +45,6 @@ struct QnCombine {
   double p[kMaxM], q[kMaxM];
 };
 
-__device__ __forceinline__ double nan_max(double a, double b) { return (isnan(a) || a >= b) ? a : b; }
-
-// fixed-order block reduction; the result is valid in thread 0
-template <bool kMax>
-__device__ double block_reduce(double v) {
-  __shared__ double warp_part[kQnThreads / 32];
-  for (int o = 16; o; o >>= 1) {
-    const double u = __shfl_xor_sync(0xffffffffu, v, o);
-    v = kMax ? nan_max(v, u) : v + u;
-  }
-  if ((threadIdx.x & 31) == 0) warp_part[threadIdx.x >> 5] = v;
-  __syncthreads();
-  double r = warp_part[0];
-  if (threadIdx.x == 0)
-    for (int w = 1; w < kQnThreads / 32; ++w) r = kMax ? nan_max(r, warp_part[w]) : r + warp_part[w];
-  return r;
-}
-
 // grid (chunks, items): part[chunk][item]
 __global__ void __launch_bounds__(kQnThreads) qn_multidot_kernel(QnItems it, long long n, double* part) {
   const int j = blockIdx.y;
@@ -71,10 +54,10 @@ __global__ void __launch_bounds__(kQnThreads) qn_multidot_kernel(QnItems it, lon
   double acc = 0.0;
   if (b) {
     for (long long i = lo + threadIdx.x; i < hi; i += kQnThreads) acc = fma(a[i], b[i], acc);
-    acc = block_reduce<false>(acc);
+    acc = block_reduce<kQnThreads, false>(acc);
   } else {
     for (long long i = lo + threadIdx.x; i < hi; i += kQnThreads) acc = nan_max(acc, fabs(a[i]));
-    acc = block_reduce<true>(acc);
+    acc = block_reduce<kQnThreads, true>(acc);
   }
   if (threadIdx.x == 0) part[(size_t)blockIdx.x * it.n + j] = acc;
 }
@@ -116,7 +99,7 @@ __global__ void __launch_bounds__(kQnThreads) qn_dot_kernel(const real* g, const
   const long long lo = (long long)blockIdx.x * kChunk, hi = min(n, lo + kChunk);
   double acc = 0.0;
   for (long long i = lo + threadIdx.x; i < hi; i += kQnThreads) acc = fma((double)g[i], d[i], acc);
-  acc = block_reduce<false>(acc);
+  acc = block_reduce<kQnThreads, false>(acc);
   if (threadIdx.x == 0) part[blockIdx.x] = acc;
 }
 
@@ -158,7 +141,7 @@ __global__ void __launch_bounds__(kQnThreads) qn_combine_kernel(QnCombine c, con
     d[i] = -v;
     acc = fma(gi, -v, acc);
   }
-  acc = block_reduce<false>(acc);
+  acc = block_reduce<kQnThreads, false>(acc);
   if (threadIdx.x == 0) part[blockIdx.x] = acc;
 }
 

@@ -38,12 +38,19 @@ EXPORTS = [
     "pinn_flops_per_eval", "pinn_adam_begin", "pinn_adam_iterate", "pinn_adam_theta",
     "pinn_term_grad_stats", "pinn_term_grad_stats_host", "pinn_set_sampler", "pinn_resample", "pinn_get_points_host",
     "pinn_comm_info", "pinn_set_sampler_ex", "pinn_qn_begin", "pinn_qn_iterate", "pinn_qn_theta",
+    "pinn_hmc_begin", "pinn_hmc_iterate", "pinn_hmc_theta",
 ]
 
 # quasi-Newton optimizer / line search kinds and run states (pinn_qn_options, pinn_qn_iterate)
 QN_LBFGS, QN_BFGS = 0, 1
 LS_HAGERZHANG, LS_BACKTRACKING = 0, 1
 QN_RUNNING, QN_CONVERGED, QN_LS_FAILED = 0, 1, 2
+
+# HMC adaptor / metric kinds (pinn_hmc_options) and the statistics columns of pinn_hmc_iterate
+HMC_ADAPT_NONE, HMC_ADAPT_STAN = 0, 1
+HMC_METRIC_UNIT, HMC_METRIC_DIAG = 0, 1
+HMC_STATS = ("step_size", "acceptance_rate", "is_accept", "log_density", "hamiltonian_energy",
+             "hamiltonian_energy_error", "numerical_error", "is_adapt")
 
 
 class EngineError(RuntimeError):
@@ -57,6 +64,12 @@ class _Instr(C.Structure):
 class _QnOptions(C.Structure):
     _fields_ = [("kind", C.c_int32), ("m", C.c_int32), ("linesearch", C.c_int32), ("_pad", C.c_int32),
                 ("initial_stepnorm", C.c_double)]
+
+
+class _HmcOptions(C.Structure):
+    _fields_ = [("n_leapfrog", C.c_int32), ("adaptor", C.c_int32), ("metric", C.c_int32), ("n_adapts", C.c_int32),
+                ("target_accept", C.c_double), ("step_size", C.c_double), ("prior_mean", C.c_double),
+                ("prior_std", C.c_double), ("seed", C.c_uint64)]
 
 
 class _NetDesc(C.Structure):
@@ -200,6 +213,12 @@ def load_library():
     lib.pinn_qn_iterate.restype = C.c_int
     lib.pinn_qn_theta.argtypes = [vp, vp]
     lib.pinn_qn_theta.restype = C.c_int
+    lib.pinn_hmc_begin.argtypes = [vp, C.POINTER(dbl), C.POINTER(_HmcOptions), C.POINTER(dbl), dbl, C.POINTER(dbl)]
+    lib.pinn_hmc_begin.restype = C.c_int
+    lib.pinn_hmc_iterate.argtypes = [vp, i32, C.POINTER(dbl), C.POINTER(dbl)]
+    lib.pinn_hmc_iterate.restype = C.c_int
+    lib.pinn_hmc_theta.argtypes = [vp, C.POINTER(dbl)]
+    lib.pinn_hmc_theta.restype = C.c_int
     _lib = lib
     return lib
 
@@ -437,6 +456,38 @@ class Engine:
     def qn_theta(self) -> np.ndarray:
         th = np.empty(self.n_theta, dtype=self.np_dtype)
         _check(self.lib.pinn_qn_theta(self._h, _ptr(th)))
+        return th
+
+    # -- device-resident HMC sampler ------------------------------------------------------------------------
+    def hmc_begin(self, theta0: np.ndarray, n_leapfrog: int = 30, adaptor: int = HMC_ADAPT_STAN,
+                  metric: int = HMC_METRIC_DIAG, n_adapts: int = 0, target_accept: float = 0.8, step_size: float = 0.0,
+                  prior_mean: float = 0.0, prior_std: float = 1.0, seed: int = 0, weights=None,
+                  ll_const: float = 0.0) -> float:
+        """Start a chain at theta0 (float64) for the log density sum_k w_k L_k + ll_const + log N(theta; prior);
+        step_size <= 0 runs find_good_stepsize.  Returns the initial step size."""
+        th = np.ascontiguousarray(theta0, dtype=np.float64)
+        if th.shape != (self.n_theta,):
+            raise ValueError("theta must have length %d" % self.n_theta)
+        opt = _HmcOptions(int(n_leapfrog), int(adaptor), int(metric), int(n_adapts), float(target_accept),
+                          float(step_size), float(prior_mean), float(prior_std), int(seed) & (2 ** 64 - 1))
+        w = self._weights(weights)
+        wp = w.ctypes.data_as(C.POINTER(C.c_double)) if w is not None else None
+        eps = C.c_double(0.0)
+        _check(self.lib.pinn_hmc_begin(self._h, th.ctypes.data_as(C.POINTER(C.c_double)), C.byref(opt), wp,
+                                       float(ll_const), C.byref(eps)))
+        return float(eps.value)
+
+    def hmc_iterate(self, n: int):
+        """n transitions: (samples [n, n_theta] float64, stats [n, 8] with the columns of HMC_STATS)."""
+        samples = np.empty((int(n), self.n_theta), dtype=np.float64)
+        stats = np.empty((int(n), len(HMC_STATS)), dtype=np.float64)
+        dp = C.POINTER(C.c_double)
+        _check(self.lib.pinn_hmc_iterate(self._h, int(n), samples.ctypes.data_as(dp), stats.ctypes.data_as(dp)))
+        return samples, stats
+
+    def hmc_theta(self) -> np.ndarray:
+        th = np.empty(self.n_theta, dtype=np.float64)
+        _check(self.lib.pinn_hmc_theta(self._h, th.ctypes.data_as(C.POINTER(C.c_double))))
         return th
 
     # -- multi-GPU --------------------------------------------------------------------------------

@@ -16,7 +16,7 @@ from . import engine as _eng
 from .engine import Engine, EngineError, NetSpec, ProblemSpec, TapSpec, TermSpec, REDUCE_MEAN, REDUCE_WSUM
 from .lowering import LoweredTerm, LoweringError, lower_equation, term_spec
 from .strategies import (AbstractTrainingStrategy, GridTraining, QuadratureTraining, QuasiRandomTraining,
-                         StochasticTraining, gauss_legendre_box, generate_quasi_random_points,
+                         StochasticTraining, _julia_range, _product_columns, gauss_legendre_box, generate_quasi_random_points,
                          generate_random_points, generate_training_sets, get_bounds, shard_range)
 from .symbolic import Equation, PDESystem, VarInfo, get_vars
 
@@ -365,8 +365,8 @@ class PhysicsInformedNN(AbstractPINN):
 class BayesianPINN(AbstractPINN):
     """``BayesianPINN(args...; dataset = nothing, kwargs...)`` (reference src/pinn_types.jl:214-245): wraps a
     PhysicsInformedNN; ``symbolic_discretize`` then builds ``full_loss_function(θ, allstd)`` = the weighted
-    log-likelihood (src/discretize.jl:653-757) that the HMC samplers of ext/bpinn consume.  The sampler itself is out of
-    scope; the likelihood and its θ-gradient come from the same fused kernel."""
+    log-likelihood (src/discretize.jl:653-757) that the HMC samplers of ext/bpinn consume; ``ahmc_bayesian_pinn_pde``
+    samples its posterior on the device.  The likelihood and its θ-gradient come from the same fused kernel."""
 
     def __init__(self, *args, dataset=None, **kwargs):
         self.pinn = PhysicsInformedNN(*args, **kwargs)
@@ -767,14 +767,11 @@ def symbolic_discretize(pde_system: PDESystem, discretization: PhysicsInformedNN
         # -W n / (2 sigma^2).  As in the reference the per-group log-likelihoods are SUMMED before the weight vector
         # multiplies them (:682-738): every weight of a group scales the whole group sum.
         n_k = np.array([point_sets[i].shape[1] for i in range(n_pde + n_bc)], dtype=np.float64)
+        rep.loglik_weights = lambda allstd: _loglik_weights(weights, n_k, n_pde, allstd)
 
         def _loglik(theta, allstd, want_grad):
             stdpdes, stdbcs, stdextra = allstd
-            sig = np.concatenate([np.asarray(stdpdes, dtype=np.float64), np.asarray(stdbcs, dtype=np.float64)])
-            if sig.shape != (n_pde + n_bc,):
-                raise ValueError("allstd: need %d pde and %d bc standard deviations" % (n_pde, n_bc))
-            Wg = np.concatenate([np.full(n_pde, weights["pde"].sum()), np.full(n_bc, weights["bc"].sum())])
-            c = -Wg * n_k / (2.0 * sig ** 2)
+            c, const = rep.loglik_weights(allstd)
             th = np.asarray(theta, dtype=dtype)
             has_add = isinstance(add, DataLoss)
             if has_add:
@@ -784,7 +781,6 @@ def symbolic_discretize(pde_system: PDESystem, discretization: PhysicsInformedNN
             else:
                 c_all = c
             total, terms, grad = eng.loss_grad_host(th, c_all, want_grad)
-            const = float(np.sum(Wg * (-0.5 * n_k * np.log(2.0 * np.pi) - n_k * np.log(sig))))
             ll = const + float(np.dot(c, np.asarray(terms[:n_pde + n_bc], dtype=np.float64)))
             if has_add:
                 s_e = float(stdextra)
@@ -796,6 +792,21 @@ def symbolic_discretize(pde_system: PDESystem, discretization: PhysicsInformedNN
         lf.full_loss_function = lambda theta, allstd: _loglik(theta, allstd, False)[0]
         lf.full_loss_gradient = lambda theta, allstd: _loglik(theta, allstd, True)
     return rep
+
+
+def _loglik_weights(weights, n_k: np.ndarray, n_pde: int, allstd):
+    """Per-term weights c_k = -W n_k / (2 σ_k²) and the constant Σ W (-n_k/2 log 2π - n_k log σ_k) of the BayesianPINN
+    log-likelihood Σ_k c_k L_k + const, L_k = mean(abs2, r_k) (src/training_strategies.jl:115-128; every weight of a
+    group scales the whole group sum, src/discretize.jl:682-738)."""
+    stdpdes, stdbcs = allstd[0], allstd[1]
+    n_bc = n_k.size - n_pde
+    sig = np.concatenate([np.asarray(stdpdes, dtype=np.float64), np.asarray(stdbcs, dtype=np.float64)])
+    if sig.shape != (n_pde + n_bc,):
+        raise ValueError("allstd: need %d pde and %d bc standard deviations" % (n_pde, n_bc))
+    Wg = np.concatenate([np.full(n_pde, weights["pde"].sum()), np.full(n_bc, weights["bc"].sum())])
+    c = -Wg * n_k / (2.0 * sig ** 2)
+    const = float(np.sum(Wg * (-0.5 * n_k * np.log(2.0 * np.pi) - n_k * np.log(sig))))
+    return c, const
 
 
 @dataclass
@@ -952,3 +963,143 @@ def solve(prob: OptimizationProblem, opt: Union[Adam, LBFGS, BFGS], maxiters: in
         if callback is not None and callback({"iter": it, "u": u}, obj):
             break
     return Solution(u.astype(prob.u0.dtype), obj, it)
+
+
+# ---- Bayesian PINN sampling (reference ext/bpinn/PDE_BPINN.jl) --------------------------------------------------------
+@dataclass
+class HMC:
+    """``AdvancedHMC.HMC(ϵ, n_leapfrog)``: fixed-length trajectories.  As in the reference, ``ϵ`` is not used: the
+    initial step size comes from ``find_good_stepsize``."""
+    step_size: float = 0.1
+    n_leapfrog: int = 30
+
+
+class StanHMCAdaptor:
+    """``Adaptor = StanHMCAdaptor``: dual averaging of the step size and Stan's windowed mass-matrix estimate."""
+
+
+class NoAdaptation:
+    """``Adaptor = NoAdaptation``: step size and metric stay as found."""
+
+
+class DiagEuclideanMetric:
+    """``Metric = DiagEuclideanMetric``: diagonal M⁻¹, adapted by the Stan adaptor."""
+
+
+class UnitEuclideanMetric:
+    """``Metric = UnitEuclideanMetric``: M = I."""
+
+
+class Leapfrog:
+    """``Integrator = Leapfrog``."""
+
+
+@dataclass
+class BPINNstats:
+    """``BPINNstats(mcmc_chain, samples, statistics)``: ``chain`` / ``samples`` are the [draw_samples, n_θ] draws,
+    ``statistics`` maps each AdvancedHMC statistic (step_size, acceptance_rate, is_accept, log_density,
+    hamiltonian_energy, hamiltonian_energy_error, numerical_error, is_adapt) to its [draw_samples] values."""
+    chain: np.ndarray
+    samples: np.ndarray
+    statistics: Dict[str, np.ndarray]
+
+
+@dataclass
+class BPINNsolution:
+    """``BPINNsolution(original, ensemblesol, estimated_nn_params, estimated_de_params, timepoints)``:
+    ``ensemblesol[k]`` is φ_k on ``timepoints[k]`` ((d_k, n_points), first input fastest) for each of the last
+    ``numensemble + 1`` samples, an array [numensemble + 1, n_points]; ``estimated_nn_params[k]`` holds network k's
+    parameters in those samples."""
+    original: BPINNstats
+    ensemblesol: List[np.ndarray]
+    estimated_nn_params: List[np.ndarray]
+    estimated_de_params: list
+    timepoints: List[np.ndarray]
+
+
+def pmean(x) -> np.ndarray:
+    """MonteCarloMeasurements' ``pmean``: the mean over samples (axis 0) of an ensemble array."""
+    return np.mean(np.asarray(x, dtype=np.float64), axis=0)
+
+
+_DEFAULT_ADAPTOR = {"Adaptor": StanHMCAdaptor, "Metric": DiagEuclideanMetric, "targetacceptancerate": 0.8}
+
+
+def ahmc_bayesian_pinn_pde(pde_system: PDESystem, discretization: BayesianPINN, *, draw_samples: int = 1000,
+                           bcstd=(0.01,), l2std=(0.05,), phystd=(0.05,), phynewstd=(0.05,), priorsNNw=(0.0, 2.0),
+                           param=(), nchains: int = 1, Kernel=None, Adaptorkwargs=None, Integratorkwargs=None,
+                           saveats=(1 / 10,), numensemble: Optional[int] = None, Dict_differentials=None,
+                           progress: bool = False, verbose: bool = False, seed: int = 0) -> BPINNsolution:
+    """``ahmc_bayesian_pinn_pde(pde_system, discretization; draw_samples, bcstd, phystd, priorsNNw, saveats, ...)``
+    (reference ext/bpinn/PDE_BPINN.jl:371-635): Hamiltonian Monte Carlo over the network parameters of a BayesianPINN,
+    target ``full_loss_function(θ, [phystd, bcstd, l2std]) + log N(θ; μ_p, σ_p² I)`` with ``priorsNNw = (μ_p, σ_p)``.
+
+    Defaults as the reference: ``HMC(0.1, 30)`` started at ``find_good_stepsize``, Stan adaptation (dual averaging to
+    acceptance 0.8, diagonal mass matrix) over the first ``min(draw_samples ÷ 10, 1000)`` transitions, warm-up samples
+    kept.  The chain runs on the device (``pinn_hmc_*``); ``seed`` keys its Philox streams (the reference uses the global
+    RNG).  ``l2std`` / ``phynewstd`` are accepted and unused: without a dataset the reference does not use them either.
+    Not supported (refused with a message): NUTS / HMCDA kernels, ``DenseEuclideanMetric``, jittered / tempered
+    leapfrog, several chains, parameter estimation, ``Dict_differentials`` and an ``additional_loss``."""
+    Kernel = HMC() if Kernel is None else Kernel
+    ak = dict(_DEFAULT_ADAPTOR, **(Adaptorkwargs or {}))
+    ik = dict({"Integrator": Leapfrog}, **(Integratorkwargs or {}))
+    if not isinstance(Kernel, HMC):
+        raise ValueError("ahmc_bayesian_pinn_pde: Kernel %r is not implemented; the device sampler runs HMC(ϵ, n_leapfrog) "
+                         "(NUTS and HMCDA are not supported)" % (Kernel,))
+    if ak["Adaptor"] not in (StanHMCAdaptor, NoAdaptation):
+        raise ValueError("ahmc_bayesian_pinn_pde: Adaptor %r is not implemented (StanHMCAdaptor or NoAdaptation)"
+                         % (ak["Adaptor"],))
+    if ak["Metric"] not in (DiagEuclideanMetric, UnitEuclideanMetric):
+        raise ValueError("ahmc_bayesian_pinn_pde: Metric %r is not implemented; DenseEuclideanMetric is not supported "
+                         "(DiagEuclideanMetric or UnitEuclideanMetric)" % (ak["Metric"],))
+    if ik["Integrator"] is not Leapfrog:
+        raise ValueError("ahmc_bayesian_pinn_pde: Integrator %r is not implemented; JitteredLeapfrog / TemperedLeapfrog "
+                         "are not supported (Leapfrog)" % (ik["Integrator"],))
+    if nchains != 1:
+        raise ValueError("ahmc_bayesian_pinn_pde: nchains = %r; one chain per call is supported" % (nchains,))
+    if not isinstance(discretization, BayesianPINN):
+        raise TypeError("ahmc_bayesian_pinn_pde: expected a BayesianPINN discretization")
+    if discretization.pinn.param_estim or len(param) > 0:
+        raise ValueError("ahmc_bayesian_pinn_pde: parameter estimation (param_estim / param) needs a dataset, which is "
+                         "not supported (reference ext/bpinn/PDE_BPINN.jl:454-460)")
+    if Dict_differentials is not None:
+        raise ValueError("ahmc_bayesian_pinn_pde: Dict_differentials (the data-collocation loss) is not supported")
+    if discretization.pinn.additional_loss is not None:
+        raise ValueError("ahmc_bayesian_pinn_pde: an additional_loss enters the log-likelihood with a weight that depends "
+                         "on its value, two evaluations per gradient; the device sampler does not support it")
+    rep = symbolic_discretize(pde_system, discretization)
+    if len(rep.domains) != len(saveats):
+        raise ValueError("Number of independent variables must match saveat inference discretization steps")
+    draw_samples = int(draw_samples)
+    numensemble = int(np.floor(draw_samples / 3)) if numensemble is None else int(numensemble)
+    if draw_samples < 1 or not 0 <= numensemble < draw_samples:
+        raise ValueError("ahmc_bayesian_pinn_pde: need draw_samples >= 1 and 0 <= numensemble < draw_samples")
+    c, const = rep.loglik_weights([phystd, bcstd, l2std])
+    mu_p, sd_p = float(priorsNNw[0]), float(priorsNNw[1])
+    n_adapts = min(draw_samples // 10, 1000)
+    eng = rep.engine
+    theta0 = np.asarray(rep.flat_init_params, dtype=np.float64)
+    eps0 = eng.hmc_begin(theta0, n_leapfrog=Kernel.n_leapfrog,
+                         adaptor=_eng.HMC_ADAPT_STAN if ak["Adaptor"] is StanHMCAdaptor else _eng.HMC_ADAPT_NONE,
+                         metric=_eng.HMC_METRIC_DIAG if ak["Metric"] is DiagEuclideanMetric else _eng.HMC_METRIC_UNIT,
+                         n_adapts=n_adapts, target_accept=float(ak["targetacceptancerate"]), step_size=0.0,
+                         prior_mean=mu_p, prior_std=sd_p, seed=seed, weights=c, ll_const=const)
+    if verbose:
+        print("Initial step size %g; current physics log-likelihood %g"
+              % (eps0, rep.loss_functions.full_loss_function(theta0, [phystd, bcstd, l2std])))
+    samples, st = eng.hmc_iterate(draw_samples)
+    statistics = {name: st[:, j].copy() for j, name in enumerate(_eng.HMC_STATS)}
+    if verbose:
+        print("Sampling complete: acceptance rate %.3f" % float(np.mean(statistics["acceptance_rate"])))
+
+    # inference (PDE_BPINN.jl:222-312): the last numensemble + 1 samples on the saveat grid of each network's inputs
+    kept = samples[draw_samples - numensemble - 1:]
+    ranges = {str(dm.variables): _julia_range(dm.domain.lo, float(h), dm.domain.hi) for dm, h in zip(rep.domains, saveats)}
+    phis = rep.phi if rep.multioutput else [rep.phi]
+    timepoints, ensemble, nn_params = [], [], []
+    for name, ph in zip(rep.depvars, phis):
+        tp = _product_columns([ranges[v] for v in rep.dict_depvar_input[name]])
+        timepoints.append(tp)
+        ensemble.append(np.stack([np.asarray(ph(tp, th), dtype=np.float64).reshape(-1) for th in kept]))
+        nn_params.append(kept[:, ph.theta_offset:ph.theta_offset + ph.chain.n_params].copy())
+    return BPINNsolution(BPINNstats(samples, samples, statistics), ensemble, nn_params, [None], timepoints)
