@@ -305,7 +305,8 @@ int pinn_qn_theta(pinn_handle h, void* host_theta_out);
 /* ---- device-resident HMC sampler (BayesianPINN posteriors) --------------------------------------------------------
  * Samples the log density l(theta) = sum_k w_k L_k(theta) + ll_const + log N(theta; prior_mean, prior_std^2 I), where
  * L_k are the engine's term losses and w_k the host weights (for a BayesianPINN: w_k = -W n_k / (2 sigma_k^2) and
- * ll_const the Gaussian normalisation, so that the first two parts are full_loss_function(theta, allstd)).
+ * ll_const the Gaussian normalisation, so that the first two parts are full_loss_function(theta, allstd)).  With
+ * pinn_hmc_begin_ex the last entries of theta (an inverse problem's theta.p) carry their own priors instead.
  * Hamiltonian Monte Carlo with a fixed number of leapfrog steps and end-point Metropolis acceptance, with AdvancedHMC's
  * defaults: find_good_stepsize for the initial step size, Nesterov dual averaging of the step size (gamma 0.05, t0 10,
  * kappa 0.75) and Stan's windowed diagonal mass-matrix adaptation (buffers 75 / 25 / 50) over the first n_adapts
@@ -337,6 +338,20 @@ typedef struct {
  * all 1) and ll_const stay fixed for the chain.  *step_size_out (nullable): the initial step size. */
 int pinn_hmc_begin(pinn_handle h, const double* host_theta0, const pinn_hmc_options* opts, const double* host_weights,
                    double ll_const, double* step_size_out);
+/* Per-entry priors of the last n_tail entries of theta (parameter estimation: theta.p), as Distributions.jl defines
+ * them: Normal(mu = a, sigma = b), LogNormal(mu = a, sigma = b) (of log x; support x > 0) and Uniform(a, b) (support
+ * a <= x <= b).  Entry j applies to theta[n_theta - n_tail + j]; the Normal(prior_mean, prior_std^2) prior of the options
+ * then covers the first n_theta - n_tail entries only.  A tail entry outside its support makes l = -Inf: the trajectory
+ * stops and the proposal is rejected with numerical_error = 1. */
+enum { PINN_HMC_PRIOR_NORMAL = 0, PINN_HMC_PRIOR_LOGNORMAL = 1, PINN_HMC_PRIOR_UNIFORM = 2 };
+typedef struct {
+  int32_t kind;              /* PINN_HMC_PRIOR_*                                                           */
+  double a, b;               /* (mu, sigma > 0) or Uniform's bounds a < b; finite                         */
+} pinn_hmc_prior;
+/* pinn_hmc_begin with tail priors tail[n_tail], 0 <= n_tail <= PINN_MAX_PARAMS and n_tail < n_theta; n_tail = 0 is
+ * pinn_hmc_begin.  theta0's tail must lie in the priors' supports. */
+int pinn_hmc_begin_ex(pinn_handle h, const double* host_theta0, const pinn_hmc_options* opts, const double* host_weights,
+                      double ll_const, const pinn_hmc_prior* tail, int32_t n_tail, double* step_size_out);
 /* Run n transitions: host_samples [n][n_theta] float64 (theta after each transition) and host_stats
  * [n][PINN_HMC_N_STATS] (each nullable).  The chain continues across calls. */
 int pinn_hmc_iterate(pinn_handle h, int32_t n, double* host_samples, double* host_stats);

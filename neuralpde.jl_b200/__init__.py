@@ -11,7 +11,8 @@ from .symbolic import (Differential, Eq, Equation, In, Interval, PDESystem, VarD
 from .lowering import LoweringError, lower_equation
 from .strategies import (AbstractTrainingStrategy, GridTraining, QuadratureTraining, QuasiRandomTraining,
                          StochasticTraining, generate_training_sets, get_bounds, shard_range)
-from .pinn import (AbstractPINN, Adam, BPINNsolution, BPINNstats, DiagEuclideanMetric, HMC, Leapfrog, NoAdaptation,
+from .pinn import (AbstractPINN, Adam, BPINNsolution, BPINNstats, DiagEuclideanMetric, HMC, Leapfrog, LogNormal,
+                   NoAdaptation, Normal, Uniform,
                    StanHMCAdaptor, UnitEuclideanMetric, ahmc_bayesian_pinn_pde, pmean, BFGS, BackTracking, BayesianPINN, Chain, DataLoss, Dense, Descent, GradientScaleAdaptiveLoss, HagerZhang, LBFGS, LogOptions, MiniMaxAdaptiveLoss,
                    NonAdaptiveLoss, ReLoBRaLoAdaptiveLoss, SoftAdaptAdaptiveLoss,
                    OptimizationFunction, OptimizationProblem, Phi, PhysicsInformedNN, PINNRepresentation, Solution,

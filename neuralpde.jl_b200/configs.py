@@ -143,4 +143,25 @@ def config5(points: int = 1 << 20, bcs_points: int = 16384, n_obs: int = 4096, w
                   param_estim=True, additional_loss=DataLoss("u", X, yobs), n_pde_points=points)
 
 
+def lorenz_bpinn(seed: int = 100, width: int = 7):
+    """The reference's inverse BayesianPINN Lorenz test (test/PDEBPINN/bpinn_pde__bpinn_pde_inv_ii_lorenz_system.jl):
+    unknown σ_ in x' = σ_ (y - x), three 1 -> width -> width -> 1 tanh networks, observations of (x, y, z) at
+    t = 0, 0.05, ..., 1 with 5 % multiplicative noise (seeded numpy in place of Julia's RNG; the ODE solved with
+    scipy's RK45 at rtol 1e-10).  Returns (pde_system, chains, dataset_pde)."""
+    from scipy.integrate import solve_ivp
+    t, s_ = parameters("t σ_")
+    x, y, z = variables("x y z")
+    Dt = Differential(t)
+    eqs = [Eq(Dt(x(t)), s_ * (y(t) - x(t))), Eq(Dt(y(t)), x(t) * (28.0 - z(t)) - y(t)),
+           Eq(Dt(z(t)), x(t) * y(t) - 8.0 / 3.0 * z(t))]
+    bcs = [Eq(x(0.0), 1.0), Eq(y(0.0), 0.0), Eq(z(0.0), 0.0)]
+    sys_ = PDESystem(eqs, bcs, [In(t, 0.0, 1.0)], [t], [x(t), y(t), z(t)], ps=[s_], defaults={s_: 1.0})
+    chains = [Chain(Dense(1, width, "tanh"), Dense(width, width, "tanh"), Dense(width, 1)) for _ in range(3)]
+    f = lambda _, u: [10.0 * (u[1] - u[0]), u[0] * (28.0 - u[2]) - u[1], u[0] * u[1] - 8.0 / 3.0 * u[2]]   # noqa: E731
+    ts = np.linspace(0.0, 1.0, 21)
+    us = solve_ivp(f, (0.0, 1.0), [1.0, 0.0, 0.0], t_eval=ts, rtol=1e-10, atol=1e-12).y
+    us = us + 0.05 * np.random.default_rng(seed).standard_normal(us.shape) * us
+    return sys_, chains, [np.stack([us[i], ts], axis=1) for i in range(3)]
+
+
 ALL = {"cfg1": config1, "cfg2": config2, "cfg3": config3, "cfg4": config4, "cfg5": config5}

@@ -3,7 +3,10 @@
 // theta, the momentum r, the gradient g of the log density, their start-of-transition copies, M^-1 and the Welford
 // window statistics are float64 on the device for both engine dtypes; every evaluation is the fused kernel (eval_step) at
 // theta rounded to the engine dtype, weighted by the fixed log-likelihood weights.  The prior's value and gradient are
-// added here.  One transition is a fixed launch sequence that the host never inspects:
+// added here: N(mean, std^2) on the first n - n_tail entries and, for parameter estimation, one Normal / LogNormal /
+// Uniform prior per entry of the last n_tail (theta.p).  A tail entry outside its prior's support has a NaN gradient, so
+// the trajectory stops there like at any other non-finite value.  One transition is a fixed launch sequence that the
+// host never inspects:
 //
 //   momentum | L x (kick / drift, fused evaluation) | closing kick + energy partials | accept (1 block) | select
 //
@@ -63,7 +66,9 @@ struct HmcArgs {
   const void* total;             // engine dtype: its value (without ll_const)
   HmcScal* S;
   double *samples, *stats;       // [rows][n], [rows][PINN_HMC_N_STATS]
-  double prior_mean, inv_var;    // prior N(mean, 1 / inv_var)
+  double prior_mean, inv_var;    // prior N(mean, 1 / inv_var) of theta[0, n - n_tail)
+  int n_tail;                    // tail[j] is the prior of theta[n - n_tail + j]
+  pinn_hmc_prior tail[PINN_MAX_PARAMS];
   double lp_const;               // ll_const + the prior's normalisation
   double delta;                  // target acceptance
   int adapt, diag, n_adapts;
@@ -88,7 +93,39 @@ __device__ __forceinline__ double normal_draw(unsigned long long seed, long long
   return (i & 1) ? rad * s : rad * co;
 }
 
+// Distributions.jl's insupport: LogNormal x > 0, Uniform a <= x <= b
+__device__ __forceinline__ bool tail_insupport(const pinn_hmc_prior& p, double x) {
+  if (p.kind == PINN_HMC_PRIOR_LOGNORMAL) return x > 0.0;
+  if (p.kind == PINN_HMC_PRIOR_UNIFORM) return x >= p.a && x <= p.b;
+  return true;
+}
+
+// d/dx logpdf: Normal -(x - mu) / s^2, LogNormal -(1 + (log x - mu) / s^2) / x, Uniform 0; NaN outside the support
+__device__ __forceinline__ double tail_grad(const pinn_hmc_prior& p, double x) {
+  if (!tail_insupport(p, x)) return NAN;
+  if (p.kind == PINN_HMC_PRIOR_NORMAL) return -(x - p.a) / (p.b * p.b);
+  if (p.kind == PINN_HMC_PRIOR_LOGNORMAL) return -(1.0 + (log(x) - p.a) / (p.b * p.b)) / x;
+  return 0.0;
+}
+
+// logpdf as Distributions.jl writes it; -Inf outside the support
+__device__ __forceinline__ double tail_logpdf(const pinn_hmc_prior& p, double x) {
+  if (!tail_insupport(p, x)) return -INFINITY;
+  if (p.kind == PINN_HMC_PRIOR_UNIFORM) return -log(p.b - p.a);
+  const double lx = p.kind == PINN_HMC_PRIOR_LOGNORMAL ? log(x) : x;
+  const double z = (lx - p.a) / p.b;
+  const double v = -(z * z + log(2.0 * M_PI)) / 2.0 - log(p.b);
+  return p.kind == PINN_HMC_PRIOR_LOGNORMAL ? v - lx : v;
+}
+
 __device__ __forceinline__ double prior_grad(const HmcArgs& a, double th) { return -(th - a.prior_mean) * a.inv_var; }
+
+// gradient of l at entry i: the physics part g_phys plus the prior's (network entries: the n_tail = 0 arithmetic)
+__device__ __forceinline__ double grad_at(const HmcArgs& a, long long i, double th, double g_phys) {
+  const long long j = i - (a.n - a.n_tail);
+  if (j < 0) return g_phys + prior_grad(a, th);
+  return g_phys + tail_grad(a.tail[j], th);
+}
 
 // start of a transition (restore = false: theta0 = theta, g0 = g) or of a find_good_stepsize trial (restore = true:
 // theta = theta0, g = g0); r = z ./ sqrt(M^-1) and the chunk's partial of r' M^-1 r
@@ -122,7 +159,7 @@ __global__ void __launch_bounds__(kHmcThreads) hmc_kick_drift_kernel(HmcArgs a, 
   if (first) {
     gi = a.g[i];
   } else {
-    gi = (double)((const real*)a.g_r)[i] + prior_grad(a, th);
+    gi = grad_at(a, i, th, (double)((const real*)a.g_r)[i]);
     a.g[i] = gi;
     if (!isfinite(gi) || (i == 0 && !isfinite((double)*(const real*)a.total))) { a.S->flag = 1; return; }
     ri += h * gi;
@@ -134,25 +171,29 @@ __global__ void __launch_bounds__(kHmcThreads) hmc_kick_drift_kernel(HmcArgs a, 
   ((real*)a.theta_r)[i] = (real)th;
 }
 
-// after the last evaluation: g, the closing half kick, and the chunk's partials of r' M^-1 r and |theta - mu|^2
+// after the last evaluation: g, the closing half kick, and the chunk's partials of r' M^-1 r and |theta - mu|^2 (the
+// latter over the Normal prior's entries only)
 template <typename real>
 __global__ void __launch_bounds__(kHmcThreads) hmc_close_kernel(HmcArgs a, const double* eps) {
   const long long lo = (long long)blockIdx.x * kChunk, hi = min(a.n, lo + kChunk);
+  const long long n_net = a.n - a.n_tail;
   const double h = 0.5 * *eps;
   const bool live = !a.S->flag;
   bool bad = blockIdx.x == 0 && threadIdx.x == 0 && !isfinite((double)*(const real*)a.total);
   double k = 0.0, p = 0.0;
   for (long long i = lo + threadIdx.x; i < hi; i += kHmcThreads) {
     const double th = a.theta[i];
-    const double gi = (double)((const real*)a.g_r)[i] + prior_grad(a, th);
+    const double gi = grad_at(a, i, th, (double)((const real*)a.g_r)[i]);
     a.g[i] = gi;
     double ri = a.r[i];
     if (live) { ri += h * gi; a.r[i] = ri; }
     bad |= !isfinite(gi) || !isfinite(ri) || !isfinite(th);
     const double mi = a.minv[i];
     k += mi * ri * ri;
-    const double d = th - a.prior_mean;
-    p += d * d;
+    if (i < n_net) {
+      const double d = th - a.prior_mean;
+      p += d * d;
+    }
   }
   if (bad) a.S->flag = 1;
   k = block_reduce<kHmcThreads, false>(k);
@@ -181,7 +222,8 @@ __global__ void __launch_bounds__(kHmcThreads) hmc_accept_kernel(HmcArgs a, int 
   const double pp = sum_chunks(a.part + 2 * a.chunks, a.chunks);
   if (threadIdx.x) return;
   HmcScal& S = *a.S;
-  const double logp1 = (double)*(const real*)a.total + a.lp_const - 0.5 * pp * a.inv_var;
+  double logp1 = (double)*(const real*)a.total + a.lp_const - 0.5 * pp * a.inv_var;
+  for (int j = 0; j < a.n_tail; ++j) logp1 += tail_logpdf(a.tail[j], a.theta[a.n - a.n_tail + j]);
   if (mode == kInit) { S.logp = logp1; return; }
   const double h0 = -S.logp + k0;
   double h1 = -logp1 + k1;
@@ -440,8 +482,23 @@ long long launches_per_transition(const pinn_engine* e, const HmcState* s) {
 using namespace pinn;
 
 static int hmc_start(pinn_handle e, const double* host_theta0, const pinn_hmc_options* opts, const double* host_weights,
-                     double ll_const, double* step_size_out) {
+                     double ll_const, const pinn_hmc_prior* tail, int32_t n_tail, double* step_size_out) {
   if (!host_theta0 || !opts) return fail("pinn_hmc_begin: null theta / options");
+  if (n_tail < 0 || n_tail > PINN_MAX_PARAMS || (long long)n_tail >= e->n_theta)
+    return fail("pinn_hmc_begin: n_tail = %d must lie in [0, min(%d, n_theta = %lld - 1)]", n_tail, PINN_MAX_PARAMS,
+                (long long)e->n_theta);
+  if (n_tail > 0 && !tail) return fail("pinn_hmc_begin: null tail priors with n_tail = %d", n_tail);
+  for (int j = 0; j < n_tail; ++j) {
+    const pinn_hmc_prior& p = tail[j];
+    if (p.kind != PINN_HMC_PRIOR_NORMAL && p.kind != PINN_HMC_PRIOR_LOGNORMAL && p.kind != PINN_HMC_PRIOR_UNIFORM)
+      return fail("pinn_hmc_begin: tail prior %d has unknown kind %d", j, p.kind);
+    if (!isfinite(p.a) || !isfinite(p.b))
+      return fail("pinn_hmc_begin: tail prior %d has a non-finite parameter (%g, %g)", j, p.a, p.b);
+    if (p.kind == PINN_HMC_PRIOR_UNIFORM && !(p.a < p.b))
+      return fail("pinn_hmc_begin: tail prior %d is Uniform(%g, %g): needs a < b", j, p.a, p.b);
+    if (p.kind != PINN_HMC_PRIOR_UNIFORM && !(p.b > 0.0))
+      return fail("pinn_hmc_begin: tail prior %d has sigma %g: must be positive", j, p.b);
+  }
   if (e->nranks > 1) return fail("pinn_hmc_begin: the sampler runs one chain on one GPU (communicator with %d ranks)", e->nranks);
   if (any_sampler(e))
     return fail("pinn_hmc_begin: HMC needs a fixed log density; a device sampler redraws the points (use fixed point sets)");
@@ -479,7 +536,10 @@ static int hmc_start(pinn_handle e, const double* host_theta0, const pinn_hmc_op
   a.total = (char*)out + (size_t)n * e->es + (size_t)e->n_terms * e->es;
   a.prior_mean = opts->prior_mean;
   a.inv_var = 1.0 / (opts->prior_std * opts->prior_std);
-  a.lp_const = ll_const - 0.5 * (double)n * log(2.0 * M_PI) - (double)n * log(opts->prior_std);
+  a.n_tail = n_tail;
+  for (int j = 0; j < n_tail; ++j) a.tail[j] = tail[j];
+  const long long n_net = n - n_tail;
+  a.lp_const = ll_const - 0.5 * (double)n_net * log(2.0 * M_PI) - (double)n_net * log(opts->prior_std);
   a.delta = opts->target_accept;
   a.adapt = opts->adaptor == PINN_HMC_ADAPT_STAN;
   a.diag = opts->metric == PINN_HMC_METRIC_DIAG;
@@ -524,14 +584,19 @@ static int hmc_start(pinn_handle e, const double* host_theta0, const pinn_hmc_op
 
 extern "C" {
 
-int pinn_hmc_begin(pinn_handle e, const double* host_theta0, const pinn_hmc_options* opts, const double* host_weights,
-                   double ll_const, double* step_size_out) {
+int pinn_hmc_begin_ex(pinn_handle e, const double* host_theta0, const pinn_hmc_options* opts, const double* host_weights,
+                      double ll_const, const pinn_hmc_prior* tail, int32_t n_tail, double* step_size_out) {
   if (!e) return fail("pinn_hmc_begin: null handle");
-  if (hmc_start(e, host_theta0, opts, host_weights, ll_const, step_size_out)) {
+  if (hmc_start(e, host_theta0, opts, host_weights, ll_const, tail, n_tail, step_size_out)) {
     hmc_release(e);              // a failed start leaves no chain: pinn_hmc_iterate refuses until the next begin
     return 1;
   }
   return 0;
+}
+
+int pinn_hmc_begin(pinn_handle e, const double* host_theta0, const pinn_hmc_options* opts, const double* host_weights,
+                   double ll_const, double* step_size_out) {
+  return pinn_hmc_begin_ex(e, host_theta0, opts, host_weights, ll_const, nullptr, 0, step_size_out);
 }
 
 int pinn_hmc_iterate(pinn_handle e, int32_t n, double* host_samples, double* host_stats) {

@@ -38,7 +38,7 @@ EXPORTS = [
     "pinn_flops_per_eval", "pinn_adam_begin", "pinn_adam_iterate", "pinn_adam_theta",
     "pinn_term_grad_stats", "pinn_term_grad_stats_host", "pinn_set_sampler", "pinn_resample", "pinn_get_points_host",
     "pinn_comm_info", "pinn_set_sampler_ex", "pinn_qn_begin", "pinn_qn_iterate", "pinn_qn_theta",
-    "pinn_hmc_begin", "pinn_hmc_iterate", "pinn_hmc_theta",
+    "pinn_hmc_begin", "pinn_hmc_iterate", "pinn_hmc_theta", "pinn_hmc_begin_ex",
 ]
 
 # quasi-Newton optimizer / line search kinds and run states (pinn_qn_options, pinn_qn_iterate)
@@ -49,6 +49,8 @@ QN_RUNNING, QN_CONVERGED, QN_LS_FAILED = 0, 1, 2
 # HMC adaptor / metric kinds (pinn_hmc_options) and the statistics columns of pinn_hmc_iterate
 HMC_ADAPT_NONE, HMC_ADAPT_STAN = 0, 1
 HMC_METRIC_UNIT, HMC_METRIC_DIAG = 0, 1
+# kinds of the per-entry priors of theta's last entries (pinn_hmc_prior)
+HMC_PRIOR_NORMAL, HMC_PRIOR_LOGNORMAL, HMC_PRIOR_UNIFORM = 0, 1, 2
 HMC_STATS = ("step_size", "acceptance_rate", "is_accept", "log_density", "hamiltonian_energy",
              "hamiltonian_energy_error", "numerical_error", "is_adapt")
 
@@ -70,6 +72,10 @@ class _HmcOptions(C.Structure):
     _fields_ = [("n_leapfrog", C.c_int32), ("adaptor", C.c_int32), ("metric", C.c_int32), ("n_adapts", C.c_int32),
                 ("target_accept", C.c_double), ("step_size", C.c_double), ("prior_mean", C.c_double),
                 ("prior_std", C.c_double), ("seed", C.c_uint64)]
+
+
+class _HmcPrior(C.Structure):
+    _fields_ = [("kind", C.c_int32), ("a", C.c_double), ("b", C.c_double)]
 
 
 class _NetDesc(C.Structure):
@@ -215,6 +221,9 @@ def load_library():
     lib.pinn_qn_theta.restype = C.c_int
     lib.pinn_hmc_begin.argtypes = [vp, C.POINTER(dbl), C.POINTER(_HmcOptions), C.POINTER(dbl), dbl, C.POINTER(dbl)]
     lib.pinn_hmc_begin.restype = C.c_int
+    lib.pinn_hmc_begin_ex.argtypes = [vp, C.POINTER(dbl), C.POINTER(_HmcOptions), C.POINTER(dbl), dbl,
+                                      C.POINTER(_HmcPrior), i32, C.POINTER(dbl)]
+    lib.pinn_hmc_begin_ex.restype = C.c_int
     lib.pinn_hmc_iterate.argtypes = [vp, i32, C.POINTER(dbl), C.POINTER(dbl)]
     lib.pinn_hmc_iterate.restype = C.c_int
     lib.pinn_hmc_theta.argtypes = [vp, C.POINTER(dbl)]
@@ -462,9 +471,11 @@ class Engine:
     def hmc_begin(self, theta0: np.ndarray, n_leapfrog: int = 30, adaptor: int = HMC_ADAPT_STAN,
                   metric: int = HMC_METRIC_DIAG, n_adapts: int = 0, target_accept: float = 0.8, step_size: float = 0.0,
                   prior_mean: float = 0.0, prior_std: float = 1.0, seed: int = 0, weights=None,
-                  ll_const: float = 0.0) -> float:
+                  ll_const: float = 0.0, tail_priors=None) -> float:
         """Start a chain at theta0 (float64) for the log density sum_k w_k L_k + ll_const + log N(theta; prior);
-        step_size <= 0 runs find_good_stepsize.  Returns the initial step size."""
+        step_size <= 0 runs find_good_stepsize.  Returns the initial step size.  ``tail_priors``: a list of
+        (HMC_PRIOR_*, a, b) for the last len(tail_priors) entries of theta, which the Normal prior then leaves out
+        (pinn_hmc_begin_ex); None calls pinn_hmc_begin."""
         th = np.ascontiguousarray(theta0, dtype=np.float64)
         if th.shape != (self.n_theta,):
             raise ValueError("theta must have length %d" % self.n_theta)
@@ -473,8 +484,14 @@ class Engine:
         w = self._weights(weights)
         wp = w.ctypes.data_as(C.POINTER(C.c_double)) if w is not None else None
         eps = C.c_double(0.0)
-        _check(self.lib.pinn_hmc_begin(self._h, th.ctypes.data_as(C.POINTER(C.c_double)), C.byref(opt), wp,
-                                       float(ll_const), C.byref(eps)))
+        if tail_priors is None:
+            _check(self.lib.pinn_hmc_begin(self._h, th.ctypes.data_as(C.POINTER(C.c_double)), C.byref(opt), wp,
+                                           float(ll_const), C.byref(eps)))
+        else:
+            tail = (_HmcPrior * max(1, len(tail_priors)))(*[_HmcPrior(int(k), float(a), float(b))
+                                                            for k, a, b in tail_priors])
+            _check(self.lib.pinn_hmc_begin_ex(self._h, th.ctypes.data_as(C.POINTER(C.c_double)), C.byref(opt), wp,
+                                              float(ll_const), tail, len(tail_priors), C.byref(eps)))
         return float(eps.value)
 
     def hmc_iterate(self, n: int):

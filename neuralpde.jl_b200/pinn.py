@@ -366,7 +366,10 @@ class BayesianPINN(AbstractPINN):
     """``BayesianPINN(args...; dataset = nothing, kwargs...)`` (reference src/pinn_types.jl:214-245): wraps a
     PhysicsInformedNN; ``symbolic_discretize`` then builds ``full_loss_function(θ, allstd)`` = the weighted
     log-likelihood (src/discretize.jl:653-757) that the HMC samplers of ext/bpinn consume; ``ahmc_bayesian_pinn_pde``
-    samples its posterior on the device.  The likelihood and its θ-gradient come from the same fused kernel."""
+    samples its posterior on the device.  The likelihood and its θ-gradient come from the same fused kernel.
+    ``dataset = [dataset_pde, dataset_bc]``: each None or a list with one ``n × (1 + d_k)`` array per dependent
+    variable, observed values in column 1 and the variable's d_k inputs after it.  Equation (bc) j is also evaluated at
+    the coordinates of dataset_pde[j] (dataset_bc[j]); with ``param_estim`` the observations enter as L2LossData."""
 
     def __init__(self, *args, dataset=None, **kwargs):
         self.pinn = PhysicsInformedNN(*args, **kwargs)
@@ -466,15 +469,15 @@ def symbolic_discretize(pde_system: PDESystem, discretization: PhysicsInformedNN
     ``rank`` / ``world`` shard every term's point set contiguously (SURVEY section 8(e))."""
     bayes = isinstance(discretization, BayesianPINN)
     if bayes:
-        if any(ds is not None for ds in discretization.dataset):
-            raise ValueError("BayesianPINN: dataset points (physics loss evaluated at observation sites, "
-                             "src/training_strategies.jl:86-113) are not supported; pass observations as a DataLoss")
+        dataset = discretization.dataset
         if not isinstance(discretization.pinn.strategy, GridTraining):
             raise ValueError("BayesianPINN: the reference defines the log-likelihood form for GridTraining only "
                              "(merge_strategy_with_loglikelihood_function, src/training_strategies.jl:50-113)")
         if discretization.pinn.adaptive_loss is not None and not isinstance(discretization.pinn.adaptive_loss, NonAdaptiveLoss):
             raise ValueError("BayesianPINN: adaptive loss weights are not supported with the log-likelihood form")
         discretization = discretization.pinn
+    else:
+        dataset = (None, None)
     if not isinstance(discretization, PhysicsInformedNN):
         raise TypeError("symbolic_discretize: expected a PhysicsInformedNN or BayesianPINN")
     d = discretization
@@ -494,6 +497,7 @@ def symbolic_discretize(pde_system: PDESystem, discretization: PhysicsInformedNN
                              % (name, c.dims[0], len(vi.dict_depvar_input[name])))
         if c.dims[-1] != 1:
             raise ValueError("chain for %s must have a 1-dimensional output" % name)
+    ds_pde, ds_bc = _bayes_dataset(dataset, vi)
 
     # ---- parameters: θ = [depvar blocks..., p] (src/discretize.jl:432-472) -----------------------------
     eq_params = [str(p) for p in pde_system.ps]
@@ -549,6 +553,31 @@ def symbolic_discretize(pde_system: PDESystem, discretization: PhysicsInformedNN
             specs.append(term_spec(lt, REDUCE_WSUM, 1.0))      # scale filled below
         else:
             specs.append(term_spec(lt, REDUCE_MEAN))
+    # BayesianPINN dataset terms (src/training_strategies.jl:84-108): equation / bc j's residual at the coordinates of
+    # dataset j, paired by zip (so the shorter list decides how many), then with param_estim one L2LossData term per
+    # dependent variable (ext/bpinn/PDE_BPINN.jl:147-180) over the dataset_pde and dataset_bc rows of that variable
+    ds_terms: List[tuple] = []           # (lowered term, (d, n) coordinates)
+    n_ds = []
+    for ds, lts, what in ((ds_pde, pde_terms, "equation"), (ds_bc, bc_terms, "boundary condition")):
+        for j, (lt, m) in enumerate(zip(lts, ds or [])):
+            X = m[:, 1:].T
+            if X.shape[0] != len(lt.indvars):
+                raise ValueError("BayesianPINN: dataset %d has %d coordinate columns but %s %d has the variables %s"
+                                 % (j + 1, X.shape[0], what, j + 1, lt.indvars))
+            specs.append(term_spec(lt, REDUCE_MEAN))
+            ds_terms.append((lt, X))
+        n_ds.append(min(len(lts), len(ds or [])))
+    l2_sets: List[np.ndarray] = []
+    if bayes and d.param_estim and (ds_pde is not None or ds_bc is not None):
+        for k, c in enumerate(chains):
+            m = np.concatenate([ds[k] for ds in (ds_pde, ds_bc) if ds is not None], axis=0)
+            din = c.dims[0]
+            rows = [None] * len(chains)
+            rows[k] = list(range(din))
+            specs.append(TermSpec(dim=din + 1, taps=[TapSpec(net=k, order=0)],
+                                  prog=[("tap", 0, 0, 0.0), ("coord", din, 0, 0.0), ("sub", 0, 1, 0.0)],
+                                  net_rows=rows, reduction=REDUCE_MEAN))
+            l2_sets.append(np.concatenate([m[:, 1:].T, m[:, :1].T], axis=0))
     add = d.additional_loss
     if add is not None and not isinstance(add, DataLoss):
         raise ValueError("additional_loss must be a DataLoss (structured data term); arbitrary closures cannot "
@@ -589,6 +618,13 @@ def symbolic_discretize(pde_system: PDESystem, discretization: PhysicsInformedNN
             specs[i].scale = 1.0 / area
     else:
         raise TypeError("unsupported training strategy %r" % (strategy,))
+    o = n_pde + n_bc
+    for i, (_, X) in enumerate(ds_terms):
+        point_sets[o + i] = X.astype(dtype)
+    o += len(ds_terms)
+    for i, m in enumerate(l2_sets):
+        point_sets[o + i] = m.astype(dtype)
+    n_main = o + len(l2_sets)             # every term but the additional loss
     if isinstance(add, DataLoss):
         X = np.asarray(add.points, dtype=dtype)
         y = np.asarray(add.values, dtype=dtype).reshape(1, -1)
@@ -601,7 +637,7 @@ def symbolic_discretize(pde_system: PDESystem, discretization: PhysicsInformedNN
     sampler_rng = np.random.default_rng(getattr(strategy, "seed", 0) + 7919 * rank)
     state = {"calls": 0}
 
-    lowered = pde_terms + bc_terms
+    lowered = pde_terms + bc_terms + [lt for lt, _ in ds_terms]
 
     def augment(i: int, pts: np.ndarray) -> np.ndarray:
         """append the hoisted coordinate-only rows of term i (float64 evaluation, then theta's eltype)"""
@@ -658,7 +694,7 @@ def symbolic_discretize(pde_system: PDESystem, discretization: PhysicsInformedNN
             point_sets[i] = pts
 
     def term_weights() -> np.ndarray:
-        w = np.concatenate([weights["pde"], weights["bc"]])
+        w = np.concatenate([weights["pde"], weights["bc"], np.zeros(n_main - n_pde - n_bc)])
         if isinstance(add, DataLoss):
             w = np.concatenate([w, weights["add"]])
         return w
@@ -743,6 +779,8 @@ def symbolic_discretize(pde_system: PDESystem, discretization: PhysicsInformedNN
         pde_indvars=[lt.indvars for lt in pde_terms], bc_indvars=[lt.indvars for lt in bc_terms],
         symbolic_pde_loss_functions=pde_terms, symbolic_bc_loss_functions=bc_terms, loss_functions=lf, engine=eng,
         term_names=["pde_%d" % (i + 1) for i in range(n_pde)] + ["bc_%d" % (j + 1) for j in range(n_bc)]
+        + ["dataset_pde_%d" % (j + 1) for j in range(n_ds[0])] + ["dataset_bc_%d" % (j + 1) for j in range(n_ds[1])]
+        + ["l2_data_%s" % name for name in (vi.depvars if l2_sets else [])]
         + (["additional"] if isinstance(add, DataLoss) else []))
     rep.point_sets = point_sets
     rep.resample = resample
@@ -765,9 +803,11 @@ def symbolic_discretize(pde_system: PDESystem, discretization: PhysicsInformedNN
         # term (get_points_loss_functions, src/training_strategies.jl:115-128) -- the sum of squares is n * mean(abs2, r),
         # which the fused kernel returns per term, and its theta-gradient is the engine's weighted gradient with weights
         # -W n / (2 sigma^2).  As in the reference the per-group log-likelihoods are SUMMED before the weight vector
-        # multiplies them (:682-738): every weight of a group scales the whole group sum.
-        n_k = np.array([point_sets[i].shape[1] for i in range(n_pde + n_bc)], dtype=np.float64)
-        rep.loglik_weights = lambda allstd: _loglik_weights(weights, n_k, n_pde, allstd)
+        # multiplies them (:682-738): every weight of a group scales the whole group sum.  Dataset terms join their
+        # group's sum; L2LossData (data=True) is the sampler's and is not part of full_loss_function.
+        n_k = np.array([point_sets[i].shape[1] for i in range(n_main)], dtype=np.float64)
+        counts = (n_pde, n_bc, n_ds[0], n_ds[1])
+        rep.loglik_weights = lambda allstd, data=False: _loglik_weights_all(weights, n_k, counts, allstd, data)
 
         def _loglik(theta, allstd, want_grad):
             stdpdes, stdbcs, stdextra = allstd
@@ -781,7 +821,7 @@ def symbolic_discretize(pde_system: PDESystem, discretization: PhysicsInformedNN
             else:
                 c_all = c
             total, terms, grad = eng.loss_grad_host(th, c_all, want_grad)
-            ll = const + float(np.dot(c, np.asarray(terms[:n_pde + n_bc], dtype=np.float64)))
+            ll = const + float(np.dot(c, np.asarray(terms[:n_main], dtype=np.float64)))
             if has_add:
                 s_e = float(stdextra)
                 ll += weights["add"][0] * (-np.log(s_e * np.sqrt(2.0 * np.pi)) - A * A / (2.0 * s_e ** 2))
@@ -807,6 +847,61 @@ def _loglik_weights(weights, n_k: np.ndarray, n_pde: int, allstd):
     c = -Wg * n_k / (2.0 * sig ** 2)
     const = float(np.sum(Wg * (-0.5 * n_k * np.log(2.0 * np.pi) - n_k * np.log(sig))))
     return c, const
+
+
+def _loglik_weights_all(weights, n_k: np.ndarray, counts, allstd, data: bool = False):
+    """Weights c and constant of the BayesianPINN log-likelihood over all its terms.  n_k holds the point counts of the
+    grid pde and bc terms, the dataset pde and bc terms (counts: the four numbers) and then the L2 data terms.
+
+    - grid terms: ``_loglik_weights``;
+    - dataset term j: c = -W n / (2 σ²) with its group's weight sum W and σ = stdpdes[j] (stdbcs[j]), plus
+      W (-n/2 log 2π - n log σ) in the constant (src/training_strategies.jl:115-128, src/discretize.jl:699-717);
+    - L2 data term i (``data``; zero otherwise): c = -n / (2 l2std[i]²) and -n/2 log 2π - n log l2std[i], no adaptive
+      weight (L2LossData, ext/bpinn/PDE_BPINN.jl:147-180)."""
+    n_pde, n_bc, n_dp, n_db = counts
+    c, const = _loglik_weights(weights, n_k[:n_pde + n_bc], n_pde, allstd)
+    o = n_pde + n_bc
+    nd, nl = n_k[o:o + n_dp + n_db], n_k[o + n_dp + n_db:]
+    sig = np.concatenate([np.asarray(allstd[0], dtype=np.float64)[:n_dp],
+                          np.asarray(allstd[1], dtype=np.float64)[:n_db]])
+    Wg = np.concatenate([np.full(n_dp, weights["pde"].sum()), np.full(n_db, weights["bc"].sum())])
+    c_d = -Wg * nd / (2.0 * sig ** 2)
+    const += float(np.sum(Wg * (-0.5 * nd * np.log(2.0 * np.pi) - nd * np.log(sig))))
+    c_l = np.zeros(nl.size)
+    if data and nl.size:
+        l2 = np.asarray(allstd[2], dtype=np.float64).reshape(-1)
+        if l2.shape != nl.shape:
+            raise ValueError("allstd: need %d l2std values, one per dependent variable" % nl.size)
+        c_l = -nl / (2.0 * l2 ** 2)
+        const += float(np.sum(-0.5 * nl * np.log(2.0 * np.pi) - nl * np.log(l2)))
+    return np.concatenate([c, c_d, c_l]), const
+
+
+def _bayes_dataset(dataset, vi: VarInfo):
+    """BayesianPINN's ``dataset = [dataset_pde, dataset_bc]``, each None or a list with one n × (1 + d_k) array per
+    dependent variable (d_k: its inputs).  Returns the two lists as float64 arrays (or None)."""
+    if len(dataset) != 2:
+        raise ValueError("BayesianPINN: dataset points: expected dataset = [dataset_pde, dataset_bc], got %d entries"
+                         % len(dataset))
+    out = []
+    for what, ds in zip(("dataset_pde", "dataset_bc"), dataset):
+        if ds is None:
+            out.append(None)
+            continue
+        if not isinstance(ds, (list, tuple)) or len(ds) != len(vi.depvars):
+            raise ValueError("BayesianPINN: dataset points: %s must be None or a list of %d arrays, one per dependent "
+                             "variable %s, each n × (1 + inputs) with the observed values in column 1"
+                             % (what, len(vi.depvars), vi.depvars))
+        mats = []
+        for name, m in zip(vi.depvars, ds):
+            a = np.asarray(m, dtype=np.float64)
+            cols = 1 + len(vi.dict_depvar_input[name])
+            if a.ndim != 2 or a.shape[0] < 1 or a.shape[1] != cols:
+                raise ValueError("BayesianPINN: dataset points: %s for %s has shape %s, expected n × %d"
+                                 % (what, name, a.shape, cols))
+            mats.append(a)
+        out.append(mats)
+    return out
 
 
 @dataclass
@@ -994,6 +1089,65 @@ class Leapfrog:
     """``Integrator = Leapfrog``."""
 
 
+@dataclass(frozen=True)
+class Normal:
+    """``Distributions.Normal(μ, σ)``, a prior of an equation parameter (``param``)."""
+    mu: float = 0.0
+    sigma: float = 1.0
+
+    def params(self):
+        return (self.mu, self.sigma)
+
+
+@dataclass(frozen=True)
+class LogNormal:
+    """``Distributions.LogNormal(μ, σ)``: log x ~ Normal(μ, σ); ``params`` are (μ, σ) of log x, not the mean."""
+    mu: float = 0.0
+    sigma: float = 1.0
+
+    def params(self):
+        return (self.mu, self.sigma)
+
+
+@dataclass(frozen=True)
+class Uniform:
+    """``Distributions.Uniform(a, b)`` on [a, b]."""
+    a: float = 0.0
+    b: float = 1.0
+
+    def params(self):
+        return (self.a, self.b)
+
+
+_PRIOR_KINDS = {Normal: _eng.HMC_PRIOR_NORMAL, LogNormal: _eng.HMC_PRIOR_LOGNORMAL, Uniform: _eng.HMC_PRIOR_UNIFORM}
+
+
+def _tail_priors(param) -> List[tuple]:
+    """The device's table for θ.p: (kind, a, b) per parameter, in the reference's order -- priorlogpdf applies
+    ``param[length(θ) - i + 1]`` to θ[i] (ext/bpinn/PDE_BPINN.jl:194-196), so θ.p[k] gets param[end - k]."""
+    out = []
+    for prior in param:
+        kind = _PRIOR_KINDS.get(type(prior))
+        if kind is None:
+            raise ValueError("ahmc_bayesian_pinn_pde: prior %r is not supported (Normal, LogNormal or Uniform)"
+                             % (prior,))
+        a, b = (float(v) for v in prior.params())
+        if not (np.isfinite(a) and np.isfinite(b)) or (kind == _eng.HMC_PRIOR_UNIFORM and not a < b) or \
+                (kind != _eng.HMC_PRIOR_UNIFORM and not b > 0.0):
+            raise ValueError("ahmc_bayesian_pinn_pde: prior %r: needs finite parameters with σ > 0 (Uniform: a < b)"
+                             % (prior,))
+        out.append((kind, a, b))
+    return out[::-1]
+
+
+def _initial_theta(flat_init_params, param) -> np.ndarray:
+    """float64 θ0: the network part of flat_init_params, then θ.p[k] = params(param[k])[1] in FORWARD order
+    (ext/bpinn/PDE_BPINN.jl:476, :499): Normal's μ, LogNormal's μ of log x, Uniform's a."""
+    th = np.array(flat_init_params, dtype=np.float64)
+    th[th.size - len(param):] = [float(p.params()[0]) for p in param]
+    return th
+
+
 @dataclass
 class BPINNstats:
     """``BPINNstats(mcmc_chain, samples, statistics)``: ``chain`` / ``samples`` are the [draw_samples, n_θ] draws,
@@ -1037,9 +1191,15 @@ def ahmc_bayesian_pinn_pde(pde_system: PDESystem, discretization: BayesianPINN, 
     Defaults as the reference: ``HMC(0.1, 30)`` started at ``find_good_stepsize``, Stan adaptation (dual averaging to
     acceptance 0.8, diagonal mass matrix) over the first ``min(draw_samples ÷ 10, 1000)`` transitions, warm-up samples
     kept.  The chain runs on the device (``pinn_hmc_*``); ``seed`` keys its Philox streams (the reference uses the global
-    RNG).  ``l2std`` / ``phynewstd`` are accepted and unused: without a dataset the reference does not use them either.
+    RNG).  ``phynewstd`` is accepted and unused (it belongs to ``Dict_differentials``).
+
+    Parameter estimation (``BayesianPINN(...; param_estim = true, dataset)`` with ``param = [prior, ...]``, one
+    Normal / LogNormal / Uniform per equation parameter): the target gains L2LossData, the observations' Gaussian
+    log-likelihood with standard deviations ``l2std`` (one per dependent variable), and θ.p gets the priors of
+    ``param`` in REVERSED order, as the reference's priorlogpdf applies them; θ.p starts at ``params(param[k])[1]``
+    (LogNormal: μ of log x).  ``estimated_de_params[k]`` holds θ.p[k] over the ensemble's samples.
     Not supported (refused with a message): NUTS / HMCDA kernels, ``DenseEuclideanMetric``, jittered / tempered
-    leapfrog, several chains, parameter estimation, ``Dict_differentials`` and an ``additional_loss``."""
+    leapfrog, several chains, ``Dict_differentials`` and an ``additional_loss``."""
     Kernel = HMC() if Kernel is None else Kernel
     ak = dict(_DEFAULT_ADAPTOR, **(Adaptorkwargs or {}))
     ik = dict({"Integrator": Leapfrog}, **(Integratorkwargs or {}))
@@ -1059,14 +1219,30 @@ def ahmc_bayesian_pinn_pde(pde_system: PDESystem, discretization: BayesianPINN, 
         raise ValueError("ahmc_bayesian_pinn_pde: nchains = %r; one chain per call is supported" % (nchains,))
     if not isinstance(discretization, BayesianPINN):
         raise TypeError("ahmc_bayesian_pinn_pde: expected a BayesianPINN discretization")
-    if discretization.pinn.param_estim or len(param) > 0:
-        raise ValueError("ahmc_bayesian_pinn_pde: parameter estimation (param_estim / param) needs a dataset, which is "
-                         "not supported (reference ext/bpinn/PDE_BPINN.jl:454-460)")
+    param_estim = discretization.pinn.param_estim
+    if len(param) > 0 and not param_estim:
+        raise ValueError("ahmc_bayesian_pinn_pde: parameter estimation: `param` priors need "
+                         "BayesianPINN(...; param_estim = true)")
+    if param_estim and len(param) == 0:       # the reference throws UndefVarError(:param) (PDE_BPINN.jl:454-455)
+        raise ValueError("ahmc_bayesian_pinn_pde: parameter estimation (param_estim = true) needs `param`, one prior "
+                         "per equation parameter")
     if Dict_differentials is not None:
         raise ValueError("ahmc_bayesian_pinn_pde: Dict_differentials (the data-collocation loss) is not supported")
     if discretization.pinn.additional_loss is not None:
         raise ValueError("ahmc_bayesian_pinn_pde: an additional_loss enters the log-likelihood with a weight that depends "
                          "on its value, two evaluations per gradient; the device sampler does not support it")
+    tail = []
+    if param_estim:
+        if all(ds is None for ds in discretization.dataset):      # UndefVarError(:dataset) (:456-457)
+            raise ValueError("ahmc_bayesian_pinn_pde: parameter estimation (param_estim = true) needs a dataset")
+        n_dv = len(get_vars(pde_system.ivs, pde_system.dvs).depvars)
+        if len(l2std) != n_dv:                                     # :458-459
+            raise ValueError("ahmc_bayesian_pinn_pde: L2 stds length must match number of dependant variables "
+                             "(%d l2std values, %d dependent variables)" % (len(l2std), n_dv))
+        if len(param) != len(pde_system.ps):
+            raise ValueError("ahmc_bayesian_pinn_pde: parameter estimation: %d priors in `param` for the %d equation "
+                             "parameters %s" % (len(param), len(pde_system.ps), [str(p) for p in pde_system.ps]))
+        tail = _tail_priors(param)
     rep = symbolic_discretize(pde_system, discretization)
     if len(rep.domains) != len(saveats):
         raise ValueError("Number of independent variables must match saveat inference discretization steps")
@@ -1074,19 +1250,28 @@ def ahmc_bayesian_pinn_pde(pde_system: PDESystem, discretization: BayesianPINN, 
     numensemble = int(np.floor(draw_samples / 3)) if numensemble is None else int(numensemble)
     if draw_samples < 1 or not 0 <= numensemble < draw_samples:
         raise ValueError("ahmc_bayesian_pinn_pde: need draw_samples >= 1 and 0 <= numensemble < draw_samples")
-    c, const = rep.loglik_weights([phystd, bcstd, l2std])
+    allstd = [phystd, bcstd, l2std]
+    c, const = rep.loglik_weights(allstd, data=True)
     mu_p, sd_p = float(priorsNNw[0]), float(priorsNNw[1])
     n_adapts = min(draw_samples // 10, 1000)
     eng = rep.engine
-    theta0 = np.asarray(rep.flat_init_params, dtype=np.float64)
+    ninv = len(tail)
+    theta0 = _initial_theta(rep.flat_init_params, param)
+    n_net = theta0.size - ninv
     eps0 = eng.hmc_begin(theta0, n_leapfrog=Kernel.n_leapfrog,
                          adaptor=_eng.HMC_ADAPT_STAN if ak["Adaptor"] is StanHMCAdaptor else _eng.HMC_ADAPT_NONE,
                          metric=_eng.HMC_METRIC_DIAG if ak["Metric"] is DiagEuclideanMetric else _eng.HMC_METRIC_UNIT,
                          n_adapts=n_adapts, target_accept=float(ak["targetacceptancerate"]), step_size=0.0,
-                         prior_mean=mu_p, prior_std=sd_p, seed=seed, weights=c, ll_const=const)
+                         prior_mean=mu_p, prior_std=sd_p, seed=seed, weights=c, ll_const=const,
+                         tail_priors=tail if ninv else None)
     if verbose:
         print("Initial step size %g; current physics log-likelihood %g"
-              % (eps0, rep.loss_functions.full_loss_function(theta0, [phystd, bcstd, l2std])))
+              % (eps0, rep.loss_functions.full_loss_function(theta0, allstd)))
+        if ninv:
+            c_phys, const_phys = rep.loglik_weights(allstd)
+            _, terms, _ = eng.loss_grad_host(theta0.astype(rep.flat_init_params.dtype), c, False)
+            sse = float(np.dot(c - c_phys, np.asarray(terms, dtype=np.float64))) + (const - const_phys)
+            print("Current SSE against dataset Log-likelihood : %g" % sse)
     samples, st = eng.hmc_iterate(draw_samples)
     statistics = {name: st[:, j].copy() for j, name in enumerate(_eng.HMC_STATS)}
     if verbose:
@@ -1102,4 +1287,5 @@ def ahmc_bayesian_pinn_pde(pde_system: PDESystem, discretization: BayesianPINN, 
         timepoints.append(tp)
         ensemble.append(np.stack([np.asarray(ph(tp, th), dtype=np.float64).reshape(-1) for th in kept]))
         nn_params.append(kept[:, ph.theta_offset:ph.theta_offset + ph.chain.n_params].copy())
-    return BPINNsolution(BPINNstats(samples, samples, statistics), ensemble, nn_params, [None], timepoints)
+    de_params = [kept[:, n_net + k].copy() for k in range(ninv)] if ninv else [None]
+    return BPINNsolution(BPINNstats(samples, samples, statistics), ensemble, nn_params, de_params, timepoints)

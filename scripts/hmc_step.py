@@ -1,7 +1,9 @@
 """Per-transition cost of the device-resident HMC sampler (pinn_hmc_*): wall time per transition and per leapfrog step
 (profiler off, graph replay, one read-back per call), launches per transition, then, in a second profiled window, the
 share of device time spent in the fused kernels (torch.profiler, CUDA activities).  Cases: the reference's 2-D Poisson
-BayesianPINN test (iv_2d_poisson: 2 -> 9 -> 9 -> 1 sigmoid, GridTraining(0.04), FFMA fp32) and config 2 (tc_split).
+BayesianPINN test (iv_2d_poisson: 2 -> 9 -> 9 -> 1 sigmoid, GridTraining(0.04), FFMA fp32), config 2 (tc_split) and the
+reference's inverse Lorenz test (inv_ii_lorenz: three 1 -> 7 -> 7 -> 1 tanh networks, GridTraining(0.01), a 21-point
+dataset per variable, σ_ estimated under a Normal(12, 2) prior, FFMA fp32).
 The chains run with a fixed step of 1e-5 and no adaptation, so that no trajectory stops early at a non-finite value and
 every transition does the full 30 steps.  One JSON line per case, led by a line with the card's name and power limit.
 usage: hmc_step.py [--transitions K] [--out FILE]"""
@@ -35,20 +37,31 @@ def make(case):
         init = npde.initialparameters(np.random.default_rng(0), chain, np.float32)
         disc = npde.BayesianPINN([chain], npde.GridTraining(0.04), init_params=init, mode="ffma")
         std = [[0.003], [0.003] * 4, [0.05]]
+    elif case == "inv_ii_lorenz":
+        sys_, chains, data = configs.lorenz_bpinn()
+        rng = np.random.default_rng(0)
+        init = np.concatenate([npde.initialparameters(rng, c, np.float32) for c in chains] + [np.ones(1, np.float32)])
+        disc = npde.BayesianPINN(chains, npde.GridTraining([0.01]), init_params=init, mode="ffma", param_estim=True,
+                                 dataset=[data, None])
+        rep = npde.symbolic_discretize(sys_, disc)
+        return rep, [[0.1] * 3, [0.3] * 3, [1.0] * 3], [(E.HMC_PRIOR_NORMAL, 12.0, 2.0)]
     else:
         cfg = configs.config2()
         disc = npde.BayesianPINN(cfg.chains[0], cfg.strategy, init_params=cfg.init_params(np.float32), mode="tc_split")
         std = [[0.05], [0.05] * 4, [0.05]]
     rep = npde.symbolic_discretize(cfg.pde_system, disc)
-    return rep, std
+    return rep, std, None
 
 
 def run(case, transitions):
-    rep, std = make(case)
+    rep, std, tail = make(case)
     eng = rep.engine
-    c, const = rep.loglik_weights(std)
-    eng.hmc_begin(rep.flat_init_params, n_leapfrog=N_LEAPFROG, adaptor=E.HMC_ADAPT_NONE, metric=E.HMC_METRIC_UNIT,
-                  step_size=1e-5, prior_std=10.0, weights=c, ll_const=const)
+    c, const = rep.loglik_weights(std, data=True)
+    th0 = rep.flat_init_params.astype(np.float64)
+    if tail:
+        th0[-len(tail):] = [a for _, a, _ in tail]
+    eng.hmc_begin(th0, n_leapfrog=N_LEAPFROG, adaptor=E.HMC_ADAPT_NONE, metric=E.HMC_METRIC_UNIT,
+                  step_size=1e-5, prior_std=10.0, weights=c, ll_const=const, tail_priors=tail)
     eng.hmc_iterate(5)                                   # warm-up: graph capture, module loads
     l0 = eng.launch_count()
     t0 = time.perf_counter()
@@ -90,7 +103,7 @@ def main():
     torch.cuda.init()
     lines = [json.dumps({"card": card(), "note": "name, power.limit, clocks.max.sm"})]
     print(lines[0], flush=True)
-    for case in ("iv_2d_poisson", "cfg2"):
+    for case in ("iv_2d_poisson", "cfg2", "inv_ii_lorenz"):
         lines.append(json.dumps(run(case, a.transitions)))
         print(lines[-1], flush=True)
     if a.out:
