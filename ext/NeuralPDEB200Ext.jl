@@ -148,6 +148,10 @@ function lower_expr!(L::Lowered, ex, env)
         throw(ArgumentError("NeuralPDEB200Ext: symbol $ex cannot appear in an expression"))
     end
     ex isa Expr || throw(ArgumentError("NeuralPDEB200Ext: cannot lower $ex"))
+    # integral(u, cord, phi, ids, integrand, lb, ub, θ): the integrand is a separate RuntimeGeneratedFunction this
+    # lowering does not read; the engine's integral terms (pinn_create_ex) are reachable from the Python layer only
+    ex.head === :call && ex.args[1] === :integral &&
+        throw(ArgumentError("NeuralPDEB200Ext: equations with Integral terms are not lowered by this extension"))
     if ex.head === :call && ex.args[1] === :u                                                  # u(cord_k, θ_k, phi_k)
         return tap!(L, net_of(ex.args[2], env), 0, Int[])
     elseif ex.head === :call && ex.args[1] === :derivative                                     # derivative(phi_k, u, cord_k, εs, order, θ_k)

@@ -15,6 +15,8 @@
  * Reference functions each entry point replaces (file:line in /root/reference):
  *   pinn_create            <- symbolic_discretize's closure construction
  *                             (src/discretize.jl:413-651), Phi (src/pinn_types.jl:79-90)
+ *   pinn_create_ex         <- the same, with get_numeric_integral's integral terms
+ *                             (src/discretize.jl:334-397, src/transform_inf_integral.jl)
  *   pinn_set_points[_host] <- train-set placement in get_loss_function
  *                             (src/training_strategies.jl:215-221 Grid, :271-282 Stochastic)
  *   pinn_loss_grad[_host]  <- full_loss_function(theta,p) (src/discretize.jl:567-598)
@@ -115,7 +117,8 @@ enum {
   PINN_OP_LOG = 14,
   PINN_OP_TANH = 15,
   PINN_OP_SQRT = 16,
-  PINN_OP_ABS = 17
+  PINN_OP_ABS = 17,
+  PINN_OP_INTEGRAL = 18   /* value of integral `a` at the term's point (pinn_create_ex only) */
 };
 
 typedef struct {
@@ -174,8 +177,45 @@ typedef struct {
   int64_t n_theta;             /* total length of theta                                  */
 } pinn_problem_desc;
 
+/* ---- integral terms (integro-differential equations) ----------------------------------------------------------
+ * An integral over 1 or 2 of the owner term's coordinates, I(p) = int g(s) ds, evaluated per collocation point p of
+ * the owner term -- the reference's get_numeric_integral (src/discretize.jl:334-397), which calls adaptive h-cubature
+ * with reltol = abstol = 1e-3.  The engine uses a fixed Gauss-Legendre rule instead: q nodes per integrating dimension
+ * (a tensor product for two), so the value is deterministic and its gradient is the exact gradient of the rule.
+ * The quadrature runs in the variable t: t_k in [lb_k, ub_k] (a constant, or an owner point row such as a hoisted
+ * coordinate expression), and the coordinate the integrand sees is x_k(t_k):
+ *   PINN_INF_NONE   x = t
+ *   PINN_INF_BOTH   x = t / (1 - t^2)             (-inf, inf)   (reference src/transform_inf_integral.jl)
+ *   PINN_INF_UPPER  x = shift + t / (1 - t)       [a, inf)
+ *   PINN_INF_LOWER  x = shift + t / (1 + t)       (-inf, b]
+ * The Jacobian of the substitution is part of the integrand's program.  The integrand's point ("node point") has
+ * dim(owner) + n_dims rows: the owner's rows with row[k] replaced by x_k, then t_0 (, t_1).  Its taps, net_rows and
+ * program (COORD / TAP / PARAM / arithmetic; the last value is g) follow pinn_term_desc.  The owner's program reads
+ * the integral with PINN_OP_INTEGRAL a.  Integral terms run on the FFMA path only. */
+#define PINN_MAX_INTEGRALS 8   /* integrals per problem */
+#define PINN_MAX_QUAD 64       /* Gauss-Legendre nodes per integrating dimension */
+enum { PINN_INF_NONE = 0, PINN_INF_BOTH = 1, PINN_INF_UPPER = 2, PINN_INF_LOWER = 3 };
+typedef struct {
+  int32_t owner;               /* term whose program reads the integral                                  */
+  int32_t n_dims;              /* integrating dimensions, 1 or 2                                          */
+  int32_t q;                   /* Gauss-Legendre nodes per dimension, 1..PINN_MAX_QUAD                    */
+  int32_t row[2];              /* owner point row of each integrating variable                           */
+  int32_t lb_row[2], ub_row[2];   /* owner point row holding the bound (in t), or -1: the constant below   */
+  double lb[2], ub[2];         /* constant bounds in t                                                   */
+  int32_t inf_kind[2];         /* PINN_INF_*                                                             */
+  double shift[2];             /* PINN_INF_UPPER / LOWER: the shift of the substitution                  */
+  int32_t n_taps;
+  const pinn_tap_desc* taps;
+  const int32_t* net_rows;     /* [n_nets][PINN_MAX_IN]: node point row feeding input j of network k     */
+  int32_t n_instr;
+  const pinn_instr* prog;
+} pinn_integral_desc;
+
 /* ---- lifecycle ---------------------------------------------------------------- */
 int pinn_create(const pinn_problem_desc* desc, pinn_handle* out);
+/* pinn_create with integral terms integrals[n_integrals] (0 <= n_integrals <= PINN_MAX_INTEGRALS; 0 is pinn_create) */
+int pinn_create_ex(const pinn_problem_desc* desc, const pinn_integral_desc* integrals, int32_t n_integrals,
+                   pinn_handle* out);
 int pinn_destroy(pinn_handle h);
 const char* pinn_last_error(void);
 int pinn_abi_version(void);
@@ -383,8 +423,12 @@ double pinn_last_kernel_ms(pinn_handle h);
 /* bytes of device workspace owned by the handle */
 int64_t pinn_workspace_bytes(pinn_handle h);
 /* algorithmic FLOPs of one pinn_loss_grad at the current point sets:
- * 6 * sum_terms N * sum_nets C * S  (SURVEY section 8(d)) */
+ * 6 * sum_terms N * sum_nets C * S  (SURVEY section 8(d)); an integral adds 2 q^n_dims integrand evaluations per point
+ * of its owner term */
 double pinn_flops_per_eval(pinn_handle h);
+/* the q-point Gauss-Legendre rule on [-1, 1] that integral terms use (nodes ascending): x[q], w[q]; 1 <= q <= 64.
+ * Host only, no device needed. */
+int pinn_quadrature_nodes(int32_t q, double* x, double* w);
 
 #ifdef __cplusplus
 }

@@ -4,10 +4,11 @@ PhysicsInformedNN / discretize interface.
 The directory name contains a dot, so import it through the root-level alias module:
 ``import neuralpde_jl_b200 as npde``.
 """
-from .engine import (Engine, EngineError, NetSpec, ProblemSpec, TapSpec, TermSpec, EXPORTS, LIB_PATH,
+from .engine import (Engine, EngineError, IntegralSpec, NetSpec, ProblemSpec, TapSpec, TermSpec, EXPORTS, LIB_PATH,
                      MODE_FFMA, MODE_TC_BF16, MODE_TC_SPLIT, REDUCE_MEAN, REDUCE_WSUM, load_library)
-from .symbolic import (Differential, Eq, Equation, In, Interval, PDESystem, VarDomain, get_argument, get_variables,
-                       get_vars, parameters, variables)
+from .symbolic import (ClosedInterval, Differential, Eq, Equation, In, Inf, Integral, Interval, PDESystem,
+                       ProductDomain, UnitInterval, UnitSquare, VarDomain, get_argument, get_variables, get_vars,
+                       parameters, variables)
 from .lowering import LoweringError, lower_equation
 from .strategies import (AbstractTrainingStrategy, GridTraining, QuadratureTraining, QuasiRandomTraining,
                          StochasticTraining, generate_training_sets, get_bounds, shard_range)

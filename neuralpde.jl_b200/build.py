@@ -36,6 +36,11 @@ UNITS = [
     ("ffma_f32_gmem.o", "ffma_inst.cu", ["-DPINN_INST_REAL=float", "-DPINN_INST_BUFS=0"]),
     ("ffma_f64_smem.o", "ffma_inst.cu", ["-DPINN_INST_REAL=double", "-DPINN_INST_BUFS=1"]),
     ("ffma_f64_gmem.o", "ffma_inst.cu", ["-DPINN_INST_REAL=double", "-DPINN_INST_BUFS=0"]),
+    # the same four with integral terms (node tiles, PINN_OP_INTEGRAL)
+    ("ffma_f32_smem_integ.o", "ffma_inst.cu", ["-DPINN_INST_REAL=float", "-DPINN_INST_BUFS=1", "-DPINN_INST_INTEG=1"]),
+    ("ffma_f32_gmem_integ.o", "ffma_inst.cu", ["-DPINN_INST_REAL=float", "-DPINN_INST_BUFS=0", "-DPINN_INST_INTEG=1"]),
+    ("ffma_f64_smem_integ.o", "ffma_inst.cu", ["-DPINN_INST_REAL=double", "-DPINN_INST_BUFS=1", "-DPINN_INST_INTEG=1"]),
+    ("ffma_f64_gmem_integ.o", "ffma_inst.cu", ["-DPINN_INST_REAL=double", "-DPINN_INST_BUFS=0", "-DPINN_INST_INTEG=1"]),
 ]
 
 

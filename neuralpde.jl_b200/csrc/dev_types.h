@@ -66,11 +66,25 @@ struct TermDyn {
   int n_tiles;
 };
 
+// one integral term (pinn_integral_desc): the node-point geometry, the Gauss-Legendre table and the integrand, planned
+// like a term over the node point (dim = owner dim + n_dims rows)
+struct DevIntegral {
+  int owner;                        // owner term
+  int slot;                         // the owner reads the value as its tap n_taps + (index among its integrals)
+  int n_dims, q;
+  int row[2], lb_row[2], ub_row[2], inf_kind[2];
+  double lb[2], ub[2], shift[2];
+  double xi[PINN_MAX_QUAD], wq[PINN_MAX_QUAD];   // nodes and weights on [-1, 1]
+  DevTerm body;
+};
+
 struct DevProblem {
   int n_nets, n_terms, n_params;
   long long param_off, n_theta;
   DevNet nets[PINN_MAX_NETS];
   DevTerm terms[PINN_MAX_TERMS];
+  int n_integrals;
+  DevIntegral integ[PINN_MAX_INTEGRALS];
 };
 
 // per term scale (L_k = scale_k * sum_p qw_p r_p^2) and loss weight, passed by value

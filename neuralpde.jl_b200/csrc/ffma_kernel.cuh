@@ -521,9 +521,223 @@ __device__ __forceinline__ real warp_sum(real v) {
 }
 
 // ------------------------------------------------------------------------------------------
-template <typename real, bool BUFS_SMEM>
-__global__ void __launch_bounds__(kThreads, 1) ffma_loss_grad_kernel(const FfmaArgs args) {
+// forward through every network term tm taps, at the point tile X ([row][point]): the outputs land in taps; save:
+// keep the pre-activations in the stash for the reverse sweep
+template <typename real>
+__device__ __forceinline__ void forward_nets(const FfmaArgs& args, const DevProblem& P, const DevTerm& tm,
+                                             const real* __restrict__ theta, const real* X, real* bufA, real* bufB,
+                                             real* wsm, real* stash, real* taps, bool save, int ldc, int tid, int warp,
+                                             int lane) {
   constexpr int TP = Cfg<real>::TP;
+  for (int slot = 0; slot < tm.n_used; ++slot) {
+    const DevNet& net = P.nets[tm.used_net[slot]];
+    const DevChan& ch = tm.chan[slot];
+    const int C = ch.C;
+    real* H = bufA;
+    real* Z = bufB;
+    init_inputs<real>(H, X, ch, net.dims[0], ldc, tid);
+    for (int l = 0; l < net.n_layers; ++l) {
+      const int n_in = net.dims[l], n_out = net.dims[l + 1];
+      const int n_in8 = (n_in + 7) & ~7, n_out8 = (n_out + 7) & ~7;
+      if (args.weights_resident) {
+        const real* Wt = wsm + net.ws_off[l];
+        const real* bs = wsm + net.bs_off[l];
+        __syncthreads();   // layer inputs visible
+        for (int ob = warp * 8; ob < n_out8; ob += kWarps * 8) {
+          PINN_DISPATCH_C(C, (gemm_fwd_block<real, CC>(H, Z, Wt + ob, bs + ob, n_in, n_out, ob, n_out8, ldc, lane)));
+        }
+        __syncthreads();
+      } else {
+        constexpr int PW = kWarps * 8;   // panel of 64 output neurons
+        for (int pb = 0; pb < n_out8; pb += PW) {
+          stage_panel<real>(theta, net, l, 0, n_in8, pb, PW, wsm, wsm + n_in8 * PW, tid);
+          __syncthreads();   // panel (and, first time, layer inputs) visible
+          const int ob = pb + warp * 8;
+          if (ob < n_out8) {
+            PINN_DISPATCH_C(C, (gemm_fwd_block<real, CC>(H, Z, wsm + warp * 8, wsm + n_in8 * PW + warp * 8, n_in,
+                                                         n_out, ob, PW, ldc, lane)));
+          }
+          __syncthreads();   // panel consumed
+        }
+      }
+      elementwise_fwd<real>(Z, stash + ch.stash_off[l], ch, net.acts[l], n_out, ldc, warp, lane, save);
+      real* t = H; H = Z; Z = t;
+      // the next layer's __syncthreads (or the one below) orders these writes
+    }
+    __syncthreads();
+    // network outputs -> taps
+    for (int i = tid; i < tm.n_taps * kTilePts; i += kThreads) {
+      int t = i / kTilePts, p = i - t * kTilePts;
+      if (tm.tap_slot[t] == slot) taps[i] = H[tm.tap_ch[t] * ldc + tm.tap_out[t] * TP + p];
+    }
+    __syncthreads();
+  }
+}
+
+// reverse sweep through every network term tm taps, from the tap adjoints tapbar, into this CTA's gradient partial
+template <typename real>
+__device__ __forceinline__ void reverse_nets(const FfmaArgs& args, const DevProblem& P, const DevTerm& tm,
+                                             const real* __restrict__ theta, const real* X, real* bufA, real* bufB,
+                                             real* wsm, const real* stash, const real* tapbar, real* partial, int ldc,
+                                             int tid, int warp, int lane) {
+  constexpr int TP = Cfg<real>::TP;
+  for (int slot = 0; slot < tm.n_used; ++slot) {
+    const DevNet& net = P.nets[tm.used_net[slot]];
+    const DevChan& ch = tm.chan[slot];
+    const int C = ch.C;
+    const int L = net.n_layers;
+    real* B = bufA;   // adjoints
+    real* H = bufB;   // rebuilt layer inputs
+    // seed: adjoint of the network outputs
+    {
+      const int n_out = net.dims[L];
+      for (int i = tid; i < C * n_out * kTilePts; i += kThreads) {
+        int p = i & (kTilePts - 1);
+        int rest = i / kTilePts;
+        int o = rest % n_out, c = rest / n_out;
+        B[c * ldc + o * TP + p] = real(0);
+      }
+      __syncthreads();
+      // several taps may name the same (channel, out) element: one thread per point accumulates
+      if (tid < kTilePts) {
+        for (int t = 0; t < tm.n_taps; ++t)
+          if (tm.tap_slot[t] == slot)
+            B[tm.tap_ch[t] * ldc + tm.tap_out[t] * TP + tid] += tapbar[t * kTilePts + tid];
+      }
+      __syncthreads();
+    }
+    for (int l = L - 1; l >= 0; --l) {
+      const int n_in = net.dims[l], n_out = net.dims[l + 1];
+      const int n_in8 = (n_in + 7) & ~7, n_out8 = (n_out + 7) & ~7;
+      elementwise_bwd<real>(B, stash + ch.stash_off[l], ch, net.acts[l], n_out, ldc, warp, lane);
+      if (l == 0) init_inputs<real>(H, X, ch, n_in, ldc, tid);
+      else rebuild_h<real>(H, stash + ch.stash_off[l - 1], ch, net.acts[l - 1], n_in, ldc, warp, lane);
+      __syncthreads();
+      PINN_DISPATCH_C(C, (gemm_wgrad<real, CC>(B, H, partial + net.w_off[l], partial + net.b_off[l], n_in,
+                                               n_out, ldc, warp, lane)));
+      if (l > 0) {
+        __syncthreads();   // wgrad finished reading H before dgrad overwrites it
+        if (args.weights_resident) {
+          const real* Wt = wsm + net.ws_off[l];
+          for (int kb = warp * 8; kb < n_in8; kb += kWarps * 8) {
+            PINN_DISPATCH_C(C, (gemm_dgrad_block<real, CC>(B, H, Wt + kb * n_out8, n_in, n_out, kb, n_out8, ldc,
+                                                           lane)));
+          }
+        } else {
+          constexpr int PW = kWarps * 8;   // panel of 64 input neurons
+          for (int pb = 0; pb < n_in8; pb += PW) {
+            stage_panel<real>(theta, net, l, pb, PW, 0, n_out8, wsm, (real*)nullptr, tid);
+            __syncthreads();
+            const int kb = pb + warp * 8;
+            if (kb < n_in8) {
+              PINN_DISPATCH_C(C, (gemm_dgrad_block<real, CC>(B, H, wsm + warp * 8 * n_out8, n_in, n_out, kb,
+                                                             n_out8, ldc, lane)));
+            }
+            __syncthreads();
+          }
+        }
+        real* t = B; B = H; H = t;
+      }
+      __syncthreads();
+    }
+  }
+}
+
+// ---- integral terms (pinn_create_ex) -----------------------------------------------------------------------------------
+// The owner tile's 32 points (lane == point) and node j of integral I give one more tile of 32 node points, lane ==
+// owner point: no cross-lane reduction, no grid barrier, no extra launch.  The forward pass runs every node tile and
+// accumulates I_p = sum_j w_j(p) g_j(p) in a register of warp 0; the reverse pass recomputes each node tile and sweeps it
+// back with the seed dtotal/dI_p * w_j(p).
+
+// node j of integral I for this lane's owner point: writes the node point (the owner's rows with the integrating rows
+// replaced by x_k(t_k), then the t_k) into Xn and returns the node weight w_j(p) = prod_k (hi_k - lo_k) / 2 * wq[j_k]
+template <typename real>
+__device__ __forceinline__ real node_tile(const DevIntegral& I, int dim, int j, const real* Xs, real* Xn, int lane) {
+  for (int r = 0; r < dim; ++r) Xn[r * kTilePts + lane] = Xs[r * kTilePts + lane];
+  real w = real(1);
+  for (int k = 0; k < I.n_dims; ++k, j /= I.q) {
+    const int jk = j % I.q;
+    const real lo = I.lb_row[k] >= 0 ? Xs[I.lb_row[k] * kTilePts + lane] : real(I.lb[k]);
+    const real hi = I.ub_row[k] >= 0 ? Xs[I.ub_row[k] * kTilePts + lane] : real(I.ub[k]);
+    const real h = real(0.5) * (hi - lo);
+    const real t = lo + h * (real(1) + real(I.xi[jk]));
+    real x = t;
+    if (I.inf_kind[k] == PINN_INF_BOTH) x = t / (real(1) - t * t);
+    else if (I.inf_kind[k] == PINN_INF_UPPER) x = real(I.shift[k]) + t / (real(1) - t);
+    else if (I.inf_kind[k] == PINN_INF_LOWER) x = real(I.shift[k]) + t / (real(1) + t);
+    Xn[I.row[k] * kTilePts + lane] = x;
+    Xn[(dim + k) * kTilePts + lane] = t;
+    w *= h * real(I.wq[jk]);
+  }
+  return w;
+}
+
+inline __device__ int node_count(const DevIntegral& I) { return I.n_dims == 2 ? I.q * I.q : I.q; }
+
+// values of term ti's integrals at the owner tile Xs: ival[k][p] for its k-th integral
+template <typename real>
+__device__ __forceinline__ void integrals_forward(const FfmaArgs& args, const DevProblem& P, int ti,
+                                                  const real* __restrict__ theta, const real* Xs, real* Xn, real* ival,
+                                                  real* bufA, real* bufB, real* wsm, real* stash, real* taps, int tid,
+                                                  int warp, int lane) {
+  int k = 0;
+  for (int i = 0; i < P.n_integrals; ++i) {
+    const DevIntegral& I = P.integ[i];
+    if (I.owner != ti) continue;
+    real acc = real(0), wj = real(0);
+    for (int j = 0; j < node_count(I); ++j) {
+      if (warp == 0) wj = node_tile<real>(I, P.terms[ti].dim, j, Xs, Xn, lane);
+      __syncthreads();
+      forward_nets<real>(args, P, I.body, theta, Xn, bufA, bufB, wsm, stash, taps, false, args.ldc, tid, warp, lane);
+      if (warp == 0)
+        acc += wj * run_program<real, kTilePts>(I.body, theta + P.param_off, Xn, taps, (real*)nullptr, (real*)nullptr,
+                                                lane, false);
+    }
+    if (warp == 0) ival[k * kTilePts + lane] = acc;
+    ++k;
+  }
+}
+
+// gradient of term ti's integrals, given ibar[k][p] = dtotal / dI_p of its k-th integral
+template <typename real>
+__device__ __forceinline__ void integrals_reverse(const FfmaArgs& args, const DevProblem& P, int ti,
+                                                  const real* __restrict__ theta, const real* Xs, real* Xn,
+                                                  const real* ibar, real* bufA, real* bufB, real* wsm, real* stash,
+                                                  real* taps, real* tapbar, real* partial, int tid, int warp, int lane) {
+  int k = 0;
+  for (int i = 0; i < P.n_integrals; ++i) {
+    const DevIntegral& I = P.integ[i];
+    if (I.owner != ti) continue;
+    const DevTerm& body = I.body;
+    real wj = real(0);
+    for (int j = 0; j < node_count(I); ++j) {
+      if (warp == 0) wj = node_tile<real>(I, P.terms[ti].dim, j, Xs, Xn, lane);
+      __syncthreads();
+      forward_nets<real>(args, P, body, theta, Xn, bufA, bufB, wsm, stash, taps, true, args.ldc, tid, warp, lane);
+      if (warp == 0) {
+        real pbar[PINN_MAX_PARAMS];
+#pragma unroll
+        for (int q = 0; q < PINN_MAX_PARAMS; ++q) pbar[q] = real(0);
+        for (int t = 0; t < body.n_taps; ++t) tapbar[t * kTilePts + lane] = real(0);
+        run_program<real, kTilePts>(body, theta + P.param_off, Xn, taps, tapbar, pbar, lane, true);
+        const real sd = ibar[k * kTilePts + lane] * wj;
+        for (int t = 0; t < body.n_taps; ++t) tapbar[t * kTilePts + lane] *= sd;
+        for (int q = 0; q < P.n_params; ++q) {
+          real v = warp_sum<real>(pbar[q] * sd);
+          if (lane == 0) partial[P.param_off + q] += v;
+        }
+      }
+      __syncthreads();
+      reverse_nets<real>(args, P, body, theta, Xn, bufA, bufB, wsm, stash, tapbar, partial, args.ldc, tid, warp, lane);
+    }
+    ++k;
+  }
+}
+
+// ------------------------------------------------------------------------------------------
+// INTEG: the problem has integral terms (pinn_create_ex); the instantiation without them is the kernel as it was
+template <typename real, bool BUFS_SMEM, bool INTEG>
+__global__ void __launch_bounds__(kThreads, 1) ffma_loss_grad_kernel(const FfmaArgs args) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const DevProblem& P = *args.prob;
@@ -547,6 +761,8 @@ __global__ void __launch_bounds__(kThreads, 1) ffma_loss_grad_kernel(const FfmaA
   real* rres = sm; sm += kTilePts;      // residual per point
   real* qws = sm; sm += kTilePts;       // quadrature weight per point (0 for padded lanes)
   double* tsum = reinterpret_cast<double*>(sm);  // [PINN_MAX_TERMS], 8-byte aligned by construction
+  real* Xn = reinterpret_cast<real*>(tsum + PINN_MAX_TERMS);   // INTEG: node-point tile
+  real* ival = Xn + (PINN_MAX_DIM + 2) * kTilePts;              // INTEG: the term's integrals, then their adjoints
 
   real* partial = reinterpret_cast<real*>(args.partial) + (long long)blockIdx.x * args.partial_stride;
   real* stash = reinterpret_cast<real*>(args.stash) + (long long)blockIdx.x * args.stash_per_cta;
@@ -593,56 +809,25 @@ __global__ void __launch_bounds__(kThreads, 1) ffma_loss_grad_kernel(const FfmaA
     for (int i = tid; i < tm.n_taps * kTilePts; i += kThreads) tapbar[i] = real(0);
     __syncthreads();
 
-    // ---- forward through every tapped network ------------------------------------------------
-    for (int slot = 0; slot < tm.n_used; ++slot) {
-      const DevNet& net = P.nets[tm.used_net[slot]];
-      const DevChan& ch = tm.chan[slot];
-      const int C = ch.C;
-      real* H = bufA;
-      real* Z = bufB;
-      init_inputs<real>(H, Xs, ch, net.dims[0], ldc, tid);
-      for (int l = 0; l < net.n_layers; ++l) {
-        const int n_in = net.dims[l], n_out = net.dims[l + 1];
-        const int n_in8 = (n_in + 7) & ~7, n_out8 = (n_out + 7) & ~7;
-        if (args.weights_resident) {
-          const real* Wt = wsm + net.ws_off[l];
-          const real* bs = wsm + net.bs_off[l];
-          __syncthreads();   // layer inputs visible
-          for (int ob = warp * 8; ob < n_out8; ob += kWarps * 8) {
-            PINN_DISPATCH_C(C, (gemm_fwd_block<real, CC>(H, Z, Wt + ob, bs + ob, n_in, n_out, ob, n_out8, ldc, lane)));
-          }
-          __syncthreads();
-        } else {
-          constexpr int PW = kWarps * 8;   // panel of 64 output neurons
-          for (int pb = 0; pb < n_out8; pb += PW) {
-            stage_panel<real>(theta, net, l, 0, n_in8, pb, PW, wsm, wsm + n_in8 * PW, tid);
-            __syncthreads();   // panel (and, first time, layer inputs) visible
-            const int ob = pb + warp * 8;
-            if (ob < n_out8) {
-              PINN_DISPATCH_C(C, (gemm_fwd_block<real, CC>(H, Z, wsm + warp * 8, wsm + n_in8 * PW + warp * 8, n_in,
-                                                           n_out, ob, PW, ldc, lane)));
-            }
-            __syncthreads();   // panel consumed
-          }
-        }
-        elementwise_fwd<real>(Z, stash + ch.stash_off[l], ch, net.acts[l], n_out, ldc, warp, lane, want_grad);
-        real* t = H; H = Z; Z = t;
-        // the next layer's __syncthreads (or the one below) orders these writes
-      }
-      __syncthreads();
-      // network outputs -> taps
-      for (int i = tid; i < tm.n_taps * kTilePts; i += kThreads) {
-        int t = i / kTilePts, p = i - t * kTilePts;
-        if (tm.tap_slot[t] == slot) taps[i] = H[tm.tap_ch[t] * ldc + tm.tap_out[t] * TP + p];
-      }
-      __syncthreads();
+    int n_int = 0;   // integrals of this term (uniform)
+    if constexpr (INTEG) {
+      for (int i = 0; i < P.n_integrals; ++i) n_int += P.integ[i].owner == ti;
+      if (n_int) integrals_forward<real>(args, P, ti, theta, Xs, Xn, ival, bufA, bufB, wsm, stash, taps, tid, warp, lane);
     }
+
+    // ---- forward through every tapped network ------------------------------------------------
+    forward_nets<real>(args, P, tm, theta, Xs, bufA, bufB, wsm, stash, taps, want_grad, ldc, tid, warp, lane);
 
     // ---- residual, loss partial, tap adjoints (warp 0, lane == point) --------------------------
     if (warp == 0) {
       real pbar[PINN_MAX_PARAMS];
 #pragma unroll
       for (int j = 0; j < PINN_MAX_PARAMS; ++j) pbar[j] = real(0);
+      if constexpr (INTEG)
+        for (int k = 0; k < n_int; ++k) {   // the program reads integral k as tap n_taps + k
+          taps[(tm.n_taps + k) * kTilePts + lane] = ival[k * kTilePts + lane];
+          tapbar[(tm.n_taps + k) * kTilePts + lane] = real(0);
+        }
       const real r = run_program<real, kTilePts>(tm, theta + P.param_off, Xs, taps, tapbar, pbar, lane, want_grad);
       const real w = qws[lane];
       rres[lane] = r;
@@ -657,6 +842,8 @@ __global__ void __launch_bounds__(kThreads, 1) ffma_loss_grad_kernel(const FfmaA
       if (want_grad) {
         const real g = real(args.seed[ti]) * w * real(2) * r;   // d total / d r_p
         for (int t = 0; t < tm.n_taps; ++t) tapbar[t * kTilePts + lane] *= g;
+        if constexpr (INTEG)
+          for (int k = 0; k < n_int; ++k) ival[k * kTilePts + lane] = tapbar[(tm.n_taps + k) * kTilePts + lane] * g;
         for (int j = 0; j < P.n_params; ++j) {
           real v = warp_sum<real>(pbar[j] * g);
           if (lane == 0) partial[P.param_off + j] += v;
@@ -666,68 +853,11 @@ __global__ void __launch_bounds__(kThreads, 1) ffma_loss_grad_kernel(const FfmaA
     __syncthreads();
 
     // ---- reverse sweep through every tapped network -----------------------------------------------
-    if (want_grad) {
-      for (int slot = 0; slot < tm.n_used; ++slot) {
-        const DevNet& net = P.nets[tm.used_net[slot]];
-        const DevChan& ch = tm.chan[slot];
-        const int C = ch.C;
-        const int L = net.n_layers;
-        real* B = bufA;   // adjoints
-        real* H = bufB;   // rebuilt layer inputs
-        // seed: adjoint of the network outputs
-        {
-          const int n_out = net.dims[L];
-          for (int i = tid; i < C * n_out * kTilePts; i += kThreads) {
-            int p = i & (kTilePts - 1);
-            int rest = i / kTilePts;
-            int o = rest % n_out, c = rest / n_out;
-            B[c * ldc + o * TP + p] = real(0);
-          }
-          __syncthreads();
-          // several taps may name the same (channel, out) element: one thread per point accumulates
-          if (tid < kTilePts) {
-            for (int t = 0; t < tm.n_taps; ++t)
-              if (tm.tap_slot[t] == slot)
-                B[tm.tap_ch[t] * ldc + tm.tap_out[t] * TP + tid] += tapbar[t * kTilePts + tid];
-          }
-          __syncthreads();
-        }
-        for (int l = L - 1; l >= 0; --l) {
-          const int n_in = net.dims[l], n_out = net.dims[l + 1];
-          const int n_in8 = (n_in + 7) & ~7, n_out8 = (n_out + 7) & ~7;
-          elementwise_bwd<real>(B, stash + ch.stash_off[l], ch, net.acts[l], n_out, ldc, warp, lane);
-          if (l == 0) init_inputs<real>(H, Xs, ch, n_in, ldc, tid);
-          else rebuild_h<real>(H, stash + ch.stash_off[l - 1], ch, net.acts[l - 1], n_in, ldc, warp, lane);
-          __syncthreads();
-          PINN_DISPATCH_C(C, (gemm_wgrad<real, CC>(B, H, partial + net.w_off[l], partial + net.b_off[l], n_in,
-                                                   n_out, ldc, warp, lane)));
-          if (l > 0) {
-            __syncthreads();   // wgrad finished reading H before dgrad overwrites it
-            if (args.weights_resident) {
-              const real* Wt = wsm + net.ws_off[l];
-              for (int kb = warp * 8; kb < n_in8; kb += kWarps * 8) {
-                PINN_DISPATCH_C(C, (gemm_dgrad_block<real, CC>(B, H, Wt + kb * n_out8, n_in, n_out, kb, n_out8, ldc,
-                                                               lane)));
-              }
-            } else {
-              constexpr int PW = kWarps * 8;   // panel of 64 input neurons
-              for (int pb = 0; pb < n_in8; pb += PW) {
-                stage_panel<real>(theta, net, l, pb, PW, 0, n_out8, wsm, (real*)nullptr, tid);
-                __syncthreads();
-                const int kb = pb + warp * 8;
-                if (kb < n_in8) {
-                  PINN_DISPATCH_C(C, (gemm_dgrad_block<real, CC>(B, H, wsm + warp * 8 * n_out8, n_in, n_out, kb,
-                                                                 n_out8, ldc, lane)));
-                }
-                __syncthreads();
-              }
-            }
-            real* t = B; B = H; H = t;
-          }
-          __syncthreads();
-        }
-      }
-    }
+    if (want_grad) reverse_nets<real>(args, P, tm, theta, Xs, bufA, bufB, wsm, stash, tapbar, partial, ldc, tid, warp, lane);
+    if constexpr (INTEG)
+      if (want_grad && n_int)
+        integrals_reverse<real>(args, P, ti, theta, Xs, Xn, ival, bufA, bufB, wsm, stash, taps, tapbar, partial, tid, warp,
+                                lane);
   }
 
   __syncthreads();

@@ -25,13 +25,15 @@ __global__ void finish_kernel(const real* __restrict__ packed, long long n_grad,
 }
 
 // ---- host-callable launchers -------------------------------------------------------------------
-size_t ffma_smem_bytes(int dtype, long long buf_elems, int w_area, bool bufs_smem) {
+// integ: after the term sums, the node-point tile ((PINN_MAX_DIM + 2) rows) and one row per integral of the term
+size_t ffma_smem_bytes(int dtype, long long buf_elems, int w_area, bool bufs_smem, bool integ) {
   size_t es = dtype == PINN_F64 ? 8 : 4;
   size_t n = (bufs_smem ? 2 * (size_t)buf_elems : 0) + (size_t)w_area + PINN_MAX_DIM * kTilePts +
              2 * PINN_MAX_TAPS * kTilePts + 2 * kTilePts;
   size_t bytes = n * es;
   bytes = (bytes + 7) & ~size_t(7);
   bytes += PINN_MAX_TERMS * sizeof(double);
+  if (integ) bytes += (size_t)(PINN_MAX_DIM + 2 + PINN_MAX_INTEGRALS) * kTilePts * es;
   return bytes;
 }
 
@@ -39,8 +41,18 @@ cudaError_t ffma_launch_float_smem(const FfmaArgs& a, int grid, size_t smem, cud
 cudaError_t ffma_launch_float_gmem(const FfmaArgs& a, int grid, size_t smem, cudaStream_t st);
 cudaError_t ffma_launch_double_smem(const FfmaArgs& a, int grid, size_t smem, cudaStream_t st);
 cudaError_t ffma_launch_double_gmem(const FfmaArgs& a, int grid, size_t smem, cudaStream_t st);
+cudaError_t ffma_launch_float_smem_integ(const FfmaArgs& a, int grid, size_t smem, cudaStream_t st);
+cudaError_t ffma_launch_float_gmem_integ(const FfmaArgs& a, int grid, size_t smem, cudaStream_t st);
+cudaError_t ffma_launch_double_smem_integ(const FfmaArgs& a, int grid, size_t smem, cudaStream_t st);
+cudaError_t ffma_launch_double_gmem_integ(const FfmaArgs& a, int grid, size_t smem, cudaStream_t st);
 
-cudaError_t ffma_launch(int dtype, bool bufs_smem, const FfmaArgs& a, int grid, size_t smem, cudaStream_t st) {
+// integ: the instantiation that evaluates integral terms on node tiles
+cudaError_t ffma_launch(int dtype, bool bufs_smem, bool integ, const FfmaArgs& a, int grid, size_t smem, cudaStream_t st) {
+  if (integ) {
+    if (dtype == PINN_F64)
+      return bufs_smem ? ffma_launch_double_smem_integ(a, grid, smem, st) : ffma_launch_double_gmem_integ(a, grid, smem, st);
+    return bufs_smem ? ffma_launch_float_smem_integ(a, grid, smem, st) : ffma_launch_float_gmem_integ(a, grid, smem, st);
+  }
   if (dtype == PINN_F64)
     return bufs_smem ? ffma_launch_double_smem(a, grid, smem, st) : ffma_launch_double_gmem(a, grid, smem, st);
   return bufs_smem ? ffma_launch_float_smem(a, grid, smem, st) : ffma_launch_float_gmem(a, grid, smem, st);

@@ -15,7 +15,7 @@
 #include "engine.h"
 
 namespace pinn {
-cudaError_t ffma_launch(int dtype, bool bufs_smem, const FfmaArgs& a, int grid, size_t smem, cudaStream_t st);
+cudaError_t ffma_launch(int dtype, bool bufs_smem, bool integ, const FfmaArgs& a, int grid, size_t smem, cudaStream_t st);
 cudaError_t grad_stats_launch(int dtype, const void* grad, long long n, double* out2, cudaStream_t st);
 cudaError_t sample_uniform_launch(int dtype, void* pts, long long n, int dim, const double* lb, const double* ub,
                                   unsigned long long seed, unsigned long long draw, const unsigned long long* draw_dev,
@@ -148,7 +148,16 @@ int pinn_destroy(pinn_handle e) {
   return 0;
 }
 
-int pinn_create(const pinn_problem_desc* d, pinn_handle* out) {
+int pinn_create(const pinn_problem_desc* d, pinn_handle* out) { return pinn_create_ex(d, nullptr, 0, out); }
+
+int pinn_quadrature_nodes(int32_t q, double* x, double* w) {
+  if (q < 1 || q > PINN_MAX_QUAD) return fail("pinn_quadrature_nodes: q=%d out of range [1,%d]", q, PINN_MAX_QUAD);
+  if (!x || !w) return fail("pinn_quadrature_nodes: null output");
+  gauss_legendre(q, x, w);
+  return 0;
+}
+
+int pinn_create_ex(const pinn_problem_desc* d, const pinn_integral_desc* integrals, int32_t n_integrals, pinn_handle* out) {
   if (!out) return fail("pinn_create: null output handle");
   *out = nullptr;
   if (!d) return fail("pinn_create: null descriptor");
@@ -166,7 +175,7 @@ int pinn_create(const pinn_problem_desc* d, pinn_handle* out) {
   int max_smem = 0;
   cudaDeviceGetAttribute(&max_smem, cudaDevAttrMaxSharedMemoryPerBlockOptin, e->device);
   if (max_smem <= 0) max_smem = 227 * 1024;
-  if (plan_problem(d, max_smem, e->plan)) { pinn_destroy(e); return 1; }
+  if (plan_problem(d, integrals, n_integrals, max_smem, e->plan)) { pinn_destroy(e); return 1; }
   const Plan& p = e->plan;
   cudaDeviceGetAttribute(&e->num_sms, cudaDevAttrMultiProcessorCount, e->device);
   if (e->num_sms <= 0) e->num_sms = 132;
@@ -308,7 +317,7 @@ static int launch_fused(pinn_engine* e, const LaunchCall& c, int grid, cudaStrea
   if (e->mode == PINN_MODE_FFMA) {
     FfmaArgs a = with_call(p.ffma, e, c);
     a.n_tiles = e->total_tiles;
-    CUDA_TRY(ffma_launch(e->dtype, p.bufs_smem, a, grid, p.smem, st));
+    CUDA_TRY(ffma_launch(e->dtype, p.bufs_smem, p.integ, a, grid, p.smem, st));
     return 0;
   }
   if (p.wide) {

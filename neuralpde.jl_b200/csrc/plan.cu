@@ -8,7 +8,7 @@
 #include "plan.h"
 
 namespace pinn {
-size_t ffma_smem_bytes(int dtype, long long buf_elems, int w_area, bool bufs_smem);   // ffma_launch.cu
+size_t ffma_smem_bytes(int dtype, long long buf_elems, int w_area, bool bufs_smem, bool integ);   // ffma_launch.cu
 
 static thread_local std::string g_err;
 int fail(const char* fmt, ...) {
@@ -68,21 +68,22 @@ void dir_pair(const DevChan& ch, const int* dir, int& a, int& b) {
   if (a > b) std::swap(a, b);
 }
 // room for one more derivative channel
-int check_room(const DevChan& ch, int t, int net) {
+int check_room(const DevChan& ch, const char* what, int t, int net) {
   if (1 + ch.n1 + ch.n2 + ch.n3 < PINN_MAX_CH) return 0;
-  return fail("pinn_create: term %d network %d needs more than %d channels", t, net, PINN_MAX_CH);
+  return fail("pinn_create: %s %d network %d needs more than %d channels", what, t, net, PINN_MAX_CH);
 }
 
 // slots (the networks the term taps, in order of first use, with the point rows feeding their inputs), then the
 // derivative channels of every slot: first derivatives (needed directly or as intermediates), then second and pure
 // third derivatives (order 3 needs the pure second derivative along the same direction as an intermediate)
-int plan_channels(const pinn_problem_desc* d, int t, const DevProblem& P, DevTerm& T, int* slot_of) {
-  const pinn_term_desc& td = d->terms[t];
+// (what, t: "term" / "integral" and its index, for the messages)
+int plan_channels(const pinn_problem_desc* d, const pinn_term_desc& td, const char* what, int t, const DevProblem& P,
+                  DevTerm& T, int* slot_of) {
   for (int k = 0; k < PINN_MAX_NETS; ++k) slot_of[k] = -1;
   T.n_used = 0;
   for (int i = 0; i < td.n_taps; ++i) {
     const pinn_tap_desc& tp = td.taps[i];
-    if (tp.net < 0 || tp.net >= d->n_nets) return fail("pinn_create: term %d tap %d names network %d", t, i, tp.net);
+    if (tp.net < 0 || tp.net >= d->n_nets) return fail("pinn_create: %s %d tap %d names network %d", what, t, i, tp.net);
     if (slot_of[tp.net] >= 0) continue;
     slot_of[tp.net] = T.n_used;
     T.used_net[T.n_used] = tp.net;
@@ -90,7 +91,7 @@ int plan_channels(const pinn_problem_desc* d, int t, const DevProblem& P, DevTer
     for (int j = 0; j < P.nets[tp.net].dims[0]; ++j) {
       int r = td.net_rows[tp.net * PINN_MAX_IN + j];
       if (r < 0 || r >= td.dim)
-        return fail("pinn_create: term %d network %d input %d maps to point row %d (dim=%d)", t, tp.net, j, r, td.dim);
+        return fail("pinn_create: %s %d network %d input %d maps to point row %d (dim=%d)", what, t, tp.net, j, r, td.dim);
       ch.rows[j] = r;
     }
     ++T.n_used;
@@ -100,16 +101,17 @@ int plan_channels(const pinn_problem_desc* d, int t, const DevProblem& P, DevTer
     const DevNet& n = P.nets[tp.net];
     DevChan& ch = T.chan[slot_of[tp.net]];
     if (tp.order < 0 || tp.order > 3)
-      return fail("pinn_create: term %d tap %d has derivative order %d; orders 0..3 are supported (order 4 and mixed "
-                  "third derivatives are not)", t, i, tp.order);
+      return fail("pinn_create: %s %d tap %d has derivative order %d; orders 0..3 are supported (order 4 and mixed "
+                  "third derivatives are not)", what, t, i, tp.order);
     if (tp.order == 3 && !(tp.dir[0] == tp.dir[1] && tp.dir[1] == tp.dir[2]))
-      return fail("pinn_create: term %d tap %d is a mixed third derivative; only pure third derivatives d^3/dx_i^3 are "
-                  "supported", t, i);
+      return fail("pinn_create: %s %d tap %d is a mixed third derivative; only pure third derivatives d^3/dx_i^3 are "
+                  "supported", what, t, i);
     if (tp.out < 0 || tp.out >= n.dims[n.n_layers])
-      return fail("pinn_create: term %d tap %d output component %d out of range", t, i, tp.out);
+      return fail("pinn_create: %s %d tap %d output component %d out of range", what, t, i, tp.out);
     for (int q = 0; q < tp.order; ++q)
       if (tp.dir[q] < 0 || tp.dir[q] >= n.dims[0])
-        return fail("pinn_create: term %d tap %d direction %d out of range for a %d-input network", t, i, tp.dir[q], n.dims[0]);
+        return fail("pinn_create: %s %d tap %d direction %d out of range for a %d-input network", what, t, i, tp.dir[q],
+                    n.dims[0]);
     for (int q = 0; q < tp.order; ++q)
       if (find_dir(ch, tp.dir[q]) < 0) ch.dir1[ch.n1++] = tp.dir[q];
   }
@@ -120,11 +122,11 @@ int plan_channels(const pinn_problem_desc* d, int t, const DevProblem& P, DevTer
     int a, b;
     dir_pair(ch, tp.dir, a, b);
     if (find_pair(ch, a, b) < 0) {
-      if (check_room(ch, t, tp.net)) return 1;
+      if (check_room(ch, what, t, tp.net)) return 1;
       ch.s_a[ch.n2] = a; ch.s_b[ch.n2] = b; ++ch.n2;
     }
     if (tp.order == 3 && find_third(ch, a) < 0) {
-      if (check_room(ch, t, tp.net)) return 1;
+      if (check_room(ch, what, t, tp.net)) return 1;
       ch.t_a[ch.n3++] = a;
     }
   }
@@ -157,8 +159,10 @@ void canonical_order(DevChan& ch) {
 }
 
 // ---- tap mapping and the residual program ----------------------------------------------------------------------------
-int plan_taps(const pinn_problem_desc* d, int t, const int* slot_of, DevTerm& T) {
-  const pinn_term_desc& td = d->terms[t];
+// PINN_OP_INTEGRAL a (terms only) becomes a TAP of index n_taps + k, k = the rank of integral a among the term's
+// integrals: the fused kernel stores the integral's value there
+int plan_taps(const pinn_problem_desc* d, const pinn_term_desc& td, const char* what, int t, const int* slot_of,
+              const pinn_integral_desc* integrals, int n_integrals, DevTerm& T) {
   for (int i = 0; i < td.n_taps; ++i) {
     const pinn_tap_desc& tp = td.taps[i];
     const DevChan& ch = T.chan[slot_of[tp.net]];
@@ -171,6 +175,7 @@ int plan_taps(const pinn_problem_desc* d, int t, const int* slot_of, DevTerm& T)
     else T.tap_ch[i] = 1 + ch.n1 + ch.n2 + find_third(ch, find_dir(ch, tp.dir[0]));
   }
   bool any_tap = false;
+  const bool is_term = strcmp(what, "term") == 0;
   for (int i = 0; i < td.n_instr; ++i) {
     const pinn_instr& in = td.prog[i];
     DevInstr& o = T.prog[i];
@@ -179,56 +184,62 @@ int plan_taps(const pinn_problem_desc* d, int t, const int* slot_of, DevTerm& T)
     switch (in.op) {
       case PINN_OP_CONST: break;
       case PINN_OP_COORD:
-        if (in.a < 0 || in.a >= td.dim) return fail("pinn_create: term %d instr %d COORD row %d out of range", t, i, in.a);
+        if (in.a < 0 || in.a >= td.dim) return fail("pinn_create: %s %d instr %d COORD row %d out of range", what, t, i, in.a);
         break;
       case PINN_OP_TAP:
-        if (in.a < 0 || in.a >= td.n_taps) return fail("pinn_create: term %d instr %d TAP %d out of range", t, i, in.a);
+        if (in.a < 0 || in.a >= td.n_taps) return fail("pinn_create: %s %d instr %d TAP %d out of range", what, t, i, in.a);
         any_tap = true;
         break;
       case PINN_OP_PARAM:
-        if (in.a < 0 || in.a >= d->n_params) return fail("pinn_create: term %d instr %d PARAM %d out of range", t, i, in.a);
+        if (in.a < 0 || in.a >= d->n_params) return fail("pinn_create: %s %d instr %d PARAM %d out of range", what, t, i, in.a);
         break;
+      case PINN_OP_INTEGRAL: {
+        if (!is_term) return fail("pinn_create: integral %d instr %d: integrals nested in an integrand are not supported", t, i);
+        if (n_integrals == 0)
+          return fail("pinn_create: term %d instr %d reads an integral; integral terms are created with pinn_create_ex", t, i);
+        if (in.a < 0 || in.a >= n_integrals) return fail("pinn_create: term %d instr %d INTEGRAL %d out of range", t, i, in.a);
+        if (integrals[in.a].owner != t)
+          return fail("pinn_create: term %d instr %d reads integral %d, which belongs to term %d", t, i, in.a,
+                      integrals[in.a].owner);
+        int k = 0;
+        for (int j = 0; j < in.a; ++j) k += integrals[j].owner == t;
+        o.op = PINN_OP_TAP; o.a = td.n_taps + k;
+        any_tap = true;
+      } break;
       case PINN_OP_ADD: case PINN_OP_SUB: case PINN_OP_MUL: case PINN_OP_DIV: case PINN_OP_POW:
-        if (!val_ok(in.a) || !val_ok(in.b)) return fail("pinn_create: term %d instr %d operand out of range", t, i);
+        if (!val_ok(in.a) || !val_ok(in.b)) return fail("pinn_create: %s %d instr %d operand out of range", what, t, i);
         break;
       case PINN_OP_NEG: case PINN_OP_POWI: case PINN_OP_SIN: case PINN_OP_COS: case PINN_OP_EXP:
       case PINN_OP_LOG: case PINN_OP_TANH: case PINN_OP_SQRT: case PINN_OP_ABS:
-        if (!val_ok(in.a)) return fail("pinn_create: term %d instr %d operand out of range", t, i);
+        if (!val_ok(in.a)) return fail("pinn_create: %s %d instr %d operand out of range", what, t, i);
         break;
       default:
-        return fail("pinn_create: term %d instr %d unknown opcode %d", t, i, in.op);
+        return fail("pinn_create: %s %d instr %d unknown opcode %d", what, t, i, in.op);
     }
   }
-  if (!any_tap) return fail("pinn_create: term %d residual program never reads a tap (nothing depends on theta)", t);
+  if (!any_tap) return fail("pinn_create: %s %d %s program never reads a tap (nothing depends on theta)", what, t,
+                           is_term ? "residual" : "integrand");
   return 0;
 }
 
-// one term: channels, the FFMA stash layout (stash_max: scalars per CTA), taps, program and FLOPs per point
-int plan_term(const pinn_problem_desc* d, int t, DevProblem& P, TermPlan& tp, int& max_c, long long& stash_max) {
-  const pinn_term_desc& td = d->terms[t];
-  DevTerm& T = P.terms[t];
-  if (td.dim < 1 || td.dim > PINN_MAX_DIM) return fail("pinn_create: term %d dim=%d out of range [1,%d]", t, td.dim, PINN_MAX_DIM);
-  if (td.n_taps < 1)
-    return fail("pinn_create: term %d has no network taps (an equation such as 0 ~ 0 cannot be trained on)", t);
-  if (td.n_taps > PINN_MAX_TAPS) return fail("pinn_create: term %d has %d taps (max %d)", t, td.n_taps, PINN_MAX_TAPS);
+// the networks of a term or an integrand: channels, the FFMA stash layout (stash_max: scalars per CTA), taps and program;
+// *flops: algorithmic flops per point, 6 * sum_nets C * S
+int plan_body(const pinn_problem_desc* d, const pinn_term_desc& td, const char* what, int t, DevProblem& P, DevTerm& T,
+              const pinn_integral_desc* integrals, int n_integrals, int& max_c, long long& stash_max, double* flops) {
+  if (td.n_taps > PINN_MAX_TAPS) return fail("pinn_create: %s %d has %d taps (max %d)", what, t, td.n_taps, PINN_MAX_TAPS);
   if (td.n_instr < 1 || td.n_instr > PINN_MAX_INSTR)
-    return fail("pinn_create: term %d program length %d out of range [1,%d]", t, td.n_instr, PINN_MAX_INSTR);
-  if (!td.taps || !td.prog || !td.net_rows) return fail("pinn_create: term %d null taps/prog/net_rows", t);
-  if (td.reduction != PINN_REDUCE_MEAN && td.reduction != PINN_REDUCE_WSUM)
-    return fail("pinn_create: term %d unknown reduction %d", t, td.reduction);
+    return fail("pinn_create: %s %d program length %d out of range [1,%d]", what, t, td.n_instr, PINN_MAX_INSTR);
+  if (!td.taps || !td.prog || !td.net_rows) return fail("pinn_create: %s %d null taps/prog/net_rows", what, t);
   T.dim = td.dim; T.n_taps = td.n_taps; T.n_instr = td.n_instr;
-  T.weighted = td.reduction == PINN_REDUCE_WSUM;
-  tp.reduction = td.reduction;
-  tp.scale = td.reduction == PINN_REDUCE_WSUM ? td.scale : 1.0;
   int slot_of[PINN_MAX_NETS];
-  if (plan_channels(d, t, P, T, slot_of)) return 1;
+  if (plan_channels(d, td, what, t, P, T, slot_of)) return 1;
   long long stash = 0;
-  double f = 0;              // algorithmic flops per point: 6 * sum_nets C * S
+  double f = 0;
   for (int s = 0; s < T.n_used; ++s) {
     DevChan& ch = T.chan[s];
     canonical_order(ch);
     ch.C = 1 + ch.n1 + ch.n2 + ch.n3;
-    if (ch.C > PINN_MAX_CH) return fail("pinn_create: term %d needs %d channels (max %d)", t, ch.C, PINN_MAX_CH);
+    if (ch.C > PINN_MAX_CH) return fail("pinn_create: %s %d needs %d channels (max %d)", what, t, ch.C, PINN_MAX_CH);
     max_c = std::max(max_c, ch.C);
     const DevNet& n = P.nets[T.used_net[s]];
     double S = 0;
@@ -240,8 +251,96 @@ int plan_term(const pinn_problem_desc* d, int t, DevProblem& P, TermPlan& tp, in
     f += 6.0 * ch.C * S;
   }
   stash_max = std::max(stash_max, stash);
-  if (plan_taps(d, t, slot_of, T)) return 1;
-  tp.flops_per_point = f;
+  if (plan_taps(d, td, what, t, slot_of, integrals, n_integrals, T)) return 1;
+  *flops = f;
+  return 0;
+}
+
+// one term
+int plan_term(const pinn_problem_desc* d, int t, const pinn_integral_desc* integrals, int n_integrals, DevProblem& P,
+              TermPlan& tp, int& max_c, long long& stash_max) {
+  const pinn_term_desc& td = d->terms[t];
+  DevTerm& T = P.terms[t];
+  int n_own = 0;
+  for (int i = 0; i < n_integrals; ++i) n_own += integrals[i].owner == t;
+  if (td.dim < 1 || td.dim > PINN_MAX_DIM) return fail("pinn_create: term %d dim=%d out of range [1,%d]", t, td.dim, PINN_MAX_DIM);
+  if (td.n_taps < 1 && n_own == 0)
+    return fail("pinn_create: term %d has no network taps (an equation such as 0 ~ 0 cannot be trained on)", t);
+  if (td.n_taps + n_own > PINN_MAX_TAPS)
+    return fail("pinn_create: term %d has %d taps and %d integrals (max %d together)", t, td.n_taps, n_own, PINN_MAX_TAPS);
+  if (td.reduction != PINN_REDUCE_MEAN && td.reduction != PINN_REDUCE_WSUM)
+    return fail("pinn_create: term %d unknown reduction %d", t, td.reduction);
+  T.weighted = td.reduction == PINN_REDUCE_WSUM;
+  tp.reduction = td.reduction;
+  tp.scale = td.reduction == PINN_REDUCE_WSUM ? td.scale : 1.0;
+  return plan_body(d, td, "term", t, P, T, integrals, n_integrals, max_c, stash_max, &tp.flops_per_point);
+}
+
+// ---- integral terms ---------------------------------------------------------------------------------------------------
+}  // namespace
+
+// q-point Gauss-Legendre rule on [-1, 1]: Newton's method on P_q from the Chebyshev-like first guess
+void gauss_legendre(int q, double* x, double* w) {
+  const double pi = 3.14159265358979323846;
+  // P_q(z) and P_q'(z) by the three-term recurrence
+  auto legendre = [q](double z, double& dp) {
+    double p0 = 1.0, p1 = 0.0;
+    for (int j = 1; j <= q; ++j) { const double p2 = p1; p1 = p0; p0 = ((2.0 * j - 1.0) * z * p1 - (j - 1.0) * p2) / j; }
+    dp = q * (z * p0 - p1) / (z * z - 1.0);
+    return p0;
+  };
+  for (int i = 0; i < q; ++i) {
+    double z = cos(pi * (i + 0.75) / (q + 0.5)), dp = 1.0;
+    for (int it = 0; it < 100; ++it) {
+      const double dz = legendre(z, dp) / dp;
+      z -= dz;
+      if (fabs(dz) < 1e-16) break;
+    }
+    legendre(z, dp);              // the weight from the derivative at the converged node
+    x[q - 1 - i] = z;             // ascending, as numpy.polynomial.legendre.leggauss
+    w[q - 1 - i] = 2.0 / ((1.0 - z * z) * dp * dp);
+  }
+}
+
+namespace {
+
+// one integral: geometry, node table and the integrand (a term over the node point); *flops: per owner point
+int plan_integral(const pinn_problem_desc* d, const pinn_integral_desc* integrals, int n_integrals, int i, DevProblem& P,
+                  int& max_c, long long& stash_max, double* flops) {
+  const pinn_integral_desc& id = integrals[i];
+  DevIntegral& I = P.integ[i];
+  if (id.owner < 0 || id.owner >= d->n_terms) return fail("pinn_create: integral %d owner term %d out of range", i, id.owner);
+  const int odim = d->terms[id.owner].dim;
+  if (id.n_dims < 1 || id.n_dims > 2)
+    return fail("pinn_create: integral %d has %d integrating dimensions (supported 1 or 2)", i, id.n_dims);
+  if (id.q < 1 || id.q > PINN_MAX_QUAD)
+    return fail("pinn_create: integral %d has q=%d Gauss-Legendre nodes per dimension (supported 1..%d)", i, id.q, PINN_MAX_QUAD);
+  I.owner = id.owner; I.n_dims = id.n_dims; I.q = id.q;
+  for (int k = 0; k < 2; ++k) { I.row[k] = 0; I.lb_row[k] = I.ub_row[k] = -1; I.inf_kind[k] = PINN_INF_NONE; }
+  for (int k = 0; k < id.n_dims; ++k) {
+    if (id.row[k] < 0 || id.row[k] >= odim)
+      return fail("pinn_create: integral %d integrating row %d out of range (owner dim=%d)", i, id.row[k], odim);
+    if (id.lb_row[k] < -1 || id.lb_row[k] >= odim || id.ub_row[k] < -1 || id.ub_row[k] >= odim)
+      return fail("pinn_create: integral %d bound row out of range (owner dim=%d)", i, odim);
+    if (id.inf_kind[k] < PINN_INF_NONE || id.inf_kind[k] > PINN_INF_LOWER)
+      return fail("pinn_create: integral %d unknown infinite-bound kind %d", i, id.inf_kind[k]);
+    I.row[k] = id.row[k]; I.lb_row[k] = id.lb_row[k]; I.ub_row[k] = id.ub_row[k]; I.inf_kind[k] = id.inf_kind[k];
+    I.lb[k] = id.lb[k]; I.ub[k] = id.ub[k]; I.shift[k] = id.shift[k];
+  }
+  if (id.n_dims == 2 && id.row[0] == id.row[1]) return fail("pinn_create: integral %d integrates row %d twice", i, id.row[0]);
+  gauss_legendre(id.q, I.xi, I.wq);
+  I.slot = d->terms[id.owner].n_taps;
+  for (int j = 0; j < i; ++j) I.slot += integrals[j].owner == id.owner;
+  pinn_term_desc td;
+  memset(&td, 0, sizeof td);
+  td.dim = odim + id.n_dims; td.n_taps = id.n_taps; td.taps = id.taps; td.net_rows = id.net_rows;
+  td.n_instr = id.n_instr; td.prog = id.prog;
+  if (td.n_taps < 1) return fail("pinn_create: integral %d has no network taps", i);
+  double f = 0;
+  if (plan_body(d, td, "integral", i, P, I.body, integrals, n_integrals, max_c, stash_max, &f)) return 1;
+  double nodes = id.q;
+  if (id.n_dims == 2) nodes *= id.q;
+  *flops = 2.0 * nodes * f;     // the forward pass, and again in the reverse sweep (recomputed per node tile)
   return 0;
 }
 
@@ -256,7 +355,7 @@ int plan_ffma(int dtype, int max_w8, long long resident, int max_c, long long st
     long long wa = o.res ? resident : panel;
     wa = (wa + 3) & ~3LL;
     if (wa > (1LL << 30)) continue;
-    size_t need = ffma_smem_bytes(dtype, a.buf_elems, (int)wa, o.bufs);
+    size_t need = ffma_smem_bytes(dtype, a.buf_elems, (int)wa, o.bufs, p.integ);
     if (need <= (size_t)max_smem) {
       p.bufs_smem = o.bufs; a.weights_resident = o.res ? 1 : 0; a.w_area = (int)wa; p.smem = need;
       return 0;
@@ -470,9 +569,15 @@ int plan_tc(const pinn_problem_desc* d, int max_smem, Plan& p) {
 }  // namespace
 
 // validation of the descriptor header, then the stages above in order
-int plan_problem(const pinn_problem_desc* d, int max_smem, Plan& p) {
+int plan_problem(const pinn_problem_desc* d, const pinn_integral_desc* integrals, int n_integrals, int max_smem, Plan& p) {
   memset(&p, 0, sizeof p);
   if (!d) return fail("pinn_create: null descriptor");
+  if (n_integrals < 0 || n_integrals > PINN_MAX_INTEGRALS)
+    return fail("pinn_create_ex: n_integrals=%d out of range [0,%d]", n_integrals, PINN_MAX_INTEGRALS);
+  if (n_integrals > 0 && !integrals) return fail("pinn_create_ex: null integrals");
+  if (n_integrals > 0 && d->mode != PINN_MODE_FFMA)
+    return fail("pinn_create_ex: integral terms run on the FFMA path (mode PINN_MODE_FFMA); the tensor-core modes do not "
+                "evaluate them");
   if (d->abi_version != PINN_ABI_VERSION)
     return fail("pinn_create: descriptor abi_version %d, library %d", d->abi_version, PINN_ABI_VERSION);
   if (d->dtype != PINN_F32 && d->dtype != PINN_F64) return fail("pinn_create: unknown dtype %d", d->dtype);
@@ -494,7 +599,14 @@ int plan_problem(const pinn_problem_desc* d, int max_smem, Plan& p) {
   long long resident = 0, stash_max = 0;
   if (plan_nets(d, P, max_w8, resident)) return 1;
   for (int t = 0; t < d->n_terms; ++t)
-    if (plan_term(d, t, P, p.term[t], max_c, stash_max)) return 1;
+    if (plan_term(d, t, integrals, n_integrals, P, p.term[t], max_c, stash_max)) return 1;
+  P.n_integrals = n_integrals;
+  p.integ = n_integrals > 0;
+  for (int i = 0; i < n_integrals; ++i) {     // after the terms: the owners' dims and tap counts are validated
+    double f = 0;
+    if (plan_integral(d, integrals, n_integrals, i, P, max_c, stash_max, &f)) return 1;
+    p.term[integrals[i].owner].flops_per_point += f;
+  }
   p.tile_pts = d->mode == PINN_MODE_FFMA ? kTilePts : kTcPts;
   if (d->mode == PINN_MODE_FFMA) return plan_ffma(d->dtype, max_w8, resident, max_c, stash_max, max_smem, p);
   return plan_tc(d, max_smem, p);

@@ -20,10 +20,15 @@ struct Plan {
   size_t smem;                     // dynamic shared memory per CTA
   bool bufs_smem;                  // FFMA: the two activation buffers live in shared memory (else in gbufs)
   bool wide;                       // tensor-core modes: tw_pack + the 128-wide kernel run instead of the narrow one
+  bool integ;                      // FFMA: the problem has integral terms (the kernel instantiation with node tiles runs)
   // launch-argument templates: the planner fills the layout, pinn_create the buffers, a launch the per-call fields
   FfmaArgs ffma; TcArgs tc; TwArgs tw; TwPackArgs pack;
 };
 
+// the q-point Gauss-Legendre rule on [-1, 1], nodes ascending
+void gauss_legendre(int q, double* x, double* w);
+
 // Pure host code (no CUDA runtime call); max_smem: the device's opt-in shared memory per block in bytes.
-int plan_problem(const pinn_problem_desc* d, int max_smem, Plan& p);
+// integrals[n_integrals]: integral terms (pinn_create_ex), none for pinn_create.
+int plan_problem(const pinn_problem_desc* d, const pinn_integral_desc* integrals, int n_integrals, int max_smem, Plan& p);
 }  // namespace pinn

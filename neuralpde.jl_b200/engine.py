@@ -26,6 +26,7 @@ ACT = {"identity": 0, "tanh": 1, "sigmoid": 2, "sin": 3, "softplus": 4, "swish":
 OP = {
     "const": 0, "coord": 1, "tap": 2, "param": 3, "add": 4, "sub": 5, "mul": 6, "div": 7, "neg": 8,
     "pow": 9, "powi": 10, "sin": 11, "cos": 12, "exp": 13, "log": 14, "tanh": 15, "sqrt": 16, "abs": 17,
+    "integral": 18,
 }
 REDUCE_MEAN, REDUCE_WSUM = 0, 1
 
@@ -38,8 +39,17 @@ EXPORTS = [
     "pinn_flops_per_eval", "pinn_adam_begin", "pinn_adam_iterate", "pinn_adam_theta",
     "pinn_term_grad_stats", "pinn_term_grad_stats_host", "pinn_set_sampler", "pinn_resample", "pinn_get_points_host",
     "pinn_comm_info", "pinn_set_sampler_ex", "pinn_qn_begin", "pinn_qn_iterate", "pinn_qn_theta",
-    "pinn_hmc_begin", "pinn_hmc_iterate", "pinn_hmc_theta", "pinn_hmc_begin_ex",
+    "pinn_hmc_begin", "pinn_hmc_iterate", "pinn_hmc_theta", "pinn_hmc_begin_ex", "pinn_create_ex",
+    "pinn_quadrature_nodes",
 ]
+
+# substitutions of infinite integration bounds (pinn_integral_desc.inf_kind) and the limits of integral terms
+INF_NONE, INF_BOTH, INF_UPPER, INF_LOWER = 0, 1, 2, 3
+MAX_INTEGRALS = 8
+MAX_QUAD = 64
+# Gauss-Legendre nodes per integrating dimension the Python layer uses.  16 meet test/Forward/forward__integral.jl's
+# rtol = 1e-5 on [0, Inf) with 300x margin (12 are the fewest that do); DESIGN section 4.7.
+DEFAULT_QUAD_NODES = 16
 
 # quasi-Newton optimizer / line search kinds and run states (pinn_qn_options, pinn_qn_iterate)
 QN_LBFGS, QN_BFGS = 0, 1
@@ -93,6 +103,14 @@ class _TermDesc(C.Structure):
                 ("reduction", C.c_int32), ("scale", C.c_double)]
 
 
+class _IntegralDesc(C.Structure):
+    _fields_ = [("owner", C.c_int32), ("n_dims", C.c_int32), ("q", C.c_int32), ("row", C.c_int32 * 2),
+                ("lb_row", C.c_int32 * 2), ("ub_row", C.c_int32 * 2), ("lb", C.c_double * 2), ("ub", C.c_double * 2),
+                ("inf_kind", C.c_int32 * 2), ("shift", C.c_double * 2), ("n_taps", C.c_int32),
+                ("taps", C.POINTER(_TapDesc)), ("net_rows", C.POINTER(C.c_int32)), ("n_instr", C.c_int32),
+                ("prog", C.POINTER(_Instr))]
+
+
 class _ProblemDesc(C.Structure):
     _fields_ = [("abi_version", C.c_int32), ("dtype", C.c_int32), ("mode", C.c_int32), ("device", C.c_int32),
                 ("n_nets", C.c_int32), ("nets", C.POINTER(_NetDesc)), ("n_terms", C.c_int32),
@@ -131,6 +149,25 @@ class TermSpec:
 
 
 @dataclass
+class IntegralSpec:
+    """One integral term (pinn_integral_desc): read by term ``owner``'s program as ("integral", index); the integrand's
+    program runs over the node point (the owner's rows with ``rows`` replaced by x(t), then the t rows)."""
+    owner: int
+    n_dims: int = 1
+    q: int = DEFAULT_QUAD_NODES
+    rows: List[int] = field(default_factory=lambda: [0, 0])
+    lb: List[float] = field(default_factory=lambda: [0.0, 0.0])
+    ub: List[float] = field(default_factory=lambda: [0.0, 0.0])
+    lb_row: List[int] = field(default_factory=lambda: [-1, -1])
+    ub_row: List[int] = field(default_factory=lambda: [-1, -1])
+    inf_kind: List[int] = field(default_factory=lambda: [0, 0])
+    shift: List[float] = field(default_factory=lambda: [0.0, 0.0])
+    taps: List[TapSpec] = field(default_factory=list)
+    prog: List[tuple] = field(default_factory=list)
+    net_rows: Optional[List[List[int]]] = None
+
+
+@dataclass
 class ProblemSpec:
     nets: List[NetSpec]
     terms: List[TermSpec]
@@ -140,6 +177,7 @@ class ProblemSpec:
     dtype: str = "float32"
     mode: int = MODE_FFMA
     device: int = 0
+    integrals: List[IntegralSpec] = field(default_factory=list)   # non-empty: created with pinn_create_ex
     _keep: list = field(default_factory=list, repr=False)
 
 
@@ -159,6 +197,10 @@ def load_library():
     vp, i32, i64, dbl = C.c_void_p, C.c_int32, C.c_int64, C.c_double
     lib.pinn_create.argtypes = [C.POINTER(_ProblemDesc), C.POINTER(vp)]
     lib.pinn_create.restype = C.c_int
+    lib.pinn_create_ex.argtypes = [C.POINTER(_ProblemDesc), C.POINTER(_IntegralDesc), C.c_int32, C.POINTER(vp)]
+    lib.pinn_create_ex.restype = C.c_int
+    lib.pinn_quadrature_nodes.argtypes = [C.c_int32, C.POINTER(C.c_double), C.POINTER(C.c_double)]
+    lib.pinn_quadrature_nodes.restype = C.c_int
     lib.pinn_destroy.argtypes = [vp]
     lib.pinn_destroy.restype = C.c_int
     lib.pinn_last_error.argtypes = []
@@ -232,6 +274,15 @@ def load_library():
     return lib
 
 
+def quadrature_nodes(q: int):
+    """(nodes, weights) of the q-point Gauss-Legendre rule on [-1, 1] that integral terms use (host only)."""
+    lib = load_library()
+    x, w = np.empty(int(q)), np.empty(int(q))
+    _check(lib.pinn_quadrature_nodes(int(q), x.ctypes.data_as(C.POINTER(C.c_double)),
+                                     w.ctypes.data_as(C.POINTER(C.c_double))))
+    return x, w
+
+
 def _check(rc: int):
     if rc != 0:
         raise EngineError(load_library().pinn_last_error().decode("utf-8", "replace"))
@@ -252,6 +303,44 @@ def _ptr(x) -> C.c_void_p:
     if hasattr(x, "data_ptr"):
         return C.c_void_p(x.data_ptr())
     raise TypeError("cannot take a pointer of %r" % type(x))
+
+
+def _marshal_body(spec: ProblemSpec, taps_l, prog_l, net_rows_l, keep):
+    """taps / net_rows / program arrays of a term or an integrand"""
+    taps = (_TapDesc * max(1, len(taps_l)))()
+    for i, tp in enumerate(taps_l):
+        taps[i].net, taps[i].out, taps[i].order = int(tp.net), int(tp.out), int(tp.order)
+        d = list(tp.dirs) + [0, 0, 0, 0]
+        for q in range(4):
+            taps[i].dir[q] = int(d[q])
+    rows = (C.c_int32 * (len(spec.nets) * MAX_IN))(*([-1] * (len(spec.nets) * MAX_IN)))
+    for k, n in enumerate(spec.nets):
+        r = net_rows_l[k] if net_rows_l is not None and k < len(net_rows_l) and net_rows_l[k] is not None \
+            else list(range(n.dims[0]))
+        for j, v in enumerate(r):
+            rows[k * MAX_IN + j] = int(v)
+    prog = (_Instr * max(1, len(prog_l)))()
+    for i, ins in enumerate(prog_l):
+        op, a, b, imm = (list(ins) + [0, 0, 0.0])[:4]
+        prog[i].op, prog[i].a, prog[i].b, prog[i].imm = OP[op], int(a), int(b), float(imm)
+    keep += [taps, rows, prog]
+    return taps, rows, prog
+
+
+def build_integrals(spec: ProblemSpec):
+    """Marshal spec.integrals into a pinn_integral_desc array (kept alive on the spec)."""
+    arr = (_IntegralDesc * max(1, len(spec.integrals)))()
+    for i, it in enumerate(spec.integrals):
+        d = arr[i]
+        d.owner, d.n_dims, d.q = int(it.owner), int(it.n_dims), int(it.q)
+        for k in range(2):
+            d.row[k], d.lb_row[k], d.ub_row[k] = int(it.rows[k]), int(it.lb_row[k]), int(it.ub_row[k])
+            d.lb[k], d.ub[k], d.shift[k] = float(it.lb[k]), float(it.ub[k]), float(it.shift[k])
+            d.inf_kind[k] = int(it.inf_kind[k])
+        d.taps, d.net_rows, d.prog = _marshal_body(spec, it.taps, it.prog, it.net_rows, spec._keep)
+        d.n_taps, d.n_instr = len(it.taps), len(it.prog)
+    spec._keep.append(arr)
+    return arr
 
 
 def build_desc(spec: ProblemSpec) -> _ProblemDesc:
@@ -318,7 +407,10 @@ class Engine:
         self.n_theta = int(spec.n_theta)
         self._h = C.c_void_p(0)
         desc = build_desc(spec)
-        _check(self.lib.pinn_create(C.byref(desc), C.byref(self._h)))
+        if spec.integrals:
+            _check(self.lib.pinn_create_ex(C.byref(desc), build_integrals(spec), len(spec.integrals), C.byref(self._h)))
+        else:
+            _check(self.lib.pinn_create(C.byref(desc), C.byref(self._h)))
         self._keep_pts = {}
 
     def close(self):

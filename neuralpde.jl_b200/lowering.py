@@ -18,8 +18,9 @@ from typing import Dict, List, Optional, Tuple
 import sympy as sp
 from sympy.core.function import AppliedUndef
 
-from .engine import TapSpec, TermSpec, REDUCE_MEAN
-from .symbolic import Equation, VarInfo, eq_indvars, expand_derivatives
+from .engine import (DEFAULT_QUAD_NODES, INF_BOTH, INF_LOWER, INF_NONE, INF_UPPER, IntegralSpec, TapSpec, TermSpec,
+                     REDUCE_MEAN)
+from .symbolic import Equation, IntegralOp, VarInfo, eq_indvars, expand_derivatives
 
 
 class LoweringError(ValueError):
@@ -35,6 +36,9 @@ class LoweredTerm:
     # coordinate-only subexpressions hoisted out of the per-step program: evaluated once per point set
     # (float64, on the host) and appended as extra rows dim, dim+1, ... of the point matrix
     extra_exprs: List[sp.Expr] = None
+    # integral terms the program reads with ("integral", k): owner -1 and k local to this term until
+    # symbolic_discretize places them
+    integrals: List[IntegralSpec] = None
 
     @property
     def dim(self) -> int:
@@ -61,16 +65,19 @@ class LoweredTerm:
 
 
 MAX_DIM = 8   # PINN_MAX_DIM
+# the reference truncates the substituted intervals of infinite bounds by 1/20 (src/transform_inf_integral.jl)
+INF_EPS = 1.0 / 20
 
 
 def _hoist_coordinate_terms(expr, coord_names, blocked_names, extras, base_dim):
     """Replace maximal coordinate-only subexpressions (no network tap, no trainable parameter) by fresh
     symbols __c<i>; trivial ones (a bare symbol / number, or fewer than 2 operations) stay inline."""
     def has_net(e):
-        return e.has(AppliedUndef) or e.has(sp.Derivative) or any(str(q) in blocked_names for q in e.free_symbols)
+        return e.has(AppliedUndef) or e.has(sp.Derivative) or e.has(IntegralOp) or \
+            any(str(q) in blocked_names for q in e.free_symbols)
 
     def rec(e):
-        if isinstance(e, (AppliedUndef, sp.Derivative, sp.Subs)):
+        if isinstance(e, (AppliedUndef, sp.Derivative, sp.Subs, IntegralOp)):
             return e
         if not has_net(e):
             names = {str(q) for q in e.free_symbols}
@@ -96,7 +103,8 @@ def _hoist_coordinate_terms(expr, coord_names, blocked_names, extras, base_dim):
 
 
 class _Emitter:
-    def __init__(self, vi: VarInfo, rows: List[str], param_index: Dict[str, int], param_values: Dict[str, float]):
+    def __init__(self, vi: VarInfo, rows: List[str], param_index: Dict[str, int], param_values: Dict[str, float],
+                 extras: Optional[List[sp.Expr]] = None, hoist: bool = False, node_vars: Optional[Dict[str, int]] = None):
         self.vi = vi
         self.rows = rows
         self.param_index = param_index
@@ -105,6 +113,10 @@ class _Emitter:
         self.taps: List[TapSpec] = []
         self._tap_ids: Dict[tuple, int] = {}
         self._cse: Dict[object, int] = {}
+        self.extras = extras if extras is not None else []   # hoisted rows (an integral's expression bounds land here)
+        self.hoist = hoist
+        self.node_vars = node_vars or {}    # integrand: quadrature variable t_k -> ("coord", -1 - k) until placed
+        self.integrals: List[IntegralSpec] = []
 
     def _push(self, op, a=0, b=0, imm=0.0) -> int:
         key = (op, a, b, float(imm))
@@ -142,6 +154,8 @@ class _Emitter:
                 return self._push("coord", a=self.rows.index(name))
             if name.startswith("__c"):
                 return self._push("coord", a=len(self.rows) + int(name[3:]))
+            if name in self.node_vars:
+                return self._push("coord", a=-1 - self.node_vars[name])
             if name in self.param_index:
                 return self._push("param", a=self.param_index[name])
             if name in self.param_values:
@@ -150,6 +164,10 @@ class _Emitter:
                 raise LoweringError(
                     "independent variable %s is not an input of any dependent variable in this equation" % name)
             raise LoweringError("unknown symbol %s (not an independent variable or a parameter with a default)" % name)
+        if isinstance(e, IntegralOp):
+            if self.node_vars:
+                raise LoweringError("integral nested in an integrand: not supported")
+            return self._push("integral", a=self.integral(e))
         if isinstance(e, AppliedUndef):
             name = e.func.__name__
             if name not in self.vi.dict_depvars:
@@ -245,15 +263,106 @@ class _Emitter:
             return self._push("mul", a=s, b=self.const(0.5))
         raise LoweringError("unsupported expression node %s in %s" % (type(e).__name__, e))
 
+    # -- integral terms --------------------------------------------------------------------------
+    def _bound_row(self, b: sp.Expr):
+        """(constant, row): a number, a coordinate row, or a coordinate expression hoisted into a row of its own."""
+        b = sp.sympify(b)
+        if b.is_number:
+            return float(b), -1
+        names = {str(q) for q in b.free_symbols}
+        if b.has(AppliedUndef) or b.has(sp.Derivative) or not names <= set(self.rows):
+            raise LoweringError("integral bound %s: bounds are numbers or functions of the equation's coordinates %s "
+                                "(bounds that depend on dependent variables are not supported)" % (b, self.rows))
+        if isinstance(b, sp.Symbol):
+            return 0.0, self.rows.index(str(b))
+        if not self.hoist:
+            raise LoweringError("integral bound %s is an expression of the coordinates; it becomes a host-evaluated row, "
+                                "which device-sampled point sets do not carry" % b)
+        for i, old in enumerate(self.extras):
+            if old == b:
+                return 0.0, len(self.rows) + i
+        if len(self.rows) + len(self.extras) >= MAX_DIM:
+            raise LoweringError("integral bound %s: no point row left (max %d)" % (b, MAX_DIM))
+        self.extras.append(b)
+        return 0.0, len(self.rows) + len(self.extras) - 1
+
+    def integral(self, e: IntegralOp) -> int:
+        """Lower one integral: the quadrature geometry, and the integrand (times the Jacobian of the reference's
+        infinite-bound substitution, src/transform_inf_integral.jl) as its own IR over the node point."""
+        integrand, vars_, lbs, ubs = e.args
+        names = [str(v) for v in vars_]
+        if len(names) > 2:
+            raise LoweringError("integral over %d variables: at most 2 integrating dimensions are supported" % len(names))
+        if len(set(names)) != len(names):
+            raise LoweringError("integral over %s names a variable twice" % names)
+        spec = IntegralSpec(owner=-1, n_dims=len(names), q=DEFAULT_QUAD_NODES)
+        tsyms = [sp.Symbol("__t%d" % k, real=True) for k in range(len(names))]
+        jac = sp.Integer(1)
+        for k, (v, lo, hi) in enumerate(zip(names, lbs, ubs)):
+            if v not in self.rows:
+                raise LoweringError("integrating variable %s is not a coordinate of the equation %s" % (v, self.rows))
+            lo_inf, hi_inf = lo == -sp.oo, hi == sp.oo
+            if lo == sp.oo or hi == -sp.oo:
+                raise LoweringError("integral over %s: empty interval [%s, %s]" % (v, lo, hi))
+            if (lo_inf or hi_inf) and len(names) > 1:
+                raise LoweringError("infinite bounds are supported for 1-dimensional integrals only")
+            t = tsyms[k]
+            kind, shift = INF_NONE, 0.0
+            if lo_inf and hi_inf:                       # x = t / (1 - t^2), t in [-1 + eps, 1 - eps]
+                kind, lo_t, hi_t = INF_BOTH, -1.0 + INF_EPS, 1.0 - INF_EPS
+                jac = jac * (1 + t ** 2) / (1 - t ** 2) ** 2
+            elif hi_inf:                                # x = a + t / (1 - t), or t / (1 - t) from a / (1 + a)
+                kind, hi_t = INF_UPPER, 1.0 - INF_EPS
+                if sp.sympify(lo).is_number:
+                    shift, lo_t = float(lo), 0.0
+                else:
+                    lo_t = lo / (1 + lo)
+                jac = jac / (1 - t) ** 2
+            elif lo_inf:                                # x = b + t / (1 + t), t in [-1 + eps, 0]
+                if not sp.sympify(hi).is_number:
+                    raise LoweringError("integral over (-Inf, %s]: an upper bound that depends on the coordinates "
+                                        "with an infinite lower bound is not supported" % hi)
+                kind, shift, lo_t, hi_t = INF_LOWER, float(hi), -1.0 + INF_EPS, 0.0
+                jac = jac / (1 + t) ** 2
+            else:
+                lo_t, hi_t = lo, hi
+            spec.rows[k] = self.rows.index(v)
+            spec.lb[k], spec.lb_row[k] = self._bound_row(lo_t)
+            spec.ub[k], spec.ub_row[k] = self._bound_row(hi_t)
+            spec.inf_kind[k], spec.shift[k] = kind, shift
+        body = expand_derivatives(integrand)
+        if not (body.has(AppliedUndef) or body.has(sp.Derivative)):
+            raise LoweringError("integrand %s contains no dependent variable: nothing to train on" % integrand)
+        em = _Emitter(self.vi, self.rows, self.param_index, self.param_values,
+                      node_vars={str(t): k for k, t in enumerate(tsyms)})
+        v = em.emit(body * jac if jac != 1 else body)
+        if v != len(em.prog) - 1:              # the last instruction is the integrand's value
+            em.prog.append(("mul", v, em.const(1.0), 0.0))
+        spec.taps, spec.prog = em.taps, em.prog
+        spec.net_rows = _net_rows(self.vi, self.rows)
+        for i, old in enumerate(self.integrals):
+            if old == spec:
+                return i
+        self.integrals.append(spec)
+        return len(self.integrals) - 1
+
+
+def _net_rows(vi: VarInfo, rows: List[str]) -> List[Optional[List[int]]]:
+    out: List[Optional[List[int]]] = []
+    for name in vi.depvars:
+        ins = vi.dict_depvar_input[name]
+        out.append([rows.index(v) for v in ins] if all(v in rows for v in ins) else None)
+    return out
+
 
 def lower_equation(eq: Equation, vi: VarInfo, param_index: Optional[Dict[str, int]] = None,
                    param_values: Optional[Dict[str, float]] = None, hoist: bool = False) -> LoweredTerm:
-    """Equation -> taps + residual program (``lhs - rhs``)."""
+    """Equation -> taps + residual program (``lhs - rhs``), and the IR of every integral it reads."""
     rows = eq_indvars(eq, vi)
-    em = _Emitter(vi, rows, param_index or {}, param_values or {})
+    extras: List[sp.Expr] = []
+    em = _Emitter(vi, rows, param_index or {}, param_values or {}, extras=extras, hoist=hoist)
     lhs = expand_derivatives(eq.lhs)
     rhs = expand_derivatives(eq.rhs)
-    extras: List[sp.Expr] = []
     if hoist:
         # trainable parameters block hoisting; parameters with fixed defaults are substituted first
         subs = {sp.Symbol(k, real=True): v for k, v in (param_values or {}).items()}
@@ -262,16 +371,13 @@ def lower_equation(eq: Equation, vi: VarInfo, param_index: Optional[Dict[str, in
     a = em.emit(lhs)
     b = em.emit(rhs)
     em.prog.append(("sub", a, b, 0.0))      # not CSE'd: must be the last instruction
-    if not em.taps:
+    if not em.taps and not em.integrals:
         raise LoweringError("equation %s contains no dependent variable: nothing to train on" % (eq,))
-    net_rows: List[Optional[List[int]]] = []
-    for name in vi.depvars:
-        ins = vi.dict_depvar_input[name]
-        if all(v in rows for v in ins):
-            net_rows.append([rows.index(v) for v in ins])
-        else:
-            net_rows.append(None)
-    return LoweredTerm(em.taps, em.prog, rows, net_rows, extras)
+    dim = len(rows) + len(extras)
+    for spec in em.integrals:                # the quadrature variables follow the owner's rows (hoisted ones included)
+        spec.prog = [("coord", dim - 1 - ins[1], 0, 0.0) if ins[0] == "coord" and ins[1] < 0 else ins
+                     for ins in spec.prog]
+    return LoweredTerm(em.taps, em.prog, rows, _net_rows(vi, rows), extras, em.integrals)
 
 
 def term_spec(lt: LoweredTerm, reduction: int = REDUCE_MEAN, scale: float = 1.0) -> TermSpec:

@@ -7,13 +7,15 @@ kernels -- there is no CPU code path here.
 """
 from __future__ import annotations
 
+import dataclasses
 from dataclasses import dataclass, field
 from typing import Callable, Dict, List, Optional, Sequence, Union
 
 import numpy as np
 
 from . import engine as _eng
-from .engine import Engine, EngineError, NetSpec, ProblemSpec, TapSpec, TermSpec, REDUCE_MEAN, REDUCE_WSUM
+from .engine import (Engine, EngineError, IntegralSpec, NetSpec, ProblemSpec, TapSpec, TermSpec, REDUCE_MEAN,
+                     REDUCE_WSUM)
 from .lowering import LoweredTerm, LoweringError, lower_equation, term_spec
 from .strategies import (AbstractTrainingStrategy, GridTraining, QuadratureTraining, QuasiRandomTraining,
                          StochasticTraining, _julia_range, _product_columns, gauss_legendre_box, generate_quasi_random_points,
@@ -593,10 +595,22 @@ def symbolic_discretize(pde_system: PDESystem, discretization: PhysicsInformedNN
                               prog=[("tap", 0, 0, 0.0), ("coord", din, 0, 0.0), ("sub", 0, 1, 0.0)],
                               net_rows=rows, reduction=REDUCE_MEAN))
 
+    # integral terms (get_numeric_integral, src/discretize.jl:334-397): one set per term that reads them -- a dataset
+    # term re-reads its equation's integrals at the dataset's coordinates -- numbered in term order
+    integrals: List[IntegralSpec] = []
+    for i, lt in enumerate(pde_terms + bc_terms + [lt for lt, _ in ds_terms]):
+        if lt.integrals:
+            base = len(integrals)
+            integrals += [dataclasses.replace(it, owner=i) for it in lt.integrals]
+            specs[i].prog = [("integral", base + ins[1], 0, 0.0) if ins[0] == "integral" else ins
+                             for ins in specs[i].prog]
+    if len(integrals) > _eng.MAX_INTEGRALS:
+        raise ValueError("the system has %d integral terms (max %d)" % (len(integrals), _eng.MAX_INTEGRALS))
+
     nets = [NetSpec(c.dims, c.acts, off) for c, off in zip(chains, offs)]
     mode = {"ffma": _eng.MODE_FFMA, "tc_bf16": _eng.MODE_TC_BF16, "tc_split": _eng.MODE_TC_SPLIT}[d.mode]
     spec = ProblemSpec(nets=nets, terms=specs, n_params=n_p, param_offset=n_net, n_theta=n_net + n_p,
-                       dtype=dtype.name, mode=mode, device=d.device)
+                       dtype=dtype.name, mode=mode, device=d.device, integrals=integrals)
 
     n_pde, n_bc = len(eqs), len(bcs)
     point_sets: List[Optional[np.ndarray]] = [None] * len(specs)

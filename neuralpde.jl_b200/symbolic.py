@@ -200,3 +200,60 @@ def expand_derivatives(expr: sp.Expr) -> sp.Expr:
     except Exception:
         return expr
     return expr if ex == 0 else ex
+
+
+# ---- integral terms (Symbolics.Integral with DomainSets domains; reference src/symbolic_utilities.jl:203-320) ------
+Inf = sp.oo
+
+
+@dataclass(frozen=True)
+class ClosedInterval:
+    """``ClosedInterval(lo, hi)``: each bound a number, ±``Inf`` or an expression of the coordinates."""
+    lo: object
+    hi: object
+
+
+def UnitInterval() -> ClosedInterval:
+    return ClosedInterval(0, 1)
+
+
+@dataclass(frozen=True)
+class ProductDomain:
+    """``ProductDomain(d1, d2)``: one interval per integrating variable, in order."""
+    domains: tuple
+
+    def __init__(self, *domains):
+        object.__setattr__(self, "domains", tuple(domains))
+
+
+def UnitSquare() -> ProductDomain:
+    return ProductDomain(UnitInterval(), UnitInterval())
+
+
+class IntegralOp(sp.Function):
+    """Unevaluated ``Integral(vars in domain)(integrand)``: args (integrand, Tuple(vars), Tuple(lbs), Tuple(ubs))."""
+    nargs = 4
+
+    @classmethod
+    def eval(cls, *args):
+        return None
+
+
+class Integral:
+    """``Integral(x in ClosedInterval(0, x))`` -> ``Integral(x, ClosedInterval(0, x))``;
+    ``Integral((x, y) in UnitSquare())`` -> ``Integral((x, y), UnitSquare())``.  Applying it to an expression gives
+    the unevaluated integral, evaluated per collocation point of the equation (lowering.py)."""
+
+    def __init__(self, variables, domain):
+        vs = tuple(variables) if isinstance(variables, (tuple, list)) else (variables,)
+        doms = domain.domains if isinstance(domain, ProductDomain) else (domain,)
+        if len(vs) != len(doms):
+            raise ValueError("Integral: %d variables over a %d-dimensional domain" % (len(vs), len(doms)))
+        if not all(isinstance(d_, ClosedInterval) for d_ in doms):
+            raise TypeError("Integral: domains are ClosedInterval / UnitInterval / UnitSquare / ProductDomain")
+        self.variables = vs
+        self.lbs = tuple(sp.sympify(d_.lo) for d_ in doms)
+        self.ubs = tuple(sp.sympify(d_.hi) for d_ in doms)
+
+    def __call__(self, expr):
+        return IntegralOp(sp.sympify(expr), sp.Tuple(*self.variables), sp.Tuple(*self.lbs), sp.Tuple(*self.ubs))
