@@ -180,7 +180,11 @@ function lower_expr!(L::Lowered, ex, env)
     elseif haskey(UNOP, f)
         return emit!(L, UNOP[f], lower_expr!(L, args[1], env))
     end
-    throw(ArgumentError("NeuralPDEB200Ext: function $f has no residual-IR opcode"))
+    # a function registered with @register_symbolic (such as phi_bound(x, y) reading a trained network) is an opaque
+    # Julia call here; the engine's fixed networks (pinn_create_ex2) are reachable from the Python layer only
+    throw(ArgumentError("NeuralPDEB200Ext: function $f has no residual-IR opcode (functions registered with " *
+                        "@register_symbolic, such as a trained network read by a neural adapter, are not lowered by " *
+                        "this extension)"))
 end
 
 """

@@ -211,11 +211,35 @@ typedef struct {
   const pinn_instr* prog;
 } pinn_integral_desc;
 
+/* ---- fixed networks (neural adapters, registered network functions) ------------------------------------------
+ * A fixed network is a Dense MLP whose parameters are not trained: a teacher a neural adapter fits its student to
+ * (reference src/neural_adapter.jl), or a trained network read through a registered function such as
+ * `phi_bound(x, y) = first(phi(vcat(x, y), res.u))` with `@register_symbolic phi_bound(x, y)`.  Its shape rules and
+ * activations are those of pinn_net_desc; its parameters live in their own buffer (flat Lux layout, the handle's dtype),
+ * outside theta.  A tap names fixed network j as net = n_nets + j (values and derivatives as for trainable networks),
+ * and a term's net_rows then has n_nets + n_fixed rows.  The forward pass runs in the fused kernel like any other tap;
+ * nothing flows back into a fixed network, so the gradient has n_theta entries as before.  FFMA path only. */
+#define PINN_MAX_FIXED_NETS 16
+typedef struct {
+  int32_t n_layers;      /* number of Dense layers                         */
+  const int32_t* dims;   /* n_layers+1 entries: in, hidden..., out         */
+  const int32_t* acts;   /* n_layers entries: PINN_ACT_* of each layer      */
+} pinn_fixed_net_desc;
+
 /* ---- lifecycle ---------------------------------------------------------------- */
 int pinn_create(const pinn_problem_desc* desc, pinn_handle* out);
 /* pinn_create with integral terms integrals[n_integrals] (0 <= n_integrals <= PINN_MAX_INTEGRALS; 0 is pinn_create) */
 int pinn_create_ex(const pinn_problem_desc* desc, const pinn_integral_desc* integrals, int32_t n_integrals,
                    pinn_handle* out);
+/* pinn_create_ex with fixed networks fixed[n_fixed] (0 <= n_fixed <= PINN_MAX_FIXED_NETS; 0 is pinn_create_ex).  Every
+ * fixed network needs its parameters (pinn_set_fixed_params[_host]) before the first evaluation. */
+int pinn_create_ex2(const pinn_problem_desc* desc, const pinn_integral_desc* integrals, int32_t n_integrals,
+                    const pinn_fixed_net_desc* fixed, int32_t n_fixed, pinn_handle* out);
+/* Parameters of fixed network j: alias a device buffer (owned by the caller while the handle uses it), or copy a host
+ * buffer into engine memory (on `stream`).  Either may be called again between evaluations to re-point it: both first
+ * wait for the device to finish the evaluations already enqueued, and the copy is complete when the call returns. */
+int pinn_set_fixed_params(pinn_handle h, int32_t j, const void* dev_params);
+int pinn_set_fixed_params_host(pinn_handle h, int32_t j, const void* host_params, void* stream);
 int pinn_destroy(pinn_handle h);
 const char* pinn_last_error(void);
 int pinn_abi_version(void);
@@ -424,7 +448,7 @@ double pinn_last_kernel_ms(pinn_handle h);
 int64_t pinn_workspace_bytes(pinn_handle h);
 /* algorithmic FLOPs of one pinn_loss_grad at the current point sets:
  * 6 * sum_terms N * sum_nets C * S  (SURVEY section 8(d)); an integral adds 2 q^n_dims integrand evaluations per point
- * of its owner term */
+ * of its owner term; a fixed network counts its forward pass only, 2 * C * S */
 double pinn_flops_per_eval(pinn_handle h);
 /* the q-point Gauss-Legendre rule on [-1, 1] that integral terms use (nodes ascending): x[q], w[q]; 1 <= q <= 64.
  * Host only, no device needed. */

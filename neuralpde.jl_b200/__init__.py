@@ -4,7 +4,7 @@ PhysicsInformedNN / discretize interface.
 The directory name contains a dot, so import it through the root-level alias module:
 ``import neuralpde_jl_b200 as npde``.
 """
-from .engine import (Engine, EngineError, IntegralSpec, NetSpec, ProblemSpec, TapSpec, TermSpec, EXPORTS, LIB_PATH,
+from .engine import (Engine, EngineError, FixedNetSpec, IntegralSpec, NetSpec, ProblemSpec, TapSpec, TermSpec, EXPORTS, LIB_PATH,
                      MODE_FFMA, MODE_TC_BF16, MODE_TC_SPLIT, REDUCE_MEAN, REDUCE_WSUM, load_library)
 from .symbolic import (ClosedInterval, Differential, Eq, Equation, In, Inf, Integral, Interval, PDESystem,
                        ProductDomain, UnitInterval, UnitSquare, VarDomain, get_argument, get_variables, get_vars,
@@ -17,6 +17,7 @@ from .pinn import (AbstractPINN, Adam, BPINNsolution, BPINNstats, DiagEuclideanM
                    StanHMCAdaptor, UnitEuclideanMetric, ahmc_bayesian_pinn_pde, pmean, BFGS, BackTracking, BayesianPINN, Chain, DataLoss, Dense, Descent, GradientScaleAdaptiveLoss, HagerZhang, LBFGS, LogOptions, MiniMaxAdaptiveLoss,
                    NonAdaptiveLoss, ReLoBRaLoAdaptiveLoss, SoftAdaptAdaptiveLoss,
                    OptimizationFunction, OptimizationProblem, Phi, PhysicsInformedNN, PINNRepresentation, Solution,
-                   discretize, initialparameters, logscalar, logvector, solve, symbolic_discretize)
+                   discretize, initialparameters, logscalar, logvector, register_symbolic, solve, symbolic_discretize)
+from .adapter import NeuralAdapterLoss, neural_adapter
 
 __all__ = [n for n in dir() if not n.startswith("_")]

@@ -41,6 +41,15 @@ UNITS = [
     ("ffma_f32_gmem_integ.o", "ffma_inst.cu", ["-DPINN_INST_REAL=float", "-DPINN_INST_BUFS=0", "-DPINN_INST_INTEG=1"]),
     ("ffma_f64_smem_integ.o", "ffma_inst.cu", ["-DPINN_INST_REAL=double", "-DPINN_INST_BUFS=1", "-DPINN_INST_INTEG=1"]),
     ("ffma_f64_gmem_integ.o", "ffma_inst.cu", ["-DPINN_INST_REAL=double", "-DPINN_INST_BUFS=0", "-DPINN_INST_INTEG=1"]),
+    # and with fixed networks (neural adapters, registered network functions), with or without integral terms
+    ("ffma_f32_smem_fixed.o", "ffma_inst.cu", ["-DPINN_INST_REAL=float", "-DPINN_INST_BUFS=1", "-DPINN_INST_INTEG=1",
+                                              "-DPINN_INST_FIXED=1"]),
+    ("ffma_f32_gmem_fixed.o", "ffma_inst.cu", ["-DPINN_INST_REAL=float", "-DPINN_INST_BUFS=0", "-DPINN_INST_INTEG=1",
+                                              "-DPINN_INST_FIXED=1"]),
+    ("ffma_f64_smem_fixed.o", "ffma_inst.cu", ["-DPINN_INST_REAL=double", "-DPINN_INST_BUFS=1", "-DPINN_INST_INTEG=1",
+                                              "-DPINN_INST_FIXED=1"]),
+    ("ffma_f64_gmem_fixed.o", "ffma_inst.cu", ["-DPINN_INST_REAL=double", "-DPINN_INST_BUFS=0", "-DPINN_INST_INTEG=1",
+                                              "-DPINN_INST_FIXED=1"]),
 ]
 
 

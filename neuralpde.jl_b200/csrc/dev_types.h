@@ -85,6 +85,12 @@ struct DevProblem {
   DevTerm terms[PINN_MAX_TERMS];
   int n_integrals;
   DevIntegral integ[PINN_MAX_INTEGRALS];
+  // fixed networks (pinn_create_ex2): a tap's network n_nets + j is fixed[j]; w_off / b_off index its own parameter
+  // buffer fixed_params[j] (written by pinn_set_fixed_params: the kernel arguments of problems without fixed networks
+  // stay as they were), not theta
+  int n_fixed;
+  DevNet fixed[PINN_MAX_FIXED_NETS];
+  const void* fixed_params[PINN_MAX_FIXED_NETS];
 };
 
 // per term scale (L_k = scale_k * sum_p qw_p r_p^2) and loss weight, passed by value
@@ -146,5 +152,6 @@ struct FfmaArgs {
   TermDyn dyn[PINN_MAX_TERMS];
   TailArgs tail;
 };
+static_assert(sizeof(FfmaArgs) <= 4096, "FFMA kernel arguments must stay under 4 KB");
 
 }  // namespace pinn

@@ -40,6 +40,9 @@ struct pinn_engine {
   long long n_theta = 0, partial_stride = 0;
   pinn::TermState term[PINN_MAX_TERMS];
   pinn::TermDyn dyn[PINN_MAX_TERMS] = {};
+  // fixed networks: the parameters each launch reads (aliased or fixed_own), engine-owned copies of the *_host variant
+  const void* fixed_ptr[PINN_MAX_FIXED_NETS] = {};
+  void* fixed_own[PINN_MAX_FIXED_NETS] = {};
   int total_tiles = 0, num_sms = 0;
   long long *tc_dbg = nullptr, *tail_dbg = nullptr;   // pinn_debug_tc_timeline / pinn_debug_tail_marks buffers
   // wide tensor path (128-wide layers): streamed weights, fp32 pre-activation stash

@@ -1,6 +1,7 @@
 // ffma_inst.cu -- one explicit instantiation of the fused kernel per translation unit
-// (compiled eight times: {float,double} x {activation buffers in smem, in global} x {without, with integral terms}) so
-// the build parallelises.  -DPINN_INST_REAL=float|double -DPINN_INST_BUFS=0|1 [-DPINN_INST_INTEG=1]
+// (compiled twelve times: {float,double} x {activation buffers in smem, in global} x {plain, with integral terms, with
+// fixed networks (and integral terms)}) so the build parallelises.
+// -DPINN_INST_REAL=float|double -DPINN_INST_BUFS=0|1 [-DPINN_INST_INTEG=1 [-DPINN_INST_FIXED=1]]
 #include "ffma_kernel.cuh"
 
 namespace pinn {
@@ -12,17 +13,24 @@ namespace pinn {
 #else
 #define PINN_BUFS_NAME gmem
 #endif
-#if PINN_INST_INTEG
+#ifndef PINN_INST_INTEG
+#define PINN_INST_INTEG 0
+#endif
+#ifndef PINN_INST_FIXED
+#define PINN_INST_FIXED 0
+#endif
+#if PINN_INST_FIXED
+#define PINN_BUFS_NAME_X PINN_CAT(PINN_BUFS_NAME, _fixed)
+#elif PINN_INST_INTEG
 #define PINN_BUFS_NAME_X PINN_CAT(PINN_BUFS_NAME, _integ)
 #else
-#define PINN_INST_INTEG 0
 #define PINN_BUFS_NAME_X PINN_BUFS_NAME
 #endif
 #define PINN_LAUNCH_NAME PINN_CAT(PINN_CAT(PINN_CAT(ffma_launch_, PINN_INST_REAL), _), PINN_BUFS_NAME_X)
 
 cudaError_t PINN_LAUNCH_NAME(const FfmaArgs& a, int grid, size_t smem, cudaStream_t st) {
-  return launch_fused_kernel<ffma_loss_grad_kernel<PINN_INST_REAL, (PINN_INST_BUFS != 0), (PINN_INST_INTEG != 0)>>(
-      a, grid, kThreads, smem, st);
+  return launch_fused_kernel<ffma_loss_grad_kernel<PINN_INST_REAL, (PINN_INST_BUFS != 0), (PINN_INST_INTEG != 0),
+                                                   (PINN_INST_FIXED != 0)>>(a, grid, kThreads, smem, st);
 }
 
 }  // namespace pinn

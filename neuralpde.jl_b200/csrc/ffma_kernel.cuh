@@ -520,17 +520,38 @@ __device__ __forceinline__ real warp_sum(real v) {
   return v;
 }
 
+// ---- fixed networks (pinn_create_ex2): network index n_nets + j is fixed network j -------------------------------------
+// FIXED: the instantiation for problems with fixed networks; without it these compile to the old reads
+template <bool FIXED>
+__device__ __forceinline__ bool is_fixed(const DevProblem& P, int k) {
+  if constexpr (FIXED) return k >= P.n_nets;
+  return false;
+}
+template <bool FIXED>
+__device__ __forceinline__ const DevNet& net_of(const DevProblem& P, int k) {
+  if constexpr (FIXED)
+    if (k >= P.n_nets) return P.fixed[k - P.n_nets];
+  return P.nets[k];
+}
+template <typename real>
+__device__ __forceinline__ const real* fixed_params(const DevProblem& P, int k) {
+  return reinterpret_cast<const real*>(P.fixed_params[k - P.n_nets]);
+}
+
 // ------------------------------------------------------------------------------------------
 // forward through every network term tm taps, at the point tile X ([row][point]): the outputs land in taps; save:
 // keep the pre-activations in the stash for the reverse sweep
-template <typename real>
+template <typename real, bool FIXED>
 __device__ __forceinline__ void forward_nets(const FfmaArgs& args, const DevProblem& P, const DevTerm& tm,
                                              const real* __restrict__ theta, const real* X, real* bufA, real* bufB,
                                              real* wsm, real* stash, real* taps, bool save, int ldc, int tid, int warp,
                                              int lane) {
   constexpr int TP = Cfg<real>::TP;
   for (int slot = 0; slot < tm.n_used; ++slot) {
-    const DevNet& net = P.nets[tm.used_net[slot]];
+    const int k = tm.used_net[slot];
+    const DevNet& net = net_of<FIXED>(P, k);
+    const bool fixed = is_fixed<FIXED>(P, k);
+    const real* src = fixed ? fixed_params<real>(P, k) : theta;   // a fixed network saves nothing to the stash
     const DevChan& ch = tm.chan[slot];
     const int C = ch.C;
     real* H = bufA;
@@ -550,7 +571,7 @@ __device__ __forceinline__ void forward_nets(const FfmaArgs& args, const DevProb
       } else {
         constexpr int PW = kWarps * 8;   // panel of 64 output neurons
         for (int pb = 0; pb < n_out8; pb += PW) {
-          stage_panel<real>(theta, net, l, 0, n_in8, pb, PW, wsm, wsm + n_in8 * PW, tid);
+          stage_panel<real>(src, net, l, 0, n_in8, pb, PW, wsm, wsm + n_in8 * PW, tid);
           __syncthreads();   // panel (and, first time, layer inputs) visible
           const int ob = pb + warp * 8;
           if (ob < n_out8) {
@@ -560,7 +581,7 @@ __device__ __forceinline__ void forward_nets(const FfmaArgs& args, const DevProb
           __syncthreads();   // panel consumed
         }
       }
-      elementwise_fwd<real>(Z, stash + ch.stash_off[l], ch, net.acts[l], n_out, ldc, warp, lane, save);
+      elementwise_fwd<real>(Z, stash + ch.stash_off[l], ch, net.acts[l], n_out, ldc, warp, lane, save && !fixed);
       real* t = H; H = Z; Z = t;
       // the next layer's __syncthreads (or the one below) orders these writes
     }
@@ -575,13 +596,15 @@ __device__ __forceinline__ void forward_nets(const FfmaArgs& args, const DevProb
 }
 
 // reverse sweep through every network term tm taps, from the tap adjoints tapbar, into this CTA's gradient partial
-template <typename real>
+// (fixed networks are skipped: their tap adjoints reach nothing trainable)
+template <typename real, bool FIXED>
 __device__ __forceinline__ void reverse_nets(const FfmaArgs& args, const DevProblem& P, const DevTerm& tm,
                                              const real* __restrict__ theta, const real* X, real* bufA, real* bufB,
                                              real* wsm, const real* stash, const real* tapbar, real* partial, int ldc,
                                              int tid, int warp, int lane) {
   constexpr int TP = Cfg<real>::TP;
   for (int slot = 0; slot < tm.n_used; ++slot) {
+    if (is_fixed<FIXED>(P, tm.used_net[slot])) continue;   // uniform over the CTA
     const DevNet& net = P.nets[tm.used_net[slot]];
     const DevChan& ch = tm.chan[slot];
     const int C = ch.C;
@@ -675,7 +698,7 @@ __device__ __forceinline__ real node_tile(const DevIntegral& I, int dim, int j, 
 inline __device__ int node_count(const DevIntegral& I) { return I.n_dims == 2 ? I.q * I.q : I.q; }
 
 // values of term ti's integrals at the owner tile Xs: ival[k][p] for its k-th integral
-template <typename real>
+template <typename real, bool FIXED>
 __device__ __forceinline__ void integrals_forward(const FfmaArgs& args, const DevProblem& P, int ti,
                                                   const real* __restrict__ theta, const real* Xs, real* Xn, real* ival,
                                                   real* bufA, real* bufB, real* wsm, real* stash, real* taps, int tid,
@@ -688,7 +711,7 @@ __device__ __forceinline__ void integrals_forward(const FfmaArgs& args, const De
     for (int j = 0; j < node_count(I); ++j) {
       if (warp == 0) wj = node_tile<real>(I, P.terms[ti].dim, j, Xs, Xn, lane);
       __syncthreads();
-      forward_nets<real>(args, P, I.body, theta, Xn, bufA, bufB, wsm, stash, taps, false, args.ldc, tid, warp, lane);
+      forward_nets<real, FIXED>(args, P, I.body, theta, Xn, bufA, bufB, wsm, stash, taps, false, args.ldc, tid, warp, lane);
       if (warp == 0)
         acc += wj * run_program<real, kTilePts>(I.body, theta + P.param_off, Xn, taps, (real*)nullptr, (real*)nullptr,
                                                 lane, false);
@@ -699,7 +722,7 @@ __device__ __forceinline__ void integrals_forward(const FfmaArgs& args, const De
 }
 
 // gradient of term ti's integrals, given ibar[k][p] = dtotal / dI_p of its k-th integral
-template <typename real>
+template <typename real, bool FIXED>
 __device__ __forceinline__ void integrals_reverse(const FfmaArgs& args, const DevProblem& P, int ti,
                                                   const real* __restrict__ theta, const real* Xs, real* Xn,
                                                   const real* ibar, real* bufA, real* bufB, real* wsm, real* stash,
@@ -713,7 +736,7 @@ __device__ __forceinline__ void integrals_reverse(const FfmaArgs& args, const De
     for (int j = 0; j < node_count(I); ++j) {
       if (warp == 0) wj = node_tile<real>(I, P.terms[ti].dim, j, Xs, Xn, lane);
       __syncthreads();
-      forward_nets<real>(args, P, body, theta, Xn, bufA, bufB, wsm, stash, taps, true, args.ldc, tid, warp, lane);
+      forward_nets<real, FIXED>(args, P, body, theta, Xn, bufA, bufB, wsm, stash, taps, true, args.ldc, tid, warp, lane);
       if (warp == 0) {
         real pbar[PINN_MAX_PARAMS];
 #pragma unroll
@@ -728,15 +751,16 @@ __device__ __forceinline__ void integrals_reverse(const FfmaArgs& args, const De
         }
       }
       __syncthreads();
-      reverse_nets<real>(args, P, body, theta, Xn, bufA, bufB, wsm, stash, tapbar, partial, args.ldc, tid, warp, lane);
+      reverse_nets<real, FIXED>(args, P, body, theta, Xn, bufA, bufB, wsm, stash, tapbar, partial, args.ldc, tid, warp, lane);
     }
     ++k;
   }
 }
 
 // ------------------------------------------------------------------------------------------
-// INTEG: the problem has integral terms (pinn_create_ex); the instantiation without them is the kernel as it was
-template <typename real, bool BUFS_SMEM, bool INTEG>
+// INTEG: the problem has integral terms (pinn_create_ex); FIXED: it has fixed networks (pinn_create_ex2), instantiated
+// with INTEG = true only.  <false, false> is the kernel without either, <true, false> the integral kernel as it was.
+template <typename real, bool BUFS_SMEM, bool INTEG, bool FIXED>
 __global__ void __launch_bounds__(kThreads, 1) ffma_loss_grad_kernel(const FfmaArgs args) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -761,8 +785,8 @@ __global__ void __launch_bounds__(kThreads, 1) ffma_loss_grad_kernel(const FfmaA
   real* rres = sm; sm += kTilePts;      // residual per point
   real* qws = sm; sm += kTilePts;       // quadrature weight per point (0 for padded lanes)
   double* tsum = reinterpret_cast<double*>(sm);  // [PINN_MAX_TERMS], 8-byte aligned by construction
-  real* Xn = reinterpret_cast<real*>(tsum + PINN_MAX_TERMS);   // INTEG: node-point tile
-  real* ival = Xn + (PINN_MAX_DIM + 2) * kTilePts;              // INTEG: the term's integrals, then their adjoints
+  real* Xn = reinterpret_cast<real*>(tsum + PINN_MAX_TERMS);   // integral terms: node-point tile
+  real* ival = Xn + (PINN_MAX_DIM + 2) * kTilePts;              // integral terms: the term's integrals, then their adjoints
 
   real* partial = reinterpret_cast<real*>(args.partial) + (long long)blockIdx.x * args.partial_stride;
   real* stash = reinterpret_cast<real*>(args.stash) + (long long)blockIdx.x * args.stash_per_cta;
@@ -780,6 +804,13 @@ __global__ void __launch_bounds__(kThreads, 1) ffma_loss_grad_kernel(const FfmaA
       for (int l = 0; l < P.nets[k].n_layers; ++l)
         stage_panel<real>(theta, P.nets[k], l, 0, (P.nets[k].dims[l] + 7) & ~7, 0, (P.nets[k].dims[l + 1] + 7) & ~7,
                           wsm + P.nets[k].ws_off[l], wsm + P.nets[k].bs_off[l], tid);
+    if constexpr (FIXED)
+      for (int j = 0; j < P.n_fixed; ++j) {
+        const DevNet& f = P.fixed[j];
+        for (int l = 0; l < f.n_layers; ++l)
+          stage_panel<real>(reinterpret_cast<const real*>(P.fixed_params[j]), f, l, 0, (f.dims[l] + 7) & ~7, 0,
+                            (f.dims[l + 1] + 7) & ~7, wsm + f.ws_off[l], wsm + f.bs_off[l], tid);
+      }
   }
   __syncthreads();
 
@@ -812,11 +843,11 @@ __global__ void __launch_bounds__(kThreads, 1) ffma_loss_grad_kernel(const FfmaA
     int n_int = 0;   // integrals of this term (uniform)
     if constexpr (INTEG) {
       for (int i = 0; i < P.n_integrals; ++i) n_int += P.integ[i].owner == ti;
-      if (n_int) integrals_forward<real>(args, P, ti, theta, Xs, Xn, ival, bufA, bufB, wsm, stash, taps, tid, warp, lane);
+      if (n_int) integrals_forward<real, FIXED>(args, P, ti, theta, Xs, Xn, ival, bufA, bufB, wsm, stash, taps, tid, warp, lane);
     }
 
     // ---- forward through every tapped network ------------------------------------------------
-    forward_nets<real>(args, P, tm, theta, Xs, bufA, bufB, wsm, stash, taps, want_grad, ldc, tid, warp, lane);
+    forward_nets<real, FIXED>(args, P, tm, theta, Xs, bufA, bufB, wsm, stash, taps, want_grad, ldc, tid, warp, lane);
 
     // ---- residual, loss partial, tap adjoints (warp 0, lane == point) --------------------------
     if (warp == 0) {
@@ -853,10 +884,10 @@ __global__ void __launch_bounds__(kThreads, 1) ffma_loss_grad_kernel(const FfmaA
     __syncthreads();
 
     // ---- reverse sweep through every tapped network -----------------------------------------------
-    if (want_grad) reverse_nets<real>(args, P, tm, theta, Xs, bufA, bufB, wsm, stash, tapbar, partial, ldc, tid, warp, lane);
+    if (want_grad) reverse_nets<real, FIXED>(args, P, tm, theta, Xs, bufA, bufB, wsm, stash, tapbar, partial, ldc, tid, warp, lane);
     if constexpr (INTEG)
       if (want_grad && n_int)
-        integrals_reverse<real>(args, P, ti, theta, Xs, Xn, ival, bufA, bufB, wsm, stash, taps, tapbar, partial, tid, warp,
+        integrals_reverse<real, FIXED>(args, P, ti, theta, Xs, Xn, ival, bufA, bufB, wsm, stash, taps, tapbar, partial, tid, warp,
                                 lane);
   }
 

@@ -45,16 +45,24 @@ cudaError_t ffma_launch_float_smem_integ(const FfmaArgs& a, int grid, size_t sme
 cudaError_t ffma_launch_float_gmem_integ(const FfmaArgs& a, int grid, size_t smem, cudaStream_t st);
 cudaError_t ffma_launch_double_smem_integ(const FfmaArgs& a, int grid, size_t smem, cudaStream_t st);
 cudaError_t ffma_launch_double_gmem_integ(const FfmaArgs& a, int grid, size_t smem, cudaStream_t st);
+cudaError_t ffma_launch_float_smem_fixed(const FfmaArgs& a, int grid, size_t smem, cudaStream_t st);
+cudaError_t ffma_launch_float_gmem_fixed(const FfmaArgs& a, int grid, size_t smem, cudaStream_t st);
+cudaError_t ffma_launch_double_smem_fixed(const FfmaArgs& a, int grid, size_t smem, cudaStream_t st);
+cudaError_t ffma_launch_double_gmem_fixed(const FfmaArgs& a, int grid, size_t smem, cudaStream_t st);
 
-// integ: the instantiation that evaluates integral terms on node tiles
-cudaError_t ffma_launch(int dtype, bool bufs_smem, bool integ, const FfmaArgs& a, int grid, size_t smem, cudaStream_t st) {
+// integ: the instantiation that evaluates integral terms on node tiles; fixed: the one that also evaluates fixed networks
+cudaError_t ffma_launch(int dtype, bool bufs_smem, bool integ, bool fixed, const FfmaArgs& a, int grid, size_t smem,
+                        cudaStream_t st) {
+  const bool f64 = dtype == PINN_F64;
+  if (fixed) {
+    if (f64) return bufs_smem ? ffma_launch_double_smem_fixed(a, grid, smem, st) : ffma_launch_double_gmem_fixed(a, grid, smem, st);
+    return bufs_smem ? ffma_launch_float_smem_fixed(a, grid, smem, st) : ffma_launch_float_gmem_fixed(a, grid, smem, st);
+  }
   if (integ) {
-    if (dtype == PINN_F64)
-      return bufs_smem ? ffma_launch_double_smem_integ(a, grid, smem, st) : ffma_launch_double_gmem_integ(a, grid, smem, st);
+    if (f64) return bufs_smem ? ffma_launch_double_smem_integ(a, grid, smem, st) : ffma_launch_double_gmem_integ(a, grid, smem, st);
     return bufs_smem ? ffma_launch_float_smem_integ(a, grid, smem, st) : ffma_launch_float_gmem_integ(a, grid, smem, st);
   }
-  if (dtype == PINN_F64)
-    return bufs_smem ? ffma_launch_double_smem(a, grid, smem, st) : ffma_launch_double_gmem(a, grid, smem, st);
+  if (f64) return bufs_smem ? ffma_launch_double_smem(a, grid, smem, st) : ffma_launch_double_gmem(a, grid, smem, st);
   return bufs_smem ? ffma_launch_float_smem(a, grid, smem, st) : ffma_launch_float_gmem(a, grid, smem, st);
 }
 

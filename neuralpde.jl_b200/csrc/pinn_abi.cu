@@ -15,7 +15,8 @@
 #include "engine.h"
 
 namespace pinn {
-cudaError_t ffma_launch(int dtype, bool bufs_smem, bool integ, const FfmaArgs& a, int grid, size_t smem, cudaStream_t st);
+cudaError_t ffma_launch(int dtype, bool bufs_smem, bool integ, bool fixed, const FfmaArgs& a, int grid, size_t smem,
+                        cudaStream_t st);
 cudaError_t grad_stats_launch(int dtype, const void* grad, long long n, double* out2, cudaStream_t st);
 cudaError_t sample_uniform_launch(int dtype, void* pts, long long n, int dim, const double* lb, const double* ub,
                                   unsigned long long seed, unsigned long long draw, const unsigned long long* draw_dev,
@@ -139,6 +140,7 @@ int pinn_destroy(pinn_handle e) {
     if (ts.own_pts) cudaFree(ts.own_pts);
     if (ts.own_qw) cudaFree(ts.own_qw);
   }
+  for (void* p : e->fixed_own) if (p) cudaFree(p);
   if (e->h_pin_in) cudaFreeHost(e->h_pin_in);
   if (e->h_pin_out) cudaFreeHost(e->h_pin_out);
   if (e->own_stream) cudaStreamDestroy(e->own_stream);
@@ -158,6 +160,11 @@ int pinn_quadrature_nodes(int32_t q, double* x, double* w) {
 }
 
 int pinn_create_ex(const pinn_problem_desc* d, const pinn_integral_desc* integrals, int32_t n_integrals, pinn_handle* out) {
+  return pinn_create_ex2(d, integrals, n_integrals, nullptr, 0, out);
+}
+
+int pinn_create_ex2(const pinn_problem_desc* d, const pinn_integral_desc* integrals, int32_t n_integrals,
+                    const pinn_fixed_net_desc* fixed, int32_t n_fixed, pinn_handle* out) {
   if (!out) return fail("pinn_create: null output handle");
   *out = nullptr;
   if (!d) return fail("pinn_create: null descriptor");
@@ -175,7 +182,7 @@ int pinn_create_ex(const pinn_problem_desc* d, const pinn_integral_desc* integra
   int max_smem = 0;
   cudaDeviceGetAttribute(&max_smem, cudaDevAttrMaxSharedMemoryPerBlockOptin, e->device);
   if (max_smem <= 0) max_smem = 227 * 1024;
-  if (plan_problem(d, integrals, n_integrals, max_smem, e->plan)) { pinn_destroy(e); return 1; }
+  if (plan_problem(d, integrals, n_integrals, fixed, n_fixed, max_smem, e->plan)) { pinn_destroy(e); return 1; }
   const Plan& p = e->plan;
   cudaDeviceGetAttribute(&e->num_sms, cudaDevAttrMultiProcessorCount, e->device);
   if (e->num_sms <= 0) e->num_sms = 132;
@@ -229,6 +236,46 @@ int pinn_create_ex(const pinn_problem_desc* d, const pinn_integral_desc* integra
   retile(e);
   *out = e;
   return 0;
+}
+
+static int check_fixed(pinn_handle e, int32_t j, const char* fn) {
+  if (!e) return fail("%s: null handle", fn);
+  if (j < 0 || j >= e->plan.prob.n_fixed)
+    return fail("%s: fixed network %d out of range [0,%d)", fn, j, e->plan.prob.n_fixed);
+  return 0;
+}
+
+// point fixed network j at p in the device copy of the problem; evaluations still in flight finish with the old pointer
+// first (the kernels read it from there, so captured Adam graphs need no re-capture)
+static int bind_fixed(pinn_engine* e, int j, const void* p) {
+  CUDA_TRY(cudaSetDevice(e->device));
+  if (e->fixed_ptr[j] == p) return 0;
+  CUDA_TRY(cudaDeviceSynchronize());
+  CUDA_TRY(cudaMemcpy(&e->dprob->fixed_params[j], &p, sizeof p, cudaMemcpyHostToDevice));
+  e->fixed_ptr[j] = p;
+  return 0;
+}
+
+int pinn_set_fixed_params(pinn_handle e, int32_t j, const void* dev_params) {
+  if (check_fixed(e, j, "pinn_set_fixed_params")) return 1;
+  if (!dev_params) return fail("pinn_set_fixed_params: null parameters");
+  return bind_fixed(e, j, dev_params);
+}
+
+int pinn_set_fixed_params_host(pinn_handle e, int32_t j, const void* host_params, void* stream) {
+  if (check_fixed(e, j, "pinn_set_fixed_params_host")) return 1;
+  if (!host_params) return fail("pinn_set_fixed_params_host: null parameters");
+  CUDA_TRY(cudaSetDevice(e->device));
+  const size_t bytes = (size_t)e->plan.fixed_len[j] * e->es;
+  if (!e->fixed_own[j]) {
+    if (dev_alloc(&e->fixed_own[j], bytes, e)) return 1;
+  } else {
+    CUDA_TRY(cudaDeviceSynchronize());   // evaluations in flight on any stream may still read the bound buffer
+  }
+  // complete before returning: later evaluations, on whatever stream, read the new parameters
+  CUDA_TRY(cudaMemcpyAsync(e->fixed_own[j], host_params, bytes, cudaMemcpyHostToDevice, (cudaStream_t)stream));
+  CUDA_TRY(cudaStreamSynchronize((cudaStream_t)stream));
+  return bind_fixed(e, j, e->fixed_own[j]);
 }
 
 static int check_term(pinn_handle e, int32_t term, const char* fn) {
@@ -317,7 +364,11 @@ static int launch_fused(pinn_engine* e, const LaunchCall& c, int grid, cudaStrea
   if (e->mode == PINN_MODE_FFMA) {
     FfmaArgs a = with_call(p.ffma, e, c);
     a.n_tiles = e->total_tiles;
-    CUDA_TRY(ffma_launch(e->dtype, p.bufs_smem, p.integ, a, grid, p.smem, st));
+    for (int j = 0; j < p.prob.n_fixed; ++j)
+      if (!e->fixed_ptr[j])
+        return fail("pinn: fixed network %d has no parameters (call pinn_set_fixed_params or pinn_set_fixed_params_host "
+                    "first)", j);
+    CUDA_TRY(ffma_launch(e->dtype, p.bufs_smem, p.integ, p.prob.n_fixed > 0, a, grid, p.smem, st));
     return 0;
   }
   if (p.wide) {

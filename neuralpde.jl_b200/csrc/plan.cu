@@ -22,40 +22,56 @@ const char* last_error() { return g_err.c_str(); }
 
 namespace {
 // ---- networks and θ layout ------------------------------------------------------------------------------------------
-// θ offsets of every layer and the FFMA path's staged (8-padded) weight layout; max_w8 and resident feed its geometry
-int plan_nets(const pinn_problem_desc* d, DevProblem& P, int& max_w8, long long& resident) {
+// one network's layer offsets (from off: θ, or a fixed network's own buffer) and the FFMA path's staged (8-padded) weight
+// layout; returns the end offset, or -1 after fail()
+long long plan_net(const char* what, int k, int n_layers, const int32_t* dims, const int32_t* acts, long long off,
+                   DevNet& n, int& max_w8, long long& resident) {
+  if (n_layers < 1 || n_layers > PINN_MAX_LAYERS)
+    return fail("pinn_create: %s %d has %d layers (supported 1..%d)", what, k, n_layers, PINN_MAX_LAYERS), -1;
+  if (!dims || !acts) return fail("pinn_create: %s %d null dims/acts", what, k), -1;
+  n.n_layers = n_layers;
+  for (int l = 0; l <= n_layers; ++l) {
+    if (dims[l] < 1) return fail("pinn_create: %s %d dims[%d]=%d must be >= 1", what, k, l, dims[l]), -1;
+    n.dims[l] = dims[l];
+    max_w8 = std::max(max_w8, (dims[l] + 7) & ~7);
+  }
+  if (n.dims[0] > PINN_MAX_IN) return fail("pinn_create: %s %d input dimension %d > %d", what, k, n.dims[0], PINN_MAX_IN), -1;
+  for (int l = 0; l < n_layers; ++l) {
+    if (acts[l] < PINN_ACT_IDENTITY || acts[l] > PINN_ACT_SWISH)
+      return fail("pinn_create: %s %d layer %d unknown activation %d", what, k, l, acts[l]), -1;
+    n.acts[l] = acts[l];
+    n.w_off[l] = off; off += (long long)n.dims[l] * n.dims[l + 1];
+    n.b_off[l] = off; off += n.dims[l + 1];
+    int in8 = (n.dims[l] + 7) & ~7, out8 = (n.dims[l + 1] + 7) & ~7;
+    n.ws_off[l] = (int)resident; resident += (long long)in8 * out8;
+    n.bs_off[l] = (int)resident; resident += out8;
+  }
+  n.max_width8 = max_w8;   // running maximum over the networks planned so far
+  return off;
+}
+
+// the trainable networks (θ layout), then the fixed ones (each from offset 0 of its own buffer; *fixed_len: its length)
+int plan_nets(const pinn_problem_desc* d, const pinn_fixed_net_desc* fixed, int n_fixed, DevProblem& P, int& max_w8,
+              long long& resident, long long* fixed_len) {
   for (int k = 0; k < d->n_nets; ++k) {
     const pinn_net_desc& nd = d->nets[k];
-    DevNet& n = P.nets[k];
-    if (nd.n_layers < 1 || nd.n_layers > PINN_MAX_LAYERS)
-      return fail("pinn_create: net %d has %d layers (supported 1..%d)", k, nd.n_layers, PINN_MAX_LAYERS);
-    if (!nd.dims || !nd.acts) return fail("pinn_create: net %d null dims/acts", k);
-    n.n_layers = nd.n_layers;
-    long long off = nd.theta_offset;
-    if (off < 0) return fail("pinn_create: net %d negative theta_offset", k);
-    for (int l = 0; l <= nd.n_layers; ++l) {
-      if (nd.dims[l] < 1) return fail("pinn_create: net %d dims[%d]=%d must be >= 1", k, l, nd.dims[l]);
-      n.dims[l] = nd.dims[l];
-      max_w8 = std::max(max_w8, (nd.dims[l] + 7) & ~7);
-    }
-    if (n.dims[0] > PINN_MAX_IN) return fail("pinn_create: net %d input dimension %d > %d", k, n.dims[0], PINN_MAX_IN);
-    for (int l = 0; l < nd.n_layers; ++l) {
-      if (nd.acts[l] < PINN_ACT_IDENTITY || nd.acts[l] > PINN_ACT_SWISH)
-        return fail("pinn_create: net %d layer %d unknown activation %d", k, l, nd.acts[l]);
-      n.acts[l] = nd.acts[l];
-      n.w_off[l] = off; off += (long long)n.dims[l] * n.dims[l + 1];
-      n.b_off[l] = off; off += n.dims[l + 1];
-      int in8 = (n.dims[l] + 7) & ~7, out8 = (n.dims[l + 1] + 7) & ~7;
-      n.ws_off[l] = (int)resident; resident += (long long)in8 * out8;
-      n.bs_off[l] = (int)resident; resident += out8;
-    }
+    if (nd.theta_offset < 0) return fail("pinn_create: net %d negative theta_offset", k);
+    const long long off = plan_net("net", k, nd.n_layers, nd.dims, nd.acts, nd.theta_offset, P.nets[k], max_w8, resident);
+    if (off < 0) return 1;
     if (off > d->n_theta)
       return fail("pinn_create: net %d parameters [%lld,%lld) exceed n_theta=%lld", k, (long long)nd.theta_offset, off,
                   (long long)d->n_theta);
-    n.max_width8 = max_w8;   // running maximum over networks 0..k
+  }
+  for (int j = 0; j < n_fixed; ++j) {
+    fixed_len[j] = plan_net("fixed network", j, fixed[j].n_layers, fixed[j].dims, fixed[j].acts, 0, P.fixed[j], max_w8,
+                            resident);
+    if (fixed_len[j] < 0) return 1;
   }
   return 0;
 }
+
+// network k of a tap: trainable (k < n_nets) or fixed network k - n_nets
+const DevNet& net_ref(const DevProblem& P, int k) { return k < P.n_nets ? P.nets[k] : P.fixed[k - P.n_nets]; }
 
 // ---- per-term channel planning ---------------------------------------------------------------------------------------
 // lookups in a slot's channel set (-1: absent): direction x in dir1, second derivative (a, b), third along dir1[a]
@@ -79,16 +95,21 @@ int check_room(const DevChan& ch, const char* what, int t, int net) {
 // (what, t: "term" / "integral" and its index, for the messages)
 int plan_channels(const pinn_problem_desc* d, const pinn_term_desc& td, const char* what, int t, const DevProblem& P,
                   DevTerm& T, int* slot_of) {
-  for (int k = 0; k < PINN_MAX_NETS; ++k) slot_of[k] = -1;
+  const int n_all = d->n_nets + P.n_fixed;
+  for (int k = 0; k < kMaxAllNets; ++k) slot_of[k] = -1;
   T.n_used = 0;
   for (int i = 0; i < td.n_taps; ++i) {
     const pinn_tap_desc& tp = td.taps[i];
-    if (tp.net < 0 || tp.net >= d->n_nets) return fail("pinn_create: %s %d tap %d names network %d", what, t, i, tp.net);
+    if (tp.net < 0 || tp.net >= n_all)
+      return fail("pinn_create: %s %d tap %d names network %d (the problem has %d trainable and %d fixed networks)", what,
+                  t, i, tp.net, d->n_nets, P.n_fixed);
     if (slot_of[tp.net] >= 0) continue;
+    if (T.n_used == PINN_MAX_NETS)
+      return fail("pinn_create: %s %d taps more than %d networks", what, t, PINN_MAX_NETS);
     slot_of[tp.net] = T.n_used;
     T.used_net[T.n_used] = tp.net;
     DevChan& ch = T.chan[T.n_used];   // zeroed with the plan: no derivative channels yet
-    for (int j = 0; j < P.nets[tp.net].dims[0]; ++j) {
+    for (int j = 0; j < net_ref(P, tp.net).dims[0]; ++j) {
       int r = td.net_rows[tp.net * PINN_MAX_IN + j];
       if (r < 0 || r >= td.dim)
         return fail("pinn_create: %s %d network %d input %d maps to point row %d (dim=%d)", what, t, tp.net, j, r, td.dim);
@@ -98,7 +119,7 @@ int plan_channels(const pinn_problem_desc* d, const pinn_term_desc& td, const ch
   }
   for (int i = 0; i < td.n_taps; ++i) {
     const pinn_tap_desc& tp = td.taps[i];
-    const DevNet& n = P.nets[tp.net];
+    const DevNet& n = net_ref(P, tp.net);
     DevChan& ch = T.chan[slot_of[tp.net]];
     if (tp.order < 0 || tp.order > 3)
       return fail("pinn_create: %s %d tap %d has derivative order %d; orders 0..3 are supported (order 4 and mixed "
@@ -231,7 +252,7 @@ int plan_body(const pinn_problem_desc* d, const pinn_term_desc& td, const char* 
     return fail("pinn_create: %s %d program length %d out of range [1,%d]", what, t, td.n_instr, PINN_MAX_INSTR);
   if (!td.taps || !td.prog || !td.net_rows) return fail("pinn_create: %s %d null taps/prog/net_rows", what, t);
   T.dim = td.dim; T.n_taps = td.n_taps; T.n_instr = td.n_instr;
-  int slot_of[PINN_MAX_NETS];
+  int slot_of[kMaxAllNets];
   if (plan_channels(d, td, what, t, P, T, slot_of)) return 1;
   long long stash = 0;
   double f = 0;
@@ -241,14 +262,15 @@ int plan_body(const pinn_problem_desc* d, const pinn_term_desc& td, const char* 
     ch.C = 1 + ch.n1 + ch.n2 + ch.n3;
     if (ch.C > PINN_MAX_CH) return fail("pinn_create: %s %d needs %d channels (max %d)", what, t, ch.C, PINN_MAX_CH);
     max_c = std::max(max_c, ch.C);
-    const DevNet& n = P.nets[T.used_net[s]];
+    const DevNet& n = net_ref(P, T.used_net[s]);
+    const bool fixed = T.used_net[s] >= P.n_nets;   // forward only: no stash, no reverse sweep
     double S = 0;
     for (int l = 0; l < n.n_layers; ++l) {
       ch.stash_off[l] = (int)stash;
-      stash += (long long)ch.C * n.dims[l + 1] * kTilePts;
+      if (!fixed) stash += (long long)ch.C * n.dims[l + 1] * kTilePts;
       S += (double)n.dims[l] * n.dims[l + 1];
     }
-    f += 6.0 * ch.C * S;
+    f += (fixed ? 2.0 : 6.0) * ch.C * S;
   }
   stash_max = std::max(stash_max, stash);
   if (plan_taps(d, td, what, t, slot_of, integrals, n_integrals, T)) return 1;
@@ -569,9 +591,16 @@ int plan_tc(const pinn_problem_desc* d, int max_smem, Plan& p) {
 }  // namespace
 
 // validation of the descriptor header, then the stages above in order
-int plan_problem(const pinn_problem_desc* d, const pinn_integral_desc* integrals, int n_integrals, int max_smem, Plan& p) {
+int plan_problem(const pinn_problem_desc* d, const pinn_integral_desc* integrals, int n_integrals,
+                 const pinn_fixed_net_desc* fixed, int n_fixed, int max_smem, Plan& p) {
   memset(&p, 0, sizeof p);
   if (!d) return fail("pinn_create: null descriptor");
+  if (n_fixed < 0 || n_fixed > PINN_MAX_FIXED_NETS)
+    return fail("pinn_create_ex2: n_fixed=%d out of range [0,%d]", n_fixed, PINN_MAX_FIXED_NETS);
+  if (n_fixed > 0 && !fixed) return fail("pinn_create_ex2: null fixed networks");
+  if (n_fixed > 0 && d->mode != PINN_MODE_FFMA)
+    return fail("pinn_create_ex2: fixed networks run on the FFMA path (mode PINN_MODE_FFMA); the tensor-core modes do not "
+                "evaluate them");
   if (n_integrals < 0 || n_integrals > PINN_MAX_INTEGRALS)
     return fail("pinn_create_ex: n_integrals=%d out of range [0,%d]", n_integrals, PINN_MAX_INTEGRALS);
   if (n_integrals > 0 && !integrals) return fail("pinn_create_ex: null integrals");
@@ -594,10 +623,10 @@ int plan_problem(const pinn_problem_desc* d, const pinn_integral_desc* integrals
                 d->n_params, (long long)d->n_theta);
   DevProblem& P = p.prob;
   P.n_nets = d->n_nets; P.n_terms = d->n_terms; P.n_params = d->n_params;
-  P.param_off = d->param_offset; P.n_theta = d->n_theta;
+  P.param_off = d->param_offset; P.n_theta = d->n_theta; P.n_fixed = n_fixed;
   int max_w8 = 8, max_c = 1;
   long long resident = 0, stash_max = 0;
-  if (plan_nets(d, P, max_w8, resident)) return 1;
+  if (plan_nets(d, fixed, n_fixed, P, max_w8, resident, p.fixed_len)) return 1;
   for (int t = 0; t < d->n_terms; ++t)
     if (plan_term(d, t, integrals, n_integrals, P, p.term[t], max_c, stash_max)) return 1;
   P.n_integrals = n_integrals;

@@ -21,6 +21,7 @@ struct Plan {
   bool bufs_smem;                  // FFMA: the two activation buffers live in shared memory (else in gbufs)
   bool wide;                       // tensor-core modes: tw_pack + the 128-wide kernel run instead of the narrow one
   bool integ;                      // FFMA: the problem has integral terms (the kernel instantiation with node tiles runs)
+  long long fixed_len[PINN_MAX_FIXED_NETS];   // scalars of each fixed network's parameter buffer
   // launch-argument templates: the planner fills the layout, pinn_create the buffers, a launch the per-call fields
   FfmaArgs ffma; TcArgs tc; TwArgs tw; TwPackArgs pack;
 };
@@ -28,7 +29,12 @@ struct Plan {
 // the q-point Gauss-Legendre rule on [-1, 1], nodes ascending
 void gauss_legendre(int q, double* x, double* w);
 
+// networks a tap may name: the trainable ones, then the fixed ones
+constexpr int kMaxAllNets = PINN_MAX_NETS + PINN_MAX_FIXED_NETS;
+
 // Pure host code (no CUDA runtime call); max_smem: the device's opt-in shared memory per block in bytes.
-// integrals[n_integrals]: integral terms (pinn_create_ex), none for pinn_create.
-int plan_problem(const pinn_problem_desc* d, const pinn_integral_desc* integrals, int n_integrals, int max_smem, Plan& p);
+// integrals[n_integrals]: integral terms (pinn_create_ex), fixed[n_fixed]: fixed networks (pinn_create_ex2); none for
+// pinn_create.
+int plan_problem(const pinn_problem_desc* d, const pinn_integral_desc* integrals, int n_integrals,
+                 const pinn_fixed_net_desc* fixed, int n_fixed, int max_smem, Plan& p);
 }  // namespace pinn

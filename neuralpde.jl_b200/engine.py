@@ -40,7 +40,7 @@ EXPORTS = [
     "pinn_term_grad_stats", "pinn_term_grad_stats_host", "pinn_set_sampler", "pinn_resample", "pinn_get_points_host",
     "pinn_comm_info", "pinn_set_sampler_ex", "pinn_qn_begin", "pinn_qn_iterate", "pinn_qn_theta",
     "pinn_hmc_begin", "pinn_hmc_iterate", "pinn_hmc_theta", "pinn_hmc_begin_ex", "pinn_create_ex",
-    "pinn_quadrature_nodes",
+    "pinn_quadrature_nodes", "pinn_create_ex2", "pinn_set_fixed_params", "pinn_set_fixed_params_host",
 ]
 
 # substitutions of infinite integration bounds (pinn_integral_desc.inf_kind) and the limits of integral terms
@@ -50,6 +50,8 @@ MAX_QUAD = 64
 # Gauss-Legendre nodes per integrating dimension the Python layer uses.  16 meet test/Forward/forward__integral.jl's
 # rtol = 1e-5 on [0, Inf) with 300x margin (12 are the fewest that do); DESIGN section 4.7.
 DEFAULT_QUAD_NODES = 16
+# fixed (non-trained) networks per problem: teachers of a neural adapter, registered network functions
+MAX_FIXED_NETS = 16
 
 # quasi-Newton optimizer / line search kinds and run states (pinn_qn_options, pinn_qn_iterate)
 QN_LBFGS, QN_BFGS = 0, 1
@@ -93,6 +95,10 @@ class _NetDesc(C.Structure):
                 ("theta_offset", C.c_int64)]
 
 
+class _FixedNetDesc(C.Structure):
+    _fields_ = [("n_layers", C.c_int32), ("dims", C.POINTER(C.c_int32)), ("acts", C.POINTER(C.c_int32))]
+
+
 class _TapDesc(C.Structure):
     _fields_ = [("net", C.c_int32), ("out", C.c_int32), ("order", C.c_int32), ("dir", C.c_int32 * 4)]
 
@@ -124,6 +130,17 @@ class NetSpec:
     dims: Sequence[int]                 # in, hidden..., out
     acts: Sequence[str]                 # one per Dense layer
     theta_offset: int = 0
+
+    @property
+    def n_params(self) -> int:
+        return sum(self.dims[i] * self.dims[i + 1] + self.dims[i + 1] for i in range(len(self.dims) - 1))
+
+
+@dataclass
+class FixedNetSpec:
+    """A network whose parameters are not trained (pinn_fixed_net_desc); taps name it as network len(nets) + j."""
+    dims: Sequence[int]
+    acts: Sequence[str]
 
     @property
     def n_params(self) -> int:
@@ -178,6 +195,7 @@ class ProblemSpec:
     mode: int = MODE_FFMA
     device: int = 0
     integrals: List[IntegralSpec] = field(default_factory=list)   # non-empty: created with pinn_create_ex
+    fixed: List[FixedNetSpec] = field(default_factory=list)       # non-empty: created with pinn_create_ex2
     _keep: list = field(default_factory=list, repr=False)
 
 
@@ -199,6 +217,13 @@ def load_library():
     lib.pinn_create.restype = C.c_int
     lib.pinn_create_ex.argtypes = [C.POINTER(_ProblemDesc), C.POINTER(_IntegralDesc), C.c_int32, C.POINTER(vp)]
     lib.pinn_create_ex.restype = C.c_int
+    lib.pinn_create_ex2.argtypes = [C.POINTER(_ProblemDesc), C.POINTER(_IntegralDesc), C.c_int32, C.POINTER(_FixedNetDesc),
+                                    C.c_int32, C.POINTER(vp)]
+    lib.pinn_create_ex2.restype = C.c_int
+    lib.pinn_set_fixed_params.argtypes = [vp, i32, vp]
+    lib.pinn_set_fixed_params.restype = C.c_int
+    lib.pinn_set_fixed_params_host.argtypes = [vp, i32, vp, vp]
+    lib.pinn_set_fixed_params_host.restype = C.c_int
     lib.pinn_quadrature_nodes.argtypes = [C.c_int32, C.POINTER(C.c_double), C.POINTER(C.c_double)]
     lib.pinn_quadrature_nodes.restype = C.c_int
     lib.pinn_destroy.argtypes = [vp]
@@ -313,8 +338,9 @@ def _marshal_body(spec: ProblemSpec, taps_l, prog_l, net_rows_l, keep):
         d = list(tp.dirs) + [0, 0, 0, 0]
         for q in range(4):
             taps[i].dir[q] = int(d[q])
-    rows = (C.c_int32 * (len(spec.nets) * MAX_IN))(*([-1] * (len(spec.nets) * MAX_IN)))
-    for k, n in enumerate(spec.nets):
+    all_nets = list(spec.nets) + list(spec.fixed)
+    rows = (C.c_int32 * (len(all_nets) * MAX_IN))(*([-1] * (len(all_nets) * MAX_IN)))
+    for k, n in enumerate(all_nets):
         r = net_rows_l[k] if net_rows_l is not None and k < len(net_rows_l) and net_rows_l[k] is not None \
             else list(range(n.dims[0]))
         for j, v in enumerate(r):
@@ -343,6 +369,18 @@ def build_integrals(spec: ProblemSpec):
     return arr
 
 
+def build_fixed(spec: ProblemSpec):
+    """Marshal spec.fixed into a pinn_fixed_net_desc array (kept alive on the spec)."""
+    arr = (_FixedNetDesc * max(1, len(spec.fixed)))()
+    for j, f in enumerate(spec.fixed):
+        dims = (C.c_int32 * len(f.dims))(*[int(v) for v in f.dims])
+        acts = (C.c_int32 * len(f.acts))(*[ACT[a] for a in f.acts])
+        arr[j].n_layers, arr[j].dims, arr[j].acts = len(f.acts), dims, acts
+        spec._keep += [dims, acts]
+    spec._keep.append(arr)
+    return arr
+
+
 def build_desc(spec: ProblemSpec) -> _ProblemDesc:
     """Marshal a ProblemSpec into the C descriptor (buffers are kept alive on the spec)."""
     keep = spec._keep
@@ -364,8 +402,9 @@ def build_desc(spec: ProblemSpec) -> _ProblemDesc:
             d = list(tp.dirs) + [0, 0, 0, 0]
             for q in range(4):
                 taps[i].dir[q] = int(d[q])
-        rows = (C.c_int32 * (len(spec.nets) * MAX_IN))(*([-1] * (len(spec.nets) * MAX_IN)))
-        for k, n in enumerate(spec.nets):
+        all_nets = list(spec.nets) + list(spec.fixed)
+        rows = (C.c_int32 * (len(all_nets) * MAX_IN))(*([-1] * (len(all_nets) * MAX_IN)))
+        for k, n in enumerate(all_nets):
             r = tm.net_rows[k] if tm.net_rows is not None and k < len(tm.net_rows) and tm.net_rows[k] is not None \
                 else list(range(n.dims[0]))
             for j, v in enumerate(r):
@@ -407,7 +446,10 @@ class Engine:
         self.n_theta = int(spec.n_theta)
         self._h = C.c_void_p(0)
         desc = build_desc(spec)
-        if spec.integrals:
+        if spec.fixed:
+            _check(self.lib.pinn_create_ex2(C.byref(desc), build_integrals(spec), len(spec.integrals), build_fixed(spec),
+                                            len(spec.fixed), C.byref(self._h)))
+        elif spec.integrals:
             _check(self.lib.pinn_create_ex(C.byref(desc), build_integrals(spec), len(spec.integrals), C.byref(self._h)))
         else:
             _check(self.lib.pinn_create(C.byref(desc), C.byref(self._h)))
@@ -423,6 +465,22 @@ class Engine:
             self.close()
         except Exception:
             pass
+
+    # -- fixed networks ---------------------------------------------------------------------------
+    def set_fixed_params(self, j: int, dev_params):
+        """Alias a device buffer (torch CUDA tensor or raw pointer) as fixed network j's parameters."""
+        self._keep_pts[("fixed", int(j))] = dev_params
+        _check(self.lib.pinn_set_fixed_params(self._h, int(j), _ptr(dev_params)))
+
+    def set_fixed_params_host(self, j: int, params: np.ndarray, stream: int = 0):
+        """Copy fixed network j's parameters (flat Lux layout) into engine memory."""
+        p = np.ascontiguousarray(params, dtype=self.np_dtype).reshape(-1)
+        if not 0 <= int(j) < len(self.spec.fixed):
+            raise ValueError("fixed network %d out of range [0, %d)" % (int(j), len(self.spec.fixed)))
+        if p.size != self.spec.fixed[int(j)].n_params:
+            raise ValueError("fixed network %d has %d parameters, got %d" % (int(j), self.spec.fixed[int(j)].n_params,
+                                                                               p.size))
+        _check(self.lib.pinn_set_fixed_params_host(self._h, int(j), _ptr(p), C.c_void_p(stream)))
 
     # -- points ---------------------------------------------------------------------------------
     def set_points(self, term: int, dev_pts, n: int, dev_weights=None):

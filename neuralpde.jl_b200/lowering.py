@@ -20,7 +20,8 @@ from sympy.core.function import AppliedUndef
 
 from .engine import (DEFAULT_QUAD_NODES, INF_BOTH, INF_LOWER, INF_NONE, INF_UPPER, IntegralSpec, TapSpec, TermSpec,
                      REDUCE_MEAN)
-from .symbolic import Equation, IntegralOp, VarInfo, eq_indvars, expand_derivatives
+from .symbolic import (Equation, FixedNet, IntegralOp, VarInfo, _depvar_apps, _eq_expr, eq_indvars, expand_derivatives,
+                       fixed_net_of)
 
 
 class LoweringError(ValueError):
@@ -65,6 +66,7 @@ class LoweredTerm:
 
 
 MAX_DIM = 8   # PINN_MAX_DIM
+MAX_FIXED_NETS = 16   # PINN_MAX_FIXED_NETS
 # the reference truncates the substituted intervals of infinite bounds by 1/20 (src/transform_inf_integral.jl)
 INF_EPS = 1.0 / 20
 
@@ -104,7 +106,8 @@ def _hoist_coordinate_terms(expr, coord_names, blocked_names, extras, base_dim):
 
 class _Emitter:
     def __init__(self, vi: VarInfo, rows: List[str], param_index: Dict[str, int], param_values: Dict[str, float],
-                 extras: Optional[List[sp.Expr]] = None, hoist: bool = False, node_vars: Optional[Dict[str, int]] = None):
+                 extras: Optional[List[sp.Expr]] = None, hoist: bool = False, node_vars: Optional[Dict[str, int]] = None,
+                 fixed: Optional[List[FixedNet]] = None, const_rows: Optional[Dict[float, int]] = None):
         self.vi = vi
         self.rows = rows
         self.param_index = param_index
@@ -117,6 +120,11 @@ class _Emitter:
         self.hoist = hoist
         self.node_vars = node_vars or {}    # integrand: quadrature variable t_k -> ("coord", -1 - k) until placed
         self.integrals: List[IntegralSpec] = []
+        # registered network functions: the problem's fixed networks (shared by its equations; tap network
+        # len(depvars) + j is fixed[j]), the point rows each one reads here, and the rows that hold constant arguments
+        self.fixed = fixed if fixed is not None else []
+        self.fixed_rows: Dict[int, List[int]] = {}
+        self.const_rows = const_rows or {}
 
     def _push(self, op, a=0, b=0, imm=0.0) -> int:
         key = (op, a, b, float(imm))
@@ -130,7 +138,43 @@ class _Emitter:
         return self._push("const", imm=float(v))
 
     def tap(self, depvar: str, dirs: Tuple[int, ...]) -> int:
-        net = self.vi.dict_depvars[depvar]
+        return self._tap_net(self.vi.dict_depvars[depvar], depvar, dirs)
+
+    def fixed_tap(self, app: AppliedUndef, dirvars: List[str]) -> int:
+        """A value or partial derivative of a registered network function at its arguments: coordinates of the
+        equation, or constants bound to the rows that hold them (``phi_bound(x_0, y)``)."""
+        name, fn = app.func.__name__, fixed_net_of(app)
+        if len(app.args) != fn.dims[0]:
+            raise LoweringError("%s called with %d arguments; its network has %d inputs" % (name, len(app.args), fn.dims[0]))
+        rows = []
+        for a in app.args:
+            if isinstance(a, sp.Symbol) and str(a) in self.rows:
+                rows.append(self.rows.index(str(a)))
+            elif a.is_number and float(a) in self.const_rows:
+                rows.append(self.const_rows[float(a)])
+            else:
+                raise LoweringError("%s(%s): arguments of a registered function are the equation's coordinates %s or "
+                                    "constants that a dependent variable of the equation takes at the same position"
+                                    % (name, ", ".join(map(str, app.args)), self.rows))
+        j = next((i for i, f in enumerate(self.fixed) if f is fn), None)
+        if j is None:
+            if len(self.fixed) >= MAX_FIXED_NETS:
+                raise LoweringError("more than %d registered network functions in one problem" % MAX_FIXED_NETS)
+            self.fixed.append(fn)
+            j = len(self.fixed) - 1
+        net = len(self.vi.depvars) + j
+        if self.fixed_rows.setdefault(net, rows) != rows:
+            raise LoweringError("%s is applied to different arguments in one equation" % name)
+        dirs = []
+        for v in dirvars:
+            pos = [i for i, a in enumerate(app.args) if isinstance(a, sp.Symbol) and str(a) == v]
+            if len(pos) != 1:
+                raise LoweringError("derivative of %s with respect to %s, which is not exactly one of its arguments %s"
+                                    % (app, v, list(app.args)))
+            dirs.append(pos[0])
+        return self._tap_net(net, name, tuple(dirs))
+
+    def _tap_net(self, net: int, depvar: str, dirs: Tuple[int, ...]) -> int:
         dirs = tuple(sorted(dirs))
         key = (net, dirs)
         if key not in self._tap_ids:
@@ -168,6 +212,8 @@ class _Emitter:
             if self.node_vars:
                 raise LoweringError("integral nested in an integrand: not supported")
             return self._push("integral", a=self.integral(e))
+        if isinstance(e, AppliedUndef) and fixed_net_of(e) is not None:
+            return self.fixed_tap(e, [])
         if isinstance(e, AppliedUndef):
             name = e.func.__name__
             if name not in self.vi.dict_depvars:
@@ -192,6 +238,8 @@ class _Emitter:
                     for v, n in inner.variable_count:
                         dvars += [str(v)] * int(n)
                     inner = inner.expr
+            if fixed_net_of(inner) is not None:
+                return self.fixed_tap(inner, dvars)
             if not (isinstance(inner, AppliedUndef) and inner.func.__name__ in self.vi.dict_depvars):
                 raise LoweringError("derivative of a non-network expression survived expand_derivatives: %s" % e)
             name = inner.func.__name__
@@ -334,17 +382,34 @@ class _Emitter:
         if not (body.has(AppliedUndef) or body.has(sp.Derivative)):
             raise LoweringError("integrand %s contains no dependent variable: nothing to train on" % integrand)
         em = _Emitter(self.vi, self.rows, self.param_index, self.param_values,
-                      node_vars={str(t): k for k, t in enumerate(tsyms)})
+                      node_vars={str(t): k for k, t in enumerate(tsyms)}, fixed=self.fixed, const_rows=self.const_rows)
         v = em.emit(body * jac if jac != 1 else body)
         if v != len(em.prog) - 1:              # the last instruction is the integrand's value
             em.prog.append(("mul", v, em.const(1.0), 0.0))
         spec.taps, spec.prog = em.taps, em.prog
-        spec.net_rows = _net_rows(self.vi, self.rows)
+        spec.net_rows = _net_rows(self.vi, self.rows) + em.fixed_net_rows()
         for i, old in enumerate(self.integrals):
             if old == spec:
                 return i
         self.integrals.append(spec)
         return len(self.integrals) - 1
+
+
+    def fixed_net_rows(self) -> List[Optional[List[int]]]:
+        """net_rows entries of the fixed networks (after the dependent variables'): None where this body taps none"""
+        n = len(self.vi.depvars)
+        return [self.fixed_rows.get(n + j) for j in range(len(self.fixed))]
+
+
+def _const_rows(eq: Equation, vi: VarInfo, rows: List[str]) -> Dict[float, int]:
+    """constant arguments of the equation's dependent variables and the point row each sits in: row i of a bc such as
+    u(x_0, y) ~ ... holds x_0 (get_argument), so a registered function applied to x_0 reads that row"""
+    out: Dict[float, int] = {}
+    for app in _depvar_apps(_eq_expr(eq), vi):
+        for a, v in zip(app.args, vi.dict_depvar_input[app.func.__name__]):
+            if a.is_number and v in rows:
+                out.setdefault(float(a), rows.index(v))
+    return out
 
 
 def _net_rows(vi: VarInfo, rows: List[str]) -> List[Optional[List[int]]]:
@@ -356,11 +421,14 @@ def _net_rows(vi: VarInfo, rows: List[str]) -> List[Optional[List[int]]]:
 
 
 def lower_equation(eq: Equation, vi: VarInfo, param_index: Optional[Dict[str, int]] = None,
-                   param_values: Optional[Dict[str, float]] = None, hoist: bool = False) -> LoweredTerm:
-    """Equation -> taps + residual program (``lhs - rhs``), and the IR of every integral it reads."""
+                   param_values: Optional[Dict[str, float]] = None, hoist: bool = False,
+                   fixed: Optional[List[FixedNet]] = None) -> LoweredTerm:
+    """Equation -> taps + residual program (``lhs - rhs``), and the IR of every integral it reads.  ``fixed``: the
+    problem's fixed networks so far (registered network functions append theirs; shared by a problem's equations)."""
     rows = eq_indvars(eq, vi)
     extras: List[sp.Expr] = []
-    em = _Emitter(vi, rows, param_index or {}, param_values or {}, extras=extras, hoist=hoist)
+    em = _Emitter(vi, rows, param_index or {}, param_values or {}, extras=extras, hoist=hoist, fixed=fixed,
+                  const_rows=_const_rows(eq, vi, rows))
     lhs = expand_derivatives(eq.lhs)
     rhs = expand_derivatives(eq.rhs)
     if hoist:
@@ -377,7 +445,7 @@ def lower_equation(eq: Equation, vi: VarInfo, param_index: Optional[Dict[str, in
     for spec in em.integrals:                # the quadrature variables follow the owner's rows (hoisted ones included)
         spec.prog = [("coord", dim - 1 - ins[1], 0, 0.0) if ins[0] == "coord" and ins[1] < 0 else ins
                      for ins in spec.prog]
-    return LoweredTerm(em.taps, em.prog, rows, _net_rows(vi, rows), extras, em.integrals)
+    return LoweredTerm(em.taps, em.prog, rows, _net_rows(vi, rows) + em.fixed_net_rows(), extras, em.integrals)
 
 
 def term_spec(lt: LoweredTerm, reduction: int = REDUCE_MEAN, scale: float = 1.0) -> TermSpec:

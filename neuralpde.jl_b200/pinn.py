@@ -14,13 +14,13 @@ from typing import Callable, Dict, List, Optional, Sequence, Union
 import numpy as np
 
 from . import engine as _eng
-from .engine import (Engine, EngineError, IntegralSpec, NetSpec, ProblemSpec, TapSpec, TermSpec, REDUCE_MEAN,
-                     REDUCE_WSUM)
+from .engine import (Engine, EngineError, FixedNetSpec, IntegralSpec, NetSpec, ProblemSpec, TapSpec, TermSpec,
+                     REDUCE_MEAN, REDUCE_WSUM)
 from .lowering import LoweredTerm, LoweringError, lower_equation, term_spec
 from .strategies import (AbstractTrainingStrategy, GridTraining, QuadratureTraining, QuasiRandomTraining,
                          StochasticTraining, _julia_range, _product_columns, gauss_legendre_box, generate_quasi_random_points,
                          generate_random_points, generate_training_sets, get_bounds, shard_range)
-from .symbolic import Equation, PDESystem, VarInfo, get_vars
+from .symbolic import Equation, FixedNet, PDESystem, VarInfo, fixed_function, get_vars
 
 _ACT_NAMES = {"identity": "identity", "tanh": "tanh", "sigmoid": "sigmoid", "σ": "sigmoid", "sin": "sin",
               "softplus": "softplus", "swish": "swish", None: "identity"}
@@ -455,6 +455,32 @@ class Phi:
         return r[0] if scalar else r.reshape(1, -1)
 
 
+def register_symbolic(phi: Phi, theta, name: str = "phi_registered"):
+    """``phi_bound(x, y) = first(phi(vcat(x, y), θ))`` followed by ``@register_symbolic phi_bound(x, y)``: a function
+    usable in equations -- applications and ``Differential``s of them -- that evaluates the trained network ``phi`` at
+    parameters ``theta`` (the full θ ``phi`` was trained with).  The network runs inside the fused kernel as a fixed
+    network: its parameters are not trained and receive no gradient."""
+    if not isinstance(phi, Phi):
+        raise TypeError("register_symbolic: expected a trained network's Phi (discretization.phi), got %r" % type(phi))
+    if phi.chain.dims[-1] != 1:
+        raise ValueError("register_symbolic: the network must have a 1-dimensional output")
+    th = np.asarray(theta, dtype=np.float64).reshape(-1)
+    if th.size < phi.theta_offset + phi.chain.n_params:
+        raise ValueError("register_symbolic: theta has %d entries, the network needs [%d, %d)"
+                         % (th.size, phi.theta_offset, phi.theta_offset + phi.chain.n_params))
+    params = th[phi.theta_offset:phi.theta_offset + phi.chain.n_params].copy()
+    return fixed_function(name, FixedNet(list(phi.chain.dims), list(phi.chain.acts), params))
+
+
+def _fixed_specs(fixed: List[FixedNet]) -> List[FixedNetSpec]:
+    return [FixedNetSpec(f.dims, f.acts) for f in fixed]
+
+
+def _upload_fixed(eng: Engine, fixed: List[FixedNet]):
+    for j, f in enumerate(fixed):
+        eng.set_fixed_params_host(j, f.params)
+
+
 # ---- discretization --------------------------------------------------------------------------------------
 def _per_term(w, n: int, what: str) -> np.ndarray:
     if np.isscalar(w):
@@ -535,8 +561,9 @@ def symbolic_discretize(pde_system: PDESystem, discretization: PhysicsInformedNN
     try:
         # points drawn on the device carry only coordinates: no host-evaluated (hoisted) rows then
         hoist = not getattr(d.strategy, "device_sampler", False)
-        pde_terms = [lower_equation(e, vi, param_index, param_values, hoist=hoist) for e in eqs]
-        bc_terms = [lower_equation(e, vi, param_index, param_values, hoist=hoist) for e in bcs]
+        fixed: List[FixedNet] = []          # registered network functions the equations apply
+        pde_terms = [lower_equation(e, vi, param_index, param_values, hoist=hoist, fixed=fixed) for e in eqs]
+        bc_terms = [lower_equation(e, vi, param_index, param_values, hoist=hoist, fixed=fixed) for e in bcs]
     except LoweringError as ex:
         raise ValueError(str(ex)) from ex
 
@@ -609,8 +636,10 @@ def symbolic_discretize(pde_system: PDESystem, discretization: PhysicsInformedNN
 
     nets = [NetSpec(c.dims, c.acts, off) for c, off in zip(chains, offs)]
     mode = {"ffma": _eng.MODE_FFMA, "tc_bf16": _eng.MODE_TC_BF16, "tc_split": _eng.MODE_TC_SPLIT}[d.mode]
+    if fixed and mode != _eng.MODE_FFMA:
+        raise ValueError("registered network functions run on the FFMA path: use mode=\"ffma\"")
     spec = ProblemSpec(nets=nets, terms=specs, n_params=n_p, param_offset=n_net, n_theta=n_net + n_p,
-                       dtype=dtype.name, mode=mode, device=d.device, integrals=integrals)
+                       dtype=dtype.name, mode=mode, device=d.device, integrals=integrals, fixed=_fixed_specs(fixed))
 
     n_pde, n_bc = len(eqs), len(bcs)
     point_sets: List[Optional[np.ndarray]] = [None] * len(specs)
@@ -647,6 +676,7 @@ def symbolic_discretize(pde_system: PDESystem, discretization: PhysicsInformedNN
         point_sets[-1] = np.concatenate([X, y], axis=0)
 
     eng = Engine(spec)
+    _upload_fixed(eng, fixed)
     n_terms = len(specs)
     sampler_rng = np.random.default_rng(getattr(strategy, "seed", 0) + 7919 * rank)
     state = {"calls": 0}

@@ -177,6 +177,25 @@ def gauss_legendre_box(bound, nodes_per_dim: int, eltype) -> Tuple[np.ndarray, n
     return pts.astype(eltype), wt.ravel(order="F").astype(eltype), float(area)
 
 
+# ---- neural adapter sets (reference src/neural_adapter.jl:1-23) --------------------------------------------------
+def adapter_training_set(domains: Sequence[VarDomain], dx, eltype) -> np.ndarray:
+    """The neural adapter's Grid set: every domain's ``infimum:dx:supremum`` span, product in domain order (first
+    variable fastest), one (d, N) matrix for the whole system (src/neural_adapter.jl:1-6)."""
+    dxs = list(dx) if isinstance(dx, (list, tuple, np.ndarray)) else [dx] * len(domains)
+    return _product_columns([_julia_range(d.domain.lo, float(h), d.domain.hi) for d, h in zip(domains, dxs)]).astype(eltype)
+
+
+def get_bounds_(domains: Sequence[VarDomain], eqs: Sequence[Equation], eltype, vi: VarInfo):
+    """``get_bounds_`` of the neural adapter (src/neural_adapter.jl:8-23): the first equation's arguments, each a
+    variable's [infimum, supremum] -- the plain domain, not shrunk as get_bounds does -- or a number's degenerate
+    interval.  Returns (args, lb, ub)."""
+    span = {str(d.variables): (d.domain.lo, d.domain.hi) for d in domains}
+    args = get_argument(list(eqs), vi)[0]
+    lb = np.array([span[a][0] if isinstance(a, str) else float(a) for a in args], dtype=eltype)
+    ub = np.array([span[a][1] if isinstance(a, str) else float(a) for a in args], dtype=eltype)
+    return args, lb, ub
+
+
 def shard_range(n: int, rank: int, world: int) -> Tuple[int, int]:
     """Contiguous shard [lo, hi) of n points for `rank` of `world` (SURVEY section 8(e))."""
     base, rem = divmod(n, world)

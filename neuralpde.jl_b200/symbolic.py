@@ -9,8 +9,9 @@ so that the parity tests read like the reference's own tests.
 """
 from __future__ import annotations
 
+import itertools
 from dataclasses import dataclass, field
-from typing import Dict, List, Sequence, Union
+from typing import Dict, List, Optional, Sequence, Union
 
 import sympy as sp
 from sympy.core.function import AppliedUndef
@@ -257,3 +258,28 @@ class Integral:
 
     def __call__(self, expr):
         return IntegralOp(sp.sympify(expr), sp.Tuple(*self.variables), sp.Tuple(*self.lbs), sp.Tuple(*self.ubs))
+
+
+# ---- registered network functions (``@register_symbolic phi_bound(x, y)``) ------------------------------------------
+@dataclass(eq=False)
+class FixedNet:
+    """A trained 1-output Dense MLP whose parameters stay fixed: dims, activations and its flat Lux parameters."""
+    dims: List[int]
+    acts: List[str]
+    params: "object"          # numpy array (float64 copy)
+
+
+_fixed_ids = itertools.count()
+
+
+def fixed_function(name: str, net: FixedNet):
+    """A sympy function whose applications (and derivatives of them) the lowering evaluates with the fixed network
+    ``net``.  Every call gives a distinct function, even under one name, so two teachers never compare equal."""
+    f = sp.Function(name, real=True, fixed_id=next(_fixed_ids))
+    f.fixed_net = net
+    return f
+
+
+def fixed_net_of(e) -> Optional[FixedNet]:
+    """The fixed network of an application of a registered function, or None."""
+    return getattr(e.func, "fixed_net", None) if isinstance(e, AppliedUndef) else None
