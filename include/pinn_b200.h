@@ -75,10 +75,14 @@ enum { PINN_F32 = 0, PINN_F64 = 1 };
 
 /* arithmetic mode of the layer contractions.
  * Shapes the tensor-core modes accept (anything else: pinn_create fails with a message, never a silent fallback):
- *   1-output networks, linear last layer, >= 2 Dense layers, PINN_F32, <= 6 taps per term, and either
- *     - every hidden width in {16, 32, 48, 64} and <= 5 propagated channels per (term, network)      [both modes], or
- *     - every hidden width in {64, 128}, at least one hidden->hidden layer; terms that need more than 4 channels
- *       are evaluated in several passes over the same weights (pure second derivatives only)   [PINN_MODE_TC_BF16]. */
+ *   1-output networks, linear last layer, >= 2 Dense layers, PINN_F32, and either
+ *     - every hidden width in {16, 32, 48, 64}, <= 6 taps per term and <= 5 propagated channels per (term, network)
+ *                                                                                                    [both modes], or
+ *     - every hidden width in {64, 128}, <= 6 taps per term, at least one hidden->hidden layer; terms that need more
+ *       than 4 channels are evaluated in several passes over the same weights (pure second derivatives only)
+ *                                                                                           [PINN_MODE_TC_BF16], or
+ *     - a hidden width of 192 or 256 and every hidden width a multiple of 64 up to 256, up to PINN_MAX_TAPS taps per
+ *       term (as far as shared memory allows), otherwise as the previous case                [PINN_MODE_TC_BF16]. */
 enum {
   PINN_MODE_FFMA = 0,      /* CUDA-core FMA in the scalar type (parity mode, fp32 / fp64)   */
   PINN_MODE_TC_BF16 = 1,   /* wgmma, bf16 operands, fp32 accumulate                          */

@@ -203,7 +203,7 @@ int pinn_create_ex2(const pinn_problem_desc* d, const pinn_integral_desc* integr
     TRY_OR_DESTROY(dev_alloc((void**)&e->tc_acc, g * (size_t)kAccCols * kAccRows * sizeof(float), e));
     if (p.wide) {
       TRY_OR_DESTROY(dev_alloc(&e->tw_zstash, g * (size_t)p.tw.zstash_per_cta * sizeof(float), e));
-      TRY_OR_DESTROY(dev_alloc(&e->tw_wpack, (size_t)std::max(p.pack.n_images, 1) * kTwImgBytes, e));
+      TRY_OR_DESTROY(dev_alloc(&e->tw_wpack, (size_t)std::max(p.pack.n_images, 1) * (p.x256 ? kTxImgBytes : kTwImgBytes), e));
       TRY_OR_DESTROY(dev_alloc((void**)&e->tw_counter, 64, e));
     }
   }
@@ -374,9 +374,9 @@ static int launch_fused(pinn_engine* e, const LaunchCall& c, int grid, cudaStrea
   if (p.wide) {
     TwPackArgs pk = p.pack;
     pk.theta = (const float*)c.theta; pk.counter_init = c.tile_begin + grid;
-    CUDA_TRY(tw_pack_launch(pk, st));
+    CUDA_TRY(p.x256 ? tx_pack_launch(pk, st) : tw_pack_launch(pk, st));
     e->launches += 1;
-    CUDA_TRY(tw_launch(with_call(p.tw, e, c), grid, p.smem, st));
+    CUDA_TRY(p.x256 ? tx_launch(with_call(p.tw, e, c), grid, p.smem, st) : tw_launch(with_call(p.tw, e, c), grid, p.smem, st));
     return 0;
   }
   CUDA_TRY(tc_launch(with_call(p.tc, e, c), grid, p.smem, st));

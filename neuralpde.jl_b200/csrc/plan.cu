@@ -398,20 +398,37 @@ int check_tc_nets(const pinn_problem_desc* d, const DevProblem& P, Plan& p, int&
         return fail("pinn_create(tc): term %d takes a third derivative; the tensor-core path propagates derivatives up to order 2 "
                     "(use PINN_MODE_FFMA)", t);
   tl_max = 0;
-  bool wide = false;
+  bool wide = false, x256 = false;
   for (int k = 0; k < d->n_nets; ++k) {
     const DevNet& n = P.nets[k];
     if (n.n_layers < 2) return fail("pinn_create(tc): net %d needs at least 2 Dense layers", k);
     if (n.dims[n.n_layers] != 1) return fail("pinn_create(tc): net %d must have a 1-dimensional output", k);
     if (n.acts[n.n_layers - 1] != PINN_ACT_IDENTITY)
       return fail("pinn_create(tc): net %d: the last layer must be linear (identity activation)", k);
-    for (int l = 1; l < n.n_layers; ++l)
+    for (int l = 1; l < n.n_layers; ++l) {
       if (n.dims[l] > 64) wide = true;
+      if (n.dims[l] == 192 || n.dims[l] == 256) x256 = true;
+    }
     if (n.n_layers - 2 > kTcMaxTL)
       return fail("pinn_create(tc): net %d has %d hidden->hidden layers (max %d)", k, n.n_layers - 2, kTcMaxTL);
     tl_max = std::max(tl_max, n.n_layers - 2);
   }
-  for (int k = 0; k < d->n_nets; ++k) {
+  if (x256) {     // the 256-wide kernel: every hidden width a multiple of 64 up to 256
+    if (d->mode != PINN_MODE_TC_BF16)
+      return fail("pinn_create(tc): PINN_MODE_TC_SPLIT supports hidden widths up to 64; 192- and 256-wide layers run in "
+                  "PINN_MODE_TC_BF16 (or PINN_MODE_FFMA for fp32 accuracy)");
+    for (int k = 0; k < d->n_nets; ++k) {
+      const DevNet& n = P.nets[k];
+      for (int l = 1; l < n.n_layers; ++l)
+        if (n.dims[l] % 64 != 0 || n.dims[l] > kTxW)
+          return fail("pinn_create(tc): net %d hidden width %d: networks with 192- or 256-wide layers need every hidden "
+                      "width to be a multiple of 64 up to %d on the tensor-core path (use PINN_MODE_FFMA for other shapes)",
+                      k, n.dims[l], kTxW);
+      if (n.n_layers < 3)
+        return fail("pinn_create(tc): net %d: the 256-wide tensor-core path needs at least one hidden->hidden layer", k);
+    }
+  }
+  for (int k = 0; !x256 && k < d->n_nets; ++k) {
     const DevNet& n = P.nets[k];
     for (int l = 1; l < n.n_layers; ++l) {
       const int w = n.dims[l];
@@ -429,6 +446,7 @@ int check_tc_nets(const pinn_problem_desc* d, const DevProblem& P, Plan& p, int&
     return fail("pinn_create(tc): PINN_MODE_TC_SPLIT supports hidden widths up to 64; 128-wide layers run in "
                 "PINN_MODE_TC_BF16 (or PINN_MODE_FFMA for fp32 accuracy)");
   p.wide = wide;
+  p.x256 = x256;
   for (int k = 0; k < PINN_MAX_NETS; ++k)    // 1: every hidden activation is tanh (fast path), 0: generic
     tc_common(p).net_ak[k] = std::all_of(P.nets[k].acts, P.nets[k].acts + std::max(P.nets[k].n_layers - 1, 0),
                                          [](int act) { return act == PINN_ACT_TANH; });
@@ -436,11 +454,12 @@ int check_tc_nets(const pinn_problem_desc* d, const DevProblem& P, Plan& p, int&
 }
 
 // channel sets and taps of every (split) term; the most slots of a term and channels of a slot
-int check_tc_terms(const DevProblem& P, bool wide, int& n_used_max, int& max_c) {
+// (max_taps: kTcMaxTaps, or kTxMaxTaps on the 256-wide kernel, whose misc region is sized for the problem's taps)
+int check_tc_terms(const DevProblem& P, bool wide, int max_taps, int& n_used_max, int& max_c) {
   n_used_max = 1; max_c = 1;
   for (int t = 0; t < P.n_terms; ++t) {
     const DevTerm& T = P.terms[t];
-    if (T.n_taps > kTcMaxTaps) return fail("pinn_create(tc): term %d has %d taps (tensor-core path: max %d)", t, T.n_taps, kTcMaxTaps);
+    if (T.n_taps > max_taps) return fail("pinn_create(tc): term %d has %d taps (tensor-core path: max %d)", t, T.n_taps, max_taps);
     n_used_max = std::max(n_used_max, T.n_used);
     for (int s = 0; s < T.n_used; ++s) {
       const DevChan& ch = T.chan[s];
@@ -543,14 +562,19 @@ int plan_tc_smem(const DevProblem& P, int max_c, int max_smem, Plan& p) {
       }
   }
   c.off_ones = take(1024);      // 1024-aligned: the regions before it are multiples of 8 KB
-  const size_t fp_bytes = ((size_t)(p.wide ? FpBlock<kTwW>::SIZE : FpBlock<kTcW>::SIZE) * 4 + 15) & ~size_t(15);
-  for (int k = 0; k < P.n_nets; ++k) (p.wide ? p.tw.off_fp[k] : p.tc.nets[k].fp) = take(fp_bytes);
+  if (p.x256) {     // one fp32 block, staged for each pass
+    p.tw.off_fp[0] = take(((size_t)FpBlock<kTxW>::SIZE * 4 + 15) & ~size_t(15));
+  } else {
+    const size_t fp_bytes = ((size_t)(p.wide ? FpBlock<kTwW>::SIZE : FpBlock<kTcW>::SIZE) * 4 + 15) & ~size_t(15);
+    for (int k = 0; k < P.n_nets; ++k) (p.wide ? p.tw.off_fp[k] : p.tc.nets[k].fp) = take(fp_bytes);
+  }
   if (p.wide) p.tw.off_nets = take(((size_t)P.n_nets * sizeof(DevNet) + 15) & ~size_t(15));
   c.off_misc = take(tc_misc_bytes(c.mx_dim, c.mx_taps));
   if (off + 1024 > (size_t)max_smem)
     return fail("pinn_create(tc): the problem needs %zu bytes of shared memory per CTA (limit %d): %s", off, max_smem,
-                p.wide ? "too many networks for the 128-wide tensor-core path"
-                       : "too many resident weight tiles / channels for the tensor-core path");
+                p.x256 ? "too many channels or taps for the 256-wide tensor-core path"
+                : p.wide ? "too many networks for the 128-wide tensor-core path"
+                         : "too many resident weight tiles / channels for the tensor-core path");
   p.smem = off;
   return 0;
 }
@@ -561,18 +585,32 @@ int plan_tc(const pinn_problem_desc* d, int max_smem, Plan& p) {
   if (check_tc_nets(d, P, p, tl_max)) return 1;
   for (int t = 0; p.wide && t < d->n_terms; ++t)
     if (split_passes(t, P.terms[t])) return 1;
-  if (check_tc_terms(P, p.wide, n_used_max, max_c)) return 1;
+  if (check_tc_terms(P, p.wide, p.x256 ? kTxMaxTaps : kTcMaxTaps, n_used_max, max_c)) return 1;
   TcCommonArgs& c = tc_common(p);
   c.tl_max = std::max(tl_max, 1);
   c.mx_dim = 1; c.mx_taps = 1;
   for (int t = 0; t < d->n_terms; ++t) { c.mx_dim = std::max(c.mx_dim, P.terms[t].dim); c.mx_taps = std::max(c.mx_taps, P.terms[t].n_taps); }
   p.tc.split = d->mode == PINN_MODE_TC_SPLIT ? 1 : 0;
   if (plan_tc_smem(P, max_c, max_smem, p)) return 1;
-  if (p.wide) {
+  if (p.x256) {
+    // per channel of a pass and half tile: inputs of the tensor layers + the last hidden activations (4 tiles each), fp32
+    // pre-activations; channels of the term with the most (sum over its passes of 2 C, tc_x256_kernel.cu tx_chan0)
+    long long nch = 1;
+    for (int t = 0; t < d->n_terms; ++t) {
+      long long n = 0;
+      for (int s = 0; s < P.terms[t].n_used; ++s) n += 2 * P.terms[t].chan[s].C;
+      nch = std::max(nch, n);
+    }
+    p.tw.hstash_per_cta = nch * (c.tl_max + 1) * 4 * kTxTileBytes;
+    p.tw.zstash_per_cta = nch * c.tl_max * kTxW * kTxPts;      // floats
+  }
+  if (p.wide && !p.x256) {
     // per pass: inputs of the tl_max tensor layers + the last hidden activations (restored for multi-pass terms)
     p.tw.hstash_per_cta = (long long)n_used_max * (tl_max + 1) * kTwMaxC * kTwNB * kTileBytes;
     p.tw.zstash_per_cta = (long long)n_used_max * tl_max * kTwMaxC * 64 * kTcPts * 2;      // floats
-    for (int k = 0; k < d->n_nets; ++k) {      // one packed weight image per tensor layer
+  }
+  if (p.wide) {      // one packed weight image per tensor layer
+    for (int k = 0; k < d->n_nets; ++k) {
       p.tw.wimg[k] = p.pack.n_images;
       for (int l = 1; l <= P.nets[k].n_layers - 2; ++l) {
         p.pack.img_net[p.pack.n_images] = (unsigned char)k;

@@ -20,6 +20,7 @@ struct Plan {
   size_t smem;                     // dynamic shared memory per CTA
   bool bufs_smem;                  // FFMA: the two activation buffers live in shared memory (else in gbufs)
   bool wide;                       // tensor-core modes: tw_pack + the 128-wide kernel run instead of the narrow one
+  bool x256;                       // (with wide) a hidden width is 192 or 256: tx_pack + the 256-wide kernel run instead
   bool integ;                      // FFMA: the problem has integral terms (the kernel instantiation with node tiles runs)
   long long fixed_len[PINN_MAX_FIXED_NETS];   // scalars of each fixed network's parameter buffer
   // launch-argument templates: the planner fills the layout, pinn_create the buffers, a launch the per-call fields

@@ -103,6 +103,17 @@ struct TwPackArgs {
 cudaError_t tw_pack_launch(const TwPackArgs& a, cudaStream_t st);
 cudaError_t tw_launch(const TwArgs& a, int grid, size_t smem, cudaStream_t st);
 
+// ---- 256-wide path (tc_x256_kernel.cu): hidden widths multiples of 64 up to 256, each 128-point tile as two 64-point
+// halves.  Launch arguments are TwArgs / TwPackArgs; off_fp[0] is the one fp32 parameter block, staged per pass.
+constexpr int kTxW = 256;              // accumulator column stride of a channel = widest supported layer
+constexpr int kTxPts = 64;             // points per half tile = rows of an operand tile
+constexpr int kTxTileBytes = kTxPts * 128;        // operand tile: 64 rows x 64 bf16
+constexpr int kTxImgBytes = 8 * kTileBytes;       // packed bf16 image of one tensor layer: [kb][128-row half of o][128 rows][64 k]
+constexpr int kTxMaxTaps = PINN_MAX_TAPS;         // the misc region is sized per problem (the other kernels keep kTcMaxTaps)
+
+cudaError_t tx_pack_launch(const TwPackArgs& a, cudaStream_t st);
+cudaError_t tx_launch(const TwArgs& a, int grid, size_t smem, cudaStream_t st);
+
 size_t tc_misc_bytes(int mx_dim, int mx_taps);
 cudaError_t tc_launch(const TcArgs& a, int grid, size_t smem, cudaStream_t st);
 

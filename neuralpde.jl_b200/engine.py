@@ -21,6 +21,8 @@ MAX_IN = 8
 MAX_TERMS = 32
 
 F32, F64 = 0, 1
+# PINN_MODE_*: FFMA (any shape, fp32 / fp64), TC_BF16 (hidden widths up to 64, 64 / 128, or multiples of 64 up to 256),
+# TC_SPLIT (hidden widths up to 64); include/pinn_b200.h lists the shapes each tensor-core mode accepts
 MODE_FFMA, MODE_TC_BF16, MODE_TC_SPLIT = 0, 1, 2
 ACT = {"identity": 0, "tanh": 1, "sigmoid": 2, "sin": 3, "softplus": 4, "swish": 5}
 OP = {

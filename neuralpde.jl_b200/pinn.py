@@ -334,7 +334,9 @@ class PhysicsInformedNN(AbstractPINN):
     additional_loss, adaptive_loss, logger, log_options, iteration)``
     (reference src/pinn_types.jl:165-211).  ``chain``: one Chain, or a list with one
     1-output Chain per dependent variable.  Engine options arrive as extra keywords:
-    ``mode`` ("ffma" | "tc_bf16" | "tc_split"), ``device``."""
+    ``mode`` ("ffma" | "tc_bf16" | "tc_split"), ``device``.  The tensor-core modes need float32 and 1-output networks
+    with a linear last layer; "tc_split" takes hidden widths 16 / 32 / 48 / 64, "tc_bf16" also 64 / 128 and any multiple
+    of 64 up to 256 (include/pinn_b200.h lists the shapes; anything else is refused with a message)."""
     chain: Union[Chain, List[Chain]]
     strategy: AbstractTrainingStrategy
     init_params: Optional[np.ndarray] = None
