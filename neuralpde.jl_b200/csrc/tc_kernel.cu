@@ -5,8 +5,10 @@
 // layers run on the tensor cores (wgmma, bf16 operands from 128B-swizzled shared-memory tiles,
 // fp32 accumulators); every derivative channel (value, d/dx_i, d2/dx_i dx_j) is its own
 // 128-row M block that shares the same weight operand.  The epilogue (bias + activation +
-// forward-mode tap chain rule, or its reverse) runs on the CUDA cores out of the accumulator
-// region and re-packs the result as the next GEMM's bf16 operand tile.
+// forward-mode tap chain rule, or its reverse) runs on the CUDA cores and re-packs the result as
+// the next GEMM's bf16 operand tile: in the forward straight from the wgmma register fragments
+// (each warpgroup owns a 64-row x 32-column block of every channel), in the reverse out of the
+// accumulator region.
 //
 //   forward, per tensor layer l :  D_c[128 x n_out] = H_c[128 x n_in] * W_l^T        (A, B K-major)
 //   backward, per tensor layer l:  Z_c   (recompute, 32-column groups)  = H_c * W_l^T
@@ -87,38 +89,100 @@ __device__ __forceinline__ void l0_fwd_loop(const LoopCtx lc, const PassInfo<N1,
   for (int c = 0; c < C; ++c) up[c] = u[c];
 }
 
-// tensor layer forward epilogue: accumulators -> bias + activation chain -> next operand tiles
-template <int N1, int N2, bool PURE, int AK>
-__device__ __forceinline__ void tl_fwd_loop(const LoopCtx lc, const Chan<N1, N2> ch, float* up) {
-  constexpr int C = 1 + N1 + N2;
-  float u[C];
+// ---- register-resident forward of a tensor layer --------------------------------------------------------------------------
+// Warpgroup wg owns the block rows [64 h, 64 h + 64) x columns [32 j, 32 j + 32) of the layer output, h = wg & 1,
+// j = wg >> 1, for every channel: d[c] holds the m64n32k16 fragment of channel c (layout: tc::wg_chain).
+// All four warpgroups issue the same instruction sequence, so the MMAs of a layer are spread evenly and stay in registers
+// until the epilogue has consumed them.
+// The block is 32 columns wide whatever the layer width: the weight tiles are zero beyond n_out, so a narrower layer
+// gets zero pre-activations in the columns it does not have, and nothing reads them.  NK = n_in / 16 k-steps and the
+// product count are compile-time, so the MMAs of the layer are one straight-line sequence (ptxas serializes wgmmas
+// whose accumulators are carried around a loop).
+template <int C, int NK, bool SPLIT>
+__device__ __forceinline__ void fwd_mma(float (&d)[C][16], uint32_t sP, uint32_t sQ, uint32_t whi, uint32_t wlo) {
+  const int wg = threadIdx.x >> 7;
+  const uint32_t aoff = (wg & 1) * 8192u, boff = (wg >> 1) * 32u * 128u;
+  const uint64_t dwhi = tc::make_desc(whi + boff, 0, 1024), dwlo = tc::make_desc(wlo + boff, 0, 1024);
+  tc::wgmma_fence();
 #pragma unroll
-  for (int c = 0; c < C; ++c) u[c] = up[c];
-#pragma unroll 1
-  for (int g = lc.g0; g < lc.g1; ++g) {
-    float z[C][GW];
+  for (int c = 0; c < C; ++c) {
+    const uint64_t dahi = tc::make_desc(sP + c * kTileBytes + aoff, 0, 1024);
+    const uint64_t dalo = tc::make_desc(sQ + c * kTileBytes + aoff, 0, 1024);
+    // the split products hi*hi, hi*lo, lo*hi accumulate into the same registers, in this order
 #pragma unroll
-    for (int c = 0; c < C; ++c) acc_ldg(lc.taddr + TM_X + c * 64 + g * GW, z[c]);
+    for (int pr = 0; pr < (SPLIT ? 3 : 1); ++pr) {
+      const uint64_t a = (pr == 2) ? dalo : dahi, b = (pr == 1) ? dwlo : dwhi;
 #pragma unroll
-    for (int i = 0; i < GW; i += 2) {
-      P2 zz[C], hv[C];
-      zz[0] = mk2(z[0][i] + lds_f32(lc.bt + (g * GW + i) * 4), z[0][i + 1] + lds_f32(lc.bt + (g * GW + i + 1) * 4));
-#pragma unroll
-      for (int c = 1; c < C; ++c) zz[c] = mk2(z[c][i], z[c][i + 1]);
-      chain_fwd<N1, N2, PURE, AK, P2>(lc.act, ch, zz, hv);
-#pragma unroll
-      for (int c = 0; c < C; ++c) { z[c][i] = hv[c].v.x; z[c][i + 1] = hv[c].v.y; }
-      if (lc.flag) {
-        const float w0 = lds_f32(lc.fp + (Fp::WL + g * GW + i) * 4), w1 = lds_f32(lc.fp + (Fp::WL + g * GW + i + 1) * 4);
-#pragma unroll
-        for (int c = 0; c < C; ++c) u[c] = fmaf(w1, hv[c].v.y, fmaf(w0, hv[c].v.x, u[c]));
-      }
+      for (int k = 0; k < NK; ++k)   // k-steps of 16 columns = 32 bytes = 2 descriptor units in both K-major operands
+        tc::wgmma_n32<0, 0>(d[c], a + 2 * k, b + 2 * k, (pr | k) ? 1u : 0u);
     }
-#pragma unroll
-    for (int c = 0; c < C; ++c) store_half(lc.tP + c * kTileBytes, lc.tQ + c * kTileBytes, lc.p, g * GW, z[c], lc.split != 0);
   }
+  tc::wgmma_commit();
+  tc::wgmma_wait0();
+}
+template <int C>
+__device__ __forceinline__ void fwd_mma_any(float (&d)[C][16], uint32_t sP, uint32_t sQ, uint32_t whi, uint32_t wlo, int nk,
+                                            bool split) {
+  switch (nk * 2 + (split ? 1 : 0)) {   // pinn_create admits widths 16, 32, 48, 64 for this kernel
+    case 2: fwd_mma<C, 1, false>(d, sP, sQ, whi, wlo); break;
+    case 3: fwd_mma<C, 1, true>(d, sP, sQ, whi, wlo); break;
+    case 4: fwd_mma<C, 2, false>(d, sP, sQ, whi, wlo); break;
+    case 5: fwd_mma<C, 2, true>(d, sP, sQ, whi, wlo); break;
+    case 6: fwd_mma<C, 3, false>(d, sP, sQ, whi, wlo); break;
+    case 7: fwd_mma<C, 3, true>(d, sP, sQ, whi, wlo); break;
+    case 8: fwd_mma<C, 4, false>(d, sP, sQ, whi, wlo); break;
+    default: fwd_mma<C, 4, true>(d, sP, sQ, whi, wlo); break;
+  }
+}
+
+// tensor layer forward epilogue on the fragments of fwd_mma: bias + activation chain -> next operand tiles (hi in P,
+// lo in Q); for the last hidden layer (flag) the last-layer dot products of the block's rows are summed over the quad
+// of lanes that share a row and added to ms.scratch (two column warpgroups per row)
+template <int N1, int N2, bool PURE, int AK, int C>
+__device__ __forceinline__ void tl_fwd_frag(const float (&d)[C][16], const LoopCtx lc, const Chan<N1, N2> ch, float* scratch) {
+  const int wg = threadIdx.x >> 7, w = (threadIdx.x >> 5) & 3;
+  const int row0 = 64 * (wg & 1) + 16 * w + (lc.lane >> 2);
+  const int col0 = 32 * (wg >> 1) + 2 * (lc.lane & 3);
+  float u[2][C];
 #pragma unroll
-  for (int c = 0; c < C; ++c) up[c] = u[c];
+  for (int r = 0; r < 2; ++r)
+#pragma unroll
+    for (int c = 0; c < C; ++c) u[r][c] = 0.f;
+#pragma unroll
+  for (int i = 0; i < 16; i += 2) {
+    const int rh = (i >> 1) & 1;
+    const int row = row0 + 8 * rh, col = col0 + 8 * (i >> 2);
+    P2 zz[C], hv[C];
+    zz[0] = mk2(d[0][i] + lds_f32(lc.bt + col * 4), d[0][i + 1] + lds_f32(lc.bt + (col + 1) * 4));
+#pragma unroll
+    for (int c = 1; c < C; ++c) zz[c] = mk2(d[c][i], d[c][i + 1]);
+    chain_fwd<N1, N2, PURE, AK, P2>(lc.act, ch, zz, hv);
+    const uint32_t off = tc::swz_off(row, col);
+#pragma unroll
+    for (int c = 0; c < C; ++c) {
+      const uint32_t hx = tc::pack_bf16(hv[c].v.x, hv[c].v.y);
+      asm volatile("st.shared.b32 [%0], %1;" ::"r"(lc.tP + c * kTileBytes + off), "r"(hx) : "memory");
+      if (lc.split)
+        asm volatile("st.shared.b32 [%0], %1;" ::"r"(lc.tQ + c * kTileBytes + off), "r"(bf16x2_lo(hv[c].v.x, hv[c].v.y, hx))
+                     : "memory");
+    }
+    if (lc.flag) {
+      const float w0 = lds_f32(lc.fp + (Fp::WL + col) * 4), w1 = lds_f32(lc.fp + (Fp::WL + col + 1) * 4);
+#pragma unroll
+      for (int c = 0; c < C; ++c) u[rh][c] = fmaf(w1, hv[c].v.y, fmaf(w0, hv[c].v.x, u[rh][c]));
+    }
+  }
+  if (lc.flag) {
+#pragma unroll
+    for (int r = 0; r < 2; ++r)
+#pragma unroll
+      for (int c = 0; c < C; ++c) {
+        float s = u[r][c];
+        s += __shfl_xor_sync(0xffffffffu, s, 1);
+        s += __shfl_xor_sync(0xffffffffu, s, 2);
+        if ((lc.lane & 3) == 0) atomicAdd(&scratch[c * kTcPts + row0 + 8 * r], s);
+      }
+  }
 }
 
 // tensor layer backward epilogue for the column group starting at c0: recomputed Z (columns Y) and output
@@ -309,32 +373,20 @@ __device__ __noinline__ uint32_t net_forward(CtaShared* cs, const DevProblem* Pp
         tc::bulk_store(stash_slot + (size_t)(l - 1) * kTcMaxC * kTileBytes + (size_t)c * kTileBytes, tP + c * kTileBytes, kTileBytes);
       tc::bulk_commit();
     }
+    float d[C][16];
     {
       const uint32_t sP = tc::smem_u32(tP), sQ = tc::smem_u32(tQ);
+      const uint32_t whi = tc::smem_u32(smem + ns.w_hi[l - 1]), wlo = tc::smem_u32(smem + ns.w_lo[l - 1]);
       const int nk = n_in / 16;
-      const uint32_t idesc = tc::make_idesc(n_out, 0, 0);
-      const uint64_t dwhi = tc::make_desc(tc::smem_u32(smem + ns.w_hi[l - 1]), 0, 1024);
-      const uint64_t dwlo = tc::make_desc(tc::smem_u32(smem + ns.w_lo[l - 1]), 0, 1024);
-#pragma unroll 1
-      for (int c = 0; c < C; ++c) {
-        const uint64_t dahi = tc::make_desc(sP + c * kTileBytes, 0, 1024);
-        const uint32_t d = accm + TM_X + c * 64;
-        mma_chain(d, dahi, dwhi, 32, 32, nk, idesc, 0);
-        if (split) {
-          const uint64_t dalo = tc::make_desc(sQ + c * kTileBytes, 0, 1024);
-          mma_chain(d, dahi, dwlo, 32, 32, nk, idesc, 1);
-          mma_chain(d, dalo, dwhi, 32, 32, nk, idesc, 1);
-        }
-      }
+      fwd_mma_any<C>(d, sP, sQ, whi, wlo, nk, split);
     }
-    dbg_mark(cs, 12);
-    __syncthreads();
     dbg_mark(cs, 13);
+    // the epilogue overwrites rows of P / Q that the other warpgroup of the row half, and the stash copies, may still read
     if (want_grad && tid == 0) tc::bulk_wait_read0();   // stash copies have finished reading P (same thread issued them)
     __syncthreads();
     dbg_mark(cs, 14);
-    const LoopCtx lc(tc::smem_u32(fp), tc::smem_u32(fp) + (Fp::BT + (l - 1) * 64) * 4, tc::smem_u32(tP), tc::smem_u32(tQ), t, act, n_out / GW, l == TL, split);
-    tl_fwd_loop<N1, N2, PURE, AK>(lc, pi.ch, u);
+    const LoopCtx lc(tc::smem_u32(fp), tc::smem_u32(fp) + (Fp::BT + (l - 1) * 64) * 4, tc::smem_u32(tP), tc::smem_u32(tQ), t, act, 0, l == TL, split);
+    tl_fwd_frag<N1, N2, PURE, AK, C>(d, lc, pi.ch, ms.scratch);
   }
   // ---- last layer (n -> 1, identity): combine the column parts of every point ---------------------------------
   finish_forward<C>(cs, tm, slot, ms, fp + Fp::BL, t, u);
