@@ -151,8 +151,18 @@ typedef struct {
   int32_t dir[4];  /* derivative directions, `order` entries used            */
 } pinn_tap_desc;
 
-enum { PINN_REDUCE_MEAN = 0, /* mean(abs2, r)            training_strategies.jl:220 */
-       PINN_REDUCE_WSUM = 1  /* scale * sum(w .* abs2(r)) fixed-node quadrature      */ };
+/* The two *_OF_SUM reductions make a FUNCTIONAL term: its program yields a value v_p per point (not a residual to
+ * square) and its loss is g(scale * sum_p w_p v_p), g = |.| or (.)^2, w_p the nullable weights of pinn_set_points (1
+ * when none are given).  It is an integral constraint such as normalisation or a zero mean (reference
+ * docs/src/tutorials/constraints.md, test/NNPDE2/additional_loss__fokker_planck.jl); for |.| the gradient uses
+ * g'(0) = 0.  At most one functional term per problem, PINN_MODE_FFMA only, no PINN_OP_INTEGRAL in its program.  Its
+ * nodes are fixed: pinn_set_sampler*, pinn_term_grad_stats and the HMC entry points refuse it, and with several ranks
+ * the whole node set goes to one rank (0 points elsewhere; pinn_set_global_count only accepts the local count),
+ * because g(sum_r S_r) != sum_r g(S_r).  pinn_term_residual returns v_p. */
+enum { PINN_REDUCE_MEAN = 0,          /* mean(abs2, r)            training_strategies.jl:220 */
+       PINN_REDUCE_WSUM = 1,          /* scale * sum(w .* abs2(r)) fixed-node quadrature      */
+       PINN_REDUCE_ABS_OF_SUM = 2,    /* abs(scale * sum(w .* v))  functional term            */
+       PINN_REDUCE_SQUARE_OF_SUM = 3  /* abs2(scale * sum(w .* v)) functional term            */ };
 
 typedef struct {
   int32_t dim;                 /* rows of the point matrix                              */
@@ -164,7 +174,7 @@ typedef struct {
   int32_t n_instr;
   const pinn_instr* prog;
   int32_t reduction;           /* PINN_REDUCE_*                                         */
-  double scale;                /* PINN_REDUCE_WSUM: multiplies the weighted sum (1/area) */
+  double scale;                /* PINN_REDUCE_WSUM / *_OF_SUM: multiplies the weighted sum */
 } pinn_term_desc;
 
 typedef struct {

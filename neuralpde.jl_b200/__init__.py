@@ -5,7 +5,8 @@ The directory name contains a dot, so import it through the root-level alias mod
 ``import neuralpde_jl_b200 as npde``.
 """
 from .engine import (Engine, EngineError, FixedNetSpec, IntegralSpec, NetSpec, ProblemSpec, TapSpec, TermSpec, EXPORTS, LIB_PATH,
-                     MODE_FFMA, MODE_TC_BF16, MODE_TC_SPLIT, REDUCE_MEAN, REDUCE_WSUM, load_library)
+                     MODE_FFMA, MODE_TC_BF16, MODE_TC_SPLIT, REDUCE_ABS_OF_SUM, REDUCE_MEAN, REDUCE_SQUARE_OF_SUM,
+                     REDUCE_WSUM, load_library)
 from .symbolic import (ClosedInterval, Differential, Eq, Equation, In, Inf, Integral, Interval, PDESystem,
                        ProductDomain, UnitInterval, UnitSquare, VarDomain, get_argument, get_variables, get_vars,
                        parameters, variables)
@@ -14,7 +15,7 @@ from .strategies import (AbstractTrainingStrategy, GridTraining, QuadratureTrain
                          StochasticTraining, generate_training_sets, get_bounds, shard_range)
 from .pinn import (AbstractPINN, Adam, BPINNsolution, BPINNstats, DiagEuclideanMetric, HMC, Leapfrog, LogNormal,
                    NoAdaptation, Normal, Uniform,
-                   StanHMCAdaptor, UnitEuclideanMetric, ahmc_bayesian_pinn_pde, pmean, BFGS, BackTracking, BayesianPINN, Chain, DataLoss, Dense, Descent, GradientScaleAdaptiveLoss, HagerZhang, LBFGS, LogOptions, MiniMaxAdaptiveLoss,
+                   StanHMCAdaptor, UnitEuclideanMetric, ahmc_bayesian_pinn_pde, pmean, BFGS, BackTracking, BayesianPINN, Chain, DataLoss, Dense, IntegralLoss, Descent, GradientScaleAdaptiveLoss, HagerZhang, LBFGS, LogOptions, MiniMaxAdaptiveLoss,
                    NonAdaptiveLoss, ReLoBRaLoAdaptiveLoss, SoftAdaptAdaptiveLoss,
                    OptimizationFunction, OptimizationProblem, Phi, PhysicsInformedNN, PINNRepresentation, Solution,
                    discretize, initialparameters, logscalar, logvector, register_symbolic, solve, symbolic_discretize)

@@ -50,6 +50,15 @@ UNITS = [
                                               "-DPINN_INST_FIXED=1"]),
     ("ffma_f64_gmem_fixed.o", "ffma_inst.cu", ["-DPINN_INST_REAL=double", "-DPINN_INST_BUFS=0", "-DPINN_INST_INTEG=1",
                                               "-DPINN_INST_FIXED=1"]),
+    # and with a functional term (integral constraints), with integral terms and fixed networks
+    ("ffma_f32_smem_func.o", "ffma_inst.cu", ["-DPINN_INST_REAL=float", "-DPINN_INST_BUFS=1", "-DPINN_INST_INTEG=1",
+                                             "-DPINN_INST_FIXED=1", "-DPINN_INST_FUNC=1"]),
+    ("ffma_f32_gmem_func.o", "ffma_inst.cu", ["-DPINN_INST_REAL=float", "-DPINN_INST_BUFS=0", "-DPINN_INST_INTEG=1",
+                                             "-DPINN_INST_FIXED=1", "-DPINN_INST_FUNC=1"]),
+    ("ffma_f64_smem_func.o", "ffma_inst.cu", ["-DPINN_INST_REAL=double", "-DPINN_INST_BUFS=1", "-DPINN_INST_INTEG=1",
+                                             "-DPINN_INST_FIXED=1", "-DPINN_INST_FUNC=1"]),
+    ("ffma_f64_gmem_func.o", "ffma_inst.cu", ["-DPINN_INST_REAL=double", "-DPINN_INST_BUFS=0", "-DPINN_INST_INTEG=1",
+                                             "-DPINN_INST_FIXED=1", "-DPINN_INST_FUNC=1"]),
 ]
 
 

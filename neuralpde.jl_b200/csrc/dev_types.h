@@ -91,6 +91,8 @@ struct DevProblem {
   int n_fixed;
   DevNet fixed[PINN_MAX_FIXED_NETS];
   const void* fixed_params[PINN_MAX_FIXED_NETS];
+  // functional term (PINN_REDUCE_*_OF_SUM): its index (-1: none) and 1 for g = (.)^2, 0 for g = |.|
+  int func_term, func_square;
 };
 
 // per term scale (L_k = scale_k * sum_p qw_p r_p^2) and loss weight, passed by value
@@ -106,7 +108,7 @@ constexpr int kTailSlots = 256;    // per-slice flags per peer (>= CTAs per laun
 struct TailState {                 // device-resident, owned by the handle (zero-initialised)
   unsigned int count, gen;         // self-resetting generation barrier over the CTAs of one launch
   unsigned int step;               // launches with a tail so far (flag value / buffer parity of the peer allreduce)
-  unsigned int pad;
+  short func_term, func_square;    // DevProblem's functional term, for the tail of its kernel (written by pinn_create)
   unsigned long long adam_t;       // optimizer steps taken (bias correction)
   unsigned long long draw;         // sampler draw counter (advanced by the tail so captured graphs resample)
 };
@@ -133,7 +135,8 @@ struct TailArgs {
 struct FfmaArgs {
   const DevProblem* prob;
   const void* theta;
-  void* partial;          // [grid][partial_stride] per-CTA gradient partials (scalar type)
+  void* partial;          // [grid][partial_stride] per-CTA gradient partials (scalar type); with a functional term the
+                          // functional's own partials G [grid][partial_stride] follow them
   long long partial_stride;   // n_theta rounded up to 4 scalars (16-byte aligned rows for the vector loads of the tail)
   double* term_sums;      // [grid][PINN_MAX_TERMS] per-CTA sum_p qw_p r_p^2
   void* stash;            // [grid][stash_per_cta]

@@ -1,7 +1,7 @@
 // ffma_inst.cu -- one explicit instantiation of the fused kernel per translation unit
-// (compiled twelve times: {float,double} x {activation buffers in smem, in global} x {plain, with integral terms, with
-// fixed networks (and integral terms)}) so the build parallelises.
-// -DPINN_INST_REAL=float|double -DPINN_INST_BUFS=0|1 [-DPINN_INST_INTEG=1 [-DPINN_INST_FIXED=1]]
+// (compiled sixteen times: {float,double} x {activation buffers in smem, in global} x {plain, with integral terms, with
+// fixed networks (and integral terms), with a functional term (and both)}) so the build parallelises.
+// -DPINN_INST_REAL=float|double -DPINN_INST_BUFS=0|1 [-DPINN_INST_INTEG=1 [-DPINN_INST_FIXED=1 [-DPINN_INST_FUNC=1]]]
 #include "ffma_kernel.cuh"
 
 namespace pinn {
@@ -19,7 +19,12 @@ namespace pinn {
 #ifndef PINN_INST_FIXED
 #define PINN_INST_FIXED 0
 #endif
-#if PINN_INST_FIXED
+#ifndef PINN_INST_FUNC
+#define PINN_INST_FUNC 0
+#endif
+#if PINN_INST_FUNC
+#define PINN_BUFS_NAME_X PINN_CAT(PINN_BUFS_NAME, _func)
+#elif PINN_INST_FIXED
 #define PINN_BUFS_NAME_X PINN_CAT(PINN_BUFS_NAME, _fixed)
 #elif PINN_INST_INTEG
 #define PINN_BUFS_NAME_X PINN_CAT(PINN_BUFS_NAME, _integ)
@@ -30,7 +35,8 @@ namespace pinn {
 
 cudaError_t PINN_LAUNCH_NAME(const FfmaArgs& a, int grid, size_t smem, cudaStream_t st) {
   return launch_fused_kernel<ffma_loss_grad_kernel<PINN_INST_REAL, (PINN_INST_BUFS != 0), (PINN_INST_INTEG != 0),
-                                                   (PINN_INST_FIXED != 0)>>(a, grid, kThreads, smem, st);
+                                                   (PINN_INST_FIXED != 0), (PINN_INST_FUNC != 0)>>(a, grid, kThreads,
+                                                                                                     smem, st);
 }
 
 }  // namespace pinn

@@ -760,7 +760,10 @@ __device__ __forceinline__ void integrals_reverse(const FfmaArgs& args, const De
 // ------------------------------------------------------------------------------------------
 // INTEG: the problem has integral terms (pinn_create_ex); FIXED: it has fixed networks (pinn_create_ex2), instantiated
 // with INTEG = true only.  <false, false> is the kernel without either, <true, false> the integral kernel as it was.
-template <typename real, bool BUFS_SMEM, bool INTEG, bool FIXED>
+// FUNC: the problem has a functional term (PINN_REDUCE_*_OF_SUM), instantiated with INTEG = FIXED = true only.  Its
+// tiles add sum_p w_p v_p to the term sum and sweep back the seed w_p into this CTA's row of the second partial G (after
+// the ordinary partials of the launch); the tail scales G by g'(S) once S is known.
+template <typename real, bool BUFS_SMEM, bool INTEG, bool FIXED, bool FUNC>
 __global__ void __launch_bounds__(kThreads, 1) ffma_loss_grad_kernel(const FfmaArgs args) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -791,6 +794,9 @@ __global__ void __launch_bounds__(kThreads, 1) ffma_loss_grad_kernel(const FfmaA
   real* partial = reinterpret_cast<real*>(args.partial) + (long long)blockIdx.x * args.partial_stride;
   real* stash = reinterpret_cast<real*>(args.stash) + (long long)blockIdx.x * args.stash_per_cta;
   const bool want_grad = (args.mode == 0);
+  real* gpart = partial;   // FUNC: this CTA's row of G
+  if constexpr (FUNC)
+    gpart = reinterpret_cast<real*>(args.partial) + ((long long)gridDim.x + blockIdx.x) * args.partial_stride;
 
   // ---- per-CTA init ------------------------------------------------------------------------
   for (long long i = tid; i < 2 * args.buf_elems; i += kThreads) {
@@ -798,6 +804,9 @@ __global__ void __launch_bounds__(kThreads, 1) ffma_loss_grad_kernel(const FfmaA
   }
   if (want_grad)
     for (long long i = tid; i < P.n_theta; i += kThreads) partial[i] = real(0);
+  if constexpr (FUNC)
+    if (want_grad)
+      for (long long i = tid; i < P.n_theta; i += kThreads) gpart[i] = real(0);
   if (tid < PINN_MAX_TERMS) tsum[tid] = 0.0;
   if (args.weights_resident) {
     for (int k = 0; k < P.n_nets; ++k)
@@ -823,6 +832,8 @@ __global__ void __launch_bounds__(kThreads, 1) ffma_loss_grad_kernel(const FfmaA
     const long long n_pts = args.dyn[ti].n;
     const real* pts = reinterpret_cast<const real*>(args.dyn[ti].pts);
     const real* qw = reinterpret_cast<const real*>(args.dyn[ti].qw);
+    bool func = false;                 // the functional term (uniform)
+    if constexpr (FUNC) func = ti == P.func_term;
 
     // ---- load the point tile ---------------------------------------------------------------
     for (int i = tid; i < tm.dim * kTilePts; i += kThreads) {
@@ -835,6 +846,8 @@ __global__ void __launch_bounds__(kThreads, 1) ffma_loss_grad_kernel(const FfmaA
       long long gp = p0 + tid;
       real w = real(0);
       if (gp < n_pts) w = tm.weighted ? qw[gp] : real(1);
+      if constexpr (FUNC)
+        if (func && gp < n_pts && qw) w = qw[gp];   // nullable weights: 1 when none are given
       qws[tid] = w;
     }
     for (int i = tid; i < tm.n_taps * kTilePts; i += kThreads) tapbar[i] = real(0);
@@ -863,6 +876,8 @@ __global__ void __launch_bounds__(kThreads, 1) ffma_loss_grad_kernel(const FfmaA
       const real w = qws[lane];
       rres[lane] = r;
       double s = (double)w * (double)r * (double)r;
+      if constexpr (FUNC)
+        if (func) s = (double)w * (double)r;     // sum_p w_p v_p
 #pragma unroll
       for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
       if (lane == 0) tsum[ti] += s;
@@ -871,20 +886,25 @@ __global__ void __launch_bounds__(kThreads, 1) ffma_loss_grad_kernel(const FfmaA
         if (gp < n_pts) reinterpret_cast<real*>(args.resid_out)[gp] = r;
       }
       if (want_grad) {
-        const real g = real(args.seed[ti]) * w * real(2) * r;   // d total / d r_p
+        real g = real(args.seed[ti]) * w * real(2) * r;   // d total / d r_p
+        real* dst = partial;
+        if constexpr (FUNC)
+          if (func) { g = w; dst = gpart; }           // d S / d v_p, into G
         for (int t = 0; t < tm.n_taps; ++t) tapbar[t * kTilePts + lane] *= g;
         if constexpr (INTEG)
           for (int k = 0; k < n_int; ++k) ival[k * kTilePts + lane] = tapbar[(tm.n_taps + k) * kTilePts + lane] * g;
         for (int j = 0; j < P.n_params; ++j) {
           real v = warp_sum<real>(pbar[j] * g);
-          if (lane == 0) partial[P.param_off + j] += v;
+          if (lane == 0) dst[P.param_off + j] += v;
         }
       }
     }
     __syncthreads();
 
     // ---- reverse sweep through every tapped network -----------------------------------------------
-    if (want_grad) reverse_nets<real, FIXED>(args, P, tm, theta, Xs, bufA, bufB, wsm, stash, tapbar, partial, ldc, tid, warp, lane);
+    if (want_grad)
+      reverse_nets<real, FIXED>(args, P, tm, theta, Xs, bufA, bufB, wsm, stash, tapbar, func ? gpart : partial, ldc, tid,
+                                warp, lane);
     if constexpr (INTEG)
       if (want_grad && n_int)
         integrals_reverse<real, FIXED>(args, P, ti, theta, Xs, Xn, ival, bufA, bufB, wsm, stash, taps, tapbar, partial, tid, warp,
@@ -895,7 +915,7 @@ __global__ void __launch_bounds__(kThreads, 1) ffma_loss_grad_kernel(const FfmaA
   if (tid < PINN_MAX_TERMS) args.term_sums[(long long)blockIdx.x * PINN_MAX_TERMS + tid] = tsum[tid];
   // gradient reduction, optimizer step and the multi-GPU sum in the kernel tail (tail.cuh)
   if (args.tail.state)
-    fused_tail<real, kThreads>(args.tail, reinterpret_cast<const real*>(args.partial), args.partial_stride, args.term_sums,
+    fused_tail<real, kThreads, FUNC>(args.tail, reinterpret_cast<const real*>(args.partial), args.partial_stride, args.term_sums,
                                P.n_theta, P.n_terms, want_grad ? 1 : 0, taps);
 }
 

@@ -49,11 +49,20 @@ cudaError_t ffma_launch_float_smem_fixed(const FfmaArgs& a, int grid, size_t sme
 cudaError_t ffma_launch_float_gmem_fixed(const FfmaArgs& a, int grid, size_t smem, cudaStream_t st);
 cudaError_t ffma_launch_double_smem_fixed(const FfmaArgs& a, int grid, size_t smem, cudaStream_t st);
 cudaError_t ffma_launch_double_gmem_fixed(const FfmaArgs& a, int grid, size_t smem, cudaStream_t st);
+cudaError_t ffma_launch_float_smem_func(const FfmaArgs& a, int grid, size_t smem, cudaStream_t st);
+cudaError_t ffma_launch_float_gmem_func(const FfmaArgs& a, int grid, size_t smem, cudaStream_t st);
+cudaError_t ffma_launch_double_smem_func(const FfmaArgs& a, int grid, size_t smem, cudaStream_t st);
+cudaError_t ffma_launch_double_gmem_func(const FfmaArgs& a, int grid, size_t smem, cudaStream_t st);
 
-// integ: the instantiation that evaluates integral terms on node tiles; fixed: the one that also evaluates fixed networks
-cudaError_t ffma_launch(int dtype, bool bufs_smem, bool integ, bool fixed, const FfmaArgs& a, int grid, size_t smem,
-                        cudaStream_t st) {
+// integ: the instantiation that evaluates integral terms on node tiles; fixed: the one that also evaluates fixed networks;
+// func: the one that also evaluates a functional term
+cudaError_t ffma_launch(int dtype, bool bufs_smem, bool integ, bool fixed, bool func, const FfmaArgs& a, int grid,
+                        size_t smem, cudaStream_t st) {
   const bool f64 = dtype == PINN_F64;
+  if (func) {
+    if (f64) return bufs_smem ? ffma_launch_double_smem_func(a, grid, smem, st) : ffma_launch_double_gmem_func(a, grid, smem, st);
+    return bufs_smem ? ffma_launch_float_smem_func(a, grid, smem, st) : ffma_launch_float_gmem_func(a, grid, smem, st);
+  }
   if (fixed) {
     if (f64) return bufs_smem ? ffma_launch_double_smem_fixed(a, grid, smem, st) : ffma_launch_double_gmem_fixed(a, grid, smem, st);
     return bufs_smem ? ffma_launch_float_smem_fixed(a, grid, smem, st) : ffma_launch_float_gmem_fixed(a, grid, smem, st);

@@ -587,6 +587,9 @@ extern "C" {
 int pinn_hmc_begin_ex(pinn_handle e, const double* host_theta0, const pinn_hmc_options* opts, const double* host_weights,
                       double ll_const, const pinn_hmc_prior* tail, int32_t n_tail, double* step_size_out) {
   if (!e) return fail("pinn_hmc_begin: null handle");
+  if (e->plan.prob.func_term >= 0)
+    return fail("pinn_hmc_begin: term %d is a functional term (an integral constraint); the log density of the sampler is "
+                "built from mean-square terms only", e->plan.prob.func_term);
   if (hmc_start(e, host_theta0, opts, host_weights, ll_const, tail, n_tail, step_size_out)) {
     hmc_release(e);              // a failed start leaves no chain: pinn_hmc_iterate refuses until the next begin
     return 1;
@@ -601,6 +604,7 @@ int pinn_hmc_begin(pinn_handle e, const double* host_theta0, const pinn_hmc_opti
 
 int pinn_hmc_iterate(pinn_handle e, int32_t n, double* host_samples, double* host_stats) {
   if (!e) return fail("pinn_hmc_iterate: null handle");
+  if (e->plan.prob.func_term >= 0) return fail("pinn_hmc_iterate: the handle has a functional term");
   if (!e->hmc) return fail("pinn_hmc_iterate: call pinn_hmc_begin first");
   if (n < 0) return fail("pinn_hmc_iterate: n = %d must be >= 0", n);
   CUDA_TRY(cudaSetDevice(e->device));

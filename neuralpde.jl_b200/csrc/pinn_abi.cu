@@ -15,8 +15,8 @@
 #include "engine.h"
 
 namespace pinn {
-cudaError_t ffma_launch(int dtype, bool bufs_smem, bool integ, bool fixed, const FfmaArgs& a, int grid, size_t smem,
-                        cudaStream_t st);
+cudaError_t ffma_launch(int dtype, bool bufs_smem, bool integ, bool fixed, bool func, const FfmaArgs& a, int grid,
+                        size_t smem, cudaStream_t st);
 cudaError_t grad_stats_launch(int dtype, const void* grad, long long n, double* out2, cudaStream_t st);
 cudaError_t sample_uniform_launch(int dtype, void* pts, long long n, int dim, const double* lb, const double* ub,
                                   unsigned long long seed, unsigned long long draw, const unsigned long long* draw_dev,
@@ -193,7 +193,9 @@ int pinn_create_ex2(const pinn_problem_desc* d, const pinn_integral_desc* integr
   if (err != cudaSuccess) { fail("pinn_create: upload failed: %s", cudaGetErrorString(err)); pinn_destroy(e); return 1; }
   const size_t g = (size_t)e->num_sms;
   e->partial_stride = (e->n_theta + 3) & ~3LL;
-  TRY_OR_DESTROY(dev_alloc(&e->partial, g * (size_t)e->partial_stride * e->es, e));
+  // a functional term's own partials G follow the ordinary ones (tail.cuh)
+  const size_t n_partials = p.prob.func_term >= 0 ? 2 * g : g;
+  TRY_OR_DESTROY(dev_alloc(&e->partial, n_partials * (size_t)e->partial_stride * e->es, e));
   TRY_OR_DESTROY(dev_alloc((void**)&e->term_sums, g * PINN_MAX_TERMS * sizeof(double), e));
   if (e->mode == PINN_MODE_FFMA) {
     TRY_OR_DESTROY(dev_alloc(&e->stash, g * (size_t)p.ffma.stash_per_cta * e->es, e));
@@ -209,7 +211,12 @@ int pinn_create_ex2(const pinn_problem_desc* d, const pinn_integral_desc* integr
   }
   TRY_OR_DESTROY(dev_alloc(&e->packed, ((size_t)e->n_theta + PINN_MAX_TERMS) * e->es, e));
   TRY_OR_DESTROY(dev_alloc((void**)&e->d_state, sizeof(TailState), e));
-  err = cudaMemset(e->d_state, 0, sizeof(TailState));
+  {
+    TailState st0;
+    memset(&st0, 0, sizeof st0);
+    st0.func_term = (short)p.prob.func_term; st0.func_square = (short)p.prob.func_square;
+    err = cudaMemcpy(e->d_state, &st0, sizeof st0, cudaMemcpyHostToDevice);
+  }
   if (err != cudaSuccess) { fail("pinn_create: state init failed: %s", cudaGetErrorString(err)); pinn_destroy(e); return 1; }
   {
     const char* to = getenv("PINN_B200_TAIL_TIMEOUT_S");
@@ -334,6 +341,10 @@ int pinn_set_points_host(pinn_handle e, int32_t term, const void* host_pts, int6
 int pinn_set_global_count(pinn_handle e, int32_t term, int64_t n_global) {
   if (check_term(e, term, "pinn_set_global_count")) return 1;
   if (n_global <= 0) return fail("pinn_set_global_count: n_global must be positive");
+  if (term == e->plan.prob.func_term && n_global != e->dyn[term].n)
+    return fail("pinn_set_global_count: term %d is a functional term: g(sum) is not the sum of the ranks' g, so its whole "
+                "node set stays on one rank (0 points on the others) and its global count is the local count %lld", term,
+                (long long)e->dyn[term].n);
   e->term[term].n_global = n_global; e->term[term].n_global_set = true;
   return 0;
 }
@@ -368,7 +379,7 @@ static int launch_fused(pinn_engine* e, const LaunchCall& c, int grid, cudaStrea
       if (!e->fixed_ptr[j])
         return fail("pinn: fixed network %d has no parameters (call pinn_set_fixed_params or pinn_set_fixed_params_host "
                     "first)", j);
-    CUDA_TRY(ffma_launch(e->dtype, p.bufs_smem, p.integ, p.prob.n_fixed > 0, a, grid, p.smem, st));
+    CUDA_TRY(ffma_launch(e->dtype, p.bufs_smem, p.integ, p.prob.n_fixed > 0, p.prob.func_term >= 0, a, grid, p.smem, st));
     return 0;
   }
   if (p.wide) {
@@ -465,7 +476,7 @@ int pinn_loss_grad(pinn_handle e, const void* dev_theta, const double* host_weig
   if (!dev_theta || !dev_term_losses || !dev_total) return fail("pinn_loss_grad: null theta/term_losses/total");
   CUDA_TRY(cudaSetDevice(e->device));
   for (int t = 0; t < e->n_terms; ++t)
-    if (e->dyn[t].n <= 0 && !(e->nranks > 1 && e->term[t].n_global_set))
+    if (e->dyn[t].n <= 0 && !(e->nranks > 1 && (e->term[t].n_global_set || t == e->plan.prob.func_term)))
       return fail("pinn_loss_grad: term %d has no points (call pinn_set_points first)", t);
   if (e->total_tiles <= 0 && e->nranks <= 1) return fail("pinn_loss_grad: no collocation points");
   return eval_step(e, dev_theta, host_weights, dev_grad, dev_term_losses, dev_total, false, (cudaStream_t)stream);
@@ -657,6 +668,8 @@ int pinn_set_sampler_ex(pinn_handle e, int32_t term, int32_t kind, int64_t n, co
   if (!host_lb || !host_ub) return fail("pinn_set_sampler: null bounds");
   if (e->plan.term[term].reduction == PINN_REDUCE_WSUM)
     return fail("pinn_set_sampler: term %d is a weighted-sum (quadrature) term; the uniform sampler serves mean(abs2) terms", term);
+  if (term == e->plan.prob.func_term)
+    return fail("pinn_set_sampler: term %d is a functional term; its nodes are fixed (pinn_set_points)", term);
   CUDA_TRY(cudaSetDevice(e->device));
   const int dim = e->plan.prob.terms[term].dim;
   TermState& ts = e->term[term];
@@ -699,6 +712,9 @@ int pinn_term_grad_stats(pinn_handle e, int32_t term, const void* dev_theta, dou
                          void* stream) {
   if (check_term(e, term, "pinn_term_grad_stats")) return 1;
   if (!dev_theta || !host_max_abs || !host_mean_abs) return fail("pinn_term_grad_stats: null theta/output");
+  if (term == e->plan.prob.func_term)
+    return fail("pinn_term_grad_stats: term %d is a functional term; its gradient is not a per-term loss gradient of the "
+                "adaptive reweighting", term);
   CUDA_TRY(cudaSetDevice(e->device));
   cudaStream_t st = (cudaStream_t)stream;
   double w[PINN_MAX_TERMS];

@@ -290,11 +290,28 @@ int plan_term(const pinn_problem_desc* d, int t, const pinn_integral_desc* integ
     return fail("pinn_create: term %d has no network taps (an equation such as 0 ~ 0 cannot be trained on)", t);
   if (td.n_taps + n_own > PINN_MAX_TAPS)
     return fail("pinn_create: term %d has %d taps and %d integrals (max %d together)", t, td.n_taps, n_own, PINN_MAX_TAPS);
-  if (td.reduction != PINN_REDUCE_MEAN && td.reduction != PINN_REDUCE_WSUM)
+  if (td.reduction < PINN_REDUCE_MEAN || td.reduction > PINN_REDUCE_SQUARE_OF_SUM)
     return fail("pinn_create: term %d unknown reduction %d", t, td.reduction);
+  const bool func = td.reduction == PINN_REDUCE_ABS_OF_SUM || td.reduction == PINN_REDUCE_SQUARE_OF_SUM;
+  if (func) {    // a functional term: g(scale * sum_p w_p v_p) (the kernel reads its nullable weights itself)
+    if (d->mode != PINN_MODE_FFMA)
+      return fail("pinn_create: term %d is a functional term; functional terms run on the FFMA path (mode PINN_MODE_FFMA)", t);
+    if (P.func_term >= 0)
+      return fail("pinn_create: term %d is a second functional term (term %d is one); a problem has at most one", t,
+                  P.func_term);
+    if (n_own > 0)
+      return fail("pinn_create: term %d is a functional term and owns integral terms; its program may not read "
+                  "PINN_OP_INTEGRAL", t);
+    for (int i = 0; i < td.n_instr && td.prog; ++i)
+      if (td.prog[i].op == PINN_OP_INTEGRAL)
+        return fail("pinn_create: term %d is a functional term and its program reads PINN_OP_INTEGRAL (instr %d); "
+                    "integrals inside a functional term are not supported", t, i);
+    P.func_term = t;
+    P.func_square = td.reduction == PINN_REDUCE_SQUARE_OF_SUM ? 1 : 0;
+  }
   T.weighted = td.reduction == PINN_REDUCE_WSUM;
   tp.reduction = td.reduction;
-  tp.scale = td.reduction == PINN_REDUCE_WSUM ? td.scale : 1.0;
+  tp.scale = td.reduction == PINN_REDUCE_MEAN ? 1.0 : td.scale;
   return plan_body(d, td, "term", t, P, T, integrals, n_integrals, max_c, stash_max, &tp.flops_per_point);
 }
 
@@ -377,7 +394,7 @@ int plan_ffma(int dtype, int max_w8, long long resident, int max_c, long long st
     long long wa = o.res ? resident : panel;
     wa = (wa + 3) & ~3LL;
     if (wa > (1LL << 30)) continue;
-    size_t need = ffma_smem_bytes(dtype, a.buf_elems, (int)wa, o.bufs, p.integ);
+    size_t need = ffma_smem_bytes(dtype, a.buf_elems, (int)wa, o.bufs, p.integ || p.func);   // FUNC runs with INTEG
     if (need <= (size_t)max_smem) {
       p.bufs_smem = o.bufs; a.weights_resident = o.res ? 1 : 0; a.w_area = (int)wa; p.smem = need;
       return 0;
@@ -662,6 +679,7 @@ int plan_problem(const pinn_problem_desc* d, const pinn_integral_desc* integrals
   DevProblem& P = p.prob;
   P.n_nets = d->n_nets; P.n_terms = d->n_terms; P.n_params = d->n_params;
   P.param_off = d->param_offset; P.n_theta = d->n_theta; P.n_fixed = n_fixed;
+  P.func_term = -1;
   int max_w8 = 8, max_c = 1;
   long long resident = 0, stash_max = 0;
   if (plan_nets(d, fixed, n_fixed, P, max_w8, resident, p.fixed_len)) return 1;
@@ -669,6 +687,7 @@ int plan_problem(const pinn_problem_desc* d, const pinn_integral_desc* integrals
     if (plan_term(d, t, integrals, n_integrals, P, p.term[t], max_c, stash_max)) return 1;
   P.n_integrals = n_integrals;
   p.integ = n_integrals > 0;
+  p.func = P.func_term >= 0;
   for (int i = 0; i < n_integrals; ++i) {     // after the terms: the owners' dims and tap counts are validated
     double f = 0;
     if (plan_integral(d, integrals, n_integrals, i, P, max_c, stash_max, &f)) return 1;

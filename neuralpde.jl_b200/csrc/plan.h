@@ -8,8 +8,8 @@ int fail(const char* fmt, ...);    // sets the message pinn_last_error returns; 
 const char* last_error();
 
 struct TermPlan {
-  int reduction;                   // PINN_REDUCE_MEAN or PINN_REDUCE_WSUM
-  double scale;                    // WSUM scale (MEAN: 1/n_global, formed at launch time)
+  int reduction;                   // PINN_REDUCE_*
+  double scale;                    // WSUM / *_OF_SUM scale (MEAN: 1/n_global, formed at launch time)
   double flops_per_point;          // algorithmic: 6 * sum over the term's networks of C * sum_l dims[l] * dims[l+1]
 };
 
@@ -22,6 +22,7 @@ struct Plan {
   bool wide;                       // tensor-core modes: tw_pack + the 128-wide kernel run instead of the narrow one
   bool x256;                       // (with wide) a hidden width is 192 or 256: tx_pack + the 256-wide kernel run instead
   bool integ;                      // FFMA: the problem has integral terms (the kernel instantiation with node tiles runs)
+  bool func;                       // FFMA: the problem has a functional term (its own kernel instantiation runs)
   long long fixed_len[PINN_MAX_FIXED_NETS];   // scalars of each fixed network's parameter buffer
   // launch-argument templates: the planner fills the layout, pinn_create the buffers, a launch the per-call fields
   FfmaArgs ffma; TcArgs tc; TwArgs tw; TwPackArgs pack;

@@ -94,7 +94,11 @@ template <> struct Vec16<double> { typedef double2 type; };
 // NT = threads per CTA.  red: NT * (16 / sizeof(real)) scalars of 16-byte aligned shared memory.  partial:
 // [gridDim.x][stride] (stride a multiple of 4 scalars); term_sums: [gridDim.x][PINN_MAX_TERMS] (this CTA's row already
 // written).  Must be called by every thread of every CTA of the launch.
-template <typename real, int NT>
+// FUNC: the problem has a functional term f (PINN_REDUCE_*_OF_SUM; st->func_term): its loss is L_f = g(scale_f S_f),
+// S_f = sum_b term_sums[b][f], and the functional's own partials G [gridDim.x][stride] follow `partial`.  Every slice
+// CTA forms S_f in the term CTA's order, kappa = w_f g'(scale_f S_f) scale_f, and reduces sum_b partial + kappa sum_b G
+// (both in the fixed order): the chain rule of g(S) needs S before any point's contribution can be scaled.
+template <typename real, int NT, bool FUNC = false>
 __device__ __noinline__ void fused_tail(const TailArgs& ta, const real* partial, long long stride, const double* term_sums,
                                         long long n_theta, int n_terms, int want_grad, real* red) {
   constexpr int V = 16 / (int)sizeof(real);   // scalars per 16-byte load: the reduction is bound by bytes in flight
@@ -171,7 +175,11 @@ __device__ __noinline__ void fused_tail(const TailArgs& ta, const real* partial,
       for (int j = 0; j < (kTailSlots + 31) / 32; ++j) s += v[j];
 #pragma unroll
       for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-      if (lane == 0) sL[k] = s * ta.sw.scale[k];
+      if (lane == 0) {
+        sL[k] = s * ta.sw.scale[k];
+        if constexpr (FUNC)
+          if (k == st->func_term) sL[k] = st->func_square ? sL[k] * sL[k] : fabs(sL[k]);
+      }
     }
     __syncthreads();
     if (tid == 0) {
@@ -226,9 +234,59 @@ __device__ __noinline__ void fused_tail(const TailArgs& ta, const real* partial,
   const long long i0 = slice_cta ? (long long)bid * S : n_theta;
   const long long i1 = (i0 + S < n_theta) ? i0 + S : n_theta;
   const int lane = tid & 31, g = tid >> 5;
+  real kappa = real(0);                            // FUNC: d total / d S_f
+  if constexpr (FUNC) {
+    __shared__ double s_kappa;
+    if (want_grad && tid < 32) {                   // S_f exactly as the term CTA sums it
+      const int f = st->func_term;
+      double v[(kTailSlots + 31) / 32];
+#pragma unroll
+      for (int j = 0; j < (kTailSlots + 31) / 32; ++j) {
+        const int b = lane + 32 * j;
+        v[j] = (b < nb) ? __ldcg(&term_sums[(long long)b * PINN_MAX_TERMS + f]) : 0.0;
+      }
+      double s = 0.0;
+#pragma unroll
+      for (int j = 0; j < (kTailSlots + 31) / 32; ++j) s += v[j];
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+      if (lane == 0) {
+        const double x = s * ta.sw.scale[f];
+        const double dg = st->func_square ? 2.0 * x : (x > 0.0 ? 1.0 : (x < 0.0 ? -1.0 : 0.0));   // sign(0) = 0
+        s_kappa = ta.sw.w[f] * dg * ta.sw.scale[f];
+      }
+    }
+    __syncthreads();
+    kappa = real(s_kappa);
+  }
   if (want_grad) {
     for (long long base = i0; base < i1; base += EW) {
       const long long i = base + (long long)V * lane;
+      real tf = real(0);                           // FUNC: kappa * sum_b G[b][i], reduced like the partials below
+      if constexpr (FUNC) {
+        real acc[V];
+#pragma unroll
+        for (int j = 0; j < V; ++j) acc[j] = real(0);
+        if (i < i1) {
+          const real* col = partial + (long long)nb * stride + i;
+#pragma unroll 8
+          for (int b = g; b < nb; b += NG) {
+            const vec_t v = __ldcg(reinterpret_cast<const vec_t*>(col + (long long)b * stride));
+            const real* pv = reinterpret_cast<const real*>(&v);
+#pragma unroll
+            for (int j = 0; j < V; ++j) acc[j] += pv[j];
+          }
+        }
+        *reinterpret_cast<vec_t*>(red + (size_t)(g * 32 + lane) * V) = *reinterpret_cast<vec_t*>(acc);
+        __syncthreads();
+        if (tid < EW && base + tid < i1) {
+          tf = red[tid];
+#pragma unroll
+          for (int k = 1; k < NG; ++k) tf += red[k * EW + tid];
+          tf *= kappa;
+        }
+        __syncthreads();
+      }
       real acc[V];
 #pragma unroll
       for (int j = 0; j < V; ++j) acc[j] = real(0);
@@ -248,6 +306,7 @@ __device__ __noinline__ void fused_tail(const TailArgs& ta, const real* partial,
         real t = red[tid];
 #pragma unroll
         for (int k = 1; k < NG; ++k) t += red[k * EW + tid];
+        if constexpr (FUNC) t += tf;
         if (multi) {
           if (W == 1) {
             push(base + tid, (unsigned int)__float_as_uint((float)t));

@@ -31,6 +31,8 @@ OP = {
     "integral": 18,
 }
 REDUCE_MEAN, REDUCE_WSUM = 0, 1
+# functional terms: g(scale * sum_p w_p v_p), g = |.| or (.)^2 (integral constraints, pinn.IntegralLoss)
+REDUCE_ABS_OF_SUM, REDUCE_SQUARE_OF_SUM = 2, 3
 
 # symbols include/pinn_b200.h declares; tests check that the library exports every one
 EXPORTS = [

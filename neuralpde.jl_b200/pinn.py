@@ -15,12 +15,12 @@ import numpy as np
 
 from . import engine as _eng
 from .engine import (Engine, EngineError, FixedNetSpec, IntegralSpec, NetSpec, ProblemSpec, TapSpec, TermSpec,
-                     REDUCE_MEAN, REDUCE_WSUM)
+                     REDUCE_ABS_OF_SUM, REDUCE_MEAN, REDUCE_SQUARE_OF_SUM, REDUCE_WSUM)
 from .lowering import LoweredTerm, LoweringError, lower_equation, term_spec
 from .strategies import (AbstractTrainingStrategy, GridTraining, QuadratureTraining, QuasiRandomTraining,
                          StochasticTraining, _julia_range, _product_columns, gauss_legendre_box, generate_quasi_random_points,
                          generate_random_points, generate_training_sets, get_bounds, shard_range)
-from .symbolic import Equation, FixedNet, PDESystem, VarInfo, fixed_function, get_vars
+from .symbolic import Equation, FixedNet, PDESystem, VarInfo, eq_indvars, fixed_function, get_vars
 
 _ACT_NAMES = {"identity": "identity", "tanh": "tanh", "sigmoid": "sigmoid", "σ": "sigmoid", "sin": "sin",
               "softplus": "softplus", "swish": "swish", None: "identity"}
@@ -323,6 +323,84 @@ class DataLoss:
     values: np.ndarray        # (n,) observations
 
 
+@dataclass
+class IntegralLoss:
+    """Native non-data ``additional_loss``: an integral constraint ``g(Σ_p w_p v_p - target)``, ``g = |·|``
+    (``norm="abs"``) or ``(·)²`` (``norm="abs2"``), ``v_p`` the integrand at node p.
+
+    The reference states such constraints as closures (test/NNPDE2/additional_loss__fokker_planck.jl:42-46,
+    docs/src/tutorials/constraints.md:58-71); a closure cannot run inside a CUDA kernel, so the engine takes this
+    structured form, as ``DataLoss`` does for data.  ``integrand`` is an expression in the independent variables, the
+    dependent variables and their derivatives, parameters and registered functions, lowered like an equation side.
+    The nodes are the engine's fixed Gauss-Legendre box on ``domains`` (``nodes_per_dim`` per variable), or explicit
+    ``points`` ((d, n), one row per argument of the dependent variables the integrand applies) with ``weights``
+    (1 when omitted).  The reference's adaptive cubature is replaced by the fixed rule.  The term runs on the FFMA
+    path; with several ranks its whole node set stays on rank 0."""
+    integrand: object
+    domains: Optional[Sequence] = None
+    _: dataclasses.KW_ONLY
+    points: Optional[np.ndarray] = None
+    weights: Optional[np.ndarray] = None
+    target: float = 0.0
+    norm: str = "abs"
+    nodes_per_dim: int = 16
+
+    def __post_init__(self):
+        if self.norm not in ("abs", "abs2"):
+            raise ValueError("IntegralLoss: norm must be \"abs\" or \"abs2\", got %r" % (self.norm,))
+        if (self.domains is None) == (self.points is None):
+            raise ValueError("IntegralLoss: give either domains (Gauss-Legendre nodes) or explicit points")
+        if self.weights is not None and self.points is None:
+            raise ValueError("IntegralLoss: weights go with explicit points")
+        if int(self.nodes_per_dim) < 1:
+            raise ValueError("IntegralLoss: nodes_per_dim must be >= 1")
+
+    def nodes(self, rows: List[str]):
+        """(points (len(rows), n), weights (n,)) in float64; row i is the variable rows[i]"""
+        if self.points is not None:
+            X = np.asarray(self.points, dtype=np.float64)
+            X = X.reshape(1, -1) if X.ndim == 1 else X
+            if X.ndim != 2 or X.shape[0] != len(rows):
+                raise ValueError("IntegralLoss: points must be (%d, n) for the variables %s, got shape %s"
+                                 % (len(rows), rows, np.shape(self.points)))
+            w = np.ones(X.shape[1]) if self.weights is None else np.asarray(self.weights, dtype=np.float64)
+            if np.ndim(w) == 0:
+                w = np.full(X.shape[1], float(w))
+            if w.shape != (X.shape[1],):
+                raise ValueError("IntegralLoss: weights must have shape (%d,), got %s" % (X.shape[1], w.shape))
+            return X, w
+        box = {str(d.variables): (float(d.domain.lo), float(d.domain.hi)) for d in self.domains}
+        missing = [r for r in rows if r not in box]
+        if missing:
+            raise ValueError("IntegralLoss: no domain for the variables %s" % missing)
+        lb = np.array([box[r][0] for r in rows])
+        ub = np.array([box[r][1] for r in rows])
+        X, w, _ = gauss_legendre_box((lb, ub), int(self.nodes_per_dim), np.float64)
+        return X, w
+
+
+def _integral_loss_term(add: IntegralLoss, vi: VarInfo, param_index, param_values, fixed):
+    """(TermSpec, points, weights) of the functional term: the program yields v_p - target / Σw, so that
+    Σ_p w_p (v_p - target / Σw) = Σ_p w_p v_p - target"""
+    import sympy as sp
+    if callable(add.integrand) and not isinstance(add.integrand, sp.Basic):
+        raise ValueError("IntegralLoss: the integrand must be an expression, not a callable")
+    integrand = sp.sympify(add.integrand)
+    rows = eq_indvars(Equation(integrand, sp.Integer(0)), vi)
+    if not rows:
+        raise ValueError("IntegralLoss: the integrand %s applies no dependent variable: nothing to train on" % integrand)
+    X, w = add.nodes(rows)
+    sw = float(np.sum(w))
+    if add.target != 0 and sw == 0:
+        raise ValueError("IntegralLoss: the weights sum to 0, so a nonzero target cannot be folded into the integrand")
+    shift = float(add.target) / sw if add.target != 0 else 0.0
+    lt = lower_equation(Equation(integrand, sp.Float(shift)), vi, param_index, param_values, hoist=False, fixed=fixed)
+    if lt.integrals:
+        raise ValueError("IntegralLoss: the integrand may not contain an Integral")
+    red = REDUCE_ABS_OF_SUM if add.norm == "abs" else REDUCE_SQUARE_OF_SUM
+    return term_spec(lt, red, 1.0), X, w
+
+
 # ---- PhysicsInformedNN -------------------------------------------------------------------------------
 class AbstractPINN:
     pass
@@ -566,6 +644,17 @@ def symbolic_discretize(pde_system: PDESystem, discretization: PhysicsInformedNN
         fixed: List[FixedNet] = []          # registered network functions the equations apply
         pde_terms = [lower_equation(e, vi, param_index, param_values, hoist=hoist, fixed=fixed) for e in eqs]
         bc_terms = [lower_equation(e, vi, param_index, param_values, hoist=hoist, fixed=fixed) for e in bcs]
+        add = d.additional_loss
+        if add is not None and not isinstance(add, (DataLoss, IntegralLoss)):
+            raise ValueError("additional_loss must be a DataLoss (data term) or an IntegralLoss (integral constraint); "
+                             "arbitrary closures cannot run inside the CUDA kernel")
+        if isinstance(add, IntegralLoss):
+            if bayes:
+                raise ValueError("BayesianPINN: an IntegralLoss has no log-likelihood form (the reference adds "
+                                 "additional_loss values as one observation); use PhysicsInformedNN")
+            if d.mode != "ffma":
+                raise ValueError("IntegralLoss: functional terms run on the FFMA path: use mode=\"ffma\"")
+            func_spec, func_pts, func_w = _integral_loss_term(add, vi, param_index, param_values, fixed)
     except LoweringError as ex:
         raise ValueError(str(ex)) from ex
 
@@ -609,10 +698,8 @@ def symbolic_discretize(pde_system: PDESystem, discretization: PhysicsInformedNN
                                   prog=[("tap", 0, 0, 0.0), ("coord", din, 0, 0.0), ("sub", 0, 1, 0.0)],
                                   net_rows=rows, reduction=REDUCE_MEAN))
             l2_sets.append(np.concatenate([m[:, 1:].T, m[:, :1].T], axis=0))
-    add = d.additional_loss
-    if add is not None and not isinstance(add, DataLoss):
-        raise ValueError("additional_loss must be a DataLoss (structured data term); arbitrary closures cannot "
-                         "run inside the CUDA kernel")
+    if isinstance(add, IntegralLoss):
+        specs.append(func_spec)
     if isinstance(add, DataLoss):
         if add.depvar not in vi.dict_depvars:
             raise ValueError("DataLoss: unknown dependent variable %s" % add.depvar)
@@ -676,6 +763,7 @@ def symbolic_discretize(pde_system: PDESystem, discretization: PhysicsInformedNN
         if X.ndim != 2 or X.shape[1] != y.shape[1]:
             raise ValueError("DataLoss: points must be (d, n) and values (n,)")
         point_sets[-1] = np.concatenate([X, y], axis=0)
+    func_term = len(specs) - 1 if isinstance(add, IntegralLoss) else -1
 
     eng = Engine(spec)
     _upload_fixed(eng, fixed)
@@ -699,6 +787,11 @@ def symbolic_discretize(pde_system: PDESystem, discretization: PhysicsInformedNN
     for i in range(n_terms):
         if point_sets[i] is not None:
             upload(i, point_sets[i], quad_w[i])
+    if func_term >= 0:
+        # g(Σ_r S_r) is not Σ_r g(S_r): the whole node set stays on rank 0, the other ranks hold none and add exactly 0
+        point_sets[func_term], quad_w[func_term] = func_pts.astype(dtype), func_w.astype(dtype)
+        n_f = func_pts.shape[1] if rank == 0 else 0
+        eng.set_points_host(func_term, point_sets[func_term][:, :n_f], quad_w[func_term][:n_f])
 
     device_sampler = isinstance(strategy, (StochasticTraining, QuasiRandomTraining)) and strategy.device_sampler
     if device_sampler:
@@ -741,7 +834,7 @@ def symbolic_discretize(pde_system: PDESystem, discretization: PhysicsInformedNN
 
     def term_weights() -> np.ndarray:
         w = np.concatenate([weights["pde"], weights["bc"], np.zeros(n_main - n_pde - n_bc)])
-        if isinstance(add, DataLoss):
+        if add is not None:
             w = np.concatenate([w, weights["add"]])
         return w
 
@@ -827,7 +920,7 @@ def symbolic_discretize(pde_system: PDESystem, discretization: PhysicsInformedNN
         term_names=["pde_%d" % (i + 1) for i in range(n_pde)] + ["bc_%d" % (j + 1) for j in range(n_bc)]
         + ["dataset_pde_%d" % (j + 1) for j in range(n_ds[0])] + ["dataset_bc_%d" % (j + 1) for j in range(n_ds[1])]
         + ["l2_data_%s" % name for name in (vi.depvars if l2_sets else [])]
-        + (["additional"] if isinstance(add, DataLoss) else []))
+        + (["additional"] if add is not None else []))
     rep.point_sets = point_sets
     rep.resample = resample
     rep.quad_weights = quad_w
