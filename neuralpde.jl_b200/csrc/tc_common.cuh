@@ -18,7 +18,7 @@ namespace pinn {
 constexpr int kNH = kTcThreads / 128;   // warps per 32-row quadrant of the accumulators: each takes 1/kNH of the columns
 static_assert(kTcThreads == 512, "the MMA chains are spread over four warpgroups");
 constexpr int GW = 4;                   // columns per epilogue granule
-constexpr int GWB = 2;                  // granule of the tensor-layer reverse epilogue (register-heaviest loop)
+constexpr int GWB = 2;                  // granule of the layer-0 reverse epilogue of tc_kernel.cu (register-heaviest loop)
 
 template <int N>
 __device__ __forceinline__ float pick(const float* v, int idx) {

@@ -6,14 +6,15 @@
 // fp32 accumulators); every derivative channel (value, d/dx_i, d2/dx_i dx_j) is its own
 // 128-row M block that shares the same weight operand.  The epilogue (bias + activation +
 // forward-mode tap chain rule, or its reverse) runs on the CUDA cores and re-packs the result as
-// the next GEMM's bf16 operand tile: in the forward straight from the wgmma register fragments
-// (each warpgroup owns a 64-row x 32-column block of every channel), in the reverse out of the
-// accumulator region.
+// the next GEMM's bf16 operand tile straight from the wgmma register fragments (each warpgroup
+// owns a 64-row x 32-column block of every channel).  The reverse sweep's MMAs of a tensor layer
+// also stay in registers; only the input adjoints (hand-off to the next layer down) and the four
+// per-warpgroup weight-gradient partials go through the accumulator region.
 //
 //   forward, per tensor layer l :  D_c[128 x n_out] = H_c[128 x n_in] * W_l^T        (A, B K-major)
-//   backward, per tensor layer l:  Z_c   (recompute, 32-column groups)  = H_c * W_l^T
-//                                  Hbar_c[128 x n_in] = Zbar_c[128 x n_out] * W_l     (B MN-major)
-//                                  Wbar_l[n_out x n_in] = sum_c Zbar_c^T * H_c         (A, B MN-major)
+//   backward, per tensor layer l:  Z_c   (recompute, all columns)   = H_c * W_l^T
+//                                  Hbar_c^T[n_in x 128] = W_l^T * Zbar_c^T            (A MN-major; 32 points per warpgroup)
+//                                  Wbar_l^T[n_in x n_out] = sum_c H_c^T * Zbar_c       (A, B MN-major; 32 points per warpgroup)
 //                                  bbar_l[n_out]        = Zbar_0^T * 1                  (B = constant ones atom)
 //   last layer                  :  wbar_L[n]            = sum_c H_c^T * ubar_c          (B = (hi, lo) pairs of ubar)
 //
@@ -45,12 +46,12 @@ struct LoopCtx {
   float* gb;              // bias gradient of the current layer (CTA partial)
   float* gw;              // weight gradient of the first layer (CTA partial)
   uint32_t taddr;         // accumulator address of the warp's row quadrant
-  int act, split, p, lane, g0, g1, c0, flag;
+  int act, split, p, lane, g0, g1, flag;
   // ng granules of the layer, spread over the kNH warps of the thread's row quadrant
   __device__ __forceinline__ LoopCtx(uint32_t fp_, uint32_t bt_, uint32_t tP_, uint32_t tQ_, const Tid& t, int act_, int ng,
-                                     int flag_, int split_ = 0, int c0_ = 0, float* gb_ = nullptr, float* gw_ = nullptr)
+                                     int flag_, int split_ = 0, float* gb_ = nullptr, float* gw_ = nullptr)
       : fp(fp_), bt(bt_), tP(tP_), tQ(tQ_), gb(gb_), gw(gw_), taddr(t.lane_addr), act(act_), split(split_), p(t.p), lane(t.lane),
-        g0(t.hh * (ng / kNH)), g1((t.hh + 1) * (ng / kNH)), c0(c0_), flag(flag_) {}
+        g0(t.hh * (ng / kNH)), g1((t.hh + 1) * (ng / kNH)), flag(flag_) {}
 };
 
 // layer 0 forward: coordinates -> H^0 tiles (+ last-layer dot when there is no tensor layer: flag)
@@ -185,47 +186,106 @@ __device__ __forceinline__ void tl_fwd_frag(const float (&d)[C][16], const LoopC
   }
 }
 
-// tensor layer backward epilogue for the column group starting at c0: recomputed Z (columns Y) and output
-// adjoints (columns X, or w_last * ubar for the last hidden layer: flag) -> Zbar tiles (the bias gradient is a
-// column sum of Zbar_0, taken by one MMA chain against the constant ones atom in net_backward)
-template <int N1, int N2, bool PURE, int AK>
-__device__ __forceinline__ void tl_bwd_loop(const LoopCtx lc, const Chan<N1, N2> ch, const float* ubp) {
-  constexpr int C = 1 + N1 + N2;
-  float ub[C];
+// ---- register-resident reverse of a tensor layer --------------------------------------------------------------------------
+// The recompute of Z is fwd_mma on the reloaded hi tiles (the forward's ownership and k order).  dgrad and wgrad are
+// transposed products so that every warpgroup takes 32 points, a 4 KB (atom-aligned) offset into the MN- or K-major tiles:
+//   dgrad: Hbar_c^T[k][p] = sum_o W_l[o][k] Zbar_c[p][o]     A = W_l MN-major (M = the 64 input columns), B = Zbar_c K-major
+//   wgrad: Wbar_l^T[k][o] = sum_c sum_p H_c[p][k] Zbar_c[p][o]   A = H_c MN-major, B = Zbar_c MN-major; partial over 32 points
+//   bias : bbar_l[o] = sum_p Zbar_0[p][o]                       A = Zbar_0 MN-major, B = the constant ones atom
+// NKO = n_out / 16 k-steps of dgrad.  Each is one straight-line sequence with one commit / wait, on all four warpgroups.
+template <int C, int NKO>
+__device__ __forceinline__ void dgrad_mma(float (&d)[C][16], uint32_t sP, uint32_t whi) {
+  const uint32_t poff = (threadIdx.x >> 7) * 32u * 128u;
+  const uint64_t dw = tc::make_desc(whi, 0, 1024);
+  tc::wgmma_fence();
 #pragma unroll
-  for (int c = 0; c < C; ++c) ub[c] = ubp[c];
-#pragma unroll 1
-  for (int g = lc.g0; g < lc.g1; ++g) {
-    const int ocol = lc.c0 + g * GWB;
-    float z[C][GWB], hb[C][GWB];
+  for (int c = 0; c < C; ++c) {
+    const uint64_t dz = tc::make_desc(sP + c * kTileBytes + poff, 0, 1024);
 #pragma unroll
-    for (int c = 0; c < C; ++c) acc_ldg(lc.taddr + TM_Y + c * 32 + g * GWB, z[c]);
-    if (!lc.flag) {
+    for (int k = 0; k < NKO; ++k)   // k-step of 16 output neurons: 16 rows (2048 bytes) of W, 32 bytes of the Zbar rows
+      tc::wgmma_n32<1, 0>(d[c], dw + 128 * k, dz + 2 * k, k ? 1u : 0u);
+  }
+  tc::wgmma_commit();
+  tc::wgmma_wait0();
+}
+template <int C>
+__device__ __forceinline__ void dgrad_mma_any(float (&d)[C][16], uint32_t sP, uint32_t whi, int nko) {
+  switch (nko) {
+    case 1: dgrad_mma<C, 1>(d, sP, whi); break;
+    case 2: dgrad_mma<C, 2>(d, sP, whi); break;
+    case 3: dgrad_mma<C, 3>(d, sP, whi); break;
+    default: dgrad_mma<C, 4>(d, sP, whi); break;
+  }
+}
+template <int C>
+__device__ __forceinline__ void wgrad_mma(float (&dw)[32], float (&db)[8], uint32_t sP, uint32_t sQ, uint32_t s_ones) {
+  const uint32_t poff = (threadIdx.x >> 7) * 32u * 128u;
+  const uint64_t d1 = tc::make_desc(s_ones, 0, 0);   // SBO = 0: every 8-point group of K reads the same ones atom
+  tc::wgmma_fence();
 #pragma unroll
-      for (int c = 0; c < C; ++c) acc_ldg(lc.taddr + TM_X + c * 64 + ocol, hb[c]);
-    }
+  for (int c = 0; c < C; ++c) {
+    const uint64_t dh = tc::make_desc(sQ + c * kTileBytes + poff, 0, 1024), dz = tc::make_desc(sP + c * kTileBytes + poff, 0, 1024);
+#pragma unroll
+    for (int k = 0; k < 2; ++k) tc::wgmma_n64<1, 1>(dw, dh + 128 * k, dz + 128 * k, (c | k) ? 1u : 0u);
+  }
+  const uint64_t dz0 = tc::make_desc(sP + poff, 0, 1024);
+#pragma unroll
+  for (int k = 0; k < 2; ++k) tc::wgmma_n16<1, 1>(db, dz0 + 128 * k, d1, k ? 1u : 0u);
+  tc::wgmma_commit();
+  tc::wgmma_wait0();
+}
+
+// store the m64nNk16 fragment d of this warpgroup (layout: tc::wg_chain) as rows of a row-major fp32 array: element
+// (row r, column n) at base[r * ld + n].  The lanes of a pair swap half of their values so that each holds four
+// consecutive columns of one row: one 16-byte store per 8-column block, and a quad writes 32 contiguous bytes of two rows.
+template <int NF>
+__device__ __forceinline__ void frag_store_rows(float* base, int ld, const float (&d)[NF]) {
+  const int w = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
+  const bool odd = (lane & 1) != 0;
+  float* row = base + (16 * w + (lane >> 2) + (odd ? 8 : 0)) * ld + 4 * ((lane >> 1) & 1);
+#pragma unroll
+  for (int j = 0; j < NF / 4; ++j) {
+    const float r0 = __shfl_xor_sync(0xffffffffu, odd ? d[4 * j] : d[4 * j + 2], 1);
+    const float r1 = __shfl_xor_sync(0xffffffffu, odd ? d[4 * j + 1] : d[4 * j + 3], 1);
+    *reinterpret_cast<float4*>(row + 8 * j) =
+        odd ? make_float4(r0, r1, d[4 * j + 2], d[4 * j + 3]) : make_float4(d[4 * j], d[4 * j + 1], r0, r1);
+  }
+}
+
+// tensor layer backward epilogue on the fragments of the recompute (ownership of fwd_mma): bias + adjoint chain -> Zbar
+// tiles (bf16 hi) in P.  The output adjoints come from the hand-off (accumulator columns TM_X + 64 c + column, row =
+// point: the dgrad of the layer above), or for the last hidden layer (flag) are w_last[column] * ubar_c[row], with
+// ubar_c[row] at ubs[c * kTcPts + row].  Columns beyond n_out get Zbar = 0 (zero weights, bias and adjoints).
+template <int N1, int N2, bool PURE, int AK, int C>
+__device__ __forceinline__ void tl_bwd_frag(const float (&d)[C][16], const LoopCtx lc, const Chan<N1, N2> ch, const float* ubs) {
+  const int wg = threadIdx.x >> 7, w = (threadIdx.x >> 5) & 3;
+  const int row0 = 64 * (wg & 1) + 16 * w + (lc.lane >> 2);
+  const int col0 = 32 * (wg >> 1) + 2 * (lc.lane & 3);
+  const float* hbar = tc::s_acc + TM_X * kAccRows;
+#pragma unroll
+  for (int i = 0; i < 16; i += 2) {
+    const int row = row0 + 8 * ((i >> 1) & 1), col = col0 + 8 * (i >> 2);
+    P2 zz[C], hv[C], zv[C];
+    zz[0] = mk2(d[0][i] + lds_f32(lc.bt + col * 4), d[0][i + 1] + lds_f32(lc.bt + (col + 1) * 4));
+#pragma unroll
+    for (int c = 1; c < C; ++c) zz[c] = mk2(d[c][i], d[c][i + 1]);
     if (lc.flag) {
+      const float w0 = lds_f32(lc.fp + (Fp::WL + col) * 4), w1 = lds_f32(lc.fp + (Fp::WL + col + 1) * 4);
 #pragma unroll
-      for (int i = 0; i < GWB; ++i) {
-        const float wl = lds_f32(lc.fp + (Fp::WL + ocol + i) * 4);
-#pragma unroll
-        for (int c = 0; c < C; ++c) hb[c][i] = wl * ub[c];
+      for (int c = 0; c < C; ++c) {
+        const float u = ubs[c * kTcPts + row];
+        hv[c] = mk2(w0 * u, w1 * u);
       }
+    } else {
+#pragma unroll
+      for (int c = 0; c < C; ++c) hv[c] = mk2(hbar[(c * 64 + col) * kAccRows + row], hbar[(c * 64 + col + 1) * kAccRows + row]);
     }
+    chain_bwd<N1, N2, PURE, AK, P2>(lc.act, ch, zz, hv, zv);
+    const uint32_t off = tc::swz_off(row, col);
 #pragma unroll
-    for (int i = 0; i < GWB; i += 2) {
-      P2 zz[C], hv[C], zv[C];
-      zz[0] = mk2(z[0][i] + lds_f32(lc.bt + (ocol + i) * 4), z[0][i + 1] + lds_f32(lc.bt + (ocol + i + 1) * 4));
-#pragma unroll
-      for (int c = 1; c < C; ++c) zz[c] = mk2(z[c][i], z[c][i + 1]);
-#pragma unroll
-      for (int c = 0; c < C; ++c) hv[c] = mk2(hb[c][i], hb[c][i + 1]);
-      chain_bwd<N1, N2, PURE, AK, P2>(lc.act, ch, zz, hv, zv);
-#pragma unroll
-      for (int c = 0; c < C; ++c) { hb[c][i] = zv[c].v.x; hb[c][i + 1] = zv[c].v.y; }
-    }
-#pragma unroll
-    for (int c = 0; c < C; ++c) store_half(lc.tP + c * kTileBytes, lc.tP, lc.p, ocol, hb[c], false);
+    for (int c = 0; c < C; ++c)
+      asm volatile("st.shared.b32 [%0], %1;" ::"r"(lc.tP + c * kTileBytes + off), "r"(tc::pack_bf16(zv[c].v.x, zv[c].v.y))
+                   : "memory");
   }
 }
 
@@ -424,11 +484,24 @@ __device__ __noinline__ uint32_t net_backward(CtaShared* cs, const DevProblem* P
   dbg_mark(cs, 20);
   float ub[C];
   gather_ubar<C>(tm, slot, ms, p, ub);
+  // the last hidden layer's epilogue reads ubar by fragment row (published by the barriers of last_layer_grad)
+  if (t.hh == 0) {
+#pragma unroll
+    for (int c = 0; c < C; ++c) ms.scratch[c * kTcPts + p] = ub[c];
+  }
   // ---- last layer: the ubar tile goes to Q, the products into accumulator columns Y ----------------------------------------
   last_layer_grad<C>(t, ub, pi.nL, partial + net.w_off[L - 1], partial + net.b_off[L - 1], tc::smem_u32(tQ), tc::smem_u32(tP),
                      kTileBytes, 0u, accm + TM_Y, kTcW);
 
   // ---- tensor layers, last to first ------------------------------------------------------------------------------------
+  // Hbar^{l-1} goes from the dgrad fragments to accumulator columns TM_X (the hand-off the next layer down reads), the
+  // four per-warpgroup partials of Wbar_l^T and bbar_l to columns TM_Y; each gradient element is then summed in
+  // warpgroup order by one thread, so the result does not depend on scheduling.
+  const uint32_t sP = tc::smem_u32(tP), sQ = tc::smem_u32(tQ);
+  const int wg = tid >> 7;
+  float* hand = tc::s_acc + TM_X * kAccRows;
+  float* wpart = tc::s_acc + TM_Y * kAccRows;   // [wg][k][o] (4 x 64 x 64), then bbar [wg][o]
+  float* bpart = wpart + 4 * 64 * 64;
   for (int l = TL; l >= 1; --l) {
     const int n_in = net.dims[l], n_out = net.dims[l + 1];
     const int act = net.acts[l];
@@ -445,51 +518,43 @@ __device__ __noinline__ uint32_t net_backward(CtaShared* cs, const DevProblem* P
     }
     wait_bar(ms.bar_ld, ld_phase);
     dbg_mark(cs, 22);
-    // recompute pre-activations in groups of <= 32 columns and turn output adjoints into Zbar tiles
-    for (int c0 = 0; c0 < n_out; c0 += 32) {
-      const int gw_cols = (n_out - c0) < 32 ? (n_out - c0) : 32;     // 32 or 16
-      __syncthreads();
-      dbg_mark(cs, 23);
-      {
-        const uint32_t sQ = tc::smem_u32(tQ);
-        const uint32_t idesc = tc::make_idesc(gw_cols, 0, 0);
-        const uint64_t dw = tc::make_desc(whi + c0 * 128, 0, 1024);
-#pragma unroll 1
-        for (int c = 0; c < C; ++c)
-          mma_chain(accm + TM_Y + c * 32, tc::make_desc(sQ + c * kTileBytes, 0, 1024), dw, 32, 32, n_in / 16, idesc, 0);
-      }
+    {
+      // recompute Z = H_hi * W_hi^T of all n_out columns, then Zbar tiles into P
+      float d[C][16];
+      fwd_mma_any<C>(d, sQ, sQ, whi, whi, n_in / 16, false);
       dbg_mark(cs, 24);
-      __syncthreads();
-      dbg_mark(cs, 25);
-      const LoopCtx lc(tc::smem_u32(fp), tc::smem_u32(bt), tc::smem_u32(tP), tc::smem_u32(tQ), t, act, gw_cols / GWB, l == TL, 0, c0);
-      tl_bwd_loop<N1, N2, PURE, AK>(lc, pi.ch, ub);
+      const LoopCtx lc(tc::smem_u32(fp), tc::smem_u32(bt), sP, sQ, t, act, 0, l == TL);
+      tl_bwd_frag<N1, N2, PURE, AK, C>(d, lc, pi.ch, ms.scratch);
     }
     tc::fence_async_smem();
     __syncthreads();
     dbg_mark(cs, 26);
     {
-      const uint32_t sP = tc::smem_u32(tP), sQ = tc::smem_u32(tQ);
-      const uint32_t s_ones = tc::smem_u32(smem + cs->off_ones);
-      // dgrad: Hbar_c = Zbar_c * W_l  -> X
-      const uint32_t idg = tc::make_idesc(n_in, 0, 1);
-      const uint64_t dw = tc::make_desc(whi, 0, 1024);
-#pragma unroll 1
-      for (int c = 0; c < C; ++c)
-        mma_chain(accm + TM_X + c * 64, tc::make_desc(sP + c * kTileBytes, 0, 1024), dw, 32, 2048, n_out / 16, idg, 0);
-      // wgrad: Wbar_l = sum_c Zbar_c^T * H_c -> Y (rows = output neurons: the 64 columns of the Zbar tiles)
-      const uint32_t iwg = tc::make_idesc(n_in, 1, 1);
-#pragma unroll 1
-      for (int c = 0; c < C; ++c)
-        mma_chain(accm + TM_Y, tc::make_desc(sP + c * kTileBytes, 0, 1024), tc::make_desc(sQ + c * kTileBytes, 0, 1024),
-                  2048, 2048, kTcPts / 16, iwg, c > 0 ? 1u : 0u);
-      // bias gradient: bbar_l[o] = sum_p Zbar_0[p][o] -> Y column 64 (B = the constant ones atom, SBO = 0, no k advance)
-      mma_chain(accm + TM_Y + 64, tc::make_desc(sP, 0, 1024), tc::make_desc(s_ones, 0, 0), 2048, 0, kTcPts / 16,
-                tc::make_idesc(16, 1, 1), 0);
+      float d[C][16];
+      dgrad_mma_any<C>(d, sP, whi, n_out / 16);
+#pragma unroll
+      for (int c = 0; c < C; ++c) frag_store_rows(hand + c * 64 * kAccRows + 32 * wg, kAccRows, d[c]);
     }
     dbg_mark(cs, 27);
+    {
+      float dw[32], db[8];
+      wgrad_mma<C>(dw, db, sP, sQ, tc::smem_u32(smem + cs->off_ones));
+      frag_store_rows(wpart + wg * 64 * 64, 64, dw);
+      // column 0 of the bias product: rows 16 w + lane / 4 (+ 8) of lanes 0, 4, ..., 28
+      if ((t.lane & 3) == 0) {
+        const int o = 16 * (t.warp & 3) + (t.lane >> 2);
+        bpart[wg * 64 + o] = db[0];
+        bpart[wg * 64 + o + 8] = db[2];
+      }
+    }
     __syncthreads();
     dbg_mark(cs, 28);
-    flush_wgrad(t, accm + TM_Y, accm + TM_Y + 64, kTcW, n_in, n_out, gw, gb);
+#pragma unroll 1
+    for (int e = tid; e < 64 * 64; e += kTcThreads) {
+      const int k = e >> 6, o = e & 63;
+      if (k < n_in && o < n_out) atomicAdd(gw + o + (long long)n_out * k, ((wpart[e] + wpart[4096 + e]) + wpart[8192 + e]) + wpart[12288 + e]);
+    }
+    if (tid < n_out) atomicAdd(gb + tid, ((bpart[tid] + bpart[64 + tid]) + bpart[128 + tid]) + bpart[192 + tid]);
   }
 
   // ---- layer 0 backward ---------------------------------------------------------------------------------------------------
@@ -499,10 +564,9 @@ __device__ __noinline__ uint32_t net_backward(CtaShared* cs, const DevProblem* P
     const int act0 = net.acts[0];
     float* gb0 = partial + net.b_off[0];
     float* gw0 = partial + net.w_off[0];
-    const uint32_t sP = tc::smem_u32(tP), sQ = tc::smem_u32(tQ);
     if (TL == 0) {
       // no tensor layer: everything on the CUDA cores (warp reduce-scatter + atomics)
-      const LoopCtx lc(tc::smem_u32(fp), tc::smem_u32(fp), sP, sQ, t, act0, pi.n1w / GW, 1, 0, 0, gb0, gw0);
+      const LoopCtx lc(tc::smem_u32(fp), tc::smem_u32(fp), sP, sQ, t, act0, pi.n1w / GW, 1, 0, gb0, gw0);
       l0_bwd_loop<N1, N2, PURE, AK>(lc, pi, x, ub);
     } else {
       // the weight / bias gradient by MMA (layer0_grad); the coordinate tiles live in Q, which is free after the last

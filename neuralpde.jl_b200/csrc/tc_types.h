@@ -26,8 +26,8 @@ struct FpBlock {
   static constexpr int SIZE = BL + 4;
 };
 // accumulator-region columns (tc_prims.cuh)
-constexpr uint32_t TM_X = 0;           // [c][64]: forward accumulators / adjoints of layer outputs
-constexpr uint32_t TM_Y = 320;         // [c][32] recompute group, or [64] weight-gradient accumulator
+constexpr uint32_t TM_X = 0;           // [c][64]: adjoints of a tensor layer's input (reverse hand-off, row = point)
+constexpr uint32_t TM_Y = 320;         // last-layer / layer-0 gradient chains, tensor-layer weight-gradient partials
 
 struct TcNetSmem {
   int w_hi[kTcMaxTL];   // byte offsets of the bf16 weight tiles
