@@ -569,8 +569,10 @@ int plan_tc_smem(const DevProblem& P, int max_c, int max_smem, Plan& p) {
     c.off_P = take((size_t)max_c * kTwNB * kTileBytes);
     p.tw.off_S = take((size_t)2 * kTwImgBytes);
   } else {
-    c.off_P = take((size_t)max_c * kTileBytes);
+    // P also holds the reverse sweep's four 16 KB weight-gradient partials (tc_kernel.cu net_backward): four tiles at least
+    c.off_P = take((size_t)std::max(max_c, 4) * kTileBytes);
     p.tc.off_Q = take((size_t)max_c * kTileBytes);
+    p.tc.off_Q_bytes = max_c * kTileBytes;
     for (int k = 0; k < P.n_nets; ++k)
       for (int l = 0; l < P.nets[k].n_layers - 2; ++l) {
         TcNetSmem& n = p.tc.nets[k];
@@ -638,7 +640,6 @@ int plan_tc(const pinn_problem_desc* d, int max_smem, Plan& p) {
   }
   TcArgs& a = p.tc;
   a.stash_per_cta = (long long)n_used_max * c.tl_max * kTcMaxC * kTileBytes;
-  a.off_Q_bytes = a.off_Q - a.off_P;   // P and Q regions have the same size
   a.n_nets = d->n_nets; a.n_terms = d->n_terms; a.n_theta = d->n_theta;
   for (int t = 0; t < d->n_terms; ++t) a.term_dim[t] = (unsigned char)P.terms[t].dim;
   return 0;

@@ -8,8 +8,8 @@
 // forward-mode tap chain rule, or its reverse) runs on the CUDA cores and re-packs the result as
 // the next GEMM's bf16 operand tile straight from the wgmma register fragments (each warpgroup
 // owns a 64-row x 32-column block of every channel).  The reverse sweep's MMAs of a tensor layer
-// also stay in registers; only the input adjoints (hand-off to the next layer down) and the four
-// per-warpgroup weight-gradient partials go through the accumulator region.
+// also stay in registers; only the input adjoints (hand-off to the next layer down) go through the
+// accumulator region, and the four per-warpgroup weight-gradient partials through shared memory.
 //
 //   forward, per tensor layer l :  D_c[128 x n_out] = H_c[128 x n_in] * W_l^T        (A, B K-major)
 //   backward, per tensor layer l:  Z_c   (recompute, all columns)   = H_c * W_l^T
@@ -494,14 +494,17 @@ __device__ __noinline__ uint32_t net_backward(CtaShared* cs, const DevProblem* P
                      kTileBytes, 0u, accm + TM_Y, kTcW);
 
   // ---- tensor layers, last to first ------------------------------------------------------------------------------------
-  // Hbar^{l-1} goes from the dgrad fragments to accumulator columns TM_X (the hand-off the next layer down reads), the
-  // four per-warpgroup partials of Wbar_l^T and bbar_l to columns TM_Y; each gradient element is then summed in
-  // warpgroup order by one thread, so the result does not depend on scheduling.
+  // Hbar^{l-1} goes from the dgrad fragments to accumulator columns TM_X (the hand-off the next layer down reads).  The
+  // four per-warpgroup partials of Wbar_l^T and bbar_l are exchanged through shared memory: once every warpgroup's wgrad
+  // has been waited for, P (Zbar) and Q (H^{l-1}) are dead.  The partials go to the first four tiles of P (plan.cu gives
+  // P at least four) and to ms.scratch, the next layer's stash reload goes to Q at the same time, and each gradient
+  // element is summed in warpgroup order by one thread, so the result does not depend on scheduling.
   const uint32_t sP = tc::smem_u32(tP), sQ = tc::smem_u32(tQ);
   const int wg = tid >> 7;
   float* hand = tc::s_acc + TM_X * kAccRows;
-  float* wpart = tc::s_acc + TM_Y * kAccRows;   // [wg][k][o] (4 x 64 x 64), then bbar [wg][o]
-  float* bpart = wpart + 4 * 64 * 64;
+  float* wpart = reinterpret_cast<float*>(tP);   // [wg][k][o] (4 x 64 x 64)
+  float* bpart = ms.scratch;                     // [wg][o]; only the last hidden layer's epilogue reads ubar from here
+  static_assert(4 * 64 <= kTcMaxC * kTcPts, "the bias partials fit ms.scratch");
   for (int l = TL; l >= 1; --l) {
     const int n_in = net.dims[l], n_out = net.dims[l + 1];
     const int act = net.acts[l];
@@ -510,8 +513,9 @@ __device__ __noinline__ uint32_t net_backward(CtaShared* cs, const DevProblem* P
     const float* bt = fp + Fp::BT + (l - 1) * 64;
     const uint32_t whi = tc::smem_u32(smem + ns.w_hi[l - 1]);
     dbg_mark(cs, 21);
-    if (tid == 0) {
-      // reload this layer's input tiles H^{l-1} (bf16 hi) from the stash into Q
+    if (tid == 0 && l == TL) {
+      // reload this layer's input tiles H^{l-1} (bf16 hi) from the stash into Q: last_layer_grad has waited for the MMA
+      // chains that read the ubar tile there.  The layers below were reloaded by the layer above them (see there).
       const uint8_t* src = stash_slot + (size_t)(l - 1) * kTcMaxC * kTileBytes;
       tc::mbar_arrive_expect_tx(ms.bar_ld, C * kTileBytes);
       for (int c = 0; c < C; ++c) tc::bulk_load(tQ + c * kTileBytes, src + (size_t)c * kTileBytes, kTileBytes, ms.bar_ld);
@@ -522,11 +526,13 @@ __device__ __noinline__ uint32_t net_backward(CtaShared* cs, const DevProblem* P
       // recompute Z = H_hi * W_hi^T of all n_out columns, then Zbar tiles into P
       float d[C][16];
       fwd_mma_any<C>(d, sQ, sQ, whi, whi, n_in / 16, false);
+      // P holds the weight-gradient partials of the layer above until every thread has summed its elements
+      __syncthreads();
       dbg_mark(cs, 24);
       const LoopCtx lc(tc::smem_u32(fp), tc::smem_u32(bt), sP, sQ, t, act, 0, l == TL);
       tl_bwd_frag<N1, N2, PURE, AK, C>(d, lc, pi.ch, ms.scratch);
     }
-    tc::fence_async_smem();
+    tc::fence_async_smem();   // Zbar (generic-proxy stores to P) -> the dgrad / wgrad MMAs (async proxy)
     __syncthreads();
     dbg_mark(cs, 26);
     {
@@ -539,6 +545,16 @@ __device__ __noinline__ uint32_t net_backward(CtaShared* cs, const DevProblem* P
     {
       float dw[32], db[8];
       wgrad_mma<C>(dw, db, sP, sQ, tc::smem_u32(smem + cs->off_ones));
+      // Every warpgroup has waited for its MMAs: P and Q may be overwritten.  Generic-proxy stores to P after async-proxy
+      // reads that have completed need no proxy fence (the fence above orders the next Zbar stores before their MMAs), and
+      // Q is written and read by the async proxy alone until the coordinate tiles, so its reload needs none either.
+      __syncthreads();
+      if (tid == 0 && l > 1) {
+        // the input tiles H^{l-2} of the next layer down travel into Q while the gradient sum below reads P
+        const uint8_t* src = stash_slot + (size_t)(l - 2) * kTcMaxC * kTileBytes;
+        tc::mbar_arrive_expect_tx(ms.bar_ld, C * kTileBytes);
+        for (int c = 0; c < C; ++c) tc::bulk_load(tQ + c * kTileBytes, src + (size_t)c * kTileBytes, kTileBytes, ms.bar_ld);
+      }
       frag_store_rows(wpart + wg * 64 * 64, 64, dw);
       // column 0 of the bias product: rows 16 w + lane / 4 (+ 8) of lanes 0, 4, ..., 28
       if ((t.lane & 3) == 0) {
@@ -559,7 +575,7 @@ __device__ __noinline__ uint32_t net_backward(CtaShared* cs, const DevProblem* P
 
   // ---- layer 0 backward ---------------------------------------------------------------------------------------------------
   {
-    __syncthreads();
+    __syncthreads();   // the last gradient sum has read P
     dbg_mark(cs, 29);
     const int act0 = net.acts[0];
     float* gb0 = partial + net.b_off[0];

@@ -27,7 +27,7 @@ struct FpBlock {
 };
 // accumulator-region columns (tc_prims.cuh)
 constexpr uint32_t TM_X = 0;           // [c][64]: adjoints of a tensor layer's input (reverse hand-off, row = point)
-constexpr uint32_t TM_Y = 320;         // last-layer / layer-0 gradient chains, tensor-layer weight-gradient partials
+constexpr uint32_t TM_Y = 320;         // last-layer / layer-0 gradient chains
 
 struct TcNetSmem {
   int w_hi[kTcMaxTL];   // byte offsets of the bf16 weight tiles

@@ -28,8 +28,8 @@ ids = (buf[:n] >> 48).astype(int); clk = buf[:n] & ((1 << 48) - 1)
 names = {1: "start", 2: "setup done", 3: "tile loaded", 4: "fwd done", 5: "program done", 6: "stash drained", 7: "end",
          10: "F enter", 11: "F l: tiles written+sync", 12: "F l: mma issued", 13: "F l: mma done", 14: "F l: stash read done+sync",
          15: "F epilogues done", 16: "F exit", 20: "B enter", 21: "B l: start (prev. layer's gradient sum)",
-         22: "B l: stash loaded", 24: "B l: recompute done", 26: "B l: zbar written+sync", 27: "B l: dgrad done+stored",
-         28: "B l: wgrad done+stored+sync", 29: "B l0 start", 30: "B exit"}
+         22: "B l: stash loaded", 24: "B l: recompute done+sync", 26: "B l: zbar written+sync", 27: "B l: dgrad done+stored",
+         28: "B l: wgrad done, partials exchanged+sync", 29: "B l0 start", 30: "B exit"}
 if which == "cfg3":     # marks of the 128-wide kernel (tc_wide_kernel.cu)
     names.update({21: "B l: start", 26: "B l: zbar epilogue+sync", 27: "B l: wgrad issued (issuing lane waits H tiles)",
                   28: "B l: wgrad done", 29: "B l: dgrad done + wgrad flushed"})
