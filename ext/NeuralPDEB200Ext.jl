@@ -19,7 +19,7 @@ const lib = "libpinn_b200"
 const PINN_ABI_VERSION = Cint(2)
 const PINN_MAX_IN = 8
 const PINN_F32, PINN_F64 = Cint(0), Cint(1)
-const PINN_MODE_FFMA, PINN_MODE_TC_BF16, PINN_MODE_TC_SPLIT = Cint(0), Cint(1), Cint(2)
+const PINN_MODE_FFMA, PINN_MODE_TC_BF16, PINN_MODE_TC_SPLIT, PINN_MODE_TC_F64 = Cint(0), Cint(1), Cint(2), Cint(3)
 const PINN_REDUCE_MEAN, PINN_REDUCE_WSUM = Cint(0), Cint(1)
 const ACT = Dict(:identity => 0, :tanh => 1, :tanh_fast => 1, :sigmoid => 2, :sigmoid_fast => 2, :σ => 2, :sin => 3,
                  :softplus => 4, :swish => 5)
@@ -50,14 +50,16 @@ check(rc) = rc == 0 || throw(ArgumentError(unsafe_string(@ccall lib.pinn_last_er
     B200PINN(inner::PhysicsInformedNN; mode = :tc_split)
 
 Sibling discretizer (extension rule: src/NeuralPDE.jl:64-71).  `mode`: `:ffma` (fp32 / fp64 parity path),
-`:tc_bf16`, `:tc_split` (tensor-core paths, Float32 theta).
+`:tc_bf16`, `:tc_split` (tensor-core paths, Float32 theta), `:tc_f64` (the parity path with its layer products on the
+FP64 tensor cores, Float64 theta).
 """
 struct B200PINN{P <: PhysicsInformedNN} <: AbstractPINN
     inner::P
     mode::Cint
 end
 B200PINN(inner::PhysicsInformedNN; mode::Symbol = :tc_split) =
-    B200PINN(inner, Dict(:ffma => PINN_MODE_FFMA, :tc_bf16 => PINN_MODE_TC_BF16, :tc_split => PINN_MODE_TC_SPLIT)[mode])
+    B200PINN(inner, Dict(:ffma => PINN_MODE_FFMA, :tc_bf16 => PINN_MODE_TC_BF16, :tc_split => PINN_MODE_TC_SPLIT,
+                         :tc_f64 => PINN_MODE_TC_F64)[mode])
 
 # ---- lowering: generated loss function (Expr) -> residual IR ---------------------------------------------------------------
 # Grammar after _transform_expression (src/symbolic_utilities.jl:132-331) and _dot_ (:29-62):

@@ -86,8 +86,13 @@ enum { PINN_F32 = 0, PINN_F64 = 1 };
 enum {
   PINN_MODE_FFMA = 0,      /* CUDA-core FMA in the scalar type (parity mode, fp32 / fp64)   */
   PINN_MODE_TC_BF16 = 1,   /* wgmma, bf16 operands, fp32 accumulate                          */
-  PINN_MODE_TC_SPLIT = 2   /* wgmma, split-bf16 x2 (3 MMAs per product), fp32 accumulate     */
+  PINN_MODE_TC_SPLIT = 2,  /* wgmma, split-bf16 x2 (3 MMAs per product), fp32 accumulate     */
+  PINN_MODE_TC_F64 = 3     /* DMMA (mma.sync m16n8k16 .f64), fp64 operands and accumulate    */
 };
+/* PINN_MODE_TC_F64 runs the kernel of PINN_MODE_FFMA with its three layer products (forward, input adjoint, weight
+ * gradient) on the FP64 tensor cores; activations, derivative channels, the residual program and the tail are the FFMA
+ * path's.  It needs PINN_F64 and accepts every shape, integral term, fixed network and functional term PINN_MODE_FFMA
+ * accepts.  Results equal PINN_MODE_FFMA's up to the summation order of the layer products. */
 
 /* activations (Lux Dense: act.(W*x .+ b)) */
 enum {
@@ -155,7 +160,7 @@ typedef struct {
  * square) and its loss is g(scale * sum_p w_p v_p), g = |.| or (.)^2, w_p the nullable weights of pinn_set_points (1
  * when none are given).  It is an integral constraint such as normalisation or a zero mean (reference
  * docs/src/tutorials/constraints.md, test/NNPDE2/additional_loss__fokker_planck.jl); for |.| the gradient uses
- * g'(0) = 0.  At most one functional term per problem, PINN_MODE_FFMA only, no PINN_OP_INTEGRAL in its program.  Its
+ * g'(0) = 0.  At most one functional term per problem, PINN_MODE_FFMA or PINN_MODE_TC_F64, no PINN_OP_INTEGRAL in its program.  Its
  * nodes are fixed: pinn_set_sampler*, pinn_term_grad_stats and the HMC entry points refuse it, and with several ranks
  * the whole node set goes to one rank (0 points elsewhere; pinn_set_global_count only accepts the local count),
  * because g(sum_r S_r) != sum_r g(S_r).  pinn_term_residual returns v_p. */

@@ -5,7 +5,7 @@ The directory name contains a dot, so import it through the root-level alias mod
 ``import neuralpde_jl_b200 as npde``.
 """
 from .engine import (Engine, EngineError, FixedNetSpec, IntegralSpec, NetSpec, ProblemSpec, TapSpec, TermSpec, EXPORTS, LIB_PATH,
-                     MODE_FFMA, MODE_TC_BF16, MODE_TC_SPLIT, REDUCE_ABS_OF_SUM, REDUCE_MEAN, REDUCE_SQUARE_OF_SUM,
+                     MODE_FFMA, MODE_TC_BF16, MODE_TC_SPLIT, MODE_TC_F64, REDUCE_ABS_OF_SUM, REDUCE_MEAN, REDUCE_SQUARE_OF_SUM,
                      REDUCE_WSUM, load_library)
 from .symbolic import (ClosedInterval, Differential, Eq, Equation, In, Inf, Integral, Interval, PDESystem,
                        ProductDomain, UnitInterval, UnitSquare, VarDomain, get_argument, get_variables, get_vars,

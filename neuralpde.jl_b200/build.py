@@ -60,6 +60,9 @@ UNITS = [
     ("ffma_f64_gmem_func.o", "ffma_inst.cu", ["-DPINN_INST_REAL=double", "-DPINN_INST_BUFS=0", "-DPINN_INST_INTEG=1",
                                              "-DPINN_INST_FIXED=1", "-DPINN_INST_FUNC=1"]),
 ]
+# PINN_MODE_TC_F64: the double instantiations again, with their layer products on the FP64 tensor cores (DMMA)
+UNITS += [(obj.replace("ffma_f64_", "ffma_f64_dmma_"), src, defs + ["-DPINN_INST_DMMA=1"])
+          for obj, src, defs in UNITS if obj.startswith("ffma_f64_")]
 
 
 def _nvcc() -> str:

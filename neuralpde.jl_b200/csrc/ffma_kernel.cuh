@@ -256,6 +256,214 @@ __device__ __forceinline__ void gemm_wgrad(const real* Zbar, const real* H, real
   }
 }
 
+// ---- the same three products on the FP64 tensor cores (PINN_MODE_TC_F64, double only) ----------------------------------
+// mma.sync m16n8k16 .f64 (DMMA.16x8x16, sm_90).  Fragments of lane = 4 g + t: A a[i] at (row g + 8 (i&1), col t + 4 (i>>1)),
+// B b[i] at (k t + 4 i, n g), C/D d[i] at (row g + 8 (i>>1), col 2 t + (i&1)).  Accumulators stay in registers; the
+// fragments are read straight from the activation buffers and the staged weight panels.  Rows or k beyond a layer's
+// width read as zero, so a partial k step adds exact zeros.  The products are calls, not inlined: inlined at every call
+// site and channel count, the global-buffer units with integral terms take cicc longer than 20 minutes to compile.
+__device__ __forceinline__ void dmma16816(double (&d)[4], const double (&a)[8], const double (&b)[4]) {
+  asm("mma.sync.aligned.m16n8k16.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5,%6,%7,%8,%9,%10,%11}, "
+      "{%12,%13,%14,%15}, {%0,%1,%2,%3};"
+      : "+d"(d[0]), "+d"(d[1]), "+d"(d[2]), "+d"(d[3])
+      : "d"(a[0]), "d"(a[1]), "d"(a[2]), "d"(a[3]), "d"(a[4]), "d"(a[5]), "d"(a[6]), "d"(a[7]), "d"(b[0]), "d"(b[1]),
+        "d"(b[2]), "d"(b[3]));
+}
+
+// Point of fragment row r (0..15) of m-tile mt, lane group g: the bits of g are spread so that the 16 lanes of a
+// half-warp hit 16 distinct 8-byte bank pairs at the fp64 row stride TP = 34 (t * TP + dmma_pt(...) covers 0..15 mod 16).
+__device__ __forceinline__ int dmma_pt(int g, int h, int mt) {
+  return (g & 1) | ((g >> 2) << 1) | (h << 2) | (((g >> 1) & 1) << 3) | (mt << 4);
+}
+
+// gemm_fwd_block on DMMA: M = the 32 points (2 m-tiles, rows permuted by dmma_pt), N = the warp's 8 output neurons, K = n_in
+template <int C>
+__device__ __noinline__ void gemm_fwd_block_dmma(const double* Hin, double* Zout, const double* Wt_blk,
+                                                    const double* bias_blk, int n_in, int n_out, int ob, int ldw, int ldc,
+                                                    int lane) {
+  constexpr int TP = Cfg<double>::TP;
+  const int g = lane >> 2, t = lane & 3;
+  double acc[C][2][4];
+#pragma unroll
+  for (int mt = 0; mt < 2; ++mt)
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      acc[0][mt][i] = bias_blk[2 * t + (i & 1)];
+#pragma unroll
+      for (int c = 1; c < C; ++c) acc[c][mt][i] = 0.0;
+    }
+  int pa[2][2];   // points of this lane's A rows
+#pragma unroll
+  for (int mt = 0; mt < 2; ++mt)
+#pragma unroll
+    for (int h = 0; h < 2; ++h) pa[mt][h] = dmma_pt(g, h, mt);
+  auto step = [&](int k0, bool tail) {
+    double b[4];
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      const int k = k0 + t + 4 * i;
+      b[i] = (!tail || k < n_in) ? Wt_blk[k * ldw + g] : 0.0;
+    }
+#pragma unroll
+    for (int c = 0; c < C; ++c)
+#pragma unroll
+      for (int mt = 0; mt < 2; ++mt) {
+        double a[8];
+#pragma unroll
+        for (int i = 0; i < 8; ++i) {
+          const int k = k0 + t + 4 * (i >> 1);
+          a[i] = (!tail || k < n_in) ? Hin[c * ldc + k * TP + pa[mt][i & 1]] : 0.0;
+        }
+        dmma16816(acc[c][mt], a, b);
+      }
+  };
+  int k0 = 0;
+#pragma unroll 1
+  for (; k0 + 16 <= n_in; k0 += 16) step(k0, false);
+  if (k0 < n_in) step(k0, true);
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    const int o = ob + 2 * t + (i & 1);
+    if (o < n_out)
+#pragma unroll
+      for (int c = 0; c < C; ++c)
+#pragma unroll
+        for (int mt = 0; mt < 2; ++mt) Zout[c * ldc + o * TP + pa[mt][i >> 1]] = acc[c][mt][i];
+  }
+}
+
+// gemm_dgrad_block on DMMA: M = the 32 points, N = the warp's 8 input neurons, K = n_out
+template <int C>
+__device__ __noinline__ void gemm_dgrad_block_dmma(const double* Zbar, double* Hout, const double* Wt_rows, int n_in,
+                                                      int n_out, int kb, int ldw, int ldc, int lane) {
+  constexpr int TP = Cfg<double>::TP;
+  const int g = lane >> 2, t = lane & 3;
+  double acc[C][2][4];
+#pragma unroll
+  for (int c = 0; c < C; ++c)
+#pragma unroll
+    for (int mt = 0; mt < 2; ++mt)
+#pragma unroll
+      for (int i = 0; i < 4; ++i) acc[c][mt][i] = 0.0;
+  int pa[2][2];
+#pragma unroll
+  for (int mt = 0; mt < 2; ++mt)
+#pragma unroll
+    for (int h = 0; h < 2; ++h) pa[mt][h] = dmma_pt(g, h, mt);
+  auto step = [&](int o0, bool tail) {
+    double b[4];
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      const int o = o0 + t + 4 * i;
+      b[i] = (!tail || o < n_out) ? Wt_rows[g * ldw + o] : 0.0;
+    }
+#pragma unroll
+    for (int c = 0; c < C; ++c)
+#pragma unroll
+      for (int mt = 0; mt < 2; ++mt) {
+        double a[8];
+#pragma unroll
+        for (int i = 0; i < 8; ++i) {
+          const int o = o0 + t + 4 * (i >> 1);
+          a[i] = (!tail || o < n_out) ? Zbar[c * ldc + o * TP + pa[mt][i & 1]] : 0.0;
+        }
+        dmma16816(acc[c][mt], a, b);
+      }
+  };
+  int o0 = 0;
+#pragma unroll 1
+  for (; o0 + 16 <= n_out; o0 += 16) step(o0, false);
+  if (o0 < n_out) step(o0, true);
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    const int k = kb + 2 * t + (i & 1);
+    if (k < n_in)
+#pragma unroll
+      for (int c = 0; c < C; ++c)
+#pragma unroll
+        for (int mt = 0; mt < 2; ++mt) Hout[c * ldc + k * TP + pa[mt][i >> 1]] = acc[c][mt][i];
+  }
+}
+
+// gemm_wgrad on DMMA: per (block of 32 outputs, warp's block of 8 inputs) M = the 32 outputs, N = the 8 inputs,
+// K = C x 32 points (k permuted within each 16 so that both operands' loads are free of bank conflicts).  Every gW
+// element has one owning lane (plain read-modify-write); the bias sum is gemm_wgrad's.
+template <int C>
+__device__ __noinline__ void gemm_wgrad_dmma(const double* Zbar, const double* H, double* gW, double* gb, int n_in,
+                                                int n_out, int ldc, int warp, int lane) {
+  constexpr int TP = Cfg<double>::TP;
+  const int g = lane >> 2, t = lane & 3;
+  int pk[4];   // point offset of k = t + 4 i within a 16-point step
+#pragma unroll
+  for (int i = 0; i < 4; ++i) pk[i] = (t & 1) | (i << 1) | ((t >> 1) << 3);
+  for (int ob = 0; ob < n_out; ob += 32) {
+    int orow[2][2];   // A rows (outputs), clamped into the layer
+#pragma unroll
+    for (int mt = 0; mt < 2; ++mt)
+#pragma unroll
+      for (int h = 0; h < 2; ++h) orow[mt][h] = min(ob + 16 * mt + 8 * h + g, n_out - 1);
+    for (int kb = warp * 8; kb < n_in; kb += kWarps * 8) {
+      double acc[2][4];
+#pragma unroll
+      for (int mt = 0; mt < 2; ++mt)
+#pragma unroll
+        for (int i = 0; i < 4; ++i) acc[mt][i] = 0.0;
+#pragma unroll
+      for (int c = 0; c < C; ++c)
+#pragma unroll
+        for (int p0 = 0; p0 < kTilePts; p0 += 16) {
+          double b[4];
+#pragma unroll
+          for (int i = 0; i < 4; ++i) b[i] = H[c * ldc + (kb + g) * TP + p0 + pk[i]];
+#pragma unroll
+          for (int mt = 0; mt < 2; ++mt) {
+            double a[8];
+#pragma unroll
+            for (int i = 0; i < 8; ++i) a[i] = Zbar[c * ldc + orow[mt][i & 1] * TP + p0 + pk[i >> 1]];
+            dmma16816(acc[mt], a, b);
+          }
+        }
+#pragma unroll
+      for (int mt = 0; mt < 2; ++mt)
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+          const int o = ob + 16 * mt + 8 * (i >> 1) + g, k = kb + 2 * t + (i & 1);
+          if (o < n_out && k < n_in) gW[o + (long long)n_out * k] += acc[mt][i];
+        }
+    }
+    if (warp == 0 && ob + lane < n_out) {
+      const int o = ob + lane;
+      double s = 0.0;
+      for (int p = 0; p < kTilePts; p += 2) {
+        double2 zv = *reinterpret_cast<const double2*>(&Zbar[o * TP + p]);
+        s += zv.x;
+        s += zv.y;
+      }
+      gb[o] += s;
+    }
+  }
+}
+
+// the layer products of the kernel instantiation: CUDA-core FMA, or DMMA (DMMA: double only)
+template <typename real, int C, bool DMMA>
+__device__ __forceinline__ void gemm_fwd(const real* Hin, real* Zout, const real* Wt_blk, const real* bias_blk, int n_in,
+                                         int n_out, int ob, int ldw, int ldc, int lane) {
+  if constexpr (DMMA) gemm_fwd_block_dmma<C>(Hin, Zout, Wt_blk, bias_blk, n_in, n_out, ob, ldw, ldc, lane);
+  else gemm_fwd_block<real, C>(Hin, Zout, Wt_blk, bias_blk, n_in, n_out, ob, ldw, ldc, lane);
+}
+template <typename real, int C, bool DMMA>
+__device__ __forceinline__ void gemm_dgrad(const real* Zbar, real* Hout, const real* Wt_rows, int n_in, int n_out, int kb,
+                                           int ldw, int ldc, int lane) {
+  if constexpr (DMMA) gemm_dgrad_block_dmma<C>(Zbar, Hout, Wt_rows, n_in, n_out, kb, ldw, ldc, lane);
+  else gemm_dgrad_block<real, C>(Zbar, Hout, Wt_rows, n_in, n_out, kb, ldw, ldc, lane);
+}
+template <typename real, int C, bool DMMA>
+__device__ __forceinline__ void gemm_wgrad_any(const real* Zbar, const real* H, real* gW, real* gb, int n_in, int n_out,
+                                               int ldc, int warp, int lane) {
+  if constexpr (DMMA) gemm_wgrad_dmma<C>(Zbar, H, gW, gb, n_in, n_out, ldc, warp, lane);
+  else gemm_wgrad<real, C>(Zbar, H, gW, gb, n_in, n_out, ldc, warp, lane);
+}
+
 #define PINN_DISPATCH_C(Cval, CALL)                                                   \
   switch (Cval) {                                                                     \
     case 1: { constexpr int CC = 1; CALL; } break;                                    \
@@ -541,7 +749,7 @@ __device__ __forceinline__ const real* fixed_params(const DevProblem& P, int k) 
 // ------------------------------------------------------------------------------------------
 // forward through every network term tm taps, at the point tile X ([row][point]): the outputs land in taps; save:
 // keep the pre-activations in the stash for the reverse sweep
-template <typename real, bool FIXED>
+template <typename real, bool FIXED, bool DMMA>
 __device__ __forceinline__ void forward_nets(const FfmaArgs& args, const DevProblem& P, const DevTerm& tm,
                                              const real* __restrict__ theta, const real* X, real* bufA, real* bufB,
                                              real* wsm, real* stash, real* taps, bool save, int ldc, int tid, int warp,
@@ -565,7 +773,7 @@ __device__ __forceinline__ void forward_nets(const FfmaArgs& args, const DevProb
         const real* bs = wsm + net.bs_off[l];
         __syncthreads();   // layer inputs visible
         for (int ob = warp * 8; ob < n_out8; ob += kWarps * 8) {
-          PINN_DISPATCH_C(C, (gemm_fwd_block<real, CC>(H, Z, Wt + ob, bs + ob, n_in, n_out, ob, n_out8, ldc, lane)));
+          PINN_DISPATCH_C(C, (gemm_fwd<real, CC, DMMA>(H, Z, Wt + ob, bs + ob, n_in, n_out, ob, n_out8, ldc, lane)));
         }
         __syncthreads();
       } else {
@@ -575,7 +783,7 @@ __device__ __forceinline__ void forward_nets(const FfmaArgs& args, const DevProb
           __syncthreads();   // panel (and, first time, layer inputs) visible
           const int ob = pb + warp * 8;
           if (ob < n_out8) {
-            PINN_DISPATCH_C(C, (gemm_fwd_block<real, CC>(H, Z, wsm + warp * 8, wsm + n_in8 * PW + warp * 8, n_in,
+            PINN_DISPATCH_C(C, (gemm_fwd<real, CC, DMMA>(H, Z, wsm + warp * 8, wsm + n_in8 * PW + warp * 8, n_in,
                                                          n_out, ob, PW, ldc, lane)));
           }
           __syncthreads();   // panel consumed
@@ -597,7 +805,7 @@ __device__ __forceinline__ void forward_nets(const FfmaArgs& args, const DevProb
 
 // reverse sweep through every network term tm taps, from the tap adjoints tapbar, into this CTA's gradient partial
 // (fixed networks are skipped: their tap adjoints reach nothing trainable)
-template <typename real, bool FIXED>
+template <typename real, bool FIXED, bool DMMA>
 __device__ __forceinline__ void reverse_nets(const FfmaArgs& args, const DevProblem& P, const DevTerm& tm,
                                              const real* __restrict__ theta, const real* X, real* bufA, real* bufB,
                                              real* wsm, const real* stash, const real* tapbar, real* partial, int ldc,
@@ -636,14 +844,14 @@ __device__ __forceinline__ void reverse_nets(const FfmaArgs& args, const DevProb
       if (l == 0) init_inputs<real>(H, X, ch, n_in, ldc, tid);
       else rebuild_h<real>(H, stash + ch.stash_off[l - 1], ch, net.acts[l - 1], n_in, ldc, warp, lane);
       __syncthreads();
-      PINN_DISPATCH_C(C, (gemm_wgrad<real, CC>(B, H, partial + net.w_off[l], partial + net.b_off[l], n_in,
+      PINN_DISPATCH_C(C, (gemm_wgrad_any<real, CC, DMMA>(B, H, partial + net.w_off[l], partial + net.b_off[l], n_in,
                                                n_out, ldc, warp, lane)));
       if (l > 0) {
         __syncthreads();   // wgrad finished reading H before dgrad overwrites it
         if (args.weights_resident) {
           const real* Wt = wsm + net.ws_off[l];
           for (int kb = warp * 8; kb < n_in8; kb += kWarps * 8) {
-            PINN_DISPATCH_C(C, (gemm_dgrad_block<real, CC>(B, H, Wt + kb * n_out8, n_in, n_out, kb, n_out8, ldc,
+            PINN_DISPATCH_C(C, (gemm_dgrad<real, CC, DMMA>(B, H, Wt + kb * n_out8, n_in, n_out, kb, n_out8, ldc,
                                                            lane)));
           }
         } else {
@@ -653,7 +861,7 @@ __device__ __forceinline__ void reverse_nets(const FfmaArgs& args, const DevProb
             __syncthreads();
             const int kb = pb + warp * 8;
             if (kb < n_in8) {
-              PINN_DISPATCH_C(C, (gemm_dgrad_block<real, CC>(B, H, wsm + warp * 8 * n_out8, n_in, n_out, kb,
+              PINN_DISPATCH_C(C, (gemm_dgrad<real, CC, DMMA>(B, H, wsm + warp * 8 * n_out8, n_in, n_out, kb,
                                                              n_out8, ldc, lane)));
             }
             __syncthreads();
@@ -698,7 +906,7 @@ __device__ __forceinline__ real node_tile(const DevIntegral& I, int dim, int j, 
 inline __device__ int node_count(const DevIntegral& I) { return I.n_dims == 2 ? I.q * I.q : I.q; }
 
 // values of term ti's integrals at the owner tile Xs: ival[k][p] for its k-th integral
-template <typename real, bool FIXED>
+template <typename real, bool FIXED, bool DMMA>
 __device__ __forceinline__ void integrals_forward(const FfmaArgs& args, const DevProblem& P, int ti,
                                                   const real* __restrict__ theta, const real* Xs, real* Xn, real* ival,
                                                   real* bufA, real* bufB, real* wsm, real* stash, real* taps, int tid,
@@ -711,7 +919,7 @@ __device__ __forceinline__ void integrals_forward(const FfmaArgs& args, const De
     for (int j = 0; j < node_count(I); ++j) {
       if (warp == 0) wj = node_tile<real>(I, P.terms[ti].dim, j, Xs, Xn, lane);
       __syncthreads();
-      forward_nets<real, FIXED>(args, P, I.body, theta, Xn, bufA, bufB, wsm, stash, taps, false, args.ldc, tid, warp, lane);
+      forward_nets<real, FIXED, DMMA>(args, P, I.body, theta, Xn, bufA, bufB, wsm, stash, taps, false, args.ldc, tid, warp, lane);
       if (warp == 0)
         acc += wj * run_program<real, kTilePts>(I.body, theta + P.param_off, Xn, taps, (real*)nullptr, (real*)nullptr,
                                                 lane, false);
@@ -722,7 +930,7 @@ __device__ __forceinline__ void integrals_forward(const FfmaArgs& args, const De
 }
 
 // gradient of term ti's integrals, given ibar[k][p] = dtotal / dI_p of its k-th integral
-template <typename real, bool FIXED>
+template <typename real, bool FIXED, bool DMMA>
 __device__ __forceinline__ void integrals_reverse(const FfmaArgs& args, const DevProblem& P, int ti,
                                                   const real* __restrict__ theta, const real* Xs, real* Xn,
                                                   const real* ibar, real* bufA, real* bufB, real* wsm, real* stash,
@@ -736,7 +944,7 @@ __device__ __forceinline__ void integrals_reverse(const FfmaArgs& args, const De
     for (int j = 0; j < node_count(I); ++j) {
       if (warp == 0) wj = node_tile<real>(I, P.terms[ti].dim, j, Xs, Xn, lane);
       __syncthreads();
-      forward_nets<real, FIXED>(args, P, body, theta, Xn, bufA, bufB, wsm, stash, taps, true, args.ldc, tid, warp, lane);
+      forward_nets<real, FIXED, DMMA>(args, P, body, theta, Xn, bufA, bufB, wsm, stash, taps, true, args.ldc, tid, warp, lane);
       if (warp == 0) {
         real pbar[PINN_MAX_PARAMS];
 #pragma unroll
@@ -751,7 +959,7 @@ __device__ __forceinline__ void integrals_reverse(const FfmaArgs& args, const De
         }
       }
       __syncthreads();
-      reverse_nets<real, FIXED>(args, P, body, theta, Xn, bufA, bufB, wsm, stash, tapbar, partial, args.ldc, tid, warp, lane);
+      reverse_nets<real, FIXED, DMMA>(args, P, body, theta, Xn, bufA, bufB, wsm, stash, tapbar, partial, args.ldc, tid, warp, lane);
     }
     ++k;
   }
@@ -763,8 +971,11 @@ __device__ __forceinline__ void integrals_reverse(const FfmaArgs& args, const De
 // FUNC: the problem has a functional term (PINN_REDUCE_*_OF_SUM), instantiated with INTEG = FIXED = true only.  Its
 // tiles add sum_p w_p v_p to the term sum and sweep back the seed w_p into this CTA's row of the second partial G (after
 // the ordinary partials of the launch); the tail scales G by g'(S) once S is known.
-template <typename real, bool BUFS_SMEM, bool INTEG, bool FIXED, bool FUNC>
+// DMMA: PINN_MODE_TC_F64, double only: the three layer products run on the FP64 tensor cores (gemm_*_dmma); everything
+// else is the FMA instantiation's.
+template <typename real, bool BUFS_SMEM, bool INTEG, bool FIXED, bool FUNC, bool DMMA>
 __global__ void __launch_bounds__(kThreads, 1) ffma_loss_grad_kernel(const FfmaArgs args) {
+  static_assert(!DMMA || sizeof(real) == 8, "the DMMA layer products are fp64");
   extern __shared__ __align__(16) unsigned char smem_raw[];
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const DevProblem& P = *args.prob;
@@ -856,11 +1067,11 @@ __global__ void __launch_bounds__(kThreads, 1) ffma_loss_grad_kernel(const FfmaA
     int n_int = 0;   // integrals of this term (uniform)
     if constexpr (INTEG) {
       for (int i = 0; i < P.n_integrals; ++i) n_int += P.integ[i].owner == ti;
-      if (n_int) integrals_forward<real, FIXED>(args, P, ti, theta, Xs, Xn, ival, bufA, bufB, wsm, stash, taps, tid, warp, lane);
+      if (n_int) integrals_forward<real, FIXED, DMMA>(args, P, ti, theta, Xs, Xn, ival, bufA, bufB, wsm, stash, taps, tid, warp, lane);
     }
 
     // ---- forward through every tapped network ------------------------------------------------
-    forward_nets<real, FIXED>(args, P, tm, theta, Xs, bufA, bufB, wsm, stash, taps, want_grad, ldc, tid, warp, lane);
+    forward_nets<real, FIXED, DMMA>(args, P, tm, theta, Xs, bufA, bufB, wsm, stash, taps, want_grad, ldc, tid, warp, lane);
 
     // ---- residual, loss partial, tap adjoints (warp 0, lane == point) --------------------------
     if (warp == 0) {
@@ -903,11 +1114,11 @@ __global__ void __launch_bounds__(kThreads, 1) ffma_loss_grad_kernel(const FfmaA
 
     // ---- reverse sweep through every tapped network -----------------------------------------------
     if (want_grad)
-      reverse_nets<real, FIXED>(args, P, tm, theta, Xs, bufA, bufB, wsm, stash, tapbar, func ? gpart : partial, ldc, tid,
+      reverse_nets<real, FIXED, DMMA>(args, P, tm, theta, Xs, bufA, bufB, wsm, stash, tapbar, func ? gpart : partial, ldc, tid,
                                 warp, lane);
     if constexpr (INTEG)
       if (want_grad && n_int)
-        integrals_reverse<real, FIXED>(args, P, ti, theta, Xs, Xn, ival, bufA, bufB, wsm, stash, taps, tapbar, partial, tid, warp,
+        integrals_reverse<real, FIXED, DMMA>(args, P, ti, theta, Xs, Xn, ival, bufA, bufB, wsm, stash, taps, tapbar, partial, tid, warp,
                                 lane);
   }
 

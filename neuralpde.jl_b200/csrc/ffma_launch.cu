@@ -53,12 +53,28 @@ cudaError_t ffma_launch_float_smem_func(const FfmaArgs& a, int grid, size_t smem
 cudaError_t ffma_launch_float_gmem_func(const FfmaArgs& a, int grid, size_t smem, cudaStream_t st);
 cudaError_t ffma_launch_double_smem_func(const FfmaArgs& a, int grid, size_t smem, cudaStream_t st);
 cudaError_t ffma_launch_double_gmem_func(const FfmaArgs& a, int grid, size_t smem, cudaStream_t st);
+cudaError_t ffma_launch_double_dmma_smem(const FfmaArgs& a, int grid, size_t smem, cudaStream_t st);
+cudaError_t ffma_launch_double_dmma_gmem(const FfmaArgs& a, int grid, size_t smem, cudaStream_t st);
+cudaError_t ffma_launch_double_dmma_smem_integ(const FfmaArgs& a, int grid, size_t smem, cudaStream_t st);
+cudaError_t ffma_launch_double_dmma_gmem_integ(const FfmaArgs& a, int grid, size_t smem, cudaStream_t st);
+cudaError_t ffma_launch_double_dmma_smem_fixed(const FfmaArgs& a, int grid, size_t smem, cudaStream_t st);
+cudaError_t ffma_launch_double_dmma_gmem_fixed(const FfmaArgs& a, int grid, size_t smem, cudaStream_t st);
+cudaError_t ffma_launch_double_dmma_smem_func(const FfmaArgs& a, int grid, size_t smem, cudaStream_t st);
+cudaError_t ffma_launch_double_dmma_gmem_func(const FfmaArgs& a, int grid, size_t smem, cudaStream_t st);
 
 // integ: the instantiation that evaluates integral terms on node tiles; fixed: the one that also evaluates fixed networks;
-// func: the one that also evaluates a functional term
-cudaError_t ffma_launch(int dtype, bool bufs_smem, bool integ, bool fixed, bool func, const FfmaArgs& a, int grid,
-                        size_t smem, cudaStream_t st) {
+// func: the one that also evaluates a functional term; dmma: the fp64 one with its layer products on DMMA
+// (PINN_MODE_TC_F64; the planner admits it with PINN_F64 only)
+cudaError_t ffma_launch(int dtype, bool bufs_smem, bool integ, bool fixed, bool func, bool dmma, const FfmaArgs& a,
+                        int grid, size_t smem, cudaStream_t st) {
   const bool f64 = dtype == PINN_F64;
+  if (dmma) {
+    if (!f64) return cudaErrorInvalidValue;
+    if (func) return bufs_smem ? ffma_launch_double_dmma_smem_func(a, grid, smem, st) : ffma_launch_double_dmma_gmem_func(a, grid, smem, st);
+    if (fixed) return bufs_smem ? ffma_launch_double_dmma_smem_fixed(a, grid, smem, st) : ffma_launch_double_dmma_gmem_fixed(a, grid, smem, st);
+    if (integ) return bufs_smem ? ffma_launch_double_dmma_smem_integ(a, grid, smem, st) : ffma_launch_double_dmma_gmem_integ(a, grid, smem, st);
+    return bufs_smem ? ffma_launch_double_dmma_smem(a, grid, smem, st) : ffma_launch_double_dmma_gmem(a, grid, smem, st);
+  }
   if (func) {
     if (f64) return bufs_smem ? ffma_launch_double_smem_func(a, grid, smem, st) : ffma_launch_double_gmem_func(a, grid, smem, st);
     return bufs_smem ? ffma_launch_float_smem_func(a, grid, smem, st) : ffma_launch_float_gmem_func(a, grid, smem, st);

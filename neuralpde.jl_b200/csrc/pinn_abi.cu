@@ -15,8 +15,8 @@
 #include "engine.h"
 
 namespace pinn {
-cudaError_t ffma_launch(int dtype, bool bufs_smem, bool integ, bool fixed, bool func, const FfmaArgs& a, int grid,
-                        size_t smem, cudaStream_t st);
+cudaError_t ffma_launch(int dtype, bool bufs_smem, bool integ, bool fixed, bool func, bool dmma, const FfmaArgs& a,
+                        int grid, size_t smem, cudaStream_t st);
 cudaError_t grad_stats_launch(int dtype, const void* grad, long long n, double* out2, cudaStream_t st);
 cudaError_t sample_uniform_launch(int dtype, void* pts, long long n, int dim, const double* lb, const double* ub,
                                   unsigned long long seed, unsigned long long draw, const unsigned long long* draw_dev,
@@ -197,7 +197,7 @@ int pinn_create_ex2(const pinn_problem_desc* d, const pinn_integral_desc* integr
   const size_t n_partials = p.prob.func_term >= 0 ? 2 * g : g;
   TRY_OR_DESTROY(dev_alloc(&e->partial, n_partials * (size_t)e->partial_stride * e->es, e));
   TRY_OR_DESTROY(dev_alloc((void**)&e->term_sums, g * PINN_MAX_TERMS * sizeof(double), e));
-  if (e->mode == PINN_MODE_FFMA) {
+  if (ffma_kernel_mode(e->mode)) {
     TRY_OR_DESTROY(dev_alloc(&e->stash, g * (size_t)p.ffma.stash_per_cta * e->es, e));
     if (!p.bufs_smem) TRY_OR_DESTROY(dev_alloc(&e->gbufs, g * 2 * (size_t)p.ffma.buf_elems * e->es, e));
   } else {
@@ -372,14 +372,15 @@ static int prepare_scales(pinn_engine* e, const double* host_weights, double* se
 // in-kernel tail (gradient reduction / optimizer / peer allreduce) and makes the launch cooperative
 static int launch_fused(pinn_engine* e, const LaunchCall& c, int grid, cudaStream_t st) {
   const Plan& p = e->plan;
-  if (e->mode == PINN_MODE_FFMA) {
+  if (ffma_kernel_mode(e->mode)) {
     FfmaArgs a = with_call(p.ffma, e, c);
     a.n_tiles = e->total_tiles;
     for (int j = 0; j < p.prob.n_fixed; ++j)
       if (!e->fixed_ptr[j])
         return fail("pinn: fixed network %d has no parameters (call pinn_set_fixed_params or pinn_set_fixed_params_host "
                     "first)", j);
-    CUDA_TRY(ffma_launch(e->dtype, p.bufs_smem, p.integ, p.prob.n_fixed > 0, p.prob.func_term >= 0, a, grid, p.smem, st));
+    CUDA_TRY(ffma_launch(e->dtype, p.bufs_smem, p.integ, p.prob.n_fixed > 0, p.prob.func_term >= 0,
+                         e->mode == PINN_MODE_TC_F64, a, grid, p.smem, st));
     return 0;
   }
   if (p.wide) {

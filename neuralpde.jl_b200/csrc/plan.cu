@@ -294,7 +294,7 @@ int plan_term(const pinn_problem_desc* d, int t, const pinn_integral_desc* integ
     return fail("pinn_create: term %d unknown reduction %d", t, td.reduction);
   const bool func = td.reduction == PINN_REDUCE_ABS_OF_SUM || td.reduction == PINN_REDUCE_SQUARE_OF_SUM;
   if (func) {    // a functional term: g(scale * sum_p w_p v_p) (the kernel reads its nullable weights itself)
-    if (d->mode != PINN_MODE_FFMA)
+    if (!ffma_kernel_mode(d->mode))
       return fail("pinn_create: term %d is a functional term; functional terms run on the FFMA path (mode PINN_MODE_FFMA)", t);
     if (P.func_term >= 0)
       return fail("pinn_create: term %d is a second functional term (term %d is one); a problem has at most one", t,
@@ -654,19 +654,22 @@ int plan_problem(const pinn_problem_desc* d, const pinn_integral_desc* integrals
   if (n_fixed < 0 || n_fixed > PINN_MAX_FIXED_NETS)
     return fail("pinn_create_ex2: n_fixed=%d out of range [0,%d]", n_fixed, PINN_MAX_FIXED_NETS);
   if (n_fixed > 0 && !fixed) return fail("pinn_create_ex2: null fixed networks");
-  if (n_fixed > 0 && d->mode != PINN_MODE_FFMA)
+  if (n_fixed > 0 && !ffma_kernel_mode(d->mode))
     return fail("pinn_create_ex2: fixed networks run on the FFMA path (mode PINN_MODE_FFMA); the tensor-core modes do not "
                 "evaluate them");
   if (n_integrals < 0 || n_integrals > PINN_MAX_INTEGRALS)
     return fail("pinn_create_ex: n_integrals=%d out of range [0,%d]", n_integrals, PINN_MAX_INTEGRALS);
   if (n_integrals > 0 && !integrals) return fail("pinn_create_ex: null integrals");
-  if (n_integrals > 0 && d->mode != PINN_MODE_FFMA)
+  if (n_integrals > 0 && !ffma_kernel_mode(d->mode))
     return fail("pinn_create_ex: integral terms run on the FFMA path (mode PINN_MODE_FFMA); the tensor-core modes do not "
                 "evaluate them");
   if (d->abi_version != PINN_ABI_VERSION)
     return fail("pinn_create: descriptor abi_version %d, library %d", d->abi_version, PINN_ABI_VERSION);
   if (d->dtype != PINN_F32 && d->dtype != PINN_F64) return fail("pinn_create: unknown dtype %d", d->dtype);
-  if (d->mode < PINN_MODE_FFMA || d->mode > PINN_MODE_TC_SPLIT) return fail("pinn_create: unknown mode %d", d->mode);
+  if (d->mode < PINN_MODE_FFMA || d->mode > PINN_MODE_TC_F64) return fail("pinn_create: unknown mode %d", d->mode);
+  if (d->mode == PINN_MODE_TC_F64 && d->dtype != PINN_F64)
+    return fail("pinn_create: PINN_MODE_TC_F64 runs the layer products on the FP64 tensor cores and needs dtype PINN_F64 "
+                "(use PINN_MODE_FFMA, PINN_MODE_TC_BF16 or PINN_MODE_TC_SPLIT for PINN_F32)");
   if (d->n_nets < 1 || d->n_nets > PINN_MAX_NETS) return fail("pinn_create: n_nets=%d out of range [1,%d]", d->n_nets, PINN_MAX_NETS);
   if (d->n_terms < 1 || d->n_terms > PINN_MAX_TERMS)
     return fail("pinn_create: n_terms=%d out of range [1,%d]", d->n_terms, PINN_MAX_TERMS);
@@ -694,8 +697,8 @@ int plan_problem(const pinn_problem_desc* d, const pinn_integral_desc* integrals
     if (plan_integral(d, integrals, n_integrals, i, P, max_c, stash_max, &f)) return 1;
     p.term[integrals[i].owner].flops_per_point += f;
   }
-  p.tile_pts = d->mode == PINN_MODE_FFMA ? kTilePts : kTcPts;
-  if (d->mode == PINN_MODE_FFMA) return plan_ffma(d->dtype, max_w8, resident, max_c, stash_max, max_smem, p);
+  p.tile_pts = ffma_kernel_mode(d->mode) ? kTilePts : kTcPts;
+  if (ffma_kernel_mode(d->mode)) return plan_ffma(d->dtype, max_w8, resident, max_c, stash_max, max_smem, p);
   return plan_tc(d, max_smem, p);
 }
 }  // namespace pinn

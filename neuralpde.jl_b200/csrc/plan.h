@@ -28,6 +28,9 @@ struct Plan {
   FfmaArgs ffma; TcArgs tc; TwArgs tw; TwPackArgs pack;
 };
 
+// the modes that run ffma_loss_grad_kernel (CUDA-core FMA, or its DMMA instantiation for PINN_MODE_TC_F64)
+inline bool ffma_kernel_mode(int mode) { return mode == PINN_MODE_FFMA || mode == PINN_MODE_TC_F64; }
+
 // the q-point Gauss-Legendre rule on [-1, 1], nodes ascending
 void gauss_legendre(int q, double* x, double* w);
 

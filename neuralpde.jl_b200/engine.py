@@ -22,8 +22,9 @@ MAX_TERMS = 32
 
 F32, F64 = 0, 1
 # PINN_MODE_*: FFMA (any shape, fp32 / fp64), TC_BF16 (hidden widths up to 64, 64 / 128, or multiples of 64 up to 256),
-# TC_SPLIT (hidden widths up to 64); include/pinn_b200.h lists the shapes each tensor-core mode accepts
-MODE_FFMA, MODE_TC_BF16, MODE_TC_SPLIT = 0, 1, 2
+# TC_SPLIT (hidden widths up to 64), TC_F64 (FFMA's shapes, fp64 only, layer products on DMMA); include/pinn_b200.h lists
+# the shapes each tensor-core mode accepts
+MODE_FFMA, MODE_TC_BF16, MODE_TC_SPLIT, MODE_TC_F64 = 0, 1, 2, 3
 ACT = {"identity": 0, "tanh": 1, "sigmoid": 2, "sin": 3, "softplus": 4, "swish": 5}
 OP = {
     "const": 0, "coord": 1, "tap": 2, "param": 3, "add": 4, "sub": 5, "mul": 6, "div": 7, "neg": 8,

@@ -22,6 +22,11 @@ from .strategies import (AbstractTrainingStrategy, GridTraining, QuadratureTrain
                          generate_random_points, generate_training_sets, get_bounds, shard_range)
 from .symbolic import Equation, FixedNet, PDESystem, VarInfo, eq_indvars, fixed_function, get_vars
 
+# PhysicsInformedNN(mode=...) -> PINN_MODE_*; "ffma" and "tc_f64" run the FFMA kernel (integral terms, fixed networks and
+# functional terms evaluate there only)
+MODES = {"ffma": _eng.MODE_FFMA, "tc_bf16": _eng.MODE_TC_BF16, "tc_split": _eng.MODE_TC_SPLIT, "tc_f64": _eng.MODE_TC_F64}
+FFMA_KERNEL_MODES = (_eng.MODE_FFMA, _eng.MODE_TC_F64)
+
 _ACT_NAMES = {"identity": "identity", "tanh": "tanh", "sigmoid": "sigmoid", "σ": "sigmoid", "sin": "sin",
               "softplus": "softplus", "swish": "swish", None: "identity"}
 
@@ -412,9 +417,11 @@ class PhysicsInformedNN(AbstractPINN):
     additional_loss, adaptive_loss, logger, log_options, iteration)``
     (reference src/pinn_types.jl:165-211).  ``chain``: one Chain, or a list with one
     1-output Chain per dependent variable.  Engine options arrive as extra keywords:
-    ``mode`` ("ffma" | "tc_bf16" | "tc_split"), ``device``.  The tensor-core modes need float32 and 1-output networks
-    with a linear last layer; "tc_split" takes hidden widths 16 / 32 / 48 / 64, "tc_bf16" also 64 / 128 and any multiple
-    of 64 up to 256 (include/pinn_b200.h lists the shapes; anything else is refused with a message)."""
+    ``mode`` ("ffma" | "tc_bf16" | "tc_split" | "tc_f64"), ``device``.  The bf16 tensor-core modes need float32 and
+    1-output networks with a linear last layer; "tc_split" takes hidden widths 16 / 32 / 48 / 64, "tc_bf16" also 64 / 128
+    and any multiple of 64 up to 256 (include/pinn_b200.h lists the shapes; anything else is refused with a message).
+    "tc_f64" needs float64 and takes everything "ffma" takes: the same kernel with its layer products on the FP64 tensor
+    cores."""
     chain: Union[Chain, List[Chain]]
     strategy: AbstractTrainingStrategy
     init_params: Optional[np.ndarray] = None
@@ -625,6 +632,9 @@ def symbolic_discretize(pde_system: PDESystem, discretization: PhysicsInformedNN
             raise ValueError("init_params has length %d, the chains%s need %d"
                              % (flat.size, " + p" if n_p else "", n_net + n_p))
     dtype = flat.dtype
+    if d.mode == "tc_f64" and dtype != np.float64:
+        raise ValueError("mode=\"tc_f64\" runs the layer products on the FP64 tensor cores and needs float64 parameters "
+                         "(init_params is %s); use mode=\"ffma\", \"tc_bf16\" or \"tc_split\" for float32" % dtype.name)
     offs, o = [], 0
     for c in chains:
         offs.append(o)
@@ -652,7 +662,7 @@ def symbolic_discretize(pde_system: PDESystem, discretization: PhysicsInformedNN
             if bayes:
                 raise ValueError("BayesianPINN: an IntegralLoss has no log-likelihood form (the reference adds "
                                  "additional_loss values as one observation); use PhysicsInformedNN")
-            if d.mode != "ffma":
+            if d.mode not in ("ffma", "tc_f64"):
                 raise ValueError("IntegralLoss: functional terms run on the FFMA path: use mode=\"ffma\"")
             func_spec, func_pts, func_w = _integral_loss_term(add, vi, param_index, param_values, fixed)
     except LoweringError as ex:
@@ -724,8 +734,8 @@ def symbolic_discretize(pde_system: PDESystem, discretization: PhysicsInformedNN
         raise ValueError("the system has %d integral terms (max %d)" % (len(integrals), _eng.MAX_INTEGRALS))
 
     nets = [NetSpec(c.dims, c.acts, off) for c, off in zip(chains, offs)]
-    mode = {"ffma": _eng.MODE_FFMA, "tc_bf16": _eng.MODE_TC_BF16, "tc_split": _eng.MODE_TC_SPLIT}[d.mode]
-    if fixed and mode != _eng.MODE_FFMA:
+    mode = MODES[d.mode]
+    if fixed and mode not in FFMA_KERNEL_MODES:
         raise ValueError("registered network functions run on the FFMA path: use mode=\"ffma\"")
     spec = ProblemSpec(nets=nets, terms=specs, n_params=n_p, param_offset=n_net, n_theta=n_net + n_p,
                        dtype=dtype.name, mode=mode, device=d.device, integrals=integrals, fixed=_fixed_specs(fixed))
