@@ -12,7 +12,7 @@ from .symbolic import (ClosedInterval, Differential, Eq, Equation, In, Inf, Inte
                        parameters, variables)
 from .lowering import LoweringError, lower_equation
 from .strategies import (AbstractTrainingStrategy, GridTraining, QuadratureTraining, QuasiRandomTraining,
-                         StochasticTraining, generate_training_sets, get_bounds, shard_range)
+                         StochasticTraining, WeightedIntervalTraining, generate_training_sets, get_bounds, shard_range)
 from .pinn import (AbstractPINN, Adam, BPINNsolution, BPINNstats, DiagEuclideanMetric, HMC, Leapfrog, LogNormal,
                    NoAdaptation, Normal, Uniform,
                    StanHMCAdaptor, UnitEuclideanMetric, ahmc_bayesian_pinn_pde, pmean, BFGS, BackTracking, BayesianPINN, Chain, DataLoss, Dense, IntegralLoss, Descent, GradientScaleAdaptiveLoss, HagerZhang, LBFGS, LogOptions, MiniMaxAdaptiveLoss,
@@ -20,5 +20,6 @@ from .pinn import (AbstractPINN, Adam, BPINNsolution, BPINNstats, DiagEuclideanM
                    OptimizationFunction, OptimizationProblem, Phi, PhysicsInformedNN, PINNRepresentation, Solution,
                    discretize, initialparameters, logscalar, logvector, register_symbolic, solve, symbolic_discretize)
 from .adapter import NeuralAdapterLoss, neural_adapter
+from .ode import NNODE, NNODERepresentation, ODEFunction, ODEProblem, ODESolution
 
 __all__ = [n for n in dir() if not n.startswith("_")]

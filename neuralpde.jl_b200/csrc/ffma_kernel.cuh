@@ -73,9 +73,33 @@ __device__ __forceinline__ real m_sigmoid(real z) {
   return e / (real(1) + e);
 }
 
-// activation value and its first four derivatives at z (the fourth enters the reverse sweep through third-derivative taps)
+// NNlib's gelu, the tanh form z/2 (1 + T), T = tanh(u), u = c (z + k z^3), and its first four derivatives: T's
+// z-derivatives by Faa di Bruno from tanh's u-derivatives t1..t4 and u1 = c (1 + 3k z^2), u2 = 6ck z, u3 = 6ck (u4 = 0)
 template <typename real>
+__device__ __forceinline__ void gelu_eval4(real z, real& a, real& d1, real& d2, real& d3, real& d4) {
+  const real c = real(0.79788456080286535588), k = real(0.044715);
+  const real z2 = z * z;
+  real t = m_tanh(c * (z + k * z2 * z));
+  real t1 = real(1) - t * t, t2 = real(-2) * t * t1, t3 = t1 * (real(6) * t * t - real(2));
+  real t4 = real(8) * t * t1 * (real(2) - real(3) * t * t);
+  real u1 = c * (real(1) + real(3) * k * z2), u2 = real(6) * c * k * z, u3 = real(6) * c * k;
+  real T1 = t1 * u1, T2 = t2 * u1 * u1 + t1 * u2;
+  real T3 = t3 * u1 * u1 * u1 + real(3) * t2 * u1 * u2 + t1 * u3;
+  real T4 = t4 * u1 * u1 * u1 * u1 + real(6) * t3 * u1 * u1 * u2 + t2 * (real(3) * u2 * u2 + real(4) * u1 * u3);
+  a = real(0.5) * z * (real(1) + t);
+  d1 = real(0.5) * (real(1) + t + z * T1);
+  d2 = real(0.5) * (real(2) * T1 + z * T2);
+  d3 = real(0.5) * (real(3) * T2 + z * T3);
+  d4 = real(0.5) * (real(4) * T3 + z * T4);
+}
+
+// activation value and its first four derivatives at z (the fourth enters the reverse sweep through third-derivative taps).
+// kGelu = false (the tensor-core kernels, which refuse gelu layers) leaves gelu out, so their code stays as it was
+template <typename real, bool kGelu = true>
 __device__ __forceinline__ void act_eval4(int act, real z, real& a, real& d1, real& d2, real& d3, real& d4) {
+  if constexpr (kGelu) {
+    if (act == PINN_ACT_GELU) { gelu_eval4<real>(z, a, d1, d2, d3, d4); return; }
+  }
   switch (act) {
     case PINN_ACT_TANH: {
       real t = m_tanh(z);
@@ -116,10 +140,10 @@ __device__ __forceinline__ void act_eval4(int act, real z, real& a, real& d1, re
       a = z; d1 = real(1); d2 = real(0); d3 = real(0); d4 = real(0);
   }
 }
-template <typename real>
+template <typename real, bool kGelu = true>
 __device__ __forceinline__ void act_eval(int act, real z, real& a, real& d1, real& d2, real& d3) {
   real d4;
-  act_eval4<real>(act, z, a, d1, d2, d3, d4);
+  act_eval4<real, kGelu>(act, z, a, d1, d2, d3, d4);
 }
 
 template <typename real> struct Cfg {

@@ -35,7 +35,7 @@ __device__ __forceinline__ void add_at(float* v, int idx, float x) {
 
 // activation value and first three derivatives.  AK = 1: tanh, 2: sigmoid (branch-free, built on
 // ex2.approx + rcp.approx: absolute error ~1e-7, far below the bf16-split operand noise);
-// AK = 0: any activation through the accurate generic evaluator.
+// AK = 0: any activation through the accurate generic evaluator (gelu excepted: check_tc_nets refuses it).
 template <int AK>
 __device__ __forceinline__ void act_eval_tc(int act, float z, float& a, float& d1, float& d2, float& d3) {
   if (AK == 1) {
@@ -48,7 +48,7 @@ __device__ __forceinline__ void act_eval_tc(int act, float z, float& a, float& d
     const float g1 = g * (1.f - g);
     a = g; d1 = g1; d2 = g1 * fmaf(-2.f, g, 1.f); d3 = g1 * fmaf(-6.f, g1, 1.f);
   } else {
-    act_eval<float>(act, z, a, d1, d2, d3);
+    act_eval<float, false>(act, z, a, d1, d2, d3);
   }
 }
 __device__ __forceinline__ int act_kind(int act) { return act == PINN_ACT_TANH ? 1 : (act == PINN_ACT_SIGMOID ? 2 : 0); }

@@ -28,7 +28,7 @@ MODES = {"ffma": _eng.MODE_FFMA, "tc_bf16": _eng.MODE_TC_BF16, "tc_split": _eng.
 FFMA_KERNEL_MODES = (_eng.MODE_FFMA, _eng.MODE_TC_F64)
 
 _ACT_NAMES = {"identity": "identity", "tanh": "tanh", "sigmoid": "sigmoid", "σ": "sigmoid", "sin": "sin",
-              "softplus": "softplus", "swish": "swish", None: "identity"}
+              "softplus": "softplus", "swish": "swish", "gelu": "gelu", None: "identity"}
 
 
 # ---- Lux stand-ins -----------------------------------------------------------------------------
@@ -1096,31 +1096,21 @@ _DEVICE_LOOP_SETS = ("point sets that live on the device: Grid, Quadrature, non-
                      "StochasticTraining(..., device_sampler=True)")
 
 
-def _solve_quasi_newton(prob: OptimizationProblem, opt, maxiters: int, callback: Optional[Callable]) -> Solution:
-    """BFGS / L-BFGS with theta, the gradient and the curvature history on the device (pinn_qn_*); the line search runs
-    on the host with one 16-byte read-back per evaluation."""
-    rep = prob.representation
-    if _host_resampled(rep):
-        raise ValueError("BFGS / LBFGS need " + _DEVICE_LOOP_SETS)
-    if not isinstance(rep.adaloss, NonAdaptiveLoss):
-        raise ValueError("BFGS / LBFGS need fixed loss weights (NonAdaptiveLoss): an adaptive loss would change the "
-                         "objective between the line search's trial points")
-    ls = opt.linesearch
+def _linesearch_kind(ls) -> int:
     if isinstance(ls, HagerZhang) and ls == HagerZhang():
-        ls_kind = _eng.LS_HAGERZHANG
-    elif isinstance(ls, BackTracking) and ls == BackTracking():
-        ls_kind = _eng.LS_BACKTRACKING
-    else:
-        raise ValueError("linesearch must be HagerZhang() or BackTracking() with their default parameters, got %r" % (ls,))
-    if isinstance(rep.strategy, QuasiRandomTraining) and not rep.strategy.device_sampler:
-        rep.resample()                               # non-resampled QuasiRandom places its points at the first loss call
-    eng = rep.engine
-    w = rep.weights
-    term_w = np.concatenate([w["pde"], w["bc"]] + ([w["add"]] if rep.additional_loss is not None else []))
+        return _eng.LS_HAGERZHANG
+    if isinstance(ls, BackTracking) and ls == BackTracking():
+        return _eng.LS_BACKTRACKING
+    raise ValueError("linesearch must be HagerZhang() or BackTracking() with their default parameters, got %r" % (ls,))
+
+
+def _qn_run(eng: Engine, u0: np.ndarray, opt, ls_kind: int, maxiters: int, callback: Optional[Callable], term_w):
+    """The device quasi-Newton run from u0: one ``maxiters`` call without a callback, one iteration per call with one.
+    Returns (θ, objective, iterations, evaluations, retcode)."""
     if isinstance(opt, LBFGS):
-        eng.qn_begin(prob.u0, _eng.QN_LBFGS, m=opt.m, linesearch=ls_kind, weights=term_w)
+        eng.qn_begin(u0, _eng.QN_LBFGS, m=opt.m, linesearch=ls_kind, weights=term_w)
     else:
-        eng.qn_begin(prob.u0, _eng.QN_BFGS, linesearch=ls_kind, initial_stepnorm=opt.initial_stepnorm, weights=term_w)
+        eng.qn_begin(u0, _eng.QN_BFGS, linesearch=ls_kind, initial_stepnorm=opt.initial_stepnorm, weights=term_w)
     f, _, status, iters, evals = eng.qn_iterate(0)
     retcode = None
     if callback is None:
@@ -1131,14 +1121,39 @@ def _solve_quasi_newton(prob: OptimizationProblem, opt, maxiters: int, callback:
             if callback({"iter": iters, "u": eng.qn_theta()}, f):
                 retcode = "Terminated"
                 break
-    rep.iteration[0] += evals                        # one loss call per evaluation, as the reference counts them
     if retcode is None:
         retcode = {_eng.QN_CONVERGED: "Success", _eng.QN_LS_FAILED: "Failure"}.get(status, "MaxIters")
-    return Solution(eng.qn_theta().astype(prob.u0.dtype), f, iters, retcode)
+    return eng.qn_theta(), f, iters, evals, retcode
 
 
-def solve(prob: OptimizationProblem, opt: Union[Adam, LBFGS, BFGS], maxiters: int = 100, callback: Optional[Callable] = None,
-          device_loop: bool = False, chunk: int = 50) -> Solution:
+def _solve_quasi_newton(prob: OptimizationProblem, opt, maxiters: int, callback: Optional[Callable]) -> Solution:
+    """BFGS / L-BFGS with theta, the gradient and the curvature history on the device (pinn_qn_*); the line search runs
+    on the host with one 16-byte read-back per evaluation."""
+    rep = prob.representation
+    if _host_resampled(rep):
+        raise ValueError("BFGS / LBFGS need " + _DEVICE_LOOP_SETS)
+    if not isinstance(rep.adaloss, NonAdaptiveLoss):
+        raise ValueError("BFGS / LBFGS need fixed loss weights (NonAdaptiveLoss): an adaptive loss would change the "
+                         "objective between the line search's trial points")
+    ls_kind = _linesearch_kind(opt.linesearch)
+    if isinstance(rep.strategy, QuasiRandomTraining) and not rep.strategy.device_sampler:
+        rep.resample()                               # non-resampled QuasiRandom places its points at the first loss call
+    w = rep.weights
+    term_w = np.concatenate([w["pde"], w["bc"]] + ([w["add"]] if rep.additional_loss is not None else []))
+    theta, f, iters, evals, retcode = _qn_run(rep.engine, prob.u0, opt, ls_kind, maxiters, callback, term_w)
+    rep.iteration[0] += evals                        # one loss call per evaluation, as the reference counts them
+    return Solution(theta.astype(prob.u0.dtype), f, iters, retcode)
+
+
+class _DefaultMaxiters(int):
+    """``solve``'s default ``maxiters`` (100 for an OptimizationProblem); an ODEProblem needs it given"""
+
+
+_MAXITERS_DEFAULT = _DefaultMaxiters(100)
+
+
+def solve(prob: OptimizationProblem, opt: Union[Adam, LBFGS, BFGS], maxiters: int = _MAXITERS_DEFAULT, callback: Optional[Callable] = None,
+          device_loop: bool = False, chunk: int = 50, **ode_kwargs) -> Solution:
     """Minimal stand-in for ``Optimization.solve(prob, opt; maxiters, callback)``.
 
     ``LBFGS()`` / ``BFGS()``: the device-resident quasi-Newton driver (pinn_qn_*), whatever ``device_loop`` says; one
@@ -1149,7 +1164,19 @@ def solve(prob: OptimizationProblem, opt: Union[Adam, LBFGS, BFGS], maxiters: in
     Default: a host Adam loop that calls the engine's loss+gradient once per iteration.
     ``device_loop=True`` (fixed point sets, or StochasticTraining with the device-side sampler, which then draws fresh
     points before every step): theta, m, v stay on the device and the Adam update is fused into the gradient reduction
-    (pinn_adam_iterate); the callback sees the loss every `chunk` steps."""
+    (pinn_adam_iterate); the callback sees the loss every `chunk` steps.
+
+    ``solve(prob::ODEProblem, alg::NNODE; maxiters, dt, abstol, saveat, ...)`` trains an NNODE (ode.py) and takes the
+    keywords of ``ode.solve``."""
+    from .ode import ODEProblem, solve_nnode
+    if isinstance(prob, ODEProblem):
+        if callback is not None or chunk != 50:
+            raise TypeError("solve(::ODEProblem, ::NNODE) takes no callback or chunk: it stops at abstol")
+        if maxiters is _MAXITERS_DEFAULT:
+            raise TypeError("solve(::ODEProblem, ::NNODE) needs maxiters")
+        return solve_nnode(prob, opt, maxiters=maxiters, device_loop=device_loop, **ode_kwargs)
+    if ode_kwargs:
+        raise TypeError("solve() got unexpected keyword arguments %s" % sorted(ode_kwargs))
     if isinstance(opt, (LBFGS, BFGS)):
         return _solve_quasi_newton(prob, opt, maxiters, callback)
     rep = prob.representation

@@ -60,6 +60,24 @@ class QuasiRandomTraining(AbstractTrainingStrategy):
 
 
 @dataclass
+class WeightedIntervalTraining(AbstractTrainingStrategy):
+    """``WeightedIntervalTraining(weights, points)`` (training_strategies.jl, NNODE only): the time span is cut into
+    ``len(weights)`` equal sub-intervals and sub-interval i gets ``trunc(points * w_i)`` uniform points, w normalised
+    to sum 1.  The points are drawn once (src/ode_solve.jl:297-316).  ``seed`` fixes the draw (the reference uses the
+    global RNG)."""
+    weights: Sequence[float]
+    points: int
+    seed: int = 0
+
+    def sample(self, t0: float, t1: float) -> np.ndarray:
+        w = np.asarray(self.weights, dtype=np.float64)
+        w = w / w.sum()
+        h = (t1 - t0) / w.size
+        rng = np.random.default_rng(self.seed)
+        return np.concatenate([rng.random(int(self.points * wi)) * h + t0 + i * h for i, wi in enumerate(w)])
+
+
+@dataclass
 class QuadratureTraining(AbstractTrainingStrategy):
     """Fixed-node tensor Gauss-Legendre quadrature of ``r^2`` over the domain:
     ``loss = sum_i w_i r(x_i)^2 / area``.
