@@ -399,7 +399,7 @@ int pinn_qn_theta(pinn_handle h, void* host_theta_out);
  * engine dtypes; the fused kernel sees theta rounded to the engine dtype.  One transition is a fixed launch sequence with
  * no host decision, captured once into a CUDA graph (PINN_B200_NO_GRAPH=1: enqueued directly).  Random numbers are
  * Philox4x32-10 draws keyed by (seed, transition, index, stream), so two runs with one seed are bit-identical.
- * Single-GPU handles with fixed point sets only (no device sampler, nranks == 1). */
+ * Single-GPU handles (nranks == 1) with fixed point sets only, unless pinn_hmc_begin_ex2 asks for PINN_HMC_REDRAW. */
 enum { PINN_HMC_ADAPT_NONE = 0, PINN_HMC_ADAPT_STAN = 1 };
 enum { PINN_HMC_METRIC_UNIT = 0, PINN_HMC_METRIC_DIAG = 1 };
 /* columns of one statistics row of pinn_hmc_iterate */
@@ -437,6 +437,19 @@ typedef struct {
  * pinn_hmc_begin.  theta0's tail must lie in the priors' supports. */
 int pinn_hmc_begin_ex(pinn_handle h, const double* host_theta0, const pinn_hmc_options* opts, const double* host_weights,
                       double ll_const, const pinn_hmc_prior* tail, int32_t n_tail, double* step_size_out);
+/* pinn_hmc_begin_ex with two additions (tail_logabs = NULL and flags = 0 is pinn_hmc_begin_ex):
+ * - tail_logabs[n_tail] (nullable, finite): l gains sum_j tail_logabs[j] * log|theta_tail_j| and its gradient
+ *   tail_logabs[j] / theta_tail_j -- the normalisation -n log|sigma(p)| of a Gaussian likelihood whose sigma is a
+ *   monomial in theta.p.  Where such an entry is 0 the value is not finite: the proposal is rejected (numerical_error = 1).
+ * - PINN_HMC_REDRAW: the handle's device samplers (pinn_set_sampler*) draw fresh points before every evaluation of the
+ *   chain -- theta0, every find_good_stepsize trial, every leapfrog step.  Evaluation j since this call (j = 0 at
+ *   theta0) uses draw index j (the sampler's draw argument 0 plus j), counted on the device, whether or not a trajectory
+ *   has stopped early.  Without the flag a handle with a device sampler is refused.  A rejected proposal returns to the
+ *   previous state with its cached log density and gradient. */
+enum { PINN_HMC_REDRAW = 1u };
+int pinn_hmc_begin_ex2(pinn_handle h, const double* host_theta0, const pinn_hmc_options* opts, const double* host_weights,
+                       double ll_const, const pinn_hmc_prior* tail, int32_t n_tail, const double* tail_logabs,
+                       uint32_t flags, double* step_size_out);
 /* Run n transitions: host_samples [n][n_theta] float64 (theta after each transition) and host_stats
  * [n][PINN_HMC_N_STATS] (each nullable).  The chain continues across calls. */
 int pinn_hmc_iterate(pinn_handle h, int32_t n, double* host_samples, double* host_stats);

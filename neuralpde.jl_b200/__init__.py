@@ -21,5 +21,6 @@ from .pinn import (AbstractPINN, Adam, BPINNsolution, BPINNstats, DiagEuclideanM
                    discretize, initialparameters, logscalar, logvector, register_symbolic, solve, symbolic_discretize)
 from .adapter import NeuralAdapterLoss, neural_adapter
 from .ode import NNODE, NNODERepresentation, ODEFunction, ODEProblem, ODESolution
+from .bpinn_ode import BNNODE, BNNODELogDensity, ahmc_bayesian_pinn_ode
 
 __all__ = [n for n in dir() if not n.startswith("_")]

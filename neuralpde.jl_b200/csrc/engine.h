@@ -104,6 +104,8 @@ bool any_sampler(const pinn_engine* e);
 // One evaluation of the hot path on stream st (fused kernel + tail, plus the allreduce steps of the NCCL fallback).
 int eval_step(pinn_engine* e, const void* theta, const double* host_weights, void* out_grad, void* out_terms,
               void* out_total, bool adam, cudaStream_t st);
+// fresh points of a device-sampled term: draw index draw + *draw_dev (draw_dev nullable)
+int draw_term(pinn_engine* e, int term, unsigned long long draw, const unsigned long long* draw_dev, cudaStream_t st);
 // frees the quasi-Newton state (qn.cu); called by pinn_destroy and by a repeated pinn_qn_begin
 void qn_release(pinn_engine* e);
 // frees the HMC sampler state and its graph (hmc.cu); called by pinn_destroy and by a repeated pinn_hmc_begin

@@ -4,11 +4,15 @@
 // window statistics are float64 on the device for both engine dtypes; every evaluation is the fused kernel (eval_step) at
 // theta rounded to the engine dtype, weighted by the fixed log-likelihood weights.  The prior's value and gradient are
 // added here: N(mean, std^2) on the first n - n_tail entries and, for parameter estimation, one Normal / LogNormal /
-// Uniform prior per entry of the last n_tail (theta.p).  A tail entry outside its prior's support has a NaN gradient, so
-// the trajectory stops there like at any other non-finite value.  One transition is a fixed launch sequence that the
-// host never inspects:
+// Uniform prior per entry of the last n_tail (theta.p), plus c_j log|theta.p_j| where a chain has tail_logabs (the
+// normalisation of a noise that depends on theta.p).  A tail entry outside its prior's support, or at 0 under a c_j != 0,
+// has a non-finite gradient, so the trajectory stops there like at any other non-finite value.  One transition is a fixed
+// launch sequence that the host never inspects:
 //
-//   momentum | L x (kick / drift, fused evaluation) | closing kick + energy partials | accept (1 block) | select
+//   momentum | L x (kick / drift, [samplers,] fused evaluation) | closing kick + energy partials | accept (1 block) | select
+//
+// With PINN_HMC_REDRAW the device samplers draw fresh points before every evaluation: draw index = the number of
+// evaluations since pinn_hmc_begin (S->draws, advanced by every kick / drift launch, stopped trajectory or not).
 //
 // so it is captured once into a CUDA graph and replayed.  Decisions (accept, step size, window ends) are made on the
 // device by the single-block accept kernel; after a non-finite value the remaining kick / drift kernels are no-ops.
@@ -52,6 +56,7 @@ struct HmcScal {
   long long win_n;               // Welford count of the current window
   long long win_n_cur;           // ... after the current transition's push (read by the select kernel)
   long long win_size, next_split;   // Stan windows: size of the current window, its last transition (-1: none left)
+  unsigned long long draws;      // evaluations since begin: the draw index of the next sampler launch
   int flag;                      // non-finite value in the current trajectory
   int accept, push, win_end;     // the current transition's decision, Welford push and window end
 };
@@ -69,6 +74,7 @@ struct HmcArgs {
   double prior_mean, inv_var;    // prior N(mean, 1 / inv_var) of theta[0, n - n_tail)
   int n_tail;                    // tail[j] is the prior of theta[n - n_tail + j]
   pinn_hmc_prior tail[PINN_MAX_PARAMS];
+  double tail_c[PINN_MAX_PARAMS];   // c_j of the c_j log|theta.p_j| terms (0: none)
   double lp_const;               // ll_const + the prior's normalisation
   double delta;                  // target acceptance
   int adapt, diag, n_adapts;
@@ -124,6 +130,7 @@ __device__ __forceinline__ double prior_grad(const HmcArgs& a, double th) { retu
 __device__ __forceinline__ double grad_at(const HmcArgs& a, long long i, double th, double g_phys) {
   const long long j = i - (a.n - a.n_tail);
   if (j < 0) return g_phys + prior_grad(a, th);
+  if (a.tail_c[j] != 0.0) return g_phys + (tail_grad(a.tail[j], th) + a.tail_c[j] / th);
   return g_phys + tail_grad(a.tail[j], th);
 }
 
@@ -153,6 +160,7 @@ __global__ void __launch_bounds__(kHmcThreads) hmc_momentum_kernel(HmcArgs a, bo
 template <typename real>
 __global__ void __launch_bounds__(kHmcThreads) hmc_kick_drift_kernel(HmcArgs a, bool first, const double* eps) {
   const long long i = (long long)blockIdx.x * kHmcThreads + threadIdx.x;
+  if (i == 0) a.S->draws += 1;   // the evaluation after this launch, whether or not the trajectory has stopped
   if (i >= a.n || a.S->flag) return;
   const double e = *eps, h = 0.5 * e;
   double th = a.theta[i], ri = a.r[i], gi;
@@ -223,7 +231,11 @@ __global__ void __launch_bounds__(kHmcThreads) hmc_accept_kernel(HmcArgs a, int 
   if (threadIdx.x) return;
   HmcScal& S = *a.S;
   double logp1 = (double)*(const real*)a.total + a.lp_const - 0.5 * pp * a.inv_var;
-  for (int j = 0; j < a.n_tail; ++j) logp1 += tail_logpdf(a.tail[j], a.theta[a.n - a.n_tail + j]);
+  for (int j = 0; j < a.n_tail; ++j) {
+    const double x = a.theta[a.n - a.n_tail + j];
+    logp1 += tail_logpdf(a.tail[j], x);
+    if (a.tail_c[j] != 0.0) logp1 += a.tail_c[j] * log(fabs(x));
+  }
   if (mode == kInit) { S.logp = logp1; return; }
   const double h0 = -S.logp + k0;
   double h1 = -logp1 + k1;
@@ -334,6 +346,7 @@ struct HmcState {
   long long t = 0;               // transitions done (host copy)
   cudaGraphExec_t graph = nullptr;
   unsigned long long graph_key = 0;
+  bool redraw = false;           // PINN_HMC_REDRAW: the device samplers draw before every evaluation
 };
 
 void hmc_release(pinn_engine* e) {
@@ -376,9 +389,12 @@ int launch_check(pinn_engine* e, int count) {
   return 0;
 }
 
-// evaluate the weighted physics log-likelihood and its gradient at theta_r
+// evaluate the weighted physics log-likelihood and its gradient at theta_r (redraw: on fresh points of draw S->draws)
 int evaluate(pinn_engine* e, HmcState* s, cudaStream_t st) {
   const HmcArgs& a = s->a;
+  if (s->redraw)
+    for (int t = 0; t < e->n_terms; ++t)
+      if (e->term[t].sampler_on && draw_term(e, t, 0, &a.S->draws, st)) return 1;
   char* out = (char*)a.total - (size_t)e->n_terms * e->es;
   return eval_step(e, a.theta_r, s->w, (void*)a.g_r, out, (void*)a.total, false, st);
 }
@@ -473,7 +489,10 @@ unsigned long long fnv1a(const void* p, size_t n, unsigned long long h) {
 }
 
 long long launches_per_transition(const pinn_engine* e, const HmcState* s) {
-  return 4 + (long long)s->opt.n_leapfrog * (2 + (e->plan.wide ? 1 : 0));
+  long long per_step = 2 + (e->plan.wide ? 1 : 0);
+  if (s->redraw)
+    for (int t = 0; t < e->n_terms; ++t) per_step += e->term[t].sampler_on ? 1 : 0;
+  return 4 + (long long)s->opt.n_leapfrog * per_step;
 }
 
 }  // namespace
@@ -482,7 +501,8 @@ long long launches_per_transition(const pinn_engine* e, const HmcState* s) {
 using namespace pinn;
 
 static int hmc_start(pinn_handle e, const double* host_theta0, const pinn_hmc_options* opts, const double* host_weights,
-                     double ll_const, const pinn_hmc_prior* tail, int32_t n_tail, double* step_size_out) {
+                     double ll_const, const pinn_hmc_prior* tail, int32_t n_tail, const double* tail_logabs,
+                     uint32_t flags, double* step_size_out) {
   if (!host_theta0 || !opts) return fail("pinn_hmc_begin: null theta / options");
   if (n_tail < 0 || n_tail > PINN_MAX_PARAMS || (long long)n_tail >= e->n_theta)
     return fail("pinn_hmc_begin: n_tail = %d must lie in [0, min(%d, n_theta = %lld - 1)]", n_tail, PINN_MAX_PARAMS,
@@ -499,8 +519,13 @@ static int hmc_start(pinn_handle e, const double* host_theta0, const pinn_hmc_op
     if (p.kind != PINN_HMC_PRIOR_UNIFORM && !(p.b > 0.0))
       return fail("pinn_hmc_begin: tail prior %d has sigma %g: must be positive", j, p.b);
   }
+  if (tail_logabs && n_tail == 0) return fail("pinn_hmc_begin: tail_logabs needs n_tail >= 1");
+  for (int j = 0; tail_logabs && j < n_tail; ++j)
+    if (!isfinite(tail_logabs[j])) return fail("pinn_hmc_begin: tail_logabs[%d] = %g is not finite", j, tail_logabs[j]);
+  if (flags & ~(uint32_t)PINN_HMC_REDRAW) return fail("pinn_hmc_begin: unknown flags 0x%x", flags);
   if (e->nranks > 1) return fail("pinn_hmc_begin: the sampler runs one chain on one GPU (communicator with %d ranks)", e->nranks);
-  if (any_sampler(e))
+  const bool redraw = (flags & PINN_HMC_REDRAW) != 0;
+  if (any_sampler(e) && !redraw)
     return fail("pinn_hmc_begin: HMC needs a fixed log density; a device sampler redraws the points (use fixed point sets)");
   if (opts->n_leapfrog < 1) return fail("pinn_hmc_begin: n_leapfrog = %d must be >= 1", opts->n_leapfrog);
   if (opts->adaptor != PINN_HMC_ADAPT_NONE && opts->adaptor != PINN_HMC_ADAPT_STAN)
@@ -519,6 +544,7 @@ static int hmc_start(pinn_handle e, const double* host_theta0, const pinn_hmc_op
   HmcState* s = new HmcState();
   e->hmc = s;
   s->opt = *opts;
+  s->redraw = redraw;
   for (int k = 0; k < e->n_terms; ++k) s->w[k] = host_weights ? host_weights[k] : 1.0;
   const long long n = e->n_theta;
   HmcArgs& a = s->a;
@@ -537,7 +563,10 @@ static int hmc_start(pinn_handle e, const double* host_theta0, const pinn_hmc_op
   a.prior_mean = opts->prior_mean;
   a.inv_var = 1.0 / (opts->prior_std * opts->prior_std);
   a.n_tail = n_tail;
-  for (int j = 0; j < n_tail; ++j) a.tail[j] = tail[j];
+  for (int j = 0; j < n_tail; ++j) {
+    a.tail[j] = tail[j];
+    a.tail_c[j] = tail_logabs ? tail_logabs[j] : 0.0;
+  }
   const long long n_net = n - n_tail;
   a.lp_const = ll_const - 0.5 * (double)n_net * log(2.0 * M_PI) - (double)n_net * log(opts->prior_std);
   a.delta = opts->target_accept;
@@ -584,17 +613,23 @@ static int hmc_start(pinn_handle e, const double* host_theta0, const pinn_hmc_op
 
 extern "C" {
 
-int pinn_hmc_begin_ex(pinn_handle e, const double* host_theta0, const pinn_hmc_options* opts, const double* host_weights,
-                      double ll_const, const pinn_hmc_prior* tail, int32_t n_tail, double* step_size_out) {
+int pinn_hmc_begin_ex2(pinn_handle e, const double* host_theta0, const pinn_hmc_options* opts, const double* host_weights,
+                       double ll_const, const pinn_hmc_prior* tail, int32_t n_tail, const double* tail_logabs,
+                       uint32_t flags, double* step_size_out) {
   if (!e) return fail("pinn_hmc_begin: null handle");
   if (e->plan.prob.func_term >= 0)
     return fail("pinn_hmc_begin: term %d is a functional term (an integral constraint); the log density of the sampler is "
                 "built from mean-square terms only", e->plan.prob.func_term);
-  if (hmc_start(e, host_theta0, opts, host_weights, ll_const, tail, n_tail, step_size_out)) {
+  if (hmc_start(e, host_theta0, opts, host_weights, ll_const, tail, n_tail, tail_logabs, flags, step_size_out)) {
     hmc_release(e);              // a failed start leaves no chain: pinn_hmc_iterate refuses until the next begin
     return 1;
   }
   return 0;
+}
+
+int pinn_hmc_begin_ex(pinn_handle e, const double* host_theta0, const pinn_hmc_options* opts, const double* host_weights,
+                      double ll_const, const pinn_hmc_prior* tail, int32_t n_tail, double* step_size_out) {
+  return pinn_hmc_begin_ex2(e, host_theta0, opts, host_weights, ll_const, tail, n_tail, nullptr, 0, step_size_out);
 }
 
 int pinn_hmc_begin(pinn_handle e, const double* host_theta0, const pinn_hmc_options* opts, const double* host_weights,
@@ -617,6 +652,14 @@ int pinn_hmc_iterate(pinn_handle e, int32_t n, double* host_samples, double* hos
     unsigned long long key = 1469598103934665603ull;
     key = fnv1a(e->dyn, sizeof e->dyn, key);
     for (const TermState& ts : e->term) key = fnv1a(&ts.n_global, sizeof ts.n_global, key);
+    if (s->redraw)
+      for (const TermState& ts : e->term) {
+        const unsigned long long reg[4] = {ts.sampler_on, (unsigned long long)ts.sampler_kind, ts.sampler_seed,
+                                           (unsigned long long)ts.sampler_n};
+        key = fnv1a(reg, sizeof reg, key);
+        key = fnv1a(ts.sampler_lb, sizeof ts.sampler_lb, key);
+        key = fnv1a(ts.sampler_ub, sizeof ts.sampler_ub, key);
+      }
     if (!s->graph || s->graph_key != key) {
       if (s->graph) { cudaGraphExecDestroy(s->graph); s->graph = nullptr; }
       cudaGraph_t g = nullptr;

@@ -529,8 +529,6 @@ int pinn_adam_begin(pinn_handle e, const void* host_theta0, double lr, double be
   return 0;
 }
 
-static int draw_term(pinn_engine* e, int term, unsigned long long draw, const unsigned long long* draw_dev, cudaStream_t st);
-
 // one iteration of the device-resident loop: fresh points for the sampled terms, then the fused step with Adam in its tail
 static int enqueue_adam_iteration(pinn_engine* e, const double* host_weights, cudaStream_t st) {
   char* dout = (char*)e->d_out;
@@ -644,8 +642,10 @@ int pinn_term_residual_host(pinn_handle e, int32_t term, const void* host_theta,
   return rc;
 }
 
+}  // extern "C"
+
 // effective draw index = draw + *draw_dev (the device counter is advanced by the tail of the device-resident loop)
-static int draw_term(pinn_engine* e, int term, unsigned long long draw, const unsigned long long* draw_dev, cudaStream_t st) {
+int pinn::draw_term(pinn_engine* e, int term, unsigned long long draw, const unsigned long long* draw_dev, cudaStream_t st) {
   const int dim = e->plan.prob.terms[term].dim;
   TermState& ts = e->term[term];
   const long long n = ts.sampler_n;
@@ -659,6 +659,8 @@ static int draw_term(pinn_engine* e, int term, unsigned long long draw, const un
   e->dyn[term].pts = ts.own_pts; e->dyn[term].qw = nullptr; e->dyn[term].n = n;
   return 0;
 }
+
+extern "C" {
 
 int pinn_set_sampler_ex(pinn_handle e, int32_t term, int32_t kind, int64_t n, const double* host_lb, const double* host_ub,
                         uint64_t seed, void* stream) {

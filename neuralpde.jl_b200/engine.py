@@ -46,6 +46,7 @@ EXPORTS = [
     "pinn_comm_info", "pinn_set_sampler_ex", "pinn_qn_begin", "pinn_qn_iterate", "pinn_qn_theta",
     "pinn_hmc_begin", "pinn_hmc_iterate", "pinn_hmc_theta", "pinn_hmc_begin_ex", "pinn_create_ex",
     "pinn_quadrature_nodes", "pinn_create_ex2", "pinn_set_fixed_params", "pinn_set_fixed_params_host",
+    "pinn_hmc_begin_ex2",
 ]
 
 # substitutions of infinite integration bounds (pinn_integral_desc.inf_kind) and the limits of integral terms
@@ -68,6 +69,8 @@ HMC_ADAPT_NONE, HMC_ADAPT_STAN = 0, 1
 HMC_METRIC_UNIT, HMC_METRIC_DIAG = 0, 1
 # kinds of the per-entry priors of theta's last entries (pinn_hmc_prior)
 HMC_PRIOR_NORMAL, HMC_PRIOR_LOGNORMAL, HMC_PRIOR_UNIFORM = 0, 1, 2
+# pinn_hmc_begin_ex2 flags: the device samplers draw fresh points before every evaluation of the chain
+HMC_REDRAW = 1
 HMC_STATS = ("step_size", "acceptance_rate", "is_accept", "log_density", "hamiltonian_energy",
              "hamiltonian_energy_error", "numerical_error", "is_adapt")
 
@@ -296,6 +299,9 @@ def load_library():
     lib.pinn_hmc_begin_ex.argtypes = [vp, C.POINTER(dbl), C.POINTER(_HmcOptions), C.POINTER(dbl), dbl,
                                       C.POINTER(_HmcPrior), i32, C.POINTER(dbl)]
     lib.pinn_hmc_begin_ex.restype = C.c_int
+    lib.pinn_hmc_begin_ex2.argtypes = [vp, C.POINTER(dbl), C.POINTER(_HmcOptions), C.POINTER(dbl), dbl,
+                                       C.POINTER(_HmcPrior), i32, C.POINTER(dbl), C.c_uint32, C.POINTER(dbl)]
+    lib.pinn_hmc_begin_ex2.restype = C.c_int
     lib.pinn_hmc_iterate.argtypes = [vp, i32, C.POINTER(dbl), C.POINTER(dbl)]
     lib.pinn_hmc_iterate.restype = C.c_int
     lib.pinn_hmc_theta.argtypes = [vp, C.POINTER(dbl)]
@@ -626,11 +632,13 @@ class Engine:
     def hmc_begin(self, theta0: np.ndarray, n_leapfrog: int = 30, adaptor: int = HMC_ADAPT_STAN,
                   metric: int = HMC_METRIC_DIAG, n_adapts: int = 0, target_accept: float = 0.8, step_size: float = 0.0,
                   prior_mean: float = 0.0, prior_std: float = 1.0, seed: int = 0, weights=None,
-                  ll_const: float = 0.0, tail_priors=None) -> float:
+                  ll_const: float = 0.0, tail_priors=None, tail_logabs=None, redraw: bool = False) -> float:
         """Start a chain at theta0 (float64) for the log density sum_k w_k L_k + ll_const + log N(theta; prior);
         step_size <= 0 runs find_good_stepsize.  Returns the initial step size.  ``tail_priors``: a list of
         (HMC_PRIOR_*, a, b) for the last len(tail_priors) entries of theta, which the Normal prior then leaves out
-        (pinn_hmc_begin_ex); None calls pinn_hmc_begin."""
+        (pinn_hmc_begin_ex); None calls pinn_hmc_begin.  ``tail_logabs``: c_j per tail entry, adding
+        c_j log|theta_tail_j| to the log density; ``redraw``: the device samplers draw fresh points before every
+        evaluation (PINN_HMC_REDRAW).  Either one calls pinn_hmc_begin_ex2."""
         th = np.ascontiguousarray(theta0, dtype=np.float64)
         if th.shape != (self.n_theta,):
             raise ValueError("theta must have length %d" % self.n_theta)
@@ -639,7 +647,19 @@ class Engine:
         w = self._weights(weights)
         wp = w.ctypes.data_as(C.POINTER(C.c_double)) if w is not None else None
         eps = C.c_double(0.0)
-        if tail_priors is None:
+        if tail_logabs is not None or redraw:
+            tp = list(tail_priors or [])
+            tail = (_HmcPrior * max(1, len(tp)))(*[_HmcPrior(int(k), float(a), float(b)) for k, a, b in tp])
+            la = None
+            if tail_logabs is not None:
+                la = np.ascontiguousarray(tail_logabs, dtype=np.float64)
+                if la.shape != (len(tp),):
+                    raise ValueError("tail_logabs needs one entry per tail prior (%d), got %s" % (len(tp), la.shape))
+            _check(self.lib.pinn_hmc_begin_ex2(self._h, th.ctypes.data_as(C.POINTER(C.c_double)), C.byref(opt), wp,
+                                               float(ll_const), tail, len(tp),
+                                               None if la is None else la.ctypes.data_as(C.POINTER(C.c_double)),
+                                               HMC_REDRAW if redraw else 0, C.byref(eps)))
+        elif tail_priors is None:
             _check(self.lib.pinn_hmc_begin(self._h, th.ctypes.data_as(C.POINTER(C.c_double)), C.byref(opt), wp,
                                            float(ll_const), C.byref(eps)))
         else:

@@ -1167,8 +1167,14 @@ def solve(prob: OptimizationProblem, opt: Union[Adam, LBFGS, BFGS], maxiters: in
     (pinn_adam_iterate); the callback sees the loss every `chunk` steps.
 
     ``solve(prob::ODEProblem, alg::NNODE; maxiters, dt, abstol, saveat, ...)`` trains an NNODE (ode.py) and takes the
-    keywords of ``ode.solve``."""
+    keywords of ``ode.solve``.  ``solve(prob::ODEProblem, alg::BNNODE; saveat)`` samples the Bayesian ODE posterior
+    (bpinn_ode.py) and returns a BPINNsolution."""
+    from .bpinn_ode import BNNODE, solve_bnnode
     from .ode import ODEProblem, solve_nnode
+    if isinstance(prob, ODEProblem) and isinstance(opt, BNNODE):
+        if callback is not None or chunk != 50 or device_loop or maxiters is not _MAXITERS_DEFAULT:
+            raise TypeError("solve(::ODEProblem, ::BNNODE) takes no maxiters, callback, chunk or device_loop")
+        return solve_bnnode(prob, opt, **ode_kwargs)
     if isinstance(prob, ODEProblem):
         if callback is not None or chunk != 50:
             raise TypeError("solve(::ODEProblem, ::NNODE) takes no callback or chunk: it stops at abstol")
@@ -1298,20 +1304,19 @@ class Uniform:
 _PRIOR_KINDS = {Normal: _eng.HMC_PRIOR_NORMAL, LogNormal: _eng.HMC_PRIOR_LOGNORMAL, Uniform: _eng.HMC_PRIOR_UNIFORM}
 
 
-def _tail_priors(param) -> List[tuple]:
+def _tail_priors(param, who: str = "ahmc_bayesian_pinn_pde") -> List[tuple]:
     """The device's table for θ.p: (kind, a, b) per parameter, in the reference's order -- priorlogpdf applies
-    ``param[length(θ) - i + 1]`` to θ[i] (ext/bpinn/PDE_BPINN.jl:194-196), so θ.p[k] gets param[end - k]."""
+    ``param[length(θ) - i + 1]`` to θ[i] (ext/bpinn/PDE_BPINN.jl:194-196), so θ.p[k] gets param[end - k].  ``who``
+    names the calling sampler in the refusals."""
     out = []
     for prior in param:
         kind = _PRIOR_KINDS.get(type(prior))
         if kind is None:
-            raise ValueError("ahmc_bayesian_pinn_pde: prior %r is not supported (Normal, LogNormal or Uniform)"
-                             % (prior,))
+            raise ValueError("%s: prior %r is not supported (Normal, LogNormal or Uniform)" % (who, prior))
         a, b = (float(v) for v in prior.params())
         if not (np.isfinite(a) and np.isfinite(b)) or (kind == _eng.HMC_PRIOR_UNIFORM and not a < b) or \
                 (kind != _eng.HMC_PRIOR_UNIFORM and not b > 0.0):
-            raise ValueError("ahmc_bayesian_pinn_pde: prior %r: needs finite parameters with σ > 0 (Uniform: a < b)"
-                             % (prior,))
+            raise ValueError("%s: prior %r: needs finite parameters with σ > 0 (Uniform: a < b)" % (who, prior))
         out.append((kind, a, b))
     return out[::-1]
 
