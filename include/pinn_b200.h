@@ -173,7 +173,9 @@ enum { PINN_REDUCE_MEAN = 0,          /* mean(abs2, r)            training_strat
 
 typedef struct {
   int32_t dim;                 /* rows of the point matrix                              */
-  int32_t n_taps;
+  int32_t n_taps;              /* 0: a parameter-only term, whose program must read PINN_OP_PARAM
+                                  (PINN_MODE_FFMA / PINN_MODE_TC_F64; the FFMA kernel runs
+                                  its program alone, no network pass)                   */
   const pinn_tap_desc* taps;
   const int32_t* net_rows;     /* [n_nets][PINN_MAX_IN]: point row feeding input j of
                                   network k (cord_k = vcat(...), discretize.jl:111-116);
@@ -312,9 +314,27 @@ int pinn_set_sampler(pinn_handle h, int32_t term, int64_t n, const double* host_
  * default `sampling_alg = LatinHypercubeSample()` (src/training_strategies.jl:285-334; QuasiMonteCarlo.sample on the host
  * + upload per call, :365-389).  Each row's n strata hold exactly one point per draw: stratum index = a keyed Feistel
  * permutation of the point index, position inside the stratum uniform (Philox).  pinn_set_sampler == kind UNIFORM. */
-enum { PINN_SAMPLER_UNIFORM = 0, PINN_SAMPLER_LHS = 1 };
+enum { PINN_SAMPLER_UNIFORM = 0, PINN_SAMPLER_LHS = 1, PINN_SAMPLER_KKL = 2 };
 int pinn_set_sampler_ex(pinn_handle h, int32_t term, int32_t kind, int64_t n, const double* host_lb, const double* host_ub,
                         uint64_t seed, void* stream);
+/* NNSDE's StochasticTraining on the device (kind PINN_SAMPLER_KKL; pinn_set_sampler_ex does not take it): the points
+ * (t, z_1..z_n_z) of a truncated Karhunen-Loeve (KKL) Wiener path, term dim = 1 + n_z.  Draw d (the host counter of
+ * pinn_resample plus the device counter, as the other samplers) fills point p = i * sub_batch + s,
+ * i < n_times, s < sub_batch:
+ *   key   = seed ^ 0xD6E8FEB86659FD93 (k0 = low 32 bits, k1 = high; no term index: every KKL term of a handle
+ *           registered with one seed sees the same draw);
+ *   U(a, b) = ((a << 32 | b) >> 11) * 2^-53 in [0, 1) from two Philox4x32-10 words;
+ *   row 0:   c = philox({i, 0xFFFFFFFF, d_lo, d_hi}),  t_i = t_lb + (t_ub - t_lb) * U(c0, c1)  (the same for all s);
+ *   rows 1 + 2j, 2 + 2j (pair j < ceil(n_z / 2); the second only while 2 + 2j <= n_z):
+ *            c = philox({q, j, d_lo, d_hi ^ 0x4B4B4C00}), q = p (weak) or q = s (flags & PINN_KKL_STRONG: a path's
+ *            z is bit-identical at all its times),
+ *            u1 = 1 - U(c0, c1) in (0, 1], u2 = U(c2, c3), r = sqrt(-2 log u1),
+ *            z_{1+2j} = r cos(2 pi u2), z_{2+2j} = r sin(2 pi u2) (Box-Muller, N(0, 1)),
+ * computed in float64 (2 pi = 6.283185307179586) and rounded to the engine dtype.  The term must be a MEAN term (as
+ * for pinn_set_sampler); n_times * sub_batch <= 2^31 - 1. */
+enum { PINN_KKL_STRONG = 1 };
+int pinn_set_sampler_kkl(pinn_handle h, int32_t term, int64_t n_times, int32_t sub_batch, int32_t n_z, double t_lb,
+                         double t_ub, uint32_t flags, uint64_t seed, void* stream);
 int pinn_resample(pinn_handle h, void* stream);
 int pinn_get_points_host(pinn_handle h, int32_t term, void* host_pts);
 

@@ -22,5 +22,6 @@ from .pinn import (AbstractPINN, Adam, BPINNsolution, BPINNstats, DiagEuclideanM
 from .adapter import NeuralAdapterLoss, neural_adapter
 from .ode import NNODE, NNODERepresentation, ODEFunction, ODEProblem, ODESolution
 from .bpinn_ode import BNNODE, BNNODELogDensity, ahmc_bayesian_pinn_ode
+from .sde import NNSDE, NNSDERepresentation, SDEProblem, SDEsol
 
 __all__ = [n for n in dir() if not n.startswith("_")]

@@ -22,6 +22,8 @@ struct TermState {
   bool sampler_on = false; int sampler_kind = 0;
   double sampler_lb[PINN_MAX_DIM] = {}, sampler_ub[PINN_MAX_DIM] = {};
   unsigned long long sampler_seed = 0; long long sampler_n = 0;
+  // PINN_SAMPLER_KKL (pinn_set_sampler_kkl): sampler_n = kkl_times * kkl_sub points, time bounds in sampler_lb/ub[0]
+  long long kkl_times = 0; int kkl_sub = 0, kkl_flags = 0;
   void *own_pts = nullptr, *own_qw = nullptr;   // engine-owned point copies
   size_t own_pts_cap = 0, own_qw_cap = 0;
 };

@@ -243,6 +243,50 @@ cudaError_t sample_uniform_launch(int dtype, void* pts, long long n, int dim, co
   return cudaGetLastError();
 }
 
+// ---- device-side KKL path sampler (NNSDE's StochasticTraining; the formula is in include/pinn_b200.h) -------------------
+__device__ __forceinline__ double u53(uint32_t a, uint32_t b) {
+  return (double)((((unsigned long long)a << 32) | b) >> 11) * (1.0 / 9007199254740992.0);
+}
+
+template <typename real>
+__global__ void __launch_bounds__(256) sample_kkl_kernel(real* pts, long long n, int sub, int n_z, double t_lb, double t_ub,
+                                                         bool strong, unsigned long long seed, unsigned long long draw,
+                                                         const unsigned long long* draw_dev) {
+  const long long p = (long long)blockIdx.x * 256 + threadIdx.x;
+  if (p >= n) return;
+  if (draw_dev) draw += *draw_dev;
+  const int dim = 1 + n_z;
+  const uint32_t i = (uint32_t)(p / sub), s = (uint32_t)(p - (long long)i * sub);
+  const uint32_t k0 = (uint32_t)seed, k1 = (uint32_t)(seed >> 32), d0 = (uint32_t)draw, d1 = (uint32_t)(draw >> 32);
+  uint32_t c[4] = {i, 0xFFFFFFFFu, d0, d1};
+  philox4x32_10(c, k0, k1);
+  pts[p * dim] = (real)(t_lb + (t_ub - t_lb) * u53(c[0], c[1]));
+  const uint32_t q = strong ? s : (uint32_t)p;
+  for (int j = 0; 2 * j < n_z; ++j) {
+    uint32_t z[4] = {q, (uint32_t)j, d0, d1 ^ 0x4B4B4C00u};
+    philox4x32_10(z, k0, k1);
+    const double u1 = 1.0 - u53(z[0], z[1]), u2 = u53(z[2], z[3]);
+    const double r = sqrt(-2.0 * log(u1));
+    double sn, cs;
+    sincos(6.283185307179586 * u2, &sn, &cs);
+    pts[p * dim + 1 + 2 * j] = (real)(r * cs);
+    if (2 + 2 * j <= n_z) pts[p * dim + 2 + 2 * j] = (real)(r * sn);
+  }
+}
+
+cudaError_t sample_kkl_launch(int dtype, void* pts, long long n_times, int sub, int n_z, double t_lb, double t_ub,
+                              bool strong, unsigned long long seed, unsigned long long draw,
+                              const unsigned long long* draw_dev, cudaStream_t st) {
+  const long long n = n_times * sub;
+  if (n <= 0) return cudaSuccess;
+  const int blocks = (int)((n + 255) / 256);
+  if (dtype == PINN_F64)
+    sample_kkl_kernel<double><<<blocks, 256, 0, st>>>((double*)pts, n, sub, n_z, t_lb, t_ub, strong, seed, draw, draw_dev);
+  else
+    sample_kkl_kernel<float><<<blocks, 256, 0, st>>>((float*)pts, n, sub, n_z, t_lb, t_ub, strong, seed, draw, draw_dev);
+  return cudaGetLastError();
+}
+
 cudaError_t grad_stats_launch(int dtype, const void* grad, long long n, double* out2, cudaStream_t st) {
   if (dtype == PINN_F64) grad_stats_kernel<double><<<1, 1024, 0, st>>>((const double*)grad, n, out2);
   else grad_stats_kernel<float><<<1, 1024, 0, st>>>((const float*)grad, n, out2);

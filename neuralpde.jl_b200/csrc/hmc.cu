@@ -654,8 +654,9 @@ int pinn_hmc_iterate(pinn_handle e, int32_t n, double* host_samples, double* hos
     for (const TermState& ts : e->term) key = fnv1a(&ts.n_global, sizeof ts.n_global, key);
     if (s->redraw)
       for (const TermState& ts : e->term) {
-        const unsigned long long reg[4] = {ts.sampler_on, (unsigned long long)ts.sampler_kind, ts.sampler_seed,
-                                           (unsigned long long)ts.sampler_n};
+        const unsigned long long reg[6] = {ts.sampler_on, (unsigned long long)ts.sampler_kind, ts.sampler_seed,
+                                           (unsigned long long)ts.sampler_n, (unsigned long long)ts.kkl_times,
+                                           (unsigned long long)ts.kkl_sub << 32 | (unsigned)ts.kkl_flags};
         key = fnv1a(reg, sizeof reg, key);
         key = fnv1a(ts.sampler_lb, sizeof ts.sampler_lb, key);
         key = fnv1a(ts.sampler_ub, sizeof ts.sampler_ub, key);

@@ -24,6 +24,9 @@ cudaError_t sample_uniform_launch(int dtype, void* pts, long long n, int dim, co
 cudaError_t sample_lhs_launch(int dtype, void* pts, long long n, int dim, const double* lb, const double* ub,
                               unsigned long long seed, unsigned long long draw, const unsigned long long* draw_dev,
                               cudaStream_t st);
+cudaError_t sample_kkl_launch(int dtype, void* pts, long long n_times, int sub, int n_z, double t_lb, double t_ub,
+                              bool strong, unsigned long long seed, unsigned long long draw,
+                              const unsigned long long* draw_dev, cudaStream_t st);
 cudaError_t finish_launch(int dtype, const void* packed, long long n_grad, int n_terms, const ScaleW& scale_w, void* out_grad,
                           void* out_terms, void* out_total, cudaStream_t st);
 }  // namespace pinn
@@ -651,7 +654,11 @@ int pinn::draw_term(pinn_engine* e, int term, unsigned long long draw, const uns
   const long long n = ts.sampler_n;
   if (grow(&ts.own_pts, &ts.own_pts_cap, (size_t)n * dim * e->es, e)) return 1;
   const unsigned long long key = ts.sampler_seed + 0x9E3779B97F4A7C15ull * (unsigned long long)(term + 1);
-  if (ts.sampler_kind == PINN_SAMPLER_LHS)
+  if (ts.sampler_kind == PINN_SAMPLER_KKL)   // keyed on the seed alone: the KKL terms of one seed share their draw
+    CUDA_TRY(sample_kkl_launch(e->dtype, ts.own_pts, ts.kkl_times, ts.kkl_sub, dim - 1, ts.sampler_lb[0], ts.sampler_ub[0],
+                               (ts.kkl_flags & PINN_KKL_STRONG) != 0, ts.sampler_seed ^ 0xD6E8FEB86659FD93ull, draw,
+                               draw_dev, st));
+  else if (ts.sampler_kind == PINN_SAMPLER_LHS)
     CUDA_TRY(sample_lhs_launch(e->dtype, ts.own_pts, n, dim, ts.sampler_lb, ts.sampler_ub, key, draw, draw_dev, st));
   else
     CUDA_TRY(sample_uniform_launch(e->dtype, ts.own_pts, n, dim, ts.sampler_lb, ts.sampler_ub, key, draw, draw_dev, st));
@@ -681,6 +688,33 @@ int pinn_set_sampler_ex(pinn_handle e, int32_t term, int32_t kind, int64_t n, co
     ts.sampler_lb[r] = host_lb[r]; ts.sampler_ub[r] = host_ub[r];
   }
   ts.sampler_on = true; ts.sampler_kind = kind; ts.sampler_seed = seed; ts.sampler_n = n;
+  if (draw_term(e, term, e->sampler_draw, &e->d_state->draw, (cudaStream_t)stream)) return 1;
+  retile(e);
+  return 0;
+}
+
+int pinn_set_sampler_kkl(pinn_handle e, int32_t term, int64_t n_times, int32_t sub_batch, int32_t n_z, double t_lb,
+                         double t_ub, uint32_t flags, uint64_t seed, void* stream) {
+  if (check_term(e, term, "pinn_set_sampler_kkl")) return 1;
+  if (n_times < 1 || sub_batch < 1)
+    return fail("pinn_set_sampler_kkl: term %d needs at least one time and one sample (n_times=%lld, sub_batch=%d)", term,
+                (long long)n_times, sub_batch);
+  if (n_times * (long long)sub_batch > 0x7fffffffLL)
+    return fail("pinn_set_sampler_kkl: at most 2^31 - 1 points per term (n_times * sub_batch)");
+  if (n_z < 0 || 1 + n_z != e->plan.prob.terms[term].dim)
+    return fail("pinn_set_sampler_kkl: term %d has %d point rows; the KKL sampler fills 1 + n_z = %d (t, z_1..z_n_z)", term,
+                e->plan.prob.terms[term].dim, 1 + n_z);
+  if (flags & ~(uint32_t)PINN_KKL_STRONG) return fail("pinn_set_sampler_kkl: unknown flags 0x%x", flags);
+  if (!(t_lb <= t_ub)) return fail("pinn_set_sampler_kkl: term %d has t_lb > t_ub", term);
+  if (e->plan.term[term].reduction == PINN_REDUCE_WSUM)
+    return fail("pinn_set_sampler_kkl: term %d is a weighted-sum (quadrature) term; the KKL sampler serves mean(abs2) terms", term);
+  if (term == e->plan.prob.func_term)
+    return fail("pinn_set_sampler_kkl: term %d is a functional term; its nodes are fixed (pinn_set_points)", term);
+  CUDA_TRY(cudaSetDevice(e->device));
+  TermState& ts = e->term[term];
+  ts.sampler_lb[0] = t_lb; ts.sampler_ub[0] = t_ub;
+  ts.kkl_times = n_times; ts.kkl_sub = sub_batch; ts.kkl_flags = (int)flags;
+  ts.sampler_on = true; ts.sampler_kind = PINN_SAMPLER_KKL; ts.sampler_seed = seed; ts.sampler_n = n_times * sub_batch;
   if (draw_term(e, term, e->sampler_draw, &e->d_state->draw, (cudaStream_t)stream)) return 1;
   retile(e);
   return 0;

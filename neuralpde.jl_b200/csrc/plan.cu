@@ -195,7 +195,7 @@ int plan_taps(const pinn_problem_desc* d, const pinn_term_desc& td, const char* 
     else if (tp.order == 2) { dir_pair(ch, tp.dir, a, b); T.tap_ch[i] = 1 + ch.n1 + find_pair(ch, a, b); }
     else T.tap_ch[i] = 1 + ch.n1 + ch.n2 + find_third(ch, find_dir(ch, tp.dir[0]));
   }
-  bool any_tap = false;
+  bool any_tap = false, any_param = false;
   const bool is_term = strcmp(what, "term") == 0;
   for (int i = 0; i < td.n_instr; ++i) {
     const pinn_instr& in = td.prog[i];
@@ -213,6 +213,7 @@ int plan_taps(const pinn_problem_desc* d, const pinn_term_desc& td, const char* 
         break;
       case PINN_OP_PARAM:
         if (in.a < 0 || in.a >= d->n_params) return fail("pinn_create: %s %d instr %d PARAM %d out of range", what, t, i, in.a);
+        any_param = true;
         break;
       case PINN_OP_INTEGRAL: {
         if (!is_term) return fail("pinn_create: integral %d instr %d: integrals nested in an integrand are not supported", t, i);
@@ -238,8 +239,10 @@ int plan_taps(const pinn_problem_desc* d, const pinn_term_desc& td, const char* 
         return fail("pinn_create: %s %d instr %d unknown opcode %d", what, t, i, in.op);
     }
   }
-  if (!any_tap) return fail("pinn_create: %s %d %s program never reads a tap (nothing depends on theta)", what, t,
-                           is_term ? "residual" : "integrand");
+  // a term without taps is a parameter-only term (plan_term): its program must read theta.p instead
+  if (!any_tap && !(is_term && td.n_taps == 0 && any_param))
+    return fail("pinn_create: %s %d %s program never reads a tap (nothing depends on theta)", what, t,
+                is_term ? "residual" : "integrand");
   return 0;
 }
 
@@ -286,7 +289,12 @@ int plan_term(const pinn_problem_desc* d, int t, const pinn_integral_desc* integ
   int n_own = 0;
   for (int i = 0; i < n_integrals; ++i) n_own += integrals[i].owner == t;
   if (td.dim < 1 || td.dim > PINN_MAX_DIM) return fail("pinn_create: term %d dim=%d out of range [1,%d]", t, td.dim, PINN_MAX_DIM);
-  if (td.n_taps < 1 && n_own == 0)
+  // a term without taps or integrals is accepted when its program reads theta.p: a parameter-only term (such as an
+  // Euler-Maruyama data loss), for which the FFMA kernel runs the residual program alone -- no network is staged,
+  // propagated, stashed or swept back, and the adjoint reaches theta.p through the program's PARAM reads
+  bool reads_param = false;
+  for (int i = 0; i < td.n_instr && td.prog; ++i) reads_param = reads_param || td.prog[i].op == PINN_OP_PARAM;
+  if (td.n_taps < 1 && n_own == 0 && !reads_param)
     return fail("pinn_create: term %d has no network taps (an equation such as 0 ~ 0 cannot be trained on)", t);
   if (td.n_taps + n_own > PINN_MAX_TAPS)
     return fail("pinn_create: term %d has %d taps and %d integrals (max %d together)", t, td.n_taps, n_own, PINN_MAX_TAPS);
@@ -480,6 +488,9 @@ int check_tc_terms(const DevProblem& P, bool wide, int max_taps, int& n_used_max
   n_used_max = 1; max_c = 1;
   for (int t = 0; t < P.n_terms; ++t) {
     const DevTerm& T = P.terms[t];
+    if (T.n_used == 0)
+      return fail("pinn_create(tc): term %d reads no network (a parameter-only term); parameter-only terms run on the FFMA "
+                  "path (PINN_MODE_FFMA, or PINN_MODE_TC_F64 for Float64)", t);
     if (T.n_taps > max_taps) return fail("pinn_create(tc): term %d has %d taps (tensor-core path: max %d)", t, T.n_taps, max_taps);
     n_used_max = std::max(n_used_max, T.n_used);
     for (int s = 0; s < T.n_used; ++s) {

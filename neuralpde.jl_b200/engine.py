@@ -46,7 +46,7 @@ EXPORTS = [
     "pinn_comm_info", "pinn_set_sampler_ex", "pinn_qn_begin", "pinn_qn_iterate", "pinn_qn_theta",
     "pinn_hmc_begin", "pinn_hmc_iterate", "pinn_hmc_theta", "pinn_hmc_begin_ex", "pinn_create_ex",
     "pinn_quadrature_nodes", "pinn_create_ex2", "pinn_set_fixed_params", "pinn_set_fixed_params_host",
-    "pinn_hmc_begin_ex2",
+    "pinn_hmc_begin_ex2", "pinn_set_sampler_kkl",
 ]
 
 # substitutions of infinite integration bounds (pinn_integral_desc.inf_kind) and the limits of integral terms
@@ -69,6 +69,8 @@ HMC_ADAPT_NONE, HMC_ADAPT_STAN = 0, 1
 HMC_METRIC_UNIT, HMC_METRIC_DIAG = 0, 1
 # kinds of the per-entry priors of theta's last entries (pinn_hmc_prior)
 HMC_PRIOR_NORMAL, HMC_PRIOR_LOGNORMAL, HMC_PRIOR_UNIFORM = 0, 1, 2
+# pinn_set_sampler_kkl flags: one coefficient vector per sample path, shared by all its times
+KKL_STRONG = 1
 # pinn_hmc_begin_ex2 flags: the device samplers draw fresh points before every evaluation of the chain
 HMC_REDRAW = 1
 HMC_STATS = ("step_size", "acceptance_rate", "is_accept", "log_density", "hamiltonian_energy",
@@ -254,6 +256,8 @@ def load_library():
     lib.pinn_set_sampler.restype = C.c_int
     lib.pinn_set_sampler_ex.argtypes = [vp, i32, i32, i64, C.POINTER(dbl), C.POINTER(dbl), C.c_uint64, vp]
     lib.pinn_set_sampler_ex.restype = C.c_int
+    lib.pinn_set_sampler_kkl.argtypes = [vp, i32, i64, i32, i32, dbl, dbl, C.c_uint32, C.c_uint64, vp]
+    lib.pinn_set_sampler_kkl.restype = C.c_int
     lib.pinn_resample.argtypes = [vp, vp]
     lib.pinn_resample.restype = C.c_int
     lib.pinn_get_points_host.argtypes = [vp, i32, vp]
@@ -524,6 +528,18 @@ class Engine:
                                             C.c_uint64(int(seed) & (2 ** 64 - 1)), C.c_void_p(stream)))
         self._n_pts = getattr(self, "_n_pts", {})
         self._n_pts[int(term)] = int(n)
+
+    def set_sampler_kkl(self, term: int, n_times: int, sub_batch: int, t_lb: float, t_ub: float, seed: int = 0,
+                        strong: bool = False, stream: int = 0):
+        """Register NNSDE's device sampler for a term with rows (t, z_1..z_n_z): n_times uniform times in [t_lb, t_ub],
+        each with sub_batch N(0, 1) coefficient vectors, independent per point, or with strong=True one per sample s
+        shared by all times (include/pinn_b200.h gives the formula).  Draws the first sample."""
+        dim = self.spec.terms[term].dim
+        _check(self.lib.pinn_set_sampler_kkl(self._h, int(term), int(n_times), int(sub_batch), dim - 1, float(t_lb),
+                                             float(t_ub), KKL_STRONG if strong else 0,
+                                             C.c_uint64(int(seed) & (2 ** 64 - 1)), C.c_void_p(stream)))
+        self._n_pts = getattr(self, "_n_pts", {})
+        self._n_pts[int(term)] = int(n_times) * int(sub_batch)
 
     def resample(self, stream: int = 0):
         """Draw the next sample of every term that has a device-side sampler."""

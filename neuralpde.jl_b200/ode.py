@@ -357,6 +357,7 @@ class NNODERepresentation:
         self.term_weights = np.asarray(weights)
         self.term_names = names
         self.sampled = sampled
+        self.loss_const = 0.0      # added to every reported loss (NNSDE's constant Euler-Maruyama terms)
         self.flat_init_params = ComponentVector(flat, n_net)
         self._engine = None
         self._calls = 0
@@ -464,22 +465,25 @@ def solve_nnode(prob: ODEProblem, alg: NNODE, *, maxiters: int, dt=None, abstol:
 
 
 def _train(rep: NNODERepresentation, opt, maxiters: int, abstol: float, verbose: bool, device_loop: bool,
-           chunk: int) -> OptimizationSolution:
+           chunk: int, who: str = "NNODE") -> OptimizationSolution:
+    """the optimizer loops of NNODE and NNSDE; every reported loss is the engine's total plus rep.loss_const"""
+    c = rep.loss_const
+
     def log(it, l):
         if verbose:
-            print("[NNODE]\tIter: [%*d/%d]\tLoss: %g" % (len(str(maxiters)), it, maxiters, l))
+            print("[%s]\tIter: [%*d/%d]\tLoss: %g" % (who, len(str(maxiters)), it, maxiters, l))
 
     def stop(state, l):
-        log(state["iter"], l)
-        return l < abstol
+        log(state["iter"], l + c)
+        return l + c < abstol
 
     eng, w = rep.engine, rep.term_weights
     if isinstance(opt, (BFGS, LBFGS)):
         th, f, iters, _, retcode = _qn_run(eng, rep.flat_init_params, opt, _linesearch_kind(opt.linesearch), maxiters,
                                            stop, w)
-        return OptimizationSolution(ComponentVector(th, rep.n_net), f, iters, retcode)
+        return OptimizationSolution(ComponentVector(th, rep.n_net), f + c, iters, retcode)
     if not isinstance(opt, Adam):
-        raise TypeError("NNODE: opt must be Adam(...), BFGS() or LBFGS(), got %r" % (opt,))
+        raise TypeError("%s: opt must be Adam(...), BFGS() or LBFGS(), got %r" % (who, opt))
     if device_loop:
         eng.adam_begin(rep.flat_init_params, opt.lr, opt.beta1, opt.beta2, opt.eps)
         done, obj = 0, float("nan")
@@ -489,7 +493,7 @@ def _train(rep: NNODERepresentation, opt, maxiters: int, abstol: float, verbose:
             done += n
             if stop({"iter": done}, obj):
                 break
-        return OptimizationSolution(ComponentVector(eng.adam_theta(), rep.n_net), obj, done, "Success")
+        return OptimizationSolution(ComponentVector(eng.adam_theta(), rep.n_net), obj + c, done, "Success")
     u = np.asarray(rep.flat_init_params, dtype=np.float64).copy()
     m, v = np.zeros_like(u), np.zeros_like(u)
     obj, it = float("nan"), 0
@@ -501,4 +505,4 @@ def _train(rep: NNODERepresentation, opt, maxiters: int, abstol: float, verbose:
         m = opt.beta1 * m + (1 - opt.beta1) * g
         v = opt.beta2 * v + (1 - opt.beta2) * g * g
         u -= opt.lr * (m / (1 - opt.beta1 ** it)) / (np.sqrt(v / (1 - opt.beta2 ** it)) + opt.eps)
-    return OptimizationSolution(ComponentVector(u.astype(rep.dtype), rep.n_net), obj, it, "Success")
+    return OptimizationSolution(ComponentVector(u.astype(rep.dtype), rep.n_net), obj + c, it, "Success")

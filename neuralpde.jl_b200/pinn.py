@@ -1168,9 +1168,17 @@ def solve(prob: OptimizationProblem, opt: Union[Adam, LBFGS, BFGS], maxiters: in
 
     ``solve(prob::ODEProblem, alg::NNODE; maxiters, dt, abstol, saveat, ...)`` trains an NNODE (ode.py) and takes the
     keywords of ``ode.solve``.  ``solve(prob::ODEProblem, alg::BNNODE; saveat)`` samples the Bayesian ODE posterior
-    (bpinn_ode.py) and returns a BPINNsolution."""
+    (bpinn_ode.py) and returns a BPINNsolution.  ``solve(prob::SDEProblem, alg::NNSDE; maxiters, dt, abstol, saveat,
+    ...)`` trains an NNSDE (sde.py) and returns an SDEsol."""
     from .bpinn_ode import BNNODE, solve_bnnode
     from .ode import ODEProblem, solve_nnode
+    from .sde import SDEProblem, solve_nnsde
+    if isinstance(prob, SDEProblem):
+        if callback is not None or chunk != 50:
+            raise TypeError("solve(::SDEProblem, ::NNSDE) takes no callback or chunk: it stops at abstol")
+        if maxiters is _MAXITERS_DEFAULT:
+            raise TypeError("solve(::SDEProblem, ::NNSDE) needs maxiters")
+        return solve_nnsde(prob, opt, maxiters=maxiters, device_loop=device_loop, **ode_kwargs)
     if isinstance(prob, ODEProblem) and isinstance(opt, BNNODE):
         if callback is not None or chunk != 50 or device_loop or maxiters is not _MAXITERS_DEFAULT:
             raise TypeError("solve(::ODEProblem, ::BNNODE) takes no maxiters, callback, chunk or device_loop")
