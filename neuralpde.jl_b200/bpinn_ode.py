@@ -10,22 +10,18 @@ WeightedIntervalTraining draw fresh times on the device before every evaluation 
 from __future__ import annotations
 
 import math
-from types import SimpleNamespace
 from typing import List, Optional
 
 import numpy as np
 import sympy as sp
 
 from . import engine as _eng
-from .engine import Engine, NetSpec, ProblemSpec, TapSpec, TermSpec, REDUCE_MEAN, REDUCE_WSUM
-from .ode import ODEProblem, _Lowering
-from .pinn import (BPINNsolution, BPINNstats, DiagEuclideanMetric, HMC, Leapfrog, MODES, NoAdaptation, StanHMCAdaptor,
-                   UnitEuclideanMetric, _tail_priors, initialparameters)
+from .engine import Engine, TapSpec, TermSpec, REDUCE_MEAN, REDUCE_WSUM
+from .ode import ODEProblem, _Evaluator, _Lowering, _TrialRepresentation, _check_mode, _init_array
+from .pinn import BPINNsolution, BPINNstats, HMC, Leapfrog, _hmc_adaptation, _tail_priors, initialparameters
 from .strategies import (GridTraining, QuadratureTraining, StochasticTraining, WeightedIntervalTraining, _julia_range,
                          gauss_legendre_box)
 
-_BNNODE_MODES = ("ffma", "tc_f64")
-_DEFAULT_ADAPTOR = {"Adaptor": StanHMCAdaptor, "Metric": DiagEuclideanMetric, "targetacceptancerate": 0.8}
 _LOG2PI = math.log(2.0 * math.pi)
 _SEED_MIX = 0xD1B54A32D192ED03      # odd: seed -> sampler key is a bijection for a fixed strategy seed
 
@@ -63,7 +59,7 @@ def _sigma_monomials(phynewstd, p_arg, p_syms: List[sp.Symbol], n: int):
 
 
 # ---- the log density --------------------------------------------------------------------------------------------
-class BNNODELogDensity:
+class BNNODELogDensity(_TrialRepresentation):
     """The engine problem of ``LogTargetDensity``: terms (``term_names``, ``kinds``), weights ``c``, constant ``const``,
     θ0, the θ.p priors in forward order (``tail``), the log|θ.p| coefficients (``tail_logabs``) and the sampled terms'
     boxes (``sampled``: (term, n, lo, hi))."""
@@ -73,15 +69,11 @@ class BNNODELogDensity:
                  mode="ffma", device=0, seed=0):
         if not isinstance(prob, ODEProblem):
             raise TypeError("ahmc_bayesian_pinn_ode: prob must be an ODEProblem")
-        if mode not in MODES:
-            raise ValueError("unknown mode %r (one of %s)" % (mode, sorted(MODES)))
-        if mode not in _BNNODE_MODES:
-            raise ValueError("ahmc_bayesian_pinn_ode runs on the FFMA kernel: mode=\"ffma\" (or \"tc_f64\" for Float64); "
-                             "the tensor-core bf16 modes propagate 1-output networks")
+        _check_mode(mode, "ahmc_bayesian_pinn_ode", "the tensor-core bf16 modes propagate 1-output networks")
         param = list(param or [])
         ninv = len(param)
         dataset = list(dataset or [])
-        lw = _Lowering(prob, SimpleNamespace(param_estim=ninv > 0))
+        lw = _Lowering(prob, ninv > 0, ["t"])
         n = lw.n
         t0, t1 = prob.tspan
         if chain.dims[0] != 1 or chain.dims[-1] != n:
@@ -128,37 +120,19 @@ class BNNODELogDensity:
         if init_params is None:
             net0 = initialparameters(np.random.default_rng(seed), chain, np.float64)
         else:
-            net0 = np.asarray(init_params)
-            if np.iscomplexobj(net0):
-                raise ValueError("ahmc_bayesian_pinn_ode: complex parameters are not supported (the engine trains real "
-                                 "networks)")
-            if net0.dtype not in (np.float32, np.float64):
-                net0 = net0.astype(np.float64)
+            net0 = _init_array(init_params, mode, "ahmc_bayesian_pinn_ode")
             if net0.shape not in ((n_net,), (n_net + ninv,)):
                 raise ValueError("init_params has length %d, the chain needs %d" % (net0.size, n_net))
             net0 = net0[:n_net]
-        dtype = net0.dtype
-        if mode == "tc_f64" and dtype != np.float64:
-            raise ValueError("mode=\"tc_f64\" runs the layer products on the FP64 tensor cores and needs float64 "
-                             "parameters (init_params is %s); use mode=\"ffma\" for float32" % dtype.name)
         self.theta0 = np.concatenate([net0.astype(np.float64), [float(p.params()[0]) for p in param]])
 
-        specs: List[TermSpec] = []
-        self.point_sets: List[Optional[np.ndarray]] = []
-        self.quad_weights: List[Optional[np.ndarray]] = []
-        c: List[float] = []
-        names: List[str] = []
-        kinds: List[str] = []
-        self.sampled = []
+        super().__init__(prob, chain, strategy, lw, net0.dtype)
+        self.kinds: List[str] = []
         consts = {"phys": 0.0, "data": 0.0, "collocation": 0.0}
 
         def add(spec, pts, w, weight, name, kind):
-            specs.append(spec)
-            self.point_sets.append(None if pts is None else np.asarray(pts, dtype=np.float64).reshape(spec.dim, -1))
-            self.quad_weights.append(None if w is None else np.asarray(w, dtype=np.float64))
-            c.append(float(weight))
-            names.append(name)
-            kinds.append(kind)
+            self.add(spec, pts, w, weight, name)
+            self.kinds.append(kind)
 
         # physloglikelihood (:136-238): Σ_k logpdf(MvNormal(r_k(t), phystd_k^2 I), 0)
         res = lw.residuals()
@@ -186,7 +160,7 @@ class BNNODELogDensity:
             for i, (m, lo, hi) in enumerate(boxes):
                 if m < 1:
                     continue
-                self.sampled.append((len(specs), m, lo, hi))
+                self.sampled.append((len(self.specs), m, lo, hi))
                 add(lw.term(res[k], ["t"], REDUCE_MEAN), None, None, -0.5 * m / s2,
                     "phys_%d" % (k + 1) if len(boxes) == 1 else "phys_%d_interval_%d" % (k + 1, i + 1), "phys")
                 consts["phys"] += -0.5 * m * (_LOG2PI + math.log(s2))
@@ -220,16 +194,9 @@ class BNNODELogDensity:
                 add(lw.term(r * inv, rows, REDUCE_WSUM), pts, W * W, -0.5, "collocation_%d" % (k + 1), "collocation")
                 consts["collocation"] += -0.5 * t_d.size * _LOG2PI - t_d.size * math.log(abs(a_k))
                 logabs -= t_d.size * e_k
-        if len(specs) > _eng.MAX_TERMS:
-            raise ValueError("ahmc_bayesian_pinn_ode: %d log-likelihood terms (max %d)" % (len(specs), _eng.MAX_TERMS))
-
-        self.spec = ProblemSpec(nets=[NetSpec(chain.dims, chain.acts, 0)], terms=specs, n_params=ninv,
-                                param_offset=n_net, n_theta=n_net + ninv, dtype=dtype.name, mode=MODES[mode],
-                                device=device)
-        self.prob, self.chain, self.strategy, self.lowering = prob, chain, strategy, lw
-        self.n, self.n_net, self.ninv, self.dtype = n, n_net, ninv, dtype
-        self.specs, self.term_names, self.kinds = specs, names, kinds
-        self.c, self.consts, self.const = np.asarray(c), consts, float(sum(consts.values()))
+        self._close("ahmc_bayesian_pinn_ode", ninv, mode, device, "log-likelihood terms")
+        self.ninv = ninv
+        self.consts, self.const = consts, float(sum(consts.values()))
         self.tail = tail
         self.tail_logabs = logabs if np.any(logabs != 0) else None
         self.dataset = dataset
@@ -237,20 +204,15 @@ class BNNODELogDensity:
         # the device samplers' key: the strategy's seed, mixed with the chain's seed so that chains with different
         # seeds see independent point draws (seed = 0 leaves the strategy's draws as NNODE makes them)
         self.sampler_seed = (int(getattr(strategy, "seed", 0)) + _SEED_MIX * int(seed)) % 2 ** 64
-        self._engine = None
 
     @property
-    def engine(self) -> Engine:
-        """The engine handle: every fixed point set uploaded, the sampled terms' device samplers registered"""
-        if self._engine is None:
-            eng = Engine(self.spec)
-            for i, (X, w) in enumerate(zip(self.point_sets, self.quad_weights)):
-                if X is not None:
-                    eng.set_points_host(i, X.astype(self.dtype), None if w is None else w.astype(self.dtype))
-            for i, m, lo, hi in self.sampled:
-                eng.set_sampler(i, m, [lo], [hi], self.sampler_seed)
-            self._engine = eng
-        return self._engine
+    def c(self) -> np.ndarray:
+        """the terms' fixed weights c_k"""
+        return self.term_weights
+
+    def _set_samplers(self, eng: Engine):
+        for i, m, lo, hi in self.sampled:
+            eng.set_sampler(i, m, [lo], [hi], self.sampler_seed)
 
     def pieces(self, theta, prior_mean: float, prior_std: float) -> dict:
         """The reference's four log-density parts at θ on the handle's current points: "phys", "prior", "data",
@@ -302,23 +264,15 @@ def ahmc_bayesian_pinn_ode(prob: ODEProblem, chain, *, strategy=GridTraining, da
     reference uses the global RNG), ``mode`` is "ffma" or "tc_f64".  d/dt is exact for both ``autodiff`` values (the
     reference's default is a forward difference).  ``phynewstd(p)`` must return constants or monomials in p.
     Refused with a message: NUTS / HMCDA, several chains, DenseEuclideanMetric, jittered / tempered leapfrog."""
-    ak = dict(_DEFAULT_ADAPTOR, **(Adaptorkwargs or {}))
     ik = dict(Integratorkwargs or {"Integrator": Leapfrog})
     mk = dict({"n_leapfrog": 30}, **(MCMCkwargs or {}))
     if not (Kernel is HMC or isinstance(Kernel, HMC)):
         raise ValueError("ahmc_bayesian_pinn_ode: Kernel %r is not implemented; the device sampler runs HMC with "
                          "MCMCkwargs n_leapfrog (NUTS and HMCDA are not supported)" % (Kernel,))
-    if ak["Adaptor"] not in (StanHMCAdaptor, NoAdaptation):
-        raise ValueError("ahmc_bayesian_pinn_ode: Adaptor %r is not implemented (StanHMCAdaptor or NoAdaptation)"
-                         % (ak["Adaptor"],))
-    if ak["Metric"] not in (DiagEuclideanMetric, UnitEuclideanMetric):
-        raise ValueError("ahmc_bayesian_pinn_ode: Metric %r is not implemented; DenseEuclideanMetric is not supported "
-                         "(DiagEuclideanMetric or UnitEuclideanMetric)" % (ak["Metric"],))
+    adaptor, metric, target_accept = _hmc_adaptation(Adaptorkwargs, nchains, "ahmc_bayesian_pinn_ode")
     if ik.get("Integrator", Leapfrog) is not Leapfrog or set(ik) - {"Integrator"}:
         raise ValueError("ahmc_bayesian_pinn_ode: Integratorkwargs %r are not implemented; JitteredLeapfrog / "
                          "TemperedLeapfrog (jitter_rate, tempering_rate) are not supported (Leapfrog)" % (ik,))
-    if nchains != 1:
-        raise ValueError("ahmc_bayesian_pinn_ode: nchains = %r; one chain per call is supported" % (nchains,))
     draw_samples = int(draw_samples)
     if draw_samples < 1:
         raise ValueError("ahmc_bayesian_pinn_ode: draw_samples = %d must be >= 1" % draw_samples)
@@ -339,11 +293,8 @@ def ahmc_bayesian_pinn_ode(prob: ODEProblem, chain, *, strategy=GridTraining, da
     if verbose:
         report("Current", th0)
     eng = ld.engine
-    eng.hmc_begin(th0, n_leapfrog=int(mk["n_leapfrog"]),
-                  adaptor=_eng.HMC_ADAPT_STAN if ak["Adaptor"] is StanHMCAdaptor else _eng.HMC_ADAPT_NONE,
-                  metric=_eng.HMC_METRIC_DIAG if ak["Metric"] is DiagEuclideanMetric else _eng.HMC_METRIC_UNIT,
-                  n_adapts=min(draw_samples // 10, 1000), target_accept=float(ak["targetacceptancerate"]),
-                  step_size=0.0, prior_mean=mu_p, prior_std=sd_p, seed=seed, weights=ld.c, ll_const=ld.const,
+    eng.hmc_begin(th0, n_leapfrog=int(mk["n_leapfrog"]), adaptor=adaptor, metric=metric,
+                  n_adapts=min(draw_samples // 10, 1000), target_accept=target_accept, step_size=0.0, prior_mean=mu_p, prior_std=sd_p, seed=seed, weights=ld.c, ll_const=ld.const,
                   tail_priors=ld.tail or None, tail_logabs=ld.tail_logabs, redraw=bool(ld.sampled))
     samples, st = eng.hmc_iterate(draw_samples)
     stats = {name: st[:, j].copy() for j, name in enumerate(_eng.HMC_STATS)}
@@ -377,16 +328,12 @@ class BNNODE:
 def _network_outputs(chain, dtype, device, ts: np.ndarray, thetas: np.ndarray) -> np.ndarray:
     """N(t) for each row of thetas (network parameters): [len(thetas), n_out, len(ts)], one value-only term per output"""
     n_out = chain.dims[-1]
-    terms = [TermSpec(dim=1, taps=[TapSpec(net=0, order=0, out=k)], prog=[("tap", 0, 0, 0.0)], net_rows=[[0]])
-             for k in range(n_out)]
-    eng = Engine(ProblemSpec(nets=[NetSpec(chain.dims, chain.acts, 0)], terms=terms, n_theta=chain.n_params,
-                             dtype=np.dtype(dtype).name, device=device))
-    for k in range(n_out):
-        eng.set_points_host(k, ts.reshape(1, -1).astype(dtype))
+    network = _Evaluator([TermSpec(dim=1, taps=[TapSpec(net=0, order=0, out=k)], prog=[("tap", 0, 0, 0.0)],
+                                   net_rows=[[0]]) for k in range(n_out)], chain, 0, dtype, device)
+    network.at(ts)
     out = np.empty((len(thetas), n_out, ts.size))
     for i, th in enumerate(thetas):
-        for k in range(n_out):
-            out[i, k] = eng.term_residual_host(k, np.asarray(th, dtype=dtype), ts.size)
+        out[i] = network(th)
     return out
 
 

@@ -6,6 +6,11 @@ The trial solution is φ(t) = u0 + (t - t0) · N(t) for one network N with one o
 dφ_k/dt - f_k(φ, p, t) = N_k + (t - t0) ∂N_k/∂t - f_k(u0 + (t - t0) N, p, t), is lowered by the equation emitter of
 lowering.py to value and d/dt taps of output k.  Every loss and gradient evaluation is one launch of the FFMA kernel.
 DESIGN section 4.12 maps the reference's loss terms onto the engine's terms.
+
+This module also holds the front end that NNODE, NNSDE (sde.py) and BNNODE (bpinn_ode.py) share: the problem checks
+(``_TrialProblem``), the lowering of φ and its residuals (``_Lowering``), the term table and engine handle
+(``_TrialRepresentation``), the value-only evaluator (``_Evaluator``), the strategy, mode and init_params checks, the
+analytic errors and the optimizer loops (``_train``).
 """
 from __future__ import annotations
 
@@ -24,9 +29,6 @@ from .strategies import (GridTraining, QuadratureTraining, QuasiRandomTraining, 
                          WeightedIntervalTraining, _julia_range, gauss_legendre_box)
 from .symbolic import VarInfo, expand_derivatives
 
-# the modes that run the FFMA kernel; the tensor-core modes propagate 1-output networks only
-_NNODE_MODES = ("ffma", "tc_f64")
-
 
 # ---- problem and algorithm ------------------------------------------------------------------------------------
 @dataclass
@@ -36,35 +38,55 @@ class ODEFunction:
     analytic: Optional[Callable] = None
 
 
-@dataclass
-class ODEProblem:
-    """``ODEProblem(f, u0, tspan, p)``: ``u0`` a number or a vector, ``f(u, p, t)`` out-of-place."""
-    f: object
-    u0: object
-    tspan: Sequence[float]
-    p: object = None
+class _TrialProblem:
+    """What ODEProblem and SDEProblem share: the checks of their fields, ``scalar``, and the name and out-of-place
+    message of the solver that traces their functions of (u, p, t)"""
+    _solver = "NNODE"
+    _out_of_place = "The NNODE solver only supports out-of-place ODE definitions, i.e. du=f(u,p,t)."
+    _components_note = ""      # appended to the component-count refusal
+    _traced = ("f",)           # the functions of (u, p, t) the solver traces
 
     def __post_init__(self):
         if not isinstance(self.f, ODEFunction):
             self.f = ODEFunction(self.f)
         if _has_complex(self.u0) or _has_complex(self.p):
-            raise ValueError("NNODE: complex u0 or p are not supported (the engine trains real networks)")
-        f = self.f.f
-        try:
-            n_args = len(inspect.signature(f).parameters)
-        except (TypeError, ValueError):
-            n_args = 3
-        if n_args == 4:
-            raise ValueError("The NNODE solver only supports out-of-place ODE definitions, i.e. du=f(u,p,t).")
+            raise ValueError("%s: complex u0 or p are not supported (the engine trains real networks)" % self._solver)
+        for name in self._traced:
+            try:
+                n_args = len(inspect.signature(self._function(name)).parameters)
+            except (TypeError, ValueError):
+                n_args = 3
+            if n_args == 4:
+                raise ValueError(self._out_of_place)
         self.tspan = (float(self.tspan[0]), float(self.tspan[1]))
+
+    def _function(self, name: str) -> Callable:
+        return self.f.f if name == "f" else getattr(self, name)
 
     @property
     def scalar(self) -> bool:
         return np.ndim(self.u0) == 0
 
 
+@dataclass
+class ODEProblem(_TrialProblem):
+    """``ODEProblem(f, u0, tspan, p)``: ``u0`` a number or a vector, ``f(u, p, t)`` out-of-place."""
+    f: object
+    u0: object
+    tspan: Sequence[float]
+    p: object = None
+
+
 def _has_complex(p) -> bool:
     return p is not None and any(isinstance(v, complex) or np.iscomplexobj(v) for v in np.ravel(np.asarray(p, dtype=object)))
+
+
+def _check_mode(mode: str, who: str, why: str):
+    """The ODE family runs on the FFMA kernel (``ffma``, or ``tc_f64`` for Float64); `why` says why the others cannot"""
+    if mode not in MODES:
+        raise ValueError("unknown mode %r (one of %s)" % (mode, sorted(MODES)))
+    if mode not in ("ffma", "tc_f64"):
+        raise ValueError("%s runs on the FFMA kernel: mode=\"ffma\" (or \"tc_f64\" for Float64); %s" % (who, why))
 
 
 class NNODE:
@@ -81,11 +103,8 @@ class NNODE:
         self.param_estim, self.additional_loss = bool(param_estim), additional_loss
         self.dataset, self.estim_collocate = list(dataset), bool(estim_collocate)
         self.mode, self.device, self.seed = mode, device, seed
-        if mode not in MODES:
-            raise ValueError("unknown mode %r (one of %s)" % (mode, sorted(MODES)))
-        if mode not in _NNODE_MODES:
-            raise ValueError("NNODE runs on the FFMA kernel: mode=\"ffma\" (or \"tc_f64\" for Float64); the tensor-core "
-                             "modes propagate 1-output networks, NNODE's network has one output per component")
+        _check_mode(mode, "NNODE", "the tensor-core modes propagate 1-output networks, NNODE's network has one output "
+                                   "per component")
         if additional_loss is not None and not isinstance(additional_loss, DataLoss):
             raise ValueError("NNODE: additional_loss must be a DataLoss(depvar=k, points=t, values=u_k) with a component "
                              "index k in place of the depvar name (the structured form of the reference's "
@@ -122,34 +141,12 @@ class OptimizationSolution:
     retcode: str
 
 
-# ---- tracing f --------------------------------------------------------------------------------------------------
+# ---- the trial solution and its residuals -----------------------------------------------------------------------
 T_SYM = sp.Symbol("t", real=True)
-
-
-def _trace(prob: ODEProblem, u_syms, p_arg) -> List[sp.Expr]:
-    """f(u, p, t) with symbols, as a list of one expression per component"""
-    try:
-        out = prob.f.f(u_syms, p_arg, T_SYM)
-    except Exception as ex:      # noqa: BLE001 -- any failure to trace is the user's f, reported with its message
-        raise ValueError("NNODE: f(u, p, t) could not be traced with symbolic u, p and t (write it with sympy "
-                         "functions such as sympy.cos): %s: %s" % (type(ex).__name__, ex)) from ex
-    if out is None:
-        raise ValueError("The NNODE solver only supports out-of-place ODE definitions, i.e. du=f(u,p,t).")
-    n = 1 if prob.scalar else len(np.ravel(prob.u0))
-    outs = list(np.ravel(np.asarray(out, dtype=object)))      # a number, or a sequence of one for a scalar u0
-    if len(outs) != n:
-        raise ValueError("NNODE: f returns %d components, u0 has %d" % (len(outs), n))
-    exprs = [sp.sympify(e) for e in outs]
-    for e in exprs:
-        if e.has(sp.I) or any(a.is_real is False for a in e.atoms(sp.Number)):
-            raise ValueError("NNODE: f is complex-valued; the engine trains real networks")
-    return exprs
 
 
 def _p_symbols(p):
     """θ.p symbols shaped like the problem's p (a number or a vector)"""
-    if p is None:
-        raise ValueError("NNODE: param_estim starts θ.p at the problem's p, and the problem has none")
     if np.ndim(p) == 0:
         return sp.Symbol("p1", real=True), ["p1"]
     names = ["p%d" % (i + 1) for i in range(len(np.ravel(p)))]
@@ -157,22 +154,48 @@ def _p_symbols(p):
 
 
 class _Lowering:
-    """The symbols of the network outputs N_k(t) and the rows / parameters the emitter reads."""
+    """The trial solution φ_k = u0_k + (t - t0) N_k of one network N whose inputs are the point rows `rows` (["t"] for
+    NNODE and BNNODE, ["t", "z1", ...] for NNSDE): the symbols of N's outputs, the θ.p symbols under `param_estim`,
+    the residuals of the problem's f and the TermSpec of an expression in them"""
 
-    def __init__(self, prob: ODEProblem, alg: NNODE):
-        self.prob = prob
+    def __init__(self, prob: _TrialProblem, param_estim: bool, rows: List[str]):
+        self.prob, self.rows = prob, list(rows)
         self.n = 1 if prob.scalar else len(np.ravel(prob.u0))
         self.u0 = np.ravel(np.asarray(prob.u0, dtype=np.float64))
         self.t0 = prob.tspan[0]
-        self.N = [sp.Function("N%d" % (k + 1))(T_SYM) for k in range(self.n)]
+        self.N = [sp.Function("N%d" % (k + 1))(*[sp.Symbol(r, real=True) for r in self.rows]) for k in range(self.n)]
         names = ["N%d" % (k + 1) for k in range(self.n)]
-        self.vi = VarInfo(depvars=names, indvars=["t"], dict_indvars={"t": 0},
-                          dict_depvars={nm: k for k, nm in enumerate(names)}, dict_depvar_input={nm: ["t"] for nm in names})
-        if alg.param_estim:
+        self.vi = VarInfo(depvars=names, indvars=list(self.rows), dict_indvars={r: i for i, r in enumerate(self.rows)},
+                          dict_depvars={nm: k for k, nm in enumerate(names)},
+                          dict_depvar_input={nm: list(self.rows) for nm in names})
+        if param_estim:
+            if prob.p is None:
+                raise ValueError("%s: param_estim starts θ.p at the problem's p, and the problem has none" % prob._solver)
             self.p_arg, pnames = _p_symbols(prob.p)
             self.param_index = {nm: i for i, nm in enumerate(pnames)}
         else:
             self.p_arg, self.param_index = prob.p, {}
+
+    def _trace(self, name: str, comps: List[sp.Expr]) -> List[sp.Expr]:
+        """the problem's function `name` (f or g) of (u, p, t) at u = comps, with symbols: one expression per
+        component"""
+        who = self.prob._solver
+        try:
+            out = self.prob._function(name)(comps[0] if self.prob.scalar else list(comps), self.p_arg, T_SYM)
+        except Exception as ex:      # noqa: BLE001 -- any failure to trace is the user's function, reported with its message
+            raise ValueError("%s: %s(u, p, t) could not be traced with symbolic u, p and t (write it with sympy "
+                             "functions such as sympy.cos): %s: %s" % (who, name, type(ex).__name__, ex)) from ex
+        if out is None:
+            raise ValueError(self.prob._out_of_place)
+        outs = list(np.ravel(np.asarray(out, dtype=object)))      # a number, or a sequence of one for a scalar u0
+        if len(outs) != self.n:
+            raise ValueError("%s: %s returns %d components, u0 has %d%s"
+                             % (who, name, len(outs), self.n, self.prob._components_note))
+        exprs = [sp.sympify(e) for e in outs]
+        for e in exprs:
+            if e.has(sp.I) or any(a.is_real is False for a in e.atoms(sp.Number)):
+                raise ValueError("%s: %s is complex-valued; the engine trains real networks" % (who, name))
+        return exprs
 
     def phi(self, k: int) -> sp.Expr:
         return self.u0[k] + (T_SYM - self.t0) * self.N[k]
@@ -180,37 +203,172 @@ class _Lowering:
     def dphi(self, k: int) -> sp.Expr:
         return self.N[k] + (T_SYM - self.t0) * sp.Derivative(self.N[k], T_SYM)
 
-    def u_arg(self, comps: List[sp.Expr]):
-        return comps[0] if self.prob.scalar else list(comps)
-
     def residuals(self) -> List[sp.Expr]:
         """r_k = dφ_k/dt - f_k(φ, p, t)"""
-        fs = _trace(self.prob, self.u_arg([self.phi(k) for k in range(self.n)]), self.p_arg)
+        fs = self._trace("f", [self.phi(k) for k in range(self.n)])
         return [self.dphi(k) - fs[k] for k in range(self.n)]
 
     def collocation_residuals(self) -> List[sp.Expr]:
         """dφ_k/dt - f_k(û, θ.p, t), û read from point rows 1..n (the observations)"""
-        uh = [sp.Symbol("uhat%d" % (j + 1), real=True) for j in range(self.n)]
-        fs = _trace(self.prob, self.u_arg(uh), self.p_arg)
+        fs = self._trace("f", [sp.Symbol("uhat%d" % (j + 1), real=True) for j in range(self.n)])
         return [self.dphi(k) - fs[k] for k in range(self.n)]
 
     def term(self, expr: sp.Expr, rows: List[str], reduction: int, scale: float = 1.0) -> TermSpec:
-        """TermSpec of the residual expr over point rows `rows`; taps of N_k become taps of output k of network 0"""
+        """TermSpec of the residual expr over point rows `rows`; taps of N_k become taps of output k of network 0, whose
+        inputs are the lowering's rows.  A residual without taps is a parameter-only term, which the engine accepts
+        only if it reads θ.p (NNSDE's Euler-Maruyama loss).  NNODE's and BNNODE's residuals always have taps: f sees φ
+        or û but never ∂N/∂t, so it cannot cancel the (t - t0) ∂N_k/∂t of dφ_k/dt, nor the N_k of φ_k - x̂."""
         em = _Emitter(self.vi, rows, self.param_index, {})
         try:
             v = em.emit(expand_derivatives(expr))
         except LoweringError as ex:
-            raise ValueError("NNODE: %s" % ex) from ex
+            raise ValueError("%s: %s" % (self.prob._solver, ex)) from ex
         em.prog.append(("sub", v, em.const(0.0), 0.0))       # the last instruction is the residual
         taps = [TapSpec(net=0, order=tp.order, dirs=tp.dirs, out=tp.net) for tp in em.taps]
-        if not taps:
-            raise ValueError("NNODE: the residual %s reads no network output" % expr)
-        return TermSpec(dim=len(rows), taps=taps, prog=em.prog, net_rows=[[rows.index("t")]], reduction=reduction,
+        return TermSpec(dim=len(rows), taps=taps, prog=em.prog,
+                        net_rows=[[rows.index(r) for r in self.rows]] if taps else None, reduction=reduction,
                         scale=scale)
 
 
+class _Evaluator:
+    """A value-only engine of one network: the value-only terms `terms` (one per quantity, all over the same point
+    rows) evaluated at the columns of the point matrix given to ``at``, for one θ per call"""
+
+    def __init__(self, terms: List[TermSpec], chain, n_params: int, dtype, device: int):
+        self.n_rows, self.dtype = terms[0].dim, np.dtype(dtype)
+        self.engine = Engine(ProblemSpec(nets=[NetSpec(chain.dims, chain.acts, 0)], terms=terms, n_params=n_params,
+                                         param_offset=chain.n_params, n_theta=chain.n_params + n_params,
+                                         dtype=self.dtype.name, mode=_eng.MODE_FFMA, device=device))
+        self.m = 0
+
+    def at(self, X):
+        """evaluate at the columns of X, (rows, m) or, with one row, any shape of m values"""
+        X = np.asarray(X, dtype=np.float64).reshape(self.n_rows, -1).astype(self.dtype)
+        for k in range(len(self.engine.spec.terms)):
+            self.engine.set_points_host(k, X)
+        self.m = X.shape[1]
+
+    def __call__(self, theta) -> np.ndarray:
+        """(len(terms), m) values at θ"""
+        th = np.asarray(theta, dtype=self.dtype)
+        out = np.empty((len(self.engine.spec.terms), self.m))
+        for k in range(out.shape[0]):
+            out[k] = self.engine.term_residual_host(k, th, self.m)
+        return out
+
+
 # ---- the engine problem -----------------------------------------------------------------------------------------
-class NNODERepresentation:
+def _strategy(alg, dt):
+    """NNODE's and NNSDE's training strategy (src/ode_solve.jl:439-451): alg.strategy, by default GridTraining(dt)
+    with a dt and QuadratureTraining without, and its refusals"""
+    strategy = alg.strategy
+    if strategy is None:
+        strategy = GridTraining(dt) if dt is not None else QuadratureTraining()
+    if isinstance(strategy, QuasiRandomTraining):
+        raise ValueError("QuasiRandomTraining is not supported by NNODE since it's for high dimensional spaces only. "
+                         "Use StochasticTraining instead.")
+    if alg.autodiff:
+        for cls in (GridTraining, StochasticTraining, WeightedIntervalTraining):
+            if isinstance(strategy, cls):
+                raise ValueError("autodiff not supported for %s." % cls.__name__)
+    if not isinstance(strategy, (GridTraining, StochasticTraining, WeightedIntervalTraining, QuadratureTraining)):
+        raise TypeError("unsupported training strategy %r" % (strategy,))
+    return strategy
+
+
+def _init_array(init_params, mode: str, who: str) -> np.ndarray:
+    """init_params as a float32 or float64 array (other real dtypes become float64), as PhysicsInformedNN takes them;
+    complex parameters, and float32 ones under tc_f64, are refused"""
+    init = np.asarray(init_params)
+    if np.iscomplexobj(init):
+        raise ValueError("%s: complex parameters are not supported (the engine trains real networks)" % who)
+    if init.dtype not in (np.float32, np.float64):
+        init = init.astype(np.float64)
+    if mode == "tc_f64" and init.dtype != np.float64:
+        raise ValueError("mode=\"tc_f64\" runs the layer products on the FP64 tensor cores and needs float64 "
+                         "parameters (init_params is %s); use mode=\"ffma\" for float32" % init.dtype.name)
+    return init
+
+
+def _theta0(alg, chain, p0: np.ndarray, who: str) -> np.ndarray:
+    """NNODE's and NNSDE's θ0 = [depvar, p] (ComponentArray(; depvar, p), src/ode_solve.jl:431-435): θ.p starts at
+    p0 unless init_params gives it"""
+    n_net = chain.n_params
+    if alg.init_params is None:
+        return np.concatenate([initialparameters(np.random.default_rng(alg.seed), chain, np.float64), p0])
+    init = _init_array(alg.init_params, alg.mode, who)
+    if init.shape == (n_net,):
+        init = np.concatenate([init, p0.astype(init.dtype)])
+    if init.shape != (n_net + p0.size,):
+        raise ValueError("init_params has length %d, the chain%s needs %d"
+                         % (init.size, " + p" if p0.size else "", n_net + p0.size))
+    return init
+
+
+class _TrialRepresentation:
+    """What the engine problems of NNODE, NNSDE and BNNODE share: the term table (``specs``, ``point_sets``,
+    ``quad_weights``, ``term_weights``, ``term_names``) that ``add`` fills and ``_close`` turns into the ProblemSpec;
+    the engine handle, created at first use with every fixed point set uploaded and the sampled terms' device
+    samplers registered by the subclass's ``_set_samplers``; ``loss_grad`` and ``trial``."""
+
+    def __init__(self, prob: _TrialProblem, chain, strategy, lowering: _Lowering, dtype):
+        self.prob, self.chain, self.strategy, self.lowering, self.dtype = prob, chain, strategy, lowering, dtype
+        self.n, self.n_net = lowering.n, chain.n_params
+        self.specs: List[TermSpec] = []
+        self.point_sets: List[Optional[np.ndarray]] = []
+        self.quad_weights: List[Optional[np.ndarray]] = []
+        self.term_weights: List[float] = []      # an array once closed
+        self.term_names: List[str] = []
+        self.sampled: list = []
+        self._engine, self._calls, self._phi = None, 0, None
+
+    def add(self, spec: TermSpec, pts, w, weight: float, name: str):
+        self.specs.append(spec)
+        self.point_sets.append(None if pts is None else np.asarray(pts, dtype=np.float64).reshape(spec.dim, -1))
+        self.quad_weights.append(None if w is None else np.asarray(w, dtype=np.float64))
+        self.term_weights.append(float(weight))
+        self.term_names.append(name)
+
+    def _close(self, who: str, n_params: int, mode: str, device: int, what: str = "loss terms"):
+        if len(self.specs) > _eng.MAX_TERMS:
+            raise ValueError("%s: %d %s (max %d)" % (who, len(self.specs), what, _eng.MAX_TERMS))
+        self.term_weights = np.asarray(self.term_weights)
+        self.spec = ProblemSpec(nets=[NetSpec(self.chain.dims, self.chain.acts, 0)], terms=self.specs,
+                                n_params=n_params, param_offset=self.n_net, n_theta=self.n_net + n_params,
+                                dtype=self.dtype.name, mode=MODES[mode], device=device)
+
+    @property
+    def engine(self) -> Engine:
+        """The engine handle, created at first use with every fixed point set uploaded and the sampled terms' device
+        samplers registered"""
+        if self._engine is None:
+            eng = Engine(self.spec)
+            for i, (X, w) in enumerate(zip(self.point_sets, self.quad_weights)):
+                if X is not None:
+                    eng.set_points_host(i, X.astype(self.dtype), None if w is None else w.astype(self.dtype))
+            self._set_samplers(eng)
+            self._engine = eng
+        return self._engine
+
+    def loss_grad(self, theta, want_grad: bool = True):
+        """(total of the engine's terms, term losses, gradient or None) at θ: one fused launch (a fresh sample of the
+        sampled terms each call after the first, as the reference draws one per loss call)"""
+        if self.sampled and self._calls > 0:
+            self.engine.resample()
+        self._calls += 1
+        return self.engine.loss_grad_host(np.asarray(theta, dtype=self.dtype), self.term_weights, want_grad)
+
+    def trial(self, theta, X) -> np.ndarray:
+        """φ at the columns of the (rows, m) inputs X (NNODE: any shape of m times), (n, m), evaluated on the device"""
+        if self._phi is None:
+            lw = self.lowering
+            self._phi = _Evaluator([lw.term(lw.phi(k), lw.rows, REDUCE_MEAN) for k in range(self.n)], self.chain,
+                                   self.spec.n_params, self.dtype, self.spec.device)
+        self._phi.at(X)
+        return self._phi(theta)
+
+
+class NNODERepresentation(_TrialRepresentation):
     """The engine problem of one ``solve(prob, alg)``: terms (``term_names``), their weights, point sets and θ0.
     ``loss_grad(θ)`` is one evaluation (a fresh stochastic sample each call, as the reference draws one per loss call)."""
 
@@ -218,26 +376,13 @@ class NNODERepresentation:
         if not isinstance(alg, NNODE):
             raise TypeError("solve(::ODEProblem, alg): alg must be an NNODE")
         chain = alg.chain
-        lw = _Lowering(prob, alg)
+        lw = _Lowering(prob, alg.param_estim, ["t"])
         n = lw.n
         t0, t1 = prob.tspan
         if chain.dims[0] != 1 or chain.dims[-1] != n:
             raise ValueError("NNODE: the chain maps t to the %d components of u0: it needs 1 input and %d outputs, has "
                              "%d and %d" % (n, n, chain.dims[0], chain.dims[-1]))
-
-        # strategy (src/ode_solve.jl:439-451) and its refusals
-        strategy = alg.strategy
-        if strategy is None:
-            strategy = GridTraining(dt) if dt is not None else QuadratureTraining()
-        if isinstance(strategy, QuasiRandomTraining):
-            raise ValueError("QuasiRandomTraining is not supported by NNODE since it's for high dimensional spaces only. "
-                             "Use StochasticTraining instead.")
-        if alg.autodiff:
-            for cls in (GridTraining, StochasticTraining, WeightedIntervalTraining):
-                if isinstance(strategy, cls):
-                    raise ValueError("autodiff not supported for %s." % cls.__name__)
-        if not isinstance(strategy, (GridTraining, StochasticTraining, WeightedIntervalTraining, QuadratureTraining)):
-            raise TypeError("unsupported training strategy %r" % (strategy,))
+        strategy = _strategy(alg, dt)
 
         # dataset (src/ode_solve.jl:455-464)
         ds = alg.dataset
@@ -255,44 +400,11 @@ class NNODERepresentation:
             raise ValueError("Invalid dataset: %d observation vectors for %d components (dataset = [x̂_1, ..., x̂_n, t, W])"
                              % (len(ds) - 2, n))
 
-        # θ = [depvar, p] (ComponentArray(; depvar, p), :431-435); dtype as PhysicsInformedNN
-        n_net = chain.n_params
         p0 = np.ravel(np.asarray(prob.p, dtype=np.float64)) if alg.param_estim else np.zeros(0)
-        if alg.init_params is None:
-            flat = np.concatenate([initialparameters(np.random.default_rng(alg.seed), chain, np.float64), p0])
-        else:
-            init = np.asarray(alg.init_params)
-            if np.iscomplexobj(init):
-                raise ValueError("NNODE: complex parameters are not supported (the engine trains real networks)")
-            if init.dtype not in (np.float32, np.float64):
-                init = init.astype(np.float64)
-            if init.shape == (n_net,):
-                init = np.concatenate([init, p0.astype(init.dtype)])
-            if init.shape != (n_net + p0.size,):
-                raise ValueError("init_params has length %d, the chain%s needs %d"
-                                 % (init.size, " + p" if p0.size else "", n_net + p0.size))
-            flat = init
-        dtype = flat.dtype
-        if alg.mode == "tc_f64" and dtype != np.float64:
-            raise ValueError("mode=\"tc_f64\" runs the layer products on the FP64 tensor cores and needs float64 "
-                             "parameters (init_params is %s); use mode=\"ffma\" for float32" % dtype.name)
-
-        # terms, point sets, weights, names
-        specs: List[TermSpec] = []
-        sets: List[Optional[np.ndarray]] = []
-        qw: List[Optional[np.ndarray]] = []
-        weights: List[float] = []
-        names: List[str] = []
+        flat = _theta0(alg, chain, p0, "NNODE")
+        super().__init__(prob, chain, strategy, lw, flat.dtype)
+        add = self.add
         res = lw.residuals()
-
-        def add(spec, pts, w, weight, name):
-            specs.append(spec)
-            sets.append(None if pts is None else np.asarray(pts, dtype=np.float64).reshape(spec.dim, -1))
-            qw.append(w)
-            weights.append(float(weight))
-            names.append(name)
-
-        sampled: List[int] = []      # StochasticTraining's terms
         if isinstance(strategy, QuadratureTraining):
             # ∫ abs2(inner_loss(t)) dt with inner_loss(t) = Σ_k r_k(t)^2 (:250): one term with residual Σ_k r_k^2
             X, w, _ = gauss_legendre_box((np.array([t0]), np.array([t1])), int(strategy.nodes_per_dim), np.float64)
@@ -309,7 +421,7 @@ class NNODERepresentation:
                 ts, n_orig = None, int(strategy.points)
             for k in range(n):
                 if ts is None:     # fresh uniform points in [t0, t1] at every evaluation (:283-294), drawn on the device
-                    sampled.append(len(specs))
+                    self.sampled.append(len(self.specs))
                     add(lw.term(res[k], ["t"], REDUCE_MEAN), None, None, 1.0 if alg.batch else n_orig, "residual_%d" % (k + 1))
                 else:
                     add(lw.term(res[k], ["t"], REDUCE_WSUM, 1.0 / ts.size if alg.batch else 1.0), ts, np.ones(ts.size),
@@ -340,67 +452,32 @@ class NNODERepresentation:
         if tstops is not None:
             tt = np.ravel(np.asarray(tstops, dtype=np.float64))
             if n_orig is not None:     # (L N + L_t N_t) / (N + N_t) (:482-499); Quadrature: L + L_t
-                weights = [w_ * n_orig / (n_orig + tt.size) for w_ in weights]
+                self.term_weights = [w_ * n_orig / (n_orig + tt.size) for w_ in self.term_weights]
             wt = 1.0 if n_orig is None else tt.size / (n_orig + tt.size)
             for k in range(n):
                 add(lw.term(res[k], ["t"], REDUCE_WSUM, 1.0 / tt.size if alg.batch else 1.0), tt, np.ones(tt.size),
                     wt, "tstops_%d" % (k + 1))
-        if len(specs) > _eng.MAX_TERMS:
-            raise ValueError("NNODE: %d loss terms (max %d)" % (len(specs), _eng.MAX_TERMS))
-
-        self.spec = ProblemSpec(nets=[NetSpec(chain.dims, chain.acts, 0)], terms=specs, n_params=p0.size,
-                                param_offset=n_net, n_theta=n_net + p0.size, dtype=dtype.name, mode=MODES[alg.mode],
-                                device=alg.device)
-        self.prob, self.alg, self.strategy, self.lowering = prob, alg, strategy, lw
-        self.n, self.n_net, self.dtype = n, n_net, dtype
-        self.specs, self.point_sets, self.quad_weights = specs, sets, qw
-        self.term_weights = np.asarray(weights)
-        self.term_names = names
-        self.sampled = sampled
+        self._close("NNODE", p0.size, alg.mode, alg.device)
+        self.alg = alg
         self.loss_const = 0.0      # added to every reported loss (NNSDE's constant Euler-Maruyama terms)
-        self.flat_init_params = ComponentVector(flat, n_net)
-        self._engine = None
-        self._calls = 0
+        self.flat_init_params = ComponentVector(flat, self.n_net)
 
-    @property
-    def engine(self) -> Engine:
-        """The engine handle, created at first use with every fixed point set uploaded and the stochastic terms'
-        device samplers registered"""
-        if self._engine is None:
-            eng = Engine(self.spec)
-            for i, (X, w) in enumerate(zip(self.point_sets, self.quad_weights)):
-                if X is not None:
-                    eng.set_points_host(i, X.astype(self.dtype), None if w is None else w.astype(self.dtype))
-            t0, t1 = self.prob.tspan
-            for i in self.sampled:
-                eng.set_sampler(i, int(self.strategy.points), [t0], [t1], int(self.strategy.seed))
-            self._engine = eng
-        return self._engine
+    def _set_samplers(self, eng: Engine):
+        t0, t1 = self.prob.tspan
+        for i in self.sampled:
+            eng.set_sampler(i, int(self.strategy.points), [t0], [t1], int(self.strategy.seed))
 
-    def loss_grad(self, theta, want_grad: bool = True):
-        """(total, term losses, gradient or None) at θ: one fused launch"""
-        if self.sampled and self._calls > 0:
-            self.engine.resample()
-        self._calls += 1
-        return self.engine.loss_grad_host(np.asarray(theta, dtype=self.dtype), self.term_weights, want_grad)
 
-    def trial(self, theta, ts) -> np.ndarray:
-        """φ(t) at the times ts, (n, len(ts)), evaluated on the device through value-only terms"""
-        ts = np.ravel(np.asarray(ts, dtype=np.float64))
-        if not hasattr(self, "_phi_engine"):
-            lw = self.lowering
-            terms = [lw.term(lw.phi(k), ["t"], REDUCE_MEAN) for k in range(self.n)]
-            self._phi_engine = Engine(ProblemSpec(nets=[NetSpec(self.alg.chain.dims, self.alg.chain.acts, 0)], terms=terms,
-                                                  n_params=self.spec.n_params, param_offset=self.n_net,
-                                                  n_theta=self.spec.n_theta, dtype=self.dtype.name,
-                                                  mode=_eng.MODE_FFMA, device=self.alg.device))
-        e = self._phi_engine
-        th = np.asarray(theta, dtype=self.dtype)
-        out = np.empty((self.n, ts.size))
-        for k in range(self.n):
-            e.set_points_host(k, ts.reshape(1, -1).astype(self.dtype))
-            out[k] = e.term_residual_host(k, th, ts.size)
-        return out
+def _analytic_errors(prob: _TrialProblem, ts: np.ndarray, U: np.ndarray) -> dict:
+    """SciMLBase's timeseries errors of the (n, len(ts)) values U against prob.f.analytic: the final, maximum and
+    root-mean-square errors; empty without an analytic solution"""
+    an = prob.f.analytic
+    if an is None:
+        return {}
+    A = np.stack([np.ravel(np.asarray(an(prob.u0, prob.p, float(ti)), dtype=np.float64)) for ti in ts], axis=1)
+    E = U - A
+    return {"final": float(np.mean(np.abs(E[:, -1]))), "l∞": float(np.max(np.abs(E))),
+            "l2": float(np.sqrt(np.mean(E ** 2)))}
 
 
 # ---- solution ---------------------------------------------------------------------------------------------------
@@ -416,14 +493,7 @@ class ODESolution:
         self.t = np.asarray(ts, dtype=np.float64)
         U = rep.trial(res.u, self.t)
         self.u = [float(U[0, i]) for i in range(self.t.size)] if rep.prob.scalar else [U[:, i].copy() for i in range(self.t.size)]
-        self.errors = {}
-        an = rep.prob.f.analytic
-        if an is not None:
-            A = np.stack([np.ravel(np.asarray(an(rep.prob.u0, rep.prob.p, float(ti)), dtype=np.float64))
-                          for ti in self.t], axis=1)
-            E = U - A
-            self.errors = {"final": float(np.mean(np.abs(E[:, -1]))), "l∞": float(np.max(np.abs(E))),
-                           "l2": float(np.sqrt(np.mean(E ** 2)))}
+        self.errors = _analytic_errors(rep.prob, self.t, U)
 
     def __call__(self, t, idxs=None):
         """φ(t): for a number t a number (scalar u0 or an integer idxs) or a vector; for an array of times one column

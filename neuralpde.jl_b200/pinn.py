@@ -1368,6 +1368,22 @@ def pmean(x) -> np.ndarray:
 _DEFAULT_ADAPTOR = {"Adaptor": StanHMCAdaptor, "Metric": DiagEuclideanMetric, "targetacceptancerate": 0.8}
 
 
+def _hmc_adaptation(Adaptorkwargs, nchains: int, who: str):
+    """The Adaptor / Metric / nchains options of the HMC samplers, checked: (adaptor, metric, target acceptance) for
+    Engine.hmc_begin"""
+    ak = dict(_DEFAULT_ADAPTOR, **(Adaptorkwargs or {}))
+    if ak["Adaptor"] not in (StanHMCAdaptor, NoAdaptation):
+        raise ValueError("%s: Adaptor %r is not implemented (StanHMCAdaptor or NoAdaptation)" % (who, ak["Adaptor"]))
+    if ak["Metric"] not in (DiagEuclideanMetric, UnitEuclideanMetric):
+        raise ValueError("%s: Metric %r is not implemented; DenseEuclideanMetric is not supported "
+                         "(DiagEuclideanMetric or UnitEuclideanMetric)" % (who, ak["Metric"]))
+    if nchains != 1:
+        raise ValueError("%s: nchains = %r; one chain per call is supported" % (who, nchains))
+    return (_eng.HMC_ADAPT_STAN if ak["Adaptor"] is StanHMCAdaptor else _eng.HMC_ADAPT_NONE,
+            _eng.HMC_METRIC_DIAG if ak["Metric"] is DiagEuclideanMetric else _eng.HMC_METRIC_UNIT,
+            float(ak["targetacceptancerate"]))
+
+
 def ahmc_bayesian_pinn_pde(pde_system: PDESystem, discretization: BayesianPINN, *, draw_samples: int = 1000,
                            bcstd=(0.01,), l2std=(0.05,), phystd=(0.05,), phynewstd=(0.05,), priorsNNw=(0.0, 2.0),
                            param=(), nchains: int = 1, Kernel=None, Adaptorkwargs=None, Integratorkwargs=None,
@@ -1390,22 +1406,14 @@ def ahmc_bayesian_pinn_pde(pde_system: PDESystem, discretization: BayesianPINN, 
     Not supported (refused with a message): NUTS / HMCDA kernels, ``DenseEuclideanMetric``, jittered / tempered
     leapfrog, several chains, ``Dict_differentials`` and an ``additional_loss``."""
     Kernel = HMC() if Kernel is None else Kernel
-    ak = dict(_DEFAULT_ADAPTOR, **(Adaptorkwargs or {}))
     ik = dict({"Integrator": Leapfrog}, **(Integratorkwargs or {}))
     if not isinstance(Kernel, HMC):
         raise ValueError("ahmc_bayesian_pinn_pde: Kernel %r is not implemented; the device sampler runs HMC(ϵ, n_leapfrog) "
                          "(NUTS and HMCDA are not supported)" % (Kernel,))
-    if ak["Adaptor"] not in (StanHMCAdaptor, NoAdaptation):
-        raise ValueError("ahmc_bayesian_pinn_pde: Adaptor %r is not implemented (StanHMCAdaptor or NoAdaptation)"
-                         % (ak["Adaptor"],))
-    if ak["Metric"] not in (DiagEuclideanMetric, UnitEuclideanMetric):
-        raise ValueError("ahmc_bayesian_pinn_pde: Metric %r is not implemented; DenseEuclideanMetric is not supported "
-                         "(DiagEuclideanMetric or UnitEuclideanMetric)" % (ak["Metric"],))
+    adaptor, metric, target_accept = _hmc_adaptation(Adaptorkwargs, nchains, "ahmc_bayesian_pinn_pde")
     if ik["Integrator"] is not Leapfrog:
         raise ValueError("ahmc_bayesian_pinn_pde: Integrator %r is not implemented; JitteredLeapfrog / TemperedLeapfrog "
                          "are not supported (Leapfrog)" % (ik["Integrator"],))
-    if nchains != 1:
-        raise ValueError("ahmc_bayesian_pinn_pde: nchains = %r; one chain per call is supported" % (nchains,))
     if not isinstance(discretization, BayesianPINN):
         raise TypeError("ahmc_bayesian_pinn_pde: expected a BayesianPINN discretization")
     param_estim = discretization.pinn.param_estim
@@ -1447,10 +1455,8 @@ def ahmc_bayesian_pinn_pde(pde_system: PDESystem, discretization: BayesianPINN, 
     ninv = len(tail)
     theta0 = _initial_theta(rep.flat_init_params, param)
     n_net = theta0.size - ninv
-    eps0 = eng.hmc_begin(theta0, n_leapfrog=Kernel.n_leapfrog,
-                         adaptor=_eng.HMC_ADAPT_STAN if ak["Adaptor"] is StanHMCAdaptor else _eng.HMC_ADAPT_NONE,
-                         metric=_eng.HMC_METRIC_DIAG if ak["Metric"] is DiagEuclideanMetric else _eng.HMC_METRIC_UNIT,
-                         n_adapts=n_adapts, target_accept=float(ak["targetacceptancerate"]), step_size=0.0,
+    eps0 = eng.hmc_begin(theta0, n_leapfrog=Kernel.n_leapfrog, adaptor=adaptor, metric=metric, n_adapts=n_adapts,
+                         target_accept=target_accept, step_size=0.0,
                          prior_mean=mu_p, prior_std=sd_p, seed=seed, weights=c, ll_const=const,
                          tail_priors=tail if ninv else None)
     if verbose:

@@ -4,13 +4,12 @@ src/NN_SDE_solve.jl).
 The network N(t, z_1..z_n) takes the time and n = chain.dims[0] - 1 N(0, 1) coefficients of the truncated
 Karhunen-Loeve (KKL) expansion of the Wiener process, W'(t) ≈ √2 Σ_j z_j cos((j - ½) π t).  The trial solution is
 φ = u0 + (t - t0) N(t, z) and the residual of component k is r_k = dφ_k/dt - f_k(φ, p, t) - g_k(φ, p, t) W'(t)
-(:256-283).  f and g are traced once with sympy symbols and lowered, as in ode.py, to value and d/dt taps of output k.
-Time is rescaled to tspan ./ tspan[end] (:774-779), and f and g see the scaled t.  DESIGN section 4.14 maps the
-reference's loss terms onto the engine's terms.
+(:256-283).  f and g are traced once with sympy symbols and lowered by ode.py's shared lowering to value and d/dt
+taps of output k.  Time is rescaled to tspan ./ tspan[end] (:774-779), and f and g see the scaled t.  DESIGN
+section 4.14 maps the reference's loss terms onto the engine's terms.
 """
 from __future__ import annotations
 
-import inspect
 from dataclasses import dataclass
 from typing import List, Optional, Sequence
 
@@ -18,23 +17,17 @@ import numpy as np
 import sympy as sp
 
 from . import engine as _eng
-from .engine import Engine, NetSpec, ProblemSpec, TermSpec, REDUCE_MEAN, REDUCE_WSUM
-from .ode import (T_SYM, ComponentVector, ODEFunction, OptimizationSolution, _has_complex, _p_symbols, _save_times,
-                  _train)
-from .pinn import MODES, initialparameters
-from .strategies import (GridTraining, QuadratureTraining, QuasiRandomTraining, StochasticTraining,
-                         WeightedIntervalTraining, _julia_range, gauss_legendre_box)
-from .symbolic import VarInfo, expand_derivatives
-from .lowering import LoweringError, _Emitter
+from .engine import Engine, REDUCE_MEAN, REDUCE_WSUM, TermSpec
+from .ode import (T_SYM, ComponentVector, OptimizationSolution, _Lowering, _TrialProblem, _TrialRepresentation,
+                  _analytic_errors, _check_mode, _save_times, _strategy, _theta0, _train)
+from .strategies import GridTraining, QuadratureTraining, StochasticTraining, _julia_range, gauss_legendre_box
 
-# the modes that run the FFMA kernel; the tensor-core modes propagate 1-output networks and no parameter-only terms
-_NNSDE_MODES = ("ffma", "tc_f64")
 _OUT_OF_PLACE = "The NNSDE solver only supports out-of-place SDE definitions, i.e. du=f(u,p,t) + g(u,p,t)*dW(t)"
 
 
 # ---- problem and algorithm ------------------------------------------------------------------------------------
 @dataclass
-class SDEProblem:
+class SDEProblem(_TrialProblem):
     """``SDEProblem(f, g, u0, tspan, p)``: out-of-place drift ``f(u, p, t)`` and diagonal noise ``g(u, p, t)``, ``u0`` a
     number or a vector.  ``f`` may be an ``ODEFunction(f, analytic)`` whose ``analytic(u0, p, t)`` is the expected
     solution E[u(t)]; the solution then carries errors of the ensemble mean."""
@@ -43,26 +36,15 @@ class SDEProblem:
     u0: object
     tspan: Sequence[float]
     p: object = None
+    _solver = "NNSDE"
+    _out_of_place = _OUT_OF_PLACE
+    _components_note = " (g is diagonal noise: one per component)"
+    _traced = ("f", "g")
 
     def __post_init__(self):
-        if not isinstance(self.f, ODEFunction):
-            self.f = ODEFunction(self.f)
-        if _has_complex(self.u0) or _has_complex(self.p):
-            raise ValueError("NNSDE: complex u0 or p are not supported (the engine trains real networks)")
-        for fn in (self.f.f, self.g):
-            try:
-                n_args = len(inspect.signature(fn).parameters)
-            except (TypeError, ValueError):
-                n_args = 3
-            if n_args == 4:
-                raise ValueError(_OUT_OF_PLACE)
-        self.tspan = (float(self.tspan[0]), float(self.tspan[1]))
+        super().__post_init__()
         if self.tspan[1] == 0.0:
             raise ValueError("NNSDE rescales time to tspan ./ tspan[end]; tspan[end] = 0 cannot be rescaled")
-
-    @property
-    def scalar(self) -> bool:
-        return np.ndim(self.u0) == 0
 
 
 class NNSDE:
@@ -81,11 +63,7 @@ class NNSDE:
         self.param_estim, self.dataset, self.data_sub_batch = bool(param_estim), list(dataset), int(data_sub_batch)
         self.numensemble, self.additional_loss = int(numensemble), additional_loss
         self.mode, self.device, self.seed = mode, device, seed
-        if mode not in MODES:
-            raise ValueError("unknown mode %r (one of %s)" % (mode, sorted(MODES)))
-        if mode not in _NNSDE_MODES:
-            raise ValueError("NNSDE runs on the FFMA kernel: mode=\"ffma\" (or \"tc_f64\" for Float64); the tensor-core "
-                             "modes propagate 1-output networks and no parameter-only terms")
+        _check_mode(mode, "NNSDE", "the tensor-core modes propagate 1-output networks and no parameter-only terms")
         if self.sub_batch < 1:
             raise ValueError("NNSDE: sub_batch must be >= 1, got %d" % self.sub_batch)
         if additional_loss is not None:
@@ -95,89 +73,33 @@ class NNSDE:
                              "means, one functional per time, and the engine evaluates at most one functional term")
 
 
-# ---- tracing f and g --------------------------------------------------------------------------------------------
-def _trace(fn, name: str, scalar: bool, n: int, u_arg, p_arg, t) -> List[sp.Expr]:
-    """fn(u, p, t) with symbols, one expression per component"""
-    try:
-        out = fn(u_arg, p_arg, t)
-    except Exception as ex:      # noqa: BLE001 -- any failure to trace is the user's function, reported with its message
-        raise ValueError("NNSDE: %s(u, p, t) could not be traced with symbolic u, p and t (write it with sympy "
-                         "functions such as sympy.cos): %s: %s" % (name, type(ex).__name__, ex)) from ex
-    if out is None:
-        raise ValueError(_OUT_OF_PLACE)
-    outs = list(np.ravel(np.asarray(out, dtype=object)))
-    if len(outs) != n:
-        raise ValueError("NNSDE: %s returns %d components, u0 has %d (g is diagonal noise: one per component)"
-                         % (name, len(outs), n))
-    exprs = [sp.sympify(e) for e in outs]
-    for e in exprs:
-        if e.has(sp.I) or any(a.is_real is False for a in e.atoms(sp.Number)):
-            raise ValueError("NNSDE: %s is complex-valued; the engine trains real networks" % name)
-    return exprs
-
-
+# ---- the residuals ----------------------------------------------------------------------------------------------
 def kkl_noise(z: Sequence[sp.Expr], t) -> sp.Expr:
     """√2 Σ_j z_j cos((j - ½) π t), the truncated KKL series of dW/dt (:262)"""
     return sp.sqrt(2) * sp.Add(*[zj * sp.cos((j + sp.Rational(1, 2)) * sp.pi * t) for j, zj in enumerate(z)])
 
 
-class _Lowering:
-    """The symbols of the network outputs N_k(t, z), the residuals and the Euler-Maruyama data terms"""
+class _SDELowering(_Lowering):
+    """The trial solution of N(t, z_1..z_n_z) on time rescaled to tspan ./ tspan[end], its KKL residuals and the
+    Euler-Maruyama data terms"""
 
-    def __init__(self, prob: SDEProblem, alg: NNSDE, n_z: int, t0: float):
-        self.prob, self.n_z, self.t0 = prob, n_z, t0
-        self.n = 1 if prob.scalar else len(np.ravel(prob.u0))
-        self.u0 = np.ravel(np.asarray(prob.u0, dtype=np.float64))
-        self.z = [sp.Symbol("z%d" % (j + 1), real=True) for j in range(n_z)]
-        self.rows = ["t"] + [str(z) for z in self.z]
-        self.N = [sp.Function("N%d" % (k + 1))(T_SYM, *self.z) for k in range(self.n)]
-        names = ["N%d" % (k + 1) for k in range(self.n)]
-        self.vi = VarInfo(depvars=names, indvars=list(self.rows), dict_indvars={r: i for i, r in enumerate(self.rows)},
-                          dict_depvars={nm: k for k, nm in enumerate(names)},
-                          dict_depvar_input={nm: list(self.rows) for nm in names})
-        if alg.param_estim:
-            if prob.p is None:
-                raise ValueError("NNSDE: param_estim starts θ.p at the problem's p, and the problem has none")
-            self.p_arg, pnames = _p_symbols(prob.p)
-            self.param_index = {nm: i for i, nm in enumerate(pnames)}
-        else:
-            self.p_arg, self.param_index = prob.p, {}
-
-    def trace(self, name: str, u_comps):
-        fn = self.prob.f.f if name == "f" else self.prob.g
-        u_arg = u_comps[0] if self.prob.scalar else list(u_comps)
-        return _trace(fn, name, self.prob.scalar, self.n, u_arg, self.p_arg, T_SYM)
-
-    def phi(self, k: int) -> sp.Expr:
-        return self.u0[k] + (T_SYM - self.t0) * self.N[k]
+    def __init__(self, prob: SDEProblem, param_estim: bool, n_z: int):
+        super().__init__(prob, param_estim, ["t"] + ["z%d" % (j + 1) for j in range(n_z)])
+        self.t0 = prob.tspan[0] / prob.tspan[1]
 
     def residuals(self) -> List[sp.Expr]:
         """r_k = dφ_k/dt - f_k(φ, p, t) - g_k(φ, p, t) √2 Σ_j z_j cos((j - ½) π t)"""
         ph = [self.phi(k) for k in range(self.n)]
-        fs, gs = self.trace("f", ph), self.trace("g", ph)
-        w = kkl_noise(self.z, T_SYM)
-        return [self.N[k] + (T_SYM - self.t0) * sp.Derivative(self.N[k], T_SYM) - fs[k] - gs[k] * w
-                for k in range(self.n)]
+        fs, gs = self._trace("f", ph), self._trace("g", ph)
+        w = kkl_noise([sp.Symbol(r, real=True) for r in self.rows[1:]], T_SYM)
+        return [self.dphi(k) - fs[k] - gs[k] * w for k in range(self.n)]
 
     def em_residuals(self) -> List[sp.Expr]:
         """generate_EM_L2loss (:452-484) on rows X, t, Δt, ΔX: ΔX - f Δt and (ΔX - f Δt)^2 - g^2 Δt"""
         X, dt, dX = (sp.Symbol(s, real=True) for s in ("X", "dt", "dX"))
-        f, g = self.trace("f", [X])[0], self.trace("g", [X])[0]
+        f, g = self._trace("f", [X])[0], self._trace("g", [X])[0]
         e = dX - f * dt
         return [e, e ** 2 - g ** 2 * dt]
-
-    def term(self, expr: sp.Expr, rows: List[str], reduction: int, scale: float = 1.0) -> TermSpec:
-        """TermSpec of the residual expr over point rows `rows`; taps of N_k become taps of output k of network 0.
-        A residual without taps is a parameter-only term and must read θ.p."""
-        em = _Emitter(self.vi, rows, self.param_index, {})
-        try:
-            v = em.emit(expand_derivatives(expr))
-        except LoweringError as ex:
-            raise ValueError("NNSDE: %s" % ex) from ex
-        em.prog.append(("sub", v, em.const(0.0), 0.0))       # the last instruction is the residual
-        taps = [_eng.TapSpec(net=0, order=tp.order, dirs=tp.dirs, out=tp.net) for tp in em.taps]
-        return TermSpec(dim=len(rows), taps=taps, prog=em.prog,
-                        net_rows=[list(range(1 + self.n_z))] if taps else None, reduction=reduction, scale=scale)
 
 
 def reads_param(spec: TermSpec) -> bool:
@@ -215,7 +137,7 @@ def _valid_dataset(ds) -> bool:
 
 
 # ---- the engine problem -----------------------------------------------------------------------------------------
-class NNSDERepresentation:
+class NNSDERepresentation(_TrialRepresentation):
     """The engine problem of one ``solve(prob, alg)``: terms (``term_names``), their weights, point sets, θ0 and
     ``loss_const`` (the Euler-Maruyama terms that do not depend on θ).  ``loss_grad(θ)`` is one evaluation of the
     engine's terms (a fresh StochasticTraining draw each call); the reference's objective is its total plus
@@ -232,7 +154,7 @@ class NNSDERepresentation:
         t0, t1 = prob.tspan[0] / prob.tspan[1], 1.0          # tspan_scale = tspan ./ tspan[end]
         if dt is not None:
             dt = dt / abs(t1 - t0)
-        lw = _Lowering(prob, alg, n_z, t0)
+        lw = _SDELowering(prob, alg.param_estim, n_z)
         n = lw.n
         if chain.dims[-1] != n or n_z < 0:
             raise ValueError("NNSDE: the chain maps (t, z_1..z_n_z) to the %d components of u0: it needs %d outputs, "
@@ -241,18 +163,7 @@ class NNSDERepresentation:
             raise ValueError("NNSDE: the chain has %d inputs (t and %d KKL coefficients); the engine's networks take at "
                              "most %d (PINN_MAX_DIM)" % (1 + n_z, n_z, _eng.MAX_IN))
 
-        strategy = alg.strategy
-        if strategy is None:
-            strategy = GridTraining(dt) if dt is not None else QuadratureTraining()
-        if isinstance(strategy, QuasiRandomTraining):
-            raise ValueError("QuasiRandomTraining is not supported by NNODE since it's for high dimensional spaces only. "
-                             "Use StochasticTraining instead.")
-        if alg.autodiff:
-            for cls in (GridTraining, StochasticTraining, WeightedIntervalTraining):
-                if isinstance(strategy, cls):
-                    raise ValueError("autodiff not supported for %s." % cls.__name__)
-        if not isinstance(strategy, (GridTraining, StochasticTraining, WeightedIntervalTraining, QuadratureTraining)):
-            raise TypeError("unsupported training strategy %r" % (strategy,))
+        strategy = _strategy(alg, dt)
         S = alg.sub_batch
         if isinstance(strategy, QuadratureTraining) and S > 1:
             raise ValueError("NNSDE: QuadratureTraining with sub_batch > 1 is not supported: its integrand squares a "
@@ -269,46 +180,14 @@ class NNSDERepresentation:
             raise ValueError("NNSDE: the Euler-Maruyama data loss (generate_EM_L2loss) observes a scalar process; u0 has "
                              "%d components" % n)
 
-        # θ = [depvar, p]; dtype as NNODE
-        n_net = chain.n_params
         p0 = np.ravel(np.asarray(prob.p, dtype=np.float64)) if alg.param_estim else np.zeros(0)
-        if alg.init_params is None:
-            flat = np.concatenate([initialparameters(np.random.default_rng(alg.seed), chain, np.float64), p0])
-        else:
-            init = np.asarray(alg.init_params)
-            if np.iscomplexobj(init):
-                raise ValueError("NNSDE: complex parameters are not supported (the engine trains real networks)")
-            if init.dtype not in (np.float32, np.float64):
-                init = init.astype(np.float64)
-            if init.shape == (n_net,):
-                init = np.concatenate([init, p0.astype(init.dtype)])
-            if init.shape != (n_net + p0.size,):
-                raise ValueError("init_params has length %d, the chain%s needs %d"
-                                 % (init.size, " + p" if p0.size else "", n_net + p0.size))
-            flat = init
-        dtype = flat.dtype
-        if alg.mode == "tc_f64" and dtype != np.float64:
-            raise ValueError("mode=\"tc_f64\" runs the layer products on the FP64 tensor cores and needs float64 "
-                             "parameters (init_params is %s); use mode=\"ffma\" for float32" % dtype.name)
-
-        specs: List[TermSpec] = []
-        sets: List[Optional[np.ndarray]] = []
-        qw: List[Optional[np.ndarray]] = []
-        weights: List[float] = []
-        names: List[str] = []
-
-        def add(spec, pts, w, weight, name):
-            specs.append(spec)
-            sets.append(None if pts is None else np.asarray(pts, dtype=np.float64).reshape(spec.dim, -1))
-            qw.append(w)
-            weights.append(float(weight))
-            names.append(name)
-
+        flat = _theta0(alg, chain, p0, "NNSDE")
+        super().__init__(prob, chain, strategy, lw, flat.dtype)
+        add = self.add
         rng = np.random.default_rng([int(alg.seed), 1])      # the host draws of z (training sets)
         res = lw.residuals()
         rows = lw.rows
         strong = alg.strong_loss
-        sampled: List[int] = []
         training_sets: list = []
         if isinstance(strategy, QuadratureTraining):
             # ∫ abs2(inner_sde_loss) dt with one z per node and sub_batch 1: residual Σ_k r_k^2 (:498-531)
@@ -320,7 +199,7 @@ class NNSDERepresentation:
             nt = int(strategy.points)
             wt = {(False, True): 1.0, (False, False): nt, (True, True): S, (True, False): nt * S}[(strong, alg.batch)]
             for k in range(n):
-                sampled.append(len(specs))
+                self.sampled.append(len(self.specs))
                 add(lw.term(res[k], rows, REDUCE_MEAN), None, None, wt, "residual_%d" % (k + 1))
         else:
             ts = (_julia_range(t0, float(strategy.dx), t1) if isinstance(strategy, GridTraining)
@@ -345,65 +224,20 @@ class NNSDERepresentation:
                 else:       # f (or g) does not read θ.p: a constant of the objective
                     fn = sp.lambdify([sp.Symbol(s, real=True) for s in ("X", "t", "dt", "dX")], e, "numpy")
                     loss_const += float(np.sum(np.asarray(fn(*P), dtype=np.float64) ** 2 * np.ones(P.shape[1])))
-        if len(specs) > _eng.MAX_TERMS:
-            raise ValueError("NNSDE: %d loss terms (max %d)" % (len(specs), _eng.MAX_TERMS))
-
-        self.spec = ProblemSpec(nets=[NetSpec(chain.dims, chain.acts, 0)], terms=specs, n_params=p0.size,
-                                param_offset=n_net, n_theta=n_net + p0.size, dtype=dtype.name, mode=MODES[alg.mode],
-                                device=alg.device)
-        self.prob, self.alg, self.strategy, self.lowering = prob, alg, strategy, lw
-        self.n, self.n_z, self.n_net, self.dtype = n, n_z, n_net, dtype
+        self._close("NNSDE", p0.size, alg.mode, alg.device)
+        self.alg, self.n_z = alg, n_z
         self.tspan_scale, self.dt = (t0, t1), dt
-        self.specs, self.point_sets, self.quad_weights = specs, sets, qw
-        self.term_weights = np.asarray(weights)
-        self.term_names = names
-        self.sampled = sampled
         self.training_sets = training_sets
         self.loss_const = loss_const
-        self.flat_init_params = ComponentVector(flat, n_net)
-        self._engine = None
-        self._calls = 0
+        self.flat_init_params = ComponentVector(flat, self.n_net)
 
-    @property
-    def engine(self) -> Engine:
-        """The engine handle, created at first use with every fixed point set uploaded and the StochasticTraining
-        terms on the device KKL sampler, all with one seed, so that every component sees the same draw"""
-        if self._engine is None:
-            eng = Engine(self.spec)
-            for i, (X, w) in enumerate(zip(self.point_sets, self.quad_weights)):
-                if X is not None:
-                    eng.set_points_host(i, X.astype(self.dtype), None if w is None else w.astype(self.dtype))
-            t0, t1 = self.tspan_scale
-            for i in self.sampled:
-                eng.set_sampler_kkl(i, int(self.strategy.points), self.alg.sub_batch, t0, t1, int(self.strategy.seed),
-                                    strong=self.alg.strong_loss)
-            self._engine = eng
-        return self._engine
-
-    def loss_grad(self, theta, want_grad: bool = True):
-        """(total of the engine's terms, term losses, gradient or None) at θ: one fused launch"""
-        if self.sampled and self._calls > 0:
-            self.engine.resample()
-        self._calls += 1
-        return self.engine.loss_grad_host(np.asarray(theta, dtype=self.dtype), self.term_weights, want_grad)
-
-    def trial(self, theta, inp) -> np.ndarray:
-        """φ at the (1 + n_z, m) inputs, (n, m), evaluated on the device through value-only terms"""
-        X = np.asarray(inp, dtype=np.float64).reshape(1 + self.n_z, -1)
-        if not hasattr(self, "_phi_engine"):
-            lw = self.lowering
-            terms = [lw.term(lw.phi(k), lw.rows, REDUCE_MEAN) for k in range(self.n)]
-            self._phi_engine = Engine(ProblemSpec(nets=[NetSpec(self.alg.chain.dims, self.alg.chain.acts, 0)], terms=terms,
-                                                  n_params=self.spec.n_params, param_offset=self.n_net,
-                                                  n_theta=self.spec.n_theta, dtype=self.dtype.name,
-                                                  mode=_eng.MODE_FFMA, device=self.alg.device))
-        e = self._phi_engine
-        th = np.asarray(theta, dtype=self.dtype)
-        out = np.empty((self.n, X.shape[1]))
-        for k in range(self.n):
-            e.set_points_host(k, X.astype(self.dtype))
-            out[k] = e.term_residual_host(k, th, X.shape[1])
-        return out
+    def _set_samplers(self, eng: Engine):
+        """the StochasticTraining terms on the device KKL sampler, all with one seed, so that every component sees the
+        same draw"""
+        t0, t1 = self.tspan_scale
+        for i in self.sampled:
+            eng.set_sampler_kkl(i, int(self.strategy.points), self.alg.sub_batch, t0, t1, int(self.strategy.seed),
+                                strong=self.alg.strong_loss)
 
 
 # ---- solution ---------------------------------------------------------------------------------------------------
@@ -470,13 +304,7 @@ def solve_nnsde(prob: SDEProblem, alg: NNSDE, *, maxiters: int, dt=None, abstol:
     U = rep.trial(res.u, np.concatenate(inputs, axis=1)).reshape(rep.n, ts.size, alg.numensemble)
     fits = [U[:, i, :].copy() for i in range(ts.size)]
     est = [U[k].T.copy() for k in range(rep.n)]
-    errors = {}
-    an = prob.f.analytic
-    if an is not None:
-        A = np.stack([np.ravel(np.asarray(an(prob.u0, prob.p, float(ti)), dtype=np.float64)) for ti in ts], axis=1)
-        E = np.stack([e.mean(axis=0) for e in est]) - A
-        errors = {"final": float(np.mean(np.abs(E[:, -1]))), "l∞": float(np.max(np.abs(E))),
-                  "l2": float(np.sqrt(np.mean(E ** 2)))}
+    errors = _analytic_errors(prob, ts, np.stack([e.mean(axis=0) for e in est]))
     rode = RODESolution(ts, est, NNSDEInterpolation(SDEPhi(rep), res.u), errors)
     return SDEsol(res, rode, est, ts, np.asarray(res.u.p).copy() if alg.param_estim else None, fits, inputs,
                   alg.numensemble, rep.training_sets, None)
