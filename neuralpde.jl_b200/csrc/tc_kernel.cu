@@ -7,14 +7,15 @@
 // 128-row M block that shares the same weight operand.  The epilogue (bias + activation +
 // forward-mode tap chain rule, or its reverse) runs on the CUDA cores and re-packs the result as
 // the next GEMM's bf16 operand tile straight from the wgmma register fragments (each warpgroup
-// owns a 64-row x 32-column block of every channel).  The reverse sweep's MMAs of a tensor layer
-// also stay in registers; only the input adjoints (hand-off to the next layer down) go through the
-// accumulator region, and the four per-warpgroup weight-gradient partials through shared memory.
+// owns a 64-row x 32-column block of every channel).  The reverse sweep runs the tensor layers of the tile as two 64-point
+// halves, one after the other, so that its MMAs stay in registers and the input adjoints handed to the next layer down
+// stay in shared memory (only the lowest layer's go to the accumulator region, for layer 0 of the whole tile); the four
+// per-warpgroup weight-gradient partials go through shared memory too.
 //
 //   forward, per tensor layer l :  D_c[128 x n_out] = H_c[128 x n_in] * W_l^T        (A, B K-major)
-//   backward, per tensor layer l:  Z_c   (recompute, all columns)   = H_c * W_l^T
-//                                  Hbar_c^T[n_in x 128] = W_l^T * Zbar_c^T            (A MN-major; 32 points per warpgroup)
-//                                  Wbar_l^T[n_in x n_out] = sum_c H_c^T * Zbar_c       (A, B MN-major; 32 points per warpgroup)
+//   backward, per half and tensor layer l:  Z_c   (recompute, 16 columns per warpgroup) = H_c * W_l^T
+//                                  Hbar_c^T[n_in x 64] = W_l^T * Zbar_c^T             (A MN-major; 16 points per warpgroup)
+//                                  Wbar_l^T[n_in x n_out] = sum_c H_c^T * Zbar_c       (A, B MN-major; 16 points per warpgroup)
 //                                  bbar_l[n_out]        = Zbar_0^T * 1                  (B = constant ones atom)
 //   last layer                  :  wbar_L[n]            = sum_c H_c^T * ubar_c          (B = (hi, lo) pairs of ubar)
 //
@@ -186,53 +187,112 @@ __device__ __forceinline__ void tl_fwd_frag(const float (&d)[C][16], const LoopC
   }
 }
 
-// ---- register-resident reverse of a tensor layer --------------------------------------------------------------------------
-// The recompute of Z is fwd_mma on the reloaded hi tiles (the forward's ownership and k order).  dgrad and wgrad are
-// transposed products so that every warpgroup takes 32 points, a 4 KB (atom-aligned) offset into the MN- or K-major tiles:
-//   dgrad: Hbar_c^T[k][p] = sum_o W_l[o][k] Zbar_c[p][o]     A = W_l MN-major (M = the 64 input columns), B = Zbar_c K-major
-//   wgrad: Wbar_l^T[k][o] = sum_c sum_p H_c[p][k] Zbar_c[p][o]   A = H_c MN-major, B = Zbar_c MN-major; partial over 32 points
-//   bias : bbar_l[o] = sum_p Zbar_0[p][o]                       A = Zbar_0 MN-major, B = the constant ones atom
-// NKO = n_out / 16 k-steps of dgrad.  Each is one straight-line sequence with one commit / wait, on all four warpgroups.
+// ---- register-resident reverse of a tensor layer, one 64-point half of the tile at a time --------------------------------------
+// The reverse sweep runs the tensor layers of the tile as two independent halves (points 64 h .. 64 h + 63), each through
+// every tensor layer before the next starts, so that the input adjoints of a layer fit in shared memory: per channel c, Q holds the
+// tile pair at Q + c * kTileBytes = the half's reloaded input rows H_c (8 KB, 64 rows) followed by its Zbar_c (8 KB), and P
+// holds the half's Hbar in fp32 (C x 16 KB, layout hb_idx).  Every warpgroup takes 16 points or 16 columns of the half:
+//   recompute: Z_c[p][o]  = sum_k H_c[p][k] W_l[o][k]           A = H_c K-major (the 64 rows), B = W_l K-major (16 columns)
+//   dgrad    : Hbar_c^T[k][p] = sum_o W_l[o][k] Zbar_c[p][o]     A = W_l MN-major (M = the 64 input columns), B = Zbar_c K-major
+//   wgrad    : Wbar_l^T[k][o] = sum_c sum_p H_c[p][k] Zbar_c[p][o]   A = H_c MN-major, B = Zbar_c MN-major; partial over 16 points
+//   bias     : bbar_l[o] = sum_p Zbar_0[p][o]                    A = Zbar_0 MN-major, B = the constant ones atom
+// Each is one straight-line sequence with one commit / wait, on all four warpgroups (NK, NKO = k-steps: compile-time).
+constexpr uint32_t kHalfBytes = kTileBytes / 2;
+
+// recompute of the half: warpgroup wg owns its 64 rows x columns [16 wg, 16 wg + 16) for every channel (m64n16 fragments,
+// layout: tc::wg_chain); the k order of fwd_mma, so Z is the forward's to the bit
+template <int C, int NK>
+__device__ __forceinline__ void rec_mma(float (&d)[C][8], uint32_t sQ, uint32_t whi) {
+  const uint64_t dw = tc::make_desc(whi + (threadIdx.x >> 7) * 16u * 128u, 0, 1024);
+  tc::wgmma_fence();
+#pragma unroll
+  for (int c = 0; c < C; ++c) {
+    const uint64_t da = tc::make_desc(sQ + c * kTileBytes, 0, 1024);
+#pragma unroll
+    for (int k = 0; k < NK; ++k) tc::wgmma_n16<0, 0>(d[c], da + 2 * k, dw + 2 * k, k ? 1u : 0u);
+  }
+  tc::wgmma_commit();
+  tc::wgmma_wait0();
+}
+template <int C>
+__device__ __forceinline__ void rec_mma_any(float (&d)[C][8], uint32_t sQ, uint32_t whi, int nk) {
+  switch (nk) {
+    case 1: rec_mma<C, 1>(d, sQ, whi); break;
+    case 2: rec_mma<C, 2>(d, sQ, whi); break;
+    case 3: rec_mma<C, 3>(d, sQ, whi); break;
+    default: rec_mma<C, 4>(d, sQ, whi); break;
+  }
+}
 template <int C, int NKO>
-__device__ __forceinline__ void dgrad_mma(float (&d)[C][16], uint32_t sP, uint32_t whi) {
-  const uint32_t poff = (threadIdx.x >> 7) * 32u * 128u;
+__device__ __forceinline__ void dgrad_mma(float (&d)[C][8], uint32_t sQ, uint32_t whi) {
+  const uint32_t poff = kHalfBytes + (threadIdx.x >> 7) * 16u * 128u;
   const uint64_t dw = tc::make_desc(whi, 0, 1024);
   tc::wgmma_fence();
 #pragma unroll
   for (int c = 0; c < C; ++c) {
-    const uint64_t dz = tc::make_desc(sP + c * kTileBytes + poff, 0, 1024);
+    const uint64_t dz = tc::make_desc(sQ + c * kTileBytes + poff, 0, 1024);
 #pragma unroll
     for (int k = 0; k < NKO; ++k)   // k-step of 16 output neurons: 16 rows (2048 bytes) of W, 32 bytes of the Zbar rows
-      tc::wgmma_n32<1, 0>(d[c], dw + 128 * k, dz + 2 * k, k ? 1u : 0u);
+      tc::wgmma_n16<1, 0>(d[c], dw + 128 * k, dz + 2 * k, k ? 1u : 0u);
   }
   tc::wgmma_commit();
   tc::wgmma_wait0();
 }
 template <int C>
-__device__ __forceinline__ void dgrad_mma_any(float (&d)[C][16], uint32_t sP, uint32_t whi, int nko) {
+__device__ __forceinline__ void dgrad_mma_any(float (&d)[C][8], uint32_t sQ, uint32_t whi, int nko) {
   switch (nko) {
-    case 1: dgrad_mma<C, 1>(d, sP, whi); break;
-    case 2: dgrad_mma<C, 2>(d, sP, whi); break;
-    case 3: dgrad_mma<C, 3>(d, sP, whi); break;
-    default: dgrad_mma<C, 4>(d, sP, whi); break;
+    case 1: dgrad_mma<C, 1>(d, sQ, whi); break;
+    case 2: dgrad_mma<C, 2>(d, sQ, whi); break;
+    case 3: dgrad_mma<C, 3>(d, sQ, whi); break;
+    default: dgrad_mma<C, 4>(d, sQ, whi); break;
   }
 }
 template <int C>
-__device__ __forceinline__ void wgrad_mma(float (&dw)[32], float (&db)[8], uint32_t sP, uint32_t sQ, uint32_t s_ones) {
-  const uint32_t poff = (threadIdx.x >> 7) * 32u * 128u;
+__device__ __forceinline__ void wgrad_mma(float (&dw)[32], float (&db)[8], uint32_t sQ, uint32_t s_ones) {
+  const uint32_t poff = (threadIdx.x >> 7) * 16u * 128u;
   const uint64_t d1 = tc::make_desc(s_ones, 0, 0);   // SBO = 0: every 8-point group of K reads the same ones atom
   tc::wgmma_fence();
 #pragma unroll
   for (int c = 0; c < C; ++c) {
-    const uint64_t dh = tc::make_desc(sQ + c * kTileBytes + poff, 0, 1024), dz = tc::make_desc(sP + c * kTileBytes + poff, 0, 1024);
-#pragma unroll
-    for (int k = 0; k < 2; ++k) tc::wgmma_n64<1, 1>(dw, dh + 128 * k, dz + 128 * k, (c | k) ? 1u : 0u);
+    const uint64_t dh = tc::make_desc(sQ + c * kTileBytes + poff, 0, 1024);
+    const uint64_t dz = tc::make_desc(sQ + c * kTileBytes + kHalfBytes + poff, 0, 1024);
+    tc::wgmma_n64<1, 1>(dw, dh, dz, c ? 1u : 0u);
   }
-  const uint64_t dz0 = tc::make_desc(sP + poff, 0, 1024);
-#pragma unroll
-  for (int k = 0; k < 2; ++k) tc::wgmma_n16<1, 1>(db, dz0 + 128 * k, d1, k ? 1u : 0u);
+  tc::wgmma_n16<1, 1>(db, tc::make_desc(sQ + kHalfBytes + poff, 0, 1024), d1, 0u);
   tc::wgmma_commit();
   tc::wgmma_wait0();
+}
+
+// Hbar of the half in P: element (channel c, input column k, point p of the half) at hb_idx.  The point index is XORed in its
+// bits 3-4 with two bits of k, so that the dgrad fragment stores (8-byte pairs of points, rows k of a quad) and the epilogue
+// loads (8 consecutive points x 4 columns k = 8 m + 2 j (+1)) both touch 32 distinct banks.
+__device__ __forceinline__ int hb_idx(int c, int k, int p) { return (c * 64 + k) * 64 + (p ^ ((((k >> 1) ^ k) & 3) << 3)); }
+
+// store the dgrad fragments (rows = input column k, columns = the warpgroup's 16 points) as the half's Hbar
+template <int C>
+__device__ __forceinline__ void hbar_store(float* hbar, const float (&d)[C][8]) {
+  const int wg = threadIdx.x >> 7, w = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
+#pragma unroll
+  for (int c = 0; c < C; ++c)
+#pragma unroll
+    for (int i = 0; i < 8; i += 2) {
+      const int k = 16 * w + (lane >> 2) + 8 * ((i >> 1) & 1), p = 16 * wg + 8 * (i >> 2) + 2 * (lane & 3);
+      *reinterpret_cast<float2*>(hbar + hb_idx(c, k, p)) = make_float2(d[c][i], d[c][i + 1]);
+    }
+}
+
+// store the dgrad fragments of the lowest tensor layer as Hbar^0 of points 64 h .. 64 h + 63 in accumulator columns X (row =
+// point of the tile), where the layer-0 reverse of the whole tile reads them once both halves are done
+template <int C>
+__device__ __forceinline__ void hbar0_store(float* hand, const float (&d)[C][8], int h) {
+  const int wg = threadIdx.x >> 7, w = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
+#pragma unroll
+  for (int c = 0; c < C; ++c)
+#pragma unroll
+    for (int i = 0; i < 8; i += 2) {
+      const int k = 16 * w + (lane >> 2) + 8 * ((i >> 1) & 1), p = 64 * h + 16 * wg + 8 * (i >> 2) + 2 * (lane & 3);
+      *reinterpret_cast<float2*>(hand + (c * 64 + k) * kAccRows + p) = make_float2(d[c][i], d[c][i + 1]);
+    }
 }
 
 // store the m64nNk16 fragment d of this warpgroup (layout: tc::wg_chain) as rows of a row-major fp32 array: element
@@ -252,18 +312,18 @@ __device__ __forceinline__ void frag_store_rows(float* base, int ld, const float
   }
 }
 
-// tensor layer backward epilogue on the fragments of the recompute (ownership of fwd_mma): bias + adjoint chain -> Zbar
-// tiles (bf16 hi) in P.  The output adjoints come from the hand-off (accumulator columns TM_X + 64 c + column, row =
-// point: the dgrad of the layer above), or for the last hidden layer (flag) are w_last[column] * ubar_c[row], with
-// ubar_c[row] at ubs[c * kTcPts + row].  Columns beyond n_out get Zbar = 0 (zero weights, bias and adjoints).
+// tensor layer backward epilogue of half h on the fragments of rec_mma: bias + adjoint chain -> Zbar tiles (bf16 hi) in Q.
+// The output adjoints come from the half's Hbar in P (the dgrad of the layer above), or for the last hidden layer (flag) are
+// w_last[column] * ubar_c[point], with ubar_c[point] at ubs[c * kTcPts + point].  Columns beyond n_out get Zbar = 0 (zero
+// weights, bias and adjoints).
 template <int N1, int N2, bool PURE, int AK, int C>
-__device__ __forceinline__ void tl_bwd_frag(const float (&d)[C][16], const LoopCtx lc, const Chan<N1, N2> ch, const float* ubs) {
+__device__ __forceinline__ void tl_bwd_frag(const float (&d)[C][8], const LoopCtx lc, const Chan<N1, N2> ch, const float* ubs,
+                                            const float* hbar, int h) {
   const int wg = threadIdx.x >> 7, w = (threadIdx.x >> 5) & 3;
-  const int row0 = 64 * (wg & 1) + 16 * w + (lc.lane >> 2);
-  const int col0 = 32 * (wg >> 1) + 2 * (lc.lane & 3);
-  const float* hbar = tc::s_acc + TM_X * kAccRows;
+  const int row0 = 16 * w + (lc.lane >> 2);
+  const int col0 = 16 * wg + 2 * (lc.lane & 3);
 #pragma unroll
-  for (int i = 0; i < 16; i += 2) {
+  for (int i = 0; i < 8; i += 2) {
     const int row = row0 + 8 * ((i >> 1) & 1), col = col0 + 8 * (i >> 2);
     P2 zz[C], hv[C], zv[C];
     zz[0] = mk2(d[0][i] + lds_f32(lc.bt + col * 4), d[0][i + 1] + lds_f32(lc.bt + (col + 1) * 4));
@@ -273,24 +333,24 @@ __device__ __forceinline__ void tl_bwd_frag(const float (&d)[C][16], const LoopC
       const float w0 = lds_f32(lc.fp + (Fp::WL + col) * 4), w1 = lds_f32(lc.fp + (Fp::WL + col + 1) * 4);
 #pragma unroll
       for (int c = 0; c < C; ++c) {
-        const float u = ubs[c * kTcPts + row];
+        const float u = ubs[c * kTcPts + 64 * h + row];
         hv[c] = mk2(w0 * u, w1 * u);
       }
     } else {
 #pragma unroll
-      for (int c = 0; c < C; ++c) hv[c] = mk2(hbar[(c * 64 + col) * kAccRows + row], hbar[(c * 64 + col + 1) * kAccRows + row]);
+      for (int c = 0; c < C; ++c) hv[c] = mk2(hbar[hb_idx(c, col, row)], hbar[hb_idx(c, col + 1, row)]);
     }
     chain_bwd<N1, N2, PURE, AK, P2>(lc.act, ch, zz, hv, zv);
-    const uint32_t off = tc::swz_off(row, col);
+    const uint32_t off = kHalfBytes + tc::swz_off(row, col);
 #pragma unroll
     for (int c = 0; c < C; ++c)
-      asm volatile("st.shared.b32 [%0], %1;" ::"r"(lc.tP + c * kTileBytes + off), "r"(tc::pack_bf16(zv[c].v.x, zv[c].v.y))
+      asm volatile("st.shared.b32 [%0], %1;" ::"r"(lc.tQ + c * kTileBytes + off), "r"(tc::pack_bf16(zv[c].v.x, zv[c].v.y))
                    : "memory");
   }
 }
 
-// layer 0 backward, tensor-core variant: adjoints of H^0 (columns X) -> Zbar^0 tiles (value + first-derivative
-// channels; bf16 hi) in P.  The weight / bias gradient is then one small MMA chain against the augmented
+// layer 0 backward, tensor-core variant: adjoints of H^0 (accumulator columns X, row = point) -> Zbar^0 tiles (value +
+// first-derivative channels; bf16 hi) in P.  The weight / bias gradient is then one small MMA chain against the augmented
 // coordinate tiles (see net_backward), so no cross-lane reductions are needed here.
 template <int N1, int N2, bool PURE, int AK>
 __device__ __forceinline__ void l0_bwd_store_loop(const LoopCtx lc, const PassInfo<N1, N2> pi, const float* xp) {
@@ -320,7 +380,7 @@ __device__ __forceinline__ void l0_bwd_store_loop(const LoopCtx lc, const PassIn
   }
 }
 
-// layer 0 backward: adjoints of H^0 (columns X, or w_last * ubar: flag) -> first-layer weight / bias gradient
+// layer 0 backward of a network without tensor layers: adjoints of H^0 (w_last * ubar) -> first-layer weight / bias gradient
 template <int N1, int N2, bool PURE, int AK>
 __device__ __forceinline__ void l0_bwd_loop(const LoopCtx lc, const PassInfo<N1, N2> pi, const float* xp, const float* ubp) {
   constexpr int C = 1 + N1 + N2;
@@ -335,16 +395,11 @@ __device__ __forceinline__ void l0_bwd_loop(const LoopCtx lc, const PassInfo<N1,
 #pragma unroll 1
   for (int g = lc.g0; g < lc.g1; ++g) {
     float hb[C][GW];
-    if (!lc.flag) {
 #pragma unroll
-      for (int c = 0; c < C; ++c) acc_ldg(lc.taddr + TM_X + c * 64 + g * GW, hb[c]);
-    } else {
+    for (int i = 0; i < GW; ++i) {
+      const float wl = lds_f32(lc.fp + (Fp::WL + g * GW + i) * 4);
 #pragma unroll
-      for (int i = 0; i < GW; ++i) {
-        const float wl = lds_f32(lc.fp + (Fp::WL + g * GW + i) * 4);
-#pragma unroll
-        for (int c = 0; c < C; ++c) hb[c][i] = wl * ub[c];
-      }
+      for (int c = 0; c < C; ++c) hb[c][i] = wl * ub[c];
     }
     float zv0[GW], zvd[N1 > 0 ? N1 : 1][GW];
 #pragma unroll
@@ -493,106 +548,129 @@ __device__ __noinline__ uint32_t net_backward(CtaShared* cs, const DevProblem* P
   last_layer_grad<C>(t, ub, pi.nL, partial + net.w_off[L - 1], partial + net.b_off[L - 1], tc::smem_u32(tQ), tc::smem_u32(tP),
                      kTileBytes, 0u, accm + TM_Y, kTcW);
 
-  // ---- tensor layers, last to first ------------------------------------------------------------------------------------
-  // Hbar^{l-1} goes from the dgrad fragments to accumulator columns TM_X (the hand-off the next layer down reads).  The
-  // four per-warpgroup partials of Wbar_l^T and bbar_l are exchanged through shared memory: once every warpgroup's wgrad
-  // has been waited for, P (Zbar) and Q (H^{l-1}) are dead.  The partials go to the first four tiles of P (plan.cu gives
-  // P at least four) and to ms.scratch, the next layer's stash reload goes to Q at the same time, and each gradient
-  // element is summed in warpgroup order by one thread, so the result does not depend on scheduling.
   const uint32_t sP = tc::smem_u32(tP), sQ = tc::smem_u32(tQ);
-  const int wg = tid >> 7;
-  float* hand = tc::s_acc + TM_X * kAccRows;
-  float* wpart = reinterpret_cast<float*>(tP);   // [wg][k][o] (4 x 64 x 64)
-  float* bpart = ms.scratch;                     // [wg][o]; only the last hidden layer's epilogue reads ubar from here
-  static_assert(4 * 64 <= kTcMaxC * kTcPts, "the bias partials fit ms.scratch");
-  for (int l = TL; l >= 1; --l) {
-    const int n_in = net.dims[l], n_out = net.dims[l + 1];
-    const int act = net.acts[l];
-    float* gb = partial + net.b_off[l];
-    float* gw = partial + net.w_off[l];
-    const float* bt = fp + Fp::BT + (l - 1) * 64;
-    const uint32_t whi = tc::smem_u32(smem + ns.w_hi[l - 1]);
-    dbg_mark(cs, 21);
-    if (tid == 0 && l == TL) {
-      // reload this layer's input tiles H^{l-1} (bf16 hi) from the stash into Q: last_layer_grad has waited for the MMA
-      // chains that read the ubar tile there.  The layers below were reloaded by the layer above them (see there).
-      const uint8_t* src = stash_slot + (size_t)(l - 1) * kTcMaxC * kTileBytes;
-      tc::mbar_arrive_expect_tx(ms.bar_ld, C * kTileBytes);
-      for (int c = 0; c < C; ++c) tc::bulk_load(tQ + c * kTileBytes, src + (size_t)c * kTileBytes, kTileBytes, ms.bar_ld);
-    }
-    wait_bar(ms.bar_ld, ld_phase);
-    dbg_mark(cs, 22);
-    {
-      // recompute Z = H_hi * W_hi^T of all n_out columns, then Zbar tiles into P
-      float d[C][16];
-      fwd_mma_any<C>(d, sQ, sQ, whi, whi, n_in / 16, false);
-      // P holds the weight-gradient partials of the layer above until every thread has summed its elements
-      __syncthreads();
-      dbg_mark(cs, 24);
-      const LoopCtx lc(tc::smem_u32(fp), tc::smem_u32(bt), sP, sQ, t, act, 0, l == TL);
-      tl_bwd_frag<N1, N2, PURE, AK, C>(d, lc, pi.ch, ms.scratch);
-    }
-    tc::fence_async_smem();   // Zbar (generic-proxy stores to P) -> the dgrad / wgrad MMAs (async proxy)
+  const int act0 = net.acts[0];
+  float* gb0 = partial + net.b_off[0];
+  float* gw0 = partial + net.w_off[0];
+  if (TL == 0) {
+    // ---- no tensor layer: layer 0 on the CUDA cores (warp reduce-scatter + atomics) -----------------------------------------
     __syncthreads();
-    dbg_mark(cs, 26);
-    {
-      float d[C][16];
-      dgrad_mma_any<C>(d, sP, whi, n_out / 16);
-#pragma unroll
-      for (int c = 0; c < C; ++c) frag_store_rows(hand + c * 64 * kAccRows + 32 * wg, kAccRows, d[c]);
-    }
-    dbg_mark(cs, 27);
-    {
-      float dw[32], db[8];
-      wgrad_mma<C>(dw, db, sP, sQ, tc::smem_u32(smem + cs->off_ones));
-      // Every warpgroup has waited for its MMAs: P and Q may be overwritten.  Generic-proxy stores to P after async-proxy
-      // reads that have completed need no proxy fence (the fence above orders the next Zbar stores before their MMAs), and
-      // Q is written and read by the async proxy alone until the coordinate tiles, so its reload needs none either.
-      __syncthreads();
-      if (tid == 0 && l > 1) {
-        // the input tiles H^{l-2} of the next layer down travel into Q while the gradient sum below reads P
-        const uint8_t* src = stash_slot + (size_t)(l - 2) * kTcMaxC * kTileBytes;
-        tc::mbar_arrive_expect_tx(ms.bar_ld, C * kTileBytes);
-        for (int c = 0; c < C; ++c) tc::bulk_load(tQ + c * kTileBytes, src + (size_t)c * kTileBytes, kTileBytes, ms.bar_ld);
-      }
-      frag_store_rows(wpart + wg * 64 * 64, 64, dw);
-      // column 0 of the bias product: rows 16 w + lane / 4 (+ 8) of lanes 0, 4, ..., 28
-      if ((t.lane & 3) == 0) {
-        const int o = 16 * (t.warp & 3) + (t.lane >> 2);
-        bpart[wg * 64 + o] = db[0];
-        bpart[wg * 64 + o + 8] = db[2];
-      }
-    }
-    __syncthreads();
-    dbg_mark(cs, 28);
-#pragma unroll 1
-    for (int e = tid; e < 64 * 64; e += kTcThreads) {
-      const int k = e >> 6, o = e & 63;
-      if (k < n_in && o < n_out) atomicAdd(gw + o + (long long)n_out * k, ((wpart[e] + wpart[4096 + e]) + wpart[8192 + e]) + wpart[12288 + e]);
-    }
-    if (tid < n_out) atomicAdd(gb + tid, ((bpart[tid] + bpart[64 + tid]) + bpart[128 + tid]) + bpart[192 + tid]);
+    dbg_mark(cs, 29);
+    const LoopCtx lc(tc::smem_u32(fp), tc::smem_u32(fp), sP, sQ, t, act0, pi.n1w / GW, 1, 0, gb0, gw0);
+    l0_bwd_loop<N1, N2, PURE, AK>(lc, pi, x, ub);
   }
 
-  // ---- layer 0 backward ---------------------------------------------------------------------------------------------------
-  {
-    __syncthreads();   // the last gradient sum has read P
-    dbg_mark(cs, 29);
-    const int act0 = net.acts[0];
-    float* gb0 = partial + net.b_off[0];
-    float* gw0 = partial + net.w_off[0];
-    if (TL == 0) {
-      // no tensor layer: everything on the CUDA cores (warp reduce-scatter + atomics)
-      const LoopCtx lc(tc::smem_u32(fp), tc::smem_u32(fp), sP, sQ, t, act0, pi.n1w / GW, 1, 0, gb0, gw0);
-      l0_bwd_loop<N1, N2, PURE, AK>(lc, pi, x, ub);
-    } else {
-      // the weight / bias gradient by MMA (layer0_grad); the coordinate tiles live in Q, which is free after the last
-      // tensor layer, and the channel count leaves a spare tile for the lo of x when N2 > 0
-      coord_tiles<N1>(t, sQ, x, pi.dir1, N2 > 0);
-      const LoopCtx lc(tc::smem_u32(fp), tc::smem_u32(fp), sP, sQ, t, act0, pi.n1w / GWB, 0);
-      l0_bwd_store_loop<N1, N2, PURE, AK>(lc, pi, x);
-      layer0_grad<N1>(t, sP, kTileBytes, 0u, sQ, N2 > 0, accm + TM_Y, kTcW, pi.n1w, pi.d_in, gw0, gb0);
+  // ---- tensor layers, last to first: one 64-point half of the tile after the other --------------------------------------------
+  // Per layer: the stash reload of the half's H^{l-1} in Q has landed -> recompute -> barrier (the half's Hbar^l in P is
+  // complete) -> Zbar epilogue into Q -> barrier -> wgrad, whose four per-warpgroup partials of Wbar_l^T go to the first four
+  // tiles of P (plan.cu gives P at least four: every epilogue has read Hbar^l), then dgrad, whose fragments stay in registers
+  // -> barrier (every MMA has read Q) -> the bias partials go to the Zbar half of Q's first tile and the reload of H^{l-2}
+  // to Q -> barrier -> each gradient element is summed in warpgroup order by one thread, which adds it to the CTA partial
+  // (half 0 before half 1, so the result does not depend on scheduling) -> barrier -> the dgrad fragments become Hbar^{l-1}
+  // in P (the lowest layer's, Hbar^0, go to accumulator columns X for layer 0 of the whole tile).  Generic-proxy stores to P and Q after async-proxy reads that have completed need no proxy fence; the fence before
+  // the MMAs orders the Zbar stores before them.
+  const int wg = tid >> 7;
+  float* hbar = reinterpret_cast<float*>(tP);                 // [c][k][point] (hb_idx), C x 16 KB
+  float* wpart = reinterpret_cast<float*>(tP);                // [wg][k][o] (4 x 64 x 64)
+  float* bpart = reinterpret_cast<float*>(tQ + kHalfBytes);   // [wg][o]
+  float* hand = tc::s_acc + TM_X * kAccRows;                  // Hbar^0 of the tile, [c][k][point]
+#pragma unroll 1
+  for (int h = 0; h < (TL > 0 ? 2 : 0); ++h) {
+    for (int l = TL; l >= 1; --l) {
+      const int n_in = net.dims[l], n_out = net.dims[l + 1];
+      const int act = net.acts[l];
+      float* gb = partial + net.b_off[l];
+      float* gw = partial + net.w_off[l];
+      const float* bt = fp + Fp::BT + (l - 1) * 64;
+      const uint32_t whi = tc::smem_u32(smem + ns.w_hi[l - 1]);
+      dbg_mark(cs, 21);
+      if (tid == 0 && l == TL) {
+        // reload the half's rows of this layer's input tiles H^{l-1} (bf16 hi) from the stash into Q: the MMAs that read Q
+        // before (last_layer_grad's ubar tile, the previous half's layer 0) have been waited for.  The layers below are
+        // reloaded by the layer above them.
+        const uint8_t* src = stash_slot + (size_t)(l - 1) * kTcMaxC * kTileBytes + h * kHalfBytes;
+        tc::mbar_arrive_expect_tx(ms.bar_ld, C * kHalfBytes);
+        for (int c = 0; c < C; ++c) tc::bulk_load(tQ + c * kTileBytes, src + (size_t)c * kTileBytes, kHalfBytes, ms.bar_ld);
+      }
+      wait_bar(ms.bar_ld, ld_phase);
+      dbg_mark(cs, 22);
+      {
+        float d[C][8];
+        rec_mma_any<C>(d, sQ, whi, n_in / 16);
+        __syncthreads();
+        dbg_mark(cs, 24);
+        const LoopCtx lc(tc::smem_u32(fp), tc::smem_u32(bt), sP, sQ, t, act, 0, l == TL);
+        tl_bwd_frag<N1, N2, PURE, AK, C>(d, lc, pi.ch, ms.scratch, hbar, h);
+      }
+      tc::fence_async_smem();   // Zbar (generic-proxy stores to Q) -> the dgrad / wgrad MMAs (async proxy)
+      __syncthreads();
+      dbg_mark(cs, 26);
+      float db0, db2;
+      {
+        float dw[32], db[8];
+        wgrad_mma<C>(dw, db, sQ, tc::smem_u32(smem + cs->off_ones));
+        frag_store_rows(wpart + wg * 64 * 64, 64, dw);
+        db0 = db[0]; db2 = db[2];   // column 0 of the bias product: rows 16 w + lane / 4 (+ 8) of lanes 0, 4, ..., 28
+      }
+      float d[C][8];
+      dgrad_mma_any<C>(d, sQ, whi, n_out / 16);
+      __syncthreads();
+      dbg_mark(cs, 27);
+      if (tid == 0 && l > 1) {
+        // the half's input tiles H^{l-2} of the next layer down travel into Q while the gradient sum below runs
+        const uint8_t* src = stash_slot + (size_t)(l - 2) * kTcMaxC * kTileBytes + h * kHalfBytes;
+        tc::mbar_arrive_expect_tx(ms.bar_ld, C * kHalfBytes);
+        for (int c = 0; c < C; ++c) tc::bulk_load(tQ + c * kTileBytes, src + (size_t)c * kTileBytes, kHalfBytes, ms.bar_ld);
+      }
+      if ((t.lane & 3) == 0) {
+        const int o = 16 * (t.warp & 3) + (t.lane >> 2);
+        bpart[wg * 64 + o] = db0;
+        bpart[wg * 64 + o + 8] = db2;
+      }
+      __syncthreads();
+      dbg_mark(cs, 28);
+      // owner-thread read-add-write: element (k, o) belongs to one thread in both halves and in every tile
+      if ((reinterpret_cast<uintptr_t>(gw) & 15) == 0) {   // n_out is a multiple of 16: four columns o per float4
+        const float4* wp4 = reinterpret_cast<const float4*>(wpart);
+#pragma unroll 1
+        for (int e = tid; e < 64 * 16; e += kTcThreads) {
+          const int k = e >> 4, o = (e & 15) * 4;
+          if (k < n_in && o < n_out) {
+            const float4 a = wp4[e], b = wp4[1024 + e], c = wp4[2048 + e], q = wp4[3072 + e];
+            float4* g = reinterpret_cast<float4*>(gw + o + (long long)n_out * k);
+            float4 v = *g;
+            v.x += ((a.x + b.x) + c.x) + q.x;
+            v.y += ((a.y + b.y) + c.y) + q.y;
+            v.z += ((a.z + b.z) + c.z) + q.z;
+            v.w += ((a.w + b.w) + c.w) + q.w;
+            *g = v;
+          }
+        }
+      } else {
+#pragma unroll 1
+        for (int e = tid; e < 64 * 64; e += kTcThreads) {
+          const int k = e >> 6, o = e & 63;
+          if (k < n_in && o < n_out) gw[o + (long long)n_out * k] += ((wpart[e] + wpart[4096 + e]) + wpart[8192 + e]) + wpart[12288 + e];
+        }
+      }
+      if (tid < n_out) gb[tid] += ((bpart[tid] + bpart[64 + tid]) + bpart[128 + tid]) + bpart[192 + tid];
+      __syncthreads();   // the sum has read P
+      if (l > 1) hbar_store<C>(hbar, d);
+      else hbar0_store<C>(hand, d, h);
     }
   }
+  if (TL > 0) {
+    // ---- layer 0 of the whole tile: Zbar^0 by the CUDA cores into P, the weight / bias gradient by MMA (layer0_grad) -------
+    // (the coordinate tiles live in Q, which is free after the last tensor layer, and the channel count leaves a spare tile
+    // for the lo of x when N2 > 0)
+    __syncthreads();   // Hbar^0 of both halves is in accumulator columns X, the last gradient sum has read P
+    dbg_mark(cs, 29);
+    coord_tiles<N1>(t, sQ, x, pi.dir1, N2 > 0);
+    const LoopCtx lc(tc::smem_u32(fp), tc::smem_u32(fp), sP, sQ, t, act0, pi.n1w / GWB, 0);
+    l0_bwd_store_loop<N1, N2, PURE, AK>(lc, pi, x);
+    layer0_grad<N1>(t, sP, kTileBytes, 0u, sQ, N2 > 0, accm + TM_Y, kTcW, pi.n1w, pi.d_in, gw0, gb0);
+  }
+
   __syncthreads();
   dbg_mark(cs, 30);
   return (ld_phase << 1) | (phase & 1u);

@@ -8,7 +8,8 @@ import neuralpde_jl_b200 as npde
 from neuralpde_jl_b200 import configs
 mode = sys.argv[1] if len(sys.argv) > 1 else "tc_split"
 which = sys.argv[2] if len(sys.argv) > 2 else "cfg2"
-cfg = configs.config3() if which == "cfg3" else configs.config2()
+n = int(sys.argv[3]) if len(sys.argv) > 3 else 128     # cfg 2 grid size: n^2 / 128 PDE tiles + 4 boundary tiles
+cfg = configs.config3() if which == "cfg3" else configs.config2(n=n)
 rep = npde.symbolic_discretize(cfg.pde_system, cfg.discretization(dtype=np.float32, mode=mode))
 eng = rep.engine
 if hasattr(rep.strategy, "points"):
