@@ -102,8 +102,10 @@ enum {
   PINN_ACT_SIN = 3,
   PINN_ACT_SOFTPLUS = 4,
   PINN_ACT_SWISH = 5,
-  PINN_ACT_GELU = 6        /* NNlib's gelu, tanh form: x/2 (1 + tanh(sqrt(2/pi) (x + 0.044715 x^3))); FFMA kernel
+  PINN_ACT_GELU = 6,       /* NNlib's gelu, tanh form: x/2 (1 + tanh(sqrt(2/pi) (x + 0.044715 x^3))); FFMA kernel
                             * (PINN_MODE_FFMA, PINN_MODE_TC_F64) only */
+  PINN_ACT_LOGCOSH = 7     /* NNlib's logcosh: x + softplus(-2x) - log 2; FFMA kernel (PINN_MODE_FFMA,
+                            * PINN_MODE_TC_F64) only */
 };
 
 /* residual-program opcodes.  The program is in SSA form: instruction i defines

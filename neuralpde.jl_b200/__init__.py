@@ -23,5 +23,6 @@ from .adapter import NeuralAdapterLoss, neural_adapter
 from .ode import NNODE, NNODERepresentation, ODEFunction, ODEProblem, ODESolution
 from .bpinn_ode import BNNODE, BNNODELogDensity, ahmc_bayesian_pinn_ode
 from .sde import NNSDE, NNSDERepresentation, SDEProblem, SDEsol
+from .sde_weak import SDEPINN
 
 __all__ = [n for n in dir() if not n.startswith("_")]

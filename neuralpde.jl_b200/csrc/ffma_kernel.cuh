@@ -93,12 +93,27 @@ __device__ __forceinline__ void gelu_eval4(real z, real& a, real& d1, real& d2, 
   d4 = real(0.5) * (real(4) * T3 + z * T4);
 }
 
+// NNlib's logcosh, z + softplus(-2z) - log 2, evaluated as |z| + log1p(exp(-2|z|)) - log 2 so that it neither
+// overflows nor cancels for large |z|.  Its derivatives are tanh's shifted by one: t, 1 - t^2, -2t(1 - t^2), ...
+template <typename real>
+__device__ __forceinline__ void logcosh_eval4(real z, real& a, real& d1, real& d2, real& d3, real& d4) {
+  const real az = m_abs(z);
+  const real t = m_tanh(z), s = real(1) - t * t;
+  a = az + m_log1p(m_exp(real(-2) * az)) - real(0.69314718055994530942);
+  d1 = t; d2 = s; d3 = real(-2) * t * s; d4 = s * (real(6) * t * t - real(2));
+}
+
 // activation value and its first four derivatives at z (the fourth enters the reverse sweep through third-derivative taps).
-// kGelu = false (the tensor-core kernels, which refuse gelu layers) leaves gelu out, so their code stays as it was
-template <typename real, bool kGelu = true>
+// kFfmaOnly = false (the tensor-core kernels, which refuse gelu and logcosh layers) leaves those two out, so their code
+// stays as it was
+template <typename real, bool kFfmaOnly = true>
 __device__ __forceinline__ void act_eval4(int act, real z, real& a, real& d1, real& d2, real& d3, real& d4) {
-  if constexpr (kGelu) {
-    if (act == PINN_ACT_GELU) { gelu_eval4<real>(z, a, d1, d2, d3, d4); return; }
+  if constexpr (kFfmaOnly) {
+    if (act >= PINN_ACT_GELU) {     // one compare on the common path, as with gelu alone
+      if (act == PINN_ACT_GELU) gelu_eval4<real>(z, a, d1, d2, d3, d4);
+      else logcosh_eval4<real>(z, a, d1, d2, d3, d4);
+      return;
+    }
   }
   switch (act) {
     case PINN_ACT_TANH: {
@@ -140,10 +155,10 @@ __device__ __forceinline__ void act_eval4(int act, real z, real& a, real& d1, re
       a = z; d1 = real(1); d2 = real(0); d3 = real(0); d4 = real(0);
   }
 }
-template <typename real, bool kGelu = true>
+template <typename real, bool kFfmaOnly = true>
 __device__ __forceinline__ void act_eval(int act, real z, real& a, real& d1, real& d2, real& d3) {
   real d4;
-  act_eval4<real, kGelu>(act, z, a, d1, d2, d3, d4);
+  act_eval4<real, kFfmaOnly>(act, z, a, d1, d2, d3, d4);
 }
 
 template <typename real> struct Cfg {

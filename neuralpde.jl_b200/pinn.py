@@ -28,7 +28,8 @@ MODES = {"ffma": _eng.MODE_FFMA, "tc_bf16": _eng.MODE_TC_BF16, "tc_split": _eng.
 FFMA_KERNEL_MODES = (_eng.MODE_FFMA, _eng.MODE_TC_F64)
 
 _ACT_NAMES = {"identity": "identity", "tanh": "tanh", "sigmoid": "sigmoid", "σ": "sigmoid", "sin": "sin",
-              "softplus": "softplus", "swish": "swish", "gelu": "gelu", None: "identity"}
+              "softplus": "softplus", "swish": "swish", "gelu": "gelu", "logcosh": "logcosh",
+              None: "identity"}
 
 
 # ---- Lux stand-ins -----------------------------------------------------------------------------
@@ -384,6 +385,16 @@ class IntegralLoss:
         return X, w
 
 
+@dataclass
+class _ResidualSumLoss:
+    """``additional_loss`` Σ_p (lhs - rhs)² of ``eq`` at the columns of ``points`` (one row per variable of the
+    equation): a weighted-sum term with unit weights and scale 1, whose integrals take ``q`` Gauss-Legendre nodes.
+    SDEPINN's norm loss Σ_t (∫ p̂(x, t) dx - 1)² is one (sde_weak.py)."""
+    eq: Equation
+    points: np.ndarray
+    q: int = _eng.MAX_QUAD
+
+
 def _integral_loss_term(add: IntegralLoss, vi: VarInfo, param_index, param_values, fixed):
     """(TermSpec, points, weights) of the functional term: the program yields v_p - target / Σw, so that
     Σ_p w_p (v_p - target / Σw) = Σ_p w_p v_p - target"""
@@ -655,7 +666,10 @@ def symbolic_discretize(pde_system: PDESystem, discretization: PhysicsInformedNN
         pde_terms = [lower_equation(e, vi, param_index, param_values, hoist=hoist, fixed=fixed) for e in eqs]
         bc_terms = [lower_equation(e, vi, param_index, param_values, hoist=hoist, fixed=fixed) for e in bcs]
         add = d.additional_loss
-        if add is not None and not isinstance(add, (DataLoss, IntegralLoss)):
+        if isinstance(add, _ResidualSumLoss):
+            add_lt = lower_equation(add.eq, vi, param_index, param_values, fixed=fixed)
+            add_lt.integrals = [dataclasses.replace(it, q=int(add.q)) for it in add_lt.integrals]
+        elif add is not None and not isinstance(add, (DataLoss, IntegralLoss)):
             raise ValueError("additional_loss must be a DataLoss (data term) or an IntegralLoss (integral constraint); "
                              "arbitrary closures cannot run inside the CUDA kernel")
         if isinstance(add, IntegralLoss):
@@ -710,6 +724,8 @@ def symbolic_discretize(pde_system: PDESystem, discretization: PhysicsInformedNN
             l2_sets.append(np.concatenate([m[:, 1:].T, m[:, :1].T], axis=0))
     if isinstance(add, IntegralLoss):
         specs.append(func_spec)
+    if isinstance(add, _ResidualSumLoss):
+        specs.append(term_spec(add_lt, REDUCE_WSUM, 1.0))
     if isinstance(add, DataLoss):
         if add.depvar not in vi.dict_depvars:
             raise ValueError("DataLoss: unknown dependent variable %s" % add.depvar)
@@ -724,7 +740,10 @@ def symbolic_discretize(pde_system: PDESystem, discretization: PhysicsInformedNN
     # integral terms (get_numeric_integral, src/discretize.jl:334-397): one set per term that reads them -- a dataset
     # term re-reads its equation's integrals at the dataset's coordinates -- numbered in term order
     integrals: List[IntegralSpec] = []
-    for i, lt in enumerate(pde_terms + bc_terms + [lt for lt, _ in ds_terms]):
+    owners = list(enumerate(pde_terms + bc_terms + [lt for lt, _ in ds_terms]))
+    if isinstance(add, _ResidualSumLoss):
+        owners.append((len(specs) - 1, add_lt))
+    for i, lt in owners:
         if lt.integrals:
             base = len(integrals)
             integrals += [dataclasses.replace(it, owner=i) for it in lt.integrals]
@@ -773,6 +792,9 @@ def symbolic_discretize(pde_system: PDESystem, discretization: PhysicsInformedNN
         if X.ndim != 2 or X.shape[1] != y.shape[1]:
             raise ValueError("DataLoss: points must be (d, n) and values (n,)")
         point_sets[-1] = np.concatenate([X, y], axis=0)
+    if isinstance(add, _ResidualSumLoss):
+        point_sets[-1] = np.asarray(add.points, dtype=dtype)
+        quad_w[-1] = np.ones(point_sets[-1].shape[1], dtype=dtype)
     func_term = len(specs) - 1 if isinstance(add, IntegralLoss) else -1
 
     eng = Engine(spec)
@@ -1169,10 +1191,16 @@ def solve(prob: OptimizationProblem, opt: Union[Adam, LBFGS, BFGS], maxiters: in
     ``solve(prob::ODEProblem, alg::NNODE; maxiters, dt, abstol, saveat, ...)`` trains an NNODE (ode.py) and takes the
     keywords of ``ode.solve``.  ``solve(prob::ODEProblem, alg::BNNODE; saveat)`` samples the Bayesian ODE posterior
     (bpinn_ode.py) and returns a BPINNsolution.  ``solve(prob::SDEProblem, alg::NNSDE; maxiters, dt, abstol, saveat,
-    ...)`` trains an NNSDE (sde.py) and returns an SDEsol."""
+    ...)`` trains an NNSDE (sde.py) and returns an SDEsol.  ``solve(prob::SDEProblem, alg::SDEPINN; maxiters = 200,
+    verbose)`` trains the density of the SDE's Fokker-Planck equation (sde_weak.py) and returns ``(res, phi)``."""
     from .bpinn_ode import BNNODE, solve_bnnode
     from .ode import ODEProblem, solve_nnode
     from .sde import SDEProblem, solve_nnsde
+    from .sde_weak import SDEPINN, solve_sdepinn
+    if isinstance(prob, SDEProblem) and isinstance(opt, SDEPINN):
+        if callback is not None or chunk != 50 or device_loop:
+            raise TypeError("solve(::SDEProblem, ::SDEPINN) takes no callback, chunk or device_loop")
+        return solve_sdepinn(prob, opt, maxiters=200 if maxiters is _MAXITERS_DEFAULT else maxiters, **ode_kwargs)
     if isinstance(prob, SDEProblem):
         if callback is not None or chunk != 50:
             raise TypeError("solve(::SDEProblem, ::NNSDE) takes no callback or chunk: it stops at abstol")
@@ -1288,6 +1316,10 @@ class Normal:
     def params(self):
         return (self.mu, self.sigma)
 
+    def pdf(self, x: float) -> float:
+        """``Distributions.pdf``"""
+        return float(np.exp(-0.5 * ((x - self.mu) / self.sigma) ** 2) / (self.sigma * np.sqrt(2.0 * np.pi)))
+
 
 @dataclass(frozen=True)
 class LogNormal:
@@ -1297,6 +1329,12 @@ class LogNormal:
 
     def params(self):
         return (self.mu, self.sigma)
+
+    def pdf(self, x: float) -> float:
+        """``Distributions.pdf``: 0 for x <= 0"""
+        if x <= 0:
+            return 0.0
+        return float(np.exp(-0.5 * ((np.log(x) - self.mu) / self.sigma) ** 2) / (x * self.sigma * np.sqrt(2.0 * np.pi)))
 
 
 @dataclass(frozen=True)

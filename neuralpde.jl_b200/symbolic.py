@@ -47,6 +47,8 @@ class Differential:
 
     def __call__(self, expr):
         expr = sp.sympify(expr)
+        if expr.is_number:          # Dx(c) = 0: SDEPINN's flux applies Dx to g(x_0, p, t)^2, a number
+            return sp.Integer(0)
         return sp.Derivative(expr, (self.x, self.order), evaluate=False)
 
 
