@@ -679,17 +679,17 @@ __device__ __forceinline__ void flush_wgrad(const Tid& t, uint32_t wcol, uint32_
 // coord_tiles writes the B tiles (rows = points, 16 columns used), kTileBytes apart from b_tile (threads 0..127):
 //   tile 0: bf16 hi of (x_0..x_7) in columns 0..7, 1.0 in column 8;  tile 1+j: 1.0 in column dir1[j];
 //   tile 1+N1: bf16 lo of x (x_lo: when the kernel has a spare tile for it)
+// coord_row writes row `row` of those tiles (the point with coordinates x)
 template <int N1>
-__device__ __forceinline__ void coord_tiles(const Tid& t, uint32_t b_tile, const float (&x)[PINN_MAX_IN],
-                                            const int (&dir1)[N1 > 0 ? N1 : 1], bool x_lo) {
-  if (t.tid >= kTcPts) return;
+__device__ __forceinline__ void coord_row(uint32_t b_tile, int row, const float (&x)[PINN_MAX_IN],
+                                          const int (&dir1)[N1 > 0 ? N1 : 1], bool x_lo) {
   uint32_t hi[4], lo[4];
 #pragma unroll
   for (int k = 0; k < 4; ++k) {
     hi[k] = tc::pack_bf16(x[2 * k], x[2 * k + 1]);
     lo[k] = bf16x2_lo(x[2 * k], x[2 * k + 1], hi[k]);
   }
-  const uint32_t c0a = b_tile + tc::swz_chunk(t.p, 0), c1a = b_tile + tc::swz_chunk(t.p, 1);
+  const uint32_t c0a = b_tile + tc::swz_chunk(row, 0), c1a = b_tile + tc::swz_chunk(row, 1);
   sts_v4(c0a, hi[0], hi[1], hi[2], hi[3]);
   sts_v4(c1a, 0x00003f80u, 0u, 0u, 0u);
   if (x_lo) {
@@ -705,6 +705,12 @@ __device__ __forceinline__ void coord_tiles(const Tid& t, uint32_t b_tile, const
     sts_v4(c0a + (1 + j) * kTileBytes, w[0], w[1], w[2], w[3]);
     sts_v4(c1a + (1 + j) * kTileBytes, 0u, 0u, 0u, 0u);
   }
+}
+template <int N1>
+__device__ __forceinline__ void coord_tiles(const Tid& t, uint32_t b_tile, const float (&x)[PINN_MAX_IN],
+                                            const int (&dir1)[N1 > 0 ? N1 : 1], bool x_lo) {
+  if (t.tid >= kTcPts) return;
+  coord_row<N1>(b_tile, t.p, x, dir1, x_lo);
 }
 // the MMA chains against the coord_tiles at b_tile and the flush into W_0 / b_0.  Zbar_c is the tile at z_tile + c * z_stride,
 // read MN-major (z_lbo: the next 64 rows of M when the first layer is wider than 64).  Publishes the tiles itself; CTA-wide.

@@ -1,16 +1,16 @@
 // tc_kernel.cu -- fused PINN loss+gradient kernel, tensor-core path (sm_90a, wgmma).
 //
 // One CTA (512 threads = 4 warpgroups) owns a tile of 128 collocation points; a point is a row
-// of the accumulator region (tc_prims.cuh) and of every operand tile.  The hidden->hidden Dense
+// of every operand tile.  The hidden->hidden Dense
 // layers run on the tensor cores (wgmma, bf16 operands from 128B-swizzled shared-memory tiles,
 // fp32 accumulators); every derivative channel (value, d/dx_i, d2/dx_i dx_j) is its own
 // 128-row M block that shares the same weight operand.  The epilogue (bias + activation +
 // forward-mode tap chain rule, or its reverse) runs on the CUDA cores and re-packs the result as
 // the next GEMM's bf16 operand tile straight from the wgmma register fragments (each warpgroup
-// owns a 64-row x 32-column block of every channel).  The reverse sweep runs the tensor layers of the tile as two 64-point
-// halves, one after the other, so that its MMAs stay in registers and the input adjoints handed to the next layer down
-// stay in shared memory (only the lowest layer's go to the accumulator region, for layer 0 of the whole tile); the four
-// per-warpgroup weight-gradient partials go through shared memory too.
+// owns a 64-row x 32-column block of every channel).  The reverse sweep runs the tensor layers and layer 0 of the tile as
+// two 64-point halves, one after the other, so that its MMAs stay in registers and the input adjoints handed to the next
+// layer down stay in shared memory; the per-warpgroup gradient partials go through shared memory too.  Only the last
+// layer's small gradient chains (last_layer_grad) still use the accumulator region of tc_prims.cuh.
 //
 //   forward, per tensor layer l :  D_c[128 x n_out] = H_c[128 x n_in] * W_l^T        (A, B K-major)
 //   backward, per half and tensor layer l:  Z_c   (recompute, 16 columns per warpgroup) = H_c * W_l^T
@@ -18,6 +18,7 @@
 //                                  Wbar_l^T[n_in x n_out] = sum_c H_c^T * Zbar_c       (A, B MN-major; 16 points per warpgroup)
 //                                  bbar_l[n_out]        = Zbar_0^T * 1                  (B = constant ones atom)
 //   last layer                  :  wbar_L[n]            = sum_c H_c^T * ubar_c          (B = (hi, lo) pairs of ubar)
+//   layer 0, per half           :  [Wbar_0 | bbar_0]^T  = Zbar^0_0^T [x | 1] + sum_j Zbar^0_(1+j)^T E_dir(j)
 //
 // The first (d -> n) and last (n -> 1) layers are tiny and stay on the CUDA cores inside the
 // same epilogues.  Arithmetic modes: PINN_MODE_TC_BF16 (one MMA per product) and
@@ -46,12 +47,11 @@ struct LoopCtx {
   uint32_t tQ;            // shared-memory address of the lo operand tiles (forward split)
   float* gb;              // bias gradient of the current layer (CTA partial)
   float* gw;              // weight gradient of the first layer (CTA partial)
-  uint32_t taddr;         // accumulator address of the warp's row quadrant
   int act, split, p, lane, g0, g1, flag;
   // ng granules of the layer, spread over the kNH warps of the thread's row quadrant
   __device__ __forceinline__ LoopCtx(uint32_t fp_, uint32_t bt_, uint32_t tP_, uint32_t tQ_, const Tid& t, int act_, int ng,
                                      int flag_, int split_ = 0, float* gb_ = nullptr, float* gw_ = nullptr)
-      : fp(fp_), bt(bt_), tP(tP_), tQ(tQ_), gb(gb_), gw(gw_), taddr(t.lane_addr), act(act_), split(split_), p(t.p), lane(t.lane),
+      : fp(fp_), bt(bt_), tP(tP_), tQ(tQ_), gb(gb_), gw(gw_), act(act_), split(split_), p(t.p), lane(t.lane),
         g0(t.hh * (ng / kNH)), g1((t.hh + 1) * (ng / kNH)), flag(flag_) {}
 };
 
@@ -263,6 +263,26 @@ __device__ __forceinline__ void wgrad_mma(float (&dw)[32], float (&db)[8], uint3
   tc::wgmma_wait0();
 }
 
+// layer-0 weight / bias gradient of the half, 16 points (one k-step) per warpgroup, as one m64n16 fragment (row = neuron o
+// of the first layer, column = input k, 8 = the bias): D = Zbar^0_0^T [x_hi | 1] (+ Zbar^0_0^T [x_lo | 0]) +
+// sum_j Zbar^0_(1+j)^T E_dir(j), in layer0_grad's product order.  Per channel tile of Q: the Zbar half holds Zbar^0_c
+// (c <= N1, MN-major, M = the 64 neurons), the H half the coordinate tile of the same index (coord_row; the x_lo tile at
+// 1 + N1 when N2 > 0).
+template <int N1, int N2>
+__device__ __forceinline__ void l0_mma(float (&d)[8], uint32_t sQ) {
+  const uint32_t poff = (threadIdx.x >> 7) * 16u * 128u;
+  const uint64_t dz0 = tc::make_desc(sQ + kHalfBytes + poff, 0, 1024);
+  tc::wgmma_fence();
+  tc::wgmma_n16<1, 1>(d, dz0, tc::make_desc(sQ + poff, 0, 1024), 0u);
+  if (N2 > 0) tc::wgmma_n16<1, 1>(d, dz0, tc::make_desc(sQ + (1 + N1) * kTileBytes + poff, 0, 1024), 1u);
+#pragma unroll
+  for (int j = 0; j < N1; ++j)
+    tc::wgmma_n16<1, 1>(d, tc::make_desc(sQ + (1 + j) * kTileBytes + kHalfBytes + poff, 0, 1024),
+                        tc::make_desc(sQ + (1 + j) * kTileBytes + poff, 0, 1024), 1u);
+  tc::wgmma_commit();
+  tc::wgmma_wait0();
+}
+
 // Hbar of the half in P: element (channel c, input column k, point p of the half) at hb_idx.  The point index is XORed in its
 // bits 3-4 with two bits of k, so that the dgrad fragment stores (8-byte pairs of points, rows k of a quad) and the epilogue
 // loads (8 consecutive points x 4 columns k = 8 m + 2 j (+1)) both touch 32 distinct banks.
@@ -278,20 +298,6 @@ __device__ __forceinline__ void hbar_store(float* hbar, const float (&d)[C][8]) 
     for (int i = 0; i < 8; i += 2) {
       const int k = 16 * w + (lane >> 2) + 8 * ((i >> 1) & 1), p = 16 * wg + 8 * (i >> 2) + 2 * (lane & 3);
       *reinterpret_cast<float2*>(hbar + hb_idx(c, k, p)) = make_float2(d[c][i], d[c][i + 1]);
-    }
-}
-
-// store the dgrad fragments of the lowest tensor layer as Hbar^0 of points 64 h .. 64 h + 63 in accumulator columns X (row =
-// point of the tile), where the layer-0 reverse of the whole tile reads them once both halves are done
-template <int C>
-__device__ __forceinline__ void hbar0_store(float* hand, const float (&d)[C][8], int h) {
-  const int wg = threadIdx.x >> 7, w = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
-#pragma unroll
-  for (int c = 0; c < C; ++c)
-#pragma unroll
-    for (int i = 0; i < 8; i += 2) {
-      const int k = 16 * w + (lane >> 2) + 8 * ((i >> 1) & 1), p = 64 * h + 16 * wg + 8 * (i >> 2) + 2 * (lane & 3);
-      *reinterpret_cast<float2*>(hand + (c * 64 + k) * kAccRows + p) = make_float2(d[c][i], d[c][i + 1]);
     }
 }
 
@@ -349,20 +355,21 @@ __device__ __forceinline__ void tl_bwd_frag(const float (&d)[C][8], const LoopCt
   }
 }
 
-// layer 0 backward, tensor-core variant: adjoints of H^0 (accumulator columns X, row = point) -> Zbar^0 tiles (value +
-// first-derivative channels; bf16 hi) in P.  The weight / bias gradient is then one small MMA chain against the augmented
-// coordinate tiles (see net_backward), so no cross-lane reductions are needed here.
+// layer 0 backward of a half, tensor-core variant: the half's Hbar^0 in P (layout hb_idx) -> Zbar^0 (value + first-derivative
+// channels; bf16 hi) in the Zbar half of Q's channel tiles, row = point of the half.  The thread takes point lc.p of the half
+// and granules [lc.g0, lc.g1).  The weight / bias gradient is then one small MMA against the augmented coordinate tiles
+// (l0_mma), so no cross-lane reductions are needed here.
 template <int N1, int N2, bool PURE, int AK>
-__device__ __forceinline__ void l0_bwd_store_loop(const LoopCtx lc, const PassInfo<N1, N2> pi, const float* xp) {
+__device__ __forceinline__ void l0_bwd_store_loop(const LoopCtx lc, const PassInfo<N1, N2> pi, const float (&x)[PINN_MAX_IN],
+                                                  const float* hbar) {
   constexpr int C = 1 + N1 + N2;
-  float x[PINN_MAX_IN];
-#pragma unroll
-  for (int k = 0; k < PINN_MAX_IN; ++k) x[k] = xp[k];
 #pragma unroll 1
   for (int g = lc.g0; g < lc.g1; ++g) {
     float hb[C][GWB];
 #pragma unroll
-    for (int c = 0; c < C; ++c) acc_ldg(lc.taddr + TM_X + c * 64 + g * GWB, hb[c]);
+    for (int c = 0; c < C; ++c)
+#pragma unroll
+      for (int i = 0; i < GWB; ++i) hb[c][i] = hbar[hb_idx(c, g * GWB + i, lc.p)];
 #pragma unroll
     for (int i = 0; i < GWB; i += 2) {
       float za[C], zb2[C];
@@ -376,7 +383,7 @@ __device__ __forceinline__ void l0_bwd_store_loop(const LoopCtx lc, const PassIn
       for (int c = 0; c <= N1; ++c) { hb[c][i] = zv[c].v.x; hb[c][i + 1] = zv[c].v.y; }
     }
 #pragma unroll
-    for (int c = 0; c <= N1; ++c) store_half(lc.tP + c * kTileBytes, lc.tP, lc.p, g * GWB, hb[c], false);
+    for (int c = 0; c <= N1; ++c) store_half(lc.tQ + c * kTileBytes + kHalfBytes, lc.tQ, lc.p, g * GWB, hb[c], false);
   }
 }
 
@@ -435,6 +442,54 @@ __device__ __forceinline__ void l0_bwd_loop(const LoopCtx lc, const PassInfo<N1,
   }
 }
 
+// layer 0 of the reverse sweep for half h (points 64 h .. 64 h + 63) of a network with tensor layers, on the half's Hbar^0 in
+// P (layout hb_idx): the augmented-coordinate tiles go to the H halves of Q (no layer below reloads it) -> barrier -> Zbar^0 by
+// the CUDA cores into the Zbar halves of Q -> barrier -> l0_mma, whose per-warpgroup fragments go to P -> barrier -> each
+// element of W_0 / b_0 is summed in warpgroup order by one thread, which adds it to the CTA partial (as for the tensor layers).
+// A call of its own: inlined into net_backward, the step faulted on the H100 when CUDA 12.9 built it with every dispatch
+// instantiation in the unit (built for fewer instantiations, the same code ran correctly).  CTA-wide.
+template <int N1, int N2, bool PURE, int AK>
+__device__ __noinline__ void l0_half(uint32_t fpa, uint8_t* tP, uint8_t* tQ, int act0, const PassInfo<N1, N2> pi, const float* xs,
+                                     const int* rows, int h, float* gw0, float* gb0) {
+  const Tid t = tid_of();
+  const int tid = t.tid, wg = tid >> 7;
+  const uint32_t sP = tc::smem_u32(tP), sQ = tc::smem_u32(tQ);
+  const float* hbar = reinterpret_cast<const float*>(tP);     // [c][k][point] (hb_idx)
+  float* lpart = reinterpret_cast<float*>(tP);                // [wg][o][16] (column k of W_0, 8 = b_0)
+  {
+    // the thread's point of the half, and an eighth of the layer's granules (n1w is a multiple of 16)
+    const int pl = 32 * (t.warp & 1) + t.lane, ng = pi.n1w / (8 * GWB);
+    float x[PINN_MAX_IN];
+#pragma unroll
+    for (int k = 0; k < PINN_MAX_IN; ++k) x[k] = (k < pi.d_in) ? xs[rows[k] * kTcPts + 64 * h + pl] : 0.f;
+    // coordinate tiles 0 .. N1 (and 1 + N1, the lo of x, when N2 > 0: C >= 2 + N1 tiles) in the H halves of Q
+    if (tid < 64) coord_row<N1>(sQ, pl, x, pi.dir1, N2 > 0);
+    __syncthreads();   // Hbar^0 of the half is in P
+    LoopCtx lc(fpa, fpa, sP, sQ, t, act0, 0, 0);
+    lc.p = pl;
+    lc.g0 = (t.warp >> 1) * ng;
+    lc.g1 = lc.g0 + ng;
+    l0_bwd_store_loop<N1, N2, PURE, AK>(lc, pi, x, hbar);
+  }
+  tc::fence_async_smem();   // Zbar^0 and the coordinate tiles (generic-proxy stores to Q) -> l0_mma
+  __syncthreads();
+  {
+    float d[8];
+    l0_mma<N1, N2>(d, sQ);
+    frag_store_rows(lpart + wg * 64 * 16, 16, d);   // Zbar^0 has read Hbar^0 in P
+  }
+  __syncthreads();
+  const int n1w = pi.n1w, d_in = pi.d_in;
+#pragma unroll 1
+  for (int e = tid; e < 64 * 16; e += kTcThreads) {
+    const int o = e >> 4, k = e & 15;
+    if (o < n1w && (k < d_in || k == 8)) {
+      float* g = (k == 8) ? gb0 + o : gw0 + o + (long long)n1w * k;
+      *g += ((lpart[e] + lpart[1024 + e]) + lpart[2048 + e]) + lpart[3072 + e];
+    }
+  }
+}
+
 // ---------------------------------------------------------------------------------------------------
 // forward of one network for the current tile, channel structure <N1, N2, PURE>.
 // `phase` bit 1 = parity of the bulk-load barrier (bit 0 unused); returned updated.
@@ -452,7 +507,6 @@ __device__ __noinline__ uint32_t net_forward(CtaShared* cs, const DevProblem* Pp
   uint8_t* tP = smem + cs->off_P;
   uint8_t* tQ = smem + cs->off_Q;
   const Misc ms = misc_of(smem + cs->off_misc, cs->mx_dim, cs->mx_taps);
-  const uint32_t accm = 0;   // accumulator address of row 0, column 0
   const bool split = cs->split != 0;
   PassInfo<N1, N2> pi;
   load_pass<N1, N2>(pi, net, dc);
@@ -523,18 +577,15 @@ __device__ __noinline__ uint32_t net_backward(CtaShared* cs, const DevProblem* P
   uint8_t* tP = smem + cs->off_P;
   uint8_t* tQ = smem + cs->off_Q;
   const Misc ms = misc_of(smem + cs->off_misc, cs->mx_dim, cs->mx_taps);
-  const uint32_t accm = 0;   // accumulator address of row 0, column 0
   float* partial = cs->partial;
   PassInfo<N1, N2> pi;
   load_pass<N1, N2>(pi, net, dc);
   const int L = pi.L, TL = pi.TL;
   const Tid t = tid_of();
-  const int tid = t.tid, p = t.p;
+  const int tid = t.tid, p = t.p, wg = tid >> 7;
   uint32_t ld_phase = (phase >> 1) & 1u;
-  float x[PINN_MAX_IN];
-#pragma unroll
-  for (int k = 0; k < PINN_MAX_IN; ++k) x[k] = (k < pi.d_in) ? ms.Xs[dc.rows[k] * kTcPts + p] : 0.f;
   uint8_t* stash_slot = cs->stash + (size_t)slot * cs->tl_max * kTcMaxC * kTileBytes;
+  const uint32_t sP = tc::smem_u32(tP), sQ = tc::smem_u32(tQ);
 
   dbg_mark(cs, 20);
   float ub[C];
@@ -545,10 +596,8 @@ __device__ __noinline__ uint32_t net_backward(CtaShared* cs, const DevProblem* P
     for (int c = 0; c < C; ++c) ms.scratch[c * kTcPts + p] = ub[c];
   }
   // ---- last layer: the ubar tile goes to Q, the products into accumulator columns Y ----------------------------------------
-  last_layer_grad<C>(t, ub, pi.nL, partial + net.w_off[L - 1], partial + net.b_off[L - 1], tc::smem_u32(tQ), tc::smem_u32(tP),
-                     kTileBytes, 0u, accm + TM_Y, kTcW);
+  last_layer_grad<C>(t, ub, pi.nL, partial + net.w_off[L - 1], partial + net.b_off[L - 1], sQ, sP, kTileBytes, 0u, TM_Y, kTcW);
 
-  const uint32_t sP = tc::smem_u32(tP), sQ = tc::smem_u32(tQ);
   const int act0 = net.acts[0];
   float* gb0 = partial + net.b_off[0];
   float* gw0 = partial + net.w_off[0];
@@ -556,24 +605,26 @@ __device__ __noinline__ uint32_t net_backward(CtaShared* cs, const DevProblem* P
     // ---- no tensor layer: layer 0 on the CUDA cores (warp reduce-scatter + atomics) -----------------------------------------
     __syncthreads();
     dbg_mark(cs, 29);
+    float x[PINN_MAX_IN];
+#pragma unroll
+    for (int k = 0; k < PINN_MAX_IN; ++k) x[k] = (k < pi.d_in) ? ms.Xs[dc.rows[k] * kTcPts + p] : 0.f;
     const LoopCtx lc(tc::smem_u32(fp), tc::smem_u32(fp), sP, sQ, t, act0, pi.n1w / GW, 1, 0, gb0, gw0);
     l0_bwd_loop<N1, N2, PURE, AK>(lc, pi, x, ub);
   }
 
-  // ---- tensor layers, last to first: one 64-point half of the tile after the other --------------------------------------------
+  // ---- tensor layers, last to first, then layer 0: one 64-point half of the tile after the other -------------------------------
   // Per layer: the stash reload of the half's H^{l-1} in Q has landed -> recompute -> barrier (the half's Hbar^l in P is
   // complete) -> Zbar epilogue into Q -> barrier -> wgrad, whose four per-warpgroup partials of Wbar_l^T go to the first four
   // tiles of P (plan.cu gives P at least four: every epilogue has read Hbar^l), then dgrad, whose fragments stay in registers
   // -> barrier (every MMA has read Q) -> the bias partials go to the Zbar half of Q's first tile and the reload of H^{l-2}
   // to Q -> barrier -> each gradient element is summed in warpgroup order by one thread, which adds it to the CTA partial
   // (half 0 before half 1, so the result does not depend on scheduling) -> barrier -> the dgrad fragments become Hbar^{l-1}
-  // in P (the lowest layer's, Hbar^0, go to accumulator columns X for layer 0 of the whole tile).  Generic-proxy stores to P and Q after async-proxy reads that have completed need no proxy fence; the fence before
+  // in P.  Generic-proxy stores to P and Q after async-proxy reads that have completed need no proxy fence; the fence before
   // the MMAs orders the Zbar stores before them.
-  const int wg = tid >> 7;
+  // Then layer 0 of the half (l0_half).
   float* hbar = reinterpret_cast<float*>(tP);                 // [c][k][point] (hb_idx), C x 16 KB
   float* wpart = reinterpret_cast<float*>(tP);                // [wg][k][o] (4 x 64 x 64)
   float* bpart = reinterpret_cast<float*>(tQ + kHalfBytes);   // [wg][o]
-  float* hand = tc::s_acc + TM_X * kAccRows;                  // Hbar^0 of the tile, [c][k][point]
 #pragma unroll 1
   for (int h = 0; h < (TL > 0 ? 2 : 0); ++h) {
     for (int l = TL; l >= 1; --l) {
@@ -586,7 +637,7 @@ __device__ __noinline__ uint32_t net_backward(CtaShared* cs, const DevProblem* P
       dbg_mark(cs, 21);
       if (tid == 0 && l == TL) {
         // reload the half's rows of this layer's input tiles H^{l-1} (bf16 hi) from the stash into Q: the MMAs that read Q
-        // before (last_layer_grad's ubar tile, the previous half's layer 0) have been waited for.  The layers below are
+        // before (last_layer_grad's ubar tile, the previous half's l0_mma) have been waited for.  The layers below are
         // reloaded by the layer above them.
         const uint8_t* src = stash_slot + (size_t)(l - 1) * kTcMaxC * kTileBytes + h * kHalfBytes;
         tc::mbar_arrive_expect_tx(ms.bar_ld, C * kHalfBytes);
@@ -655,20 +706,12 @@ __device__ __noinline__ uint32_t net_backward(CtaShared* cs, const DevProblem* P
       }
       if (tid < n_out) gb[tid] += ((bpart[tid] + bpart[64 + tid]) + bpart[128 + tid]) + bpart[192 + tid];
       __syncthreads();   // the sum has read P
-      if (l > 1) hbar_store<C>(hbar, d);
-      else hbar0_store<C>(hand, d, h);
+      hbar_store<C>(hbar, d);
     }
-  }
-  if (TL > 0) {
-    // ---- layer 0 of the whole tile: Zbar^0 by the CUDA cores into P, the weight / bias gradient by MMA (layer0_grad) -------
-    // (the coordinate tiles live in Q, which is free after the last tensor layer, and the channel count leaves a spare tile
-    // for the lo of x when N2 > 0)
-    __syncthreads();   // Hbar^0 of both halves is in accumulator columns X, the last gradient sum has read P
+    // ---- layer 0 of the half -------------------------------------------------------------------------------------------------
     dbg_mark(cs, 29);
-    coord_tiles<N1>(t, sQ, x, pi.dir1, N2 > 0);
-    const LoopCtx lc(tc::smem_u32(fp), tc::smem_u32(fp), sP, sQ, t, act0, pi.n1w / GWB, 0);
-    l0_bwd_store_loop<N1, N2, PURE, AK>(lc, pi, x);
-    layer0_grad<N1>(t, sP, kTileBytes, 0u, sQ, N2 > 0, accm + TM_Y, kTcW, pi.n1w, pi.d_in, gw0, gb0);
+    l0_half<N1, N2, PURE, AK>(tc::smem_u32(fp), tP, tQ, act0, pi, ms.Xs, dc.rows, h, gw0, gb0);
+    // the next half's first P store (the top layer's wgrad partials) follows two barriers: the sum above has read P by then
   }
 
   __syncthreads();
