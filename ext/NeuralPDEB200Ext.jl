@@ -22,7 +22,7 @@ const PINN_F32, PINN_F64 = Cint(0), Cint(1)
 const PINN_MODE_FFMA, PINN_MODE_TC_BF16, PINN_MODE_TC_SPLIT, PINN_MODE_TC_F64 = Cint(0), Cint(1), Cint(2), Cint(3)
 const PINN_REDUCE_MEAN, PINN_REDUCE_WSUM = Cint(0), Cint(1)
 const ACT = Dict(:identity => 0, :tanh => 1, :tanh_fast => 1, :sigmoid => 2, :sigmoid_fast => 2, :σ => 2, :sin => 3,
-                 :softplus => 4, :swish => 5, :logcosh => 7)
+                 :softplus => 4, :swish => 5, :logcosh => 7, :cos => 8)
 const OPC = Dict(:const => 0, :coord => 1, :tap => 2, :param => 3, :add => 4, :sub => 5, :mul => 6, :div => 7, :neg => 8,
                  :pow => 9, :powi => 10, :sin => 11, :cos => 12, :exp => 13, :log => 14, :tanh => 15, :sqrt => 16, :abs => 17)
 

@@ -104,8 +104,9 @@ enum {
   PINN_ACT_SWISH = 5,
   PINN_ACT_GELU = 6,       /* NNlib's gelu, tanh form: x/2 (1 + tanh(sqrt(2/pi) (x + 0.044715 x^3))); FFMA kernel
                             * (PINN_MODE_FFMA, PINN_MODE_TC_F64) only */
-  PINN_ACT_LOGCOSH = 7     /* NNlib's logcosh: x + softplus(-2x) - log 2; FFMA kernel (PINN_MODE_FFMA,
+  PINN_ACT_LOGCOSH = 7,    /* NNlib's logcosh: x + softplus(-2x) - log 2; FFMA kernel (PINN_MODE_FFMA,
                             * PINN_MODE_TC_F64) only */
+  PINN_ACT_COS = 8         /* cos x; FFMA kernel (PINN_MODE_FFMA, PINN_MODE_TC_F64) only */
 };
 
 /* residual-program opcodes.  The program is in SSA form: instruction i defines

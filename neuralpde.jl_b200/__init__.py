@@ -24,5 +24,6 @@ from .ode import NNODE, NNODERepresentation, ODEFunction, ODEProblem, ODESolutio
 from .bpinn_ode import BNNODE, BNNODELogDensity, ahmc_bayesian_pinn_ode
 from .sde import NNSDE, NNSDERepresentation, SDEProblem, SDEsol
 from .sde_weak import SDEPINN
+from .dae import DAEFunction, DAEProblem, DAESolution, NNDAE, NNDAERepresentation
 
 __all__ = [n for n in dir() if not n.startswith("_")]

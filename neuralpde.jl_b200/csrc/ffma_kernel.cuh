@@ -104,14 +104,20 @@ __device__ __forceinline__ void logcosh_eval4(real z, real& a, real& d1, real& d
 }
 
 // activation value and its first four derivatives at z (the fourth enters the reverse sweep through third-derivative taps).
-// kFfmaOnly = false (the tensor-core kernels, which refuse gelu and logcosh layers) leaves those two out, so their code
-// stays as it was
+// kFfmaOnly = false (the tensor-core kernels, which refuse gelu, logcosh and cos layers) leaves those three out, so their
+// code stays as it was
 template <typename real, bool kFfmaOnly = true>
 __device__ __forceinline__ void act_eval4(int act, real z, real& a, real& d1, real& d2, real& d3, real& d4) {
   if constexpr (kFfmaOnly) {
     if (act >= PINN_ACT_GELU) {     // one compare on the common path, as with gelu alone
-      if (act == PINN_ACT_GELU) gelu_eval4<real>(z, a, d1, d2, d3, d4);
-      else logcosh_eval4<real>(z, a, d1, d2, d3, d4);
+      if (act == PINN_ACT_GELU) {
+        gelu_eval4<real>(z, a, d1, d2, d3, d4);
+      } else if (act == PINN_ACT_LOGCOSH) {
+        logcosh_eval4<real>(z, a, d1, d2, d3, d4);
+      } else {
+        const real s = m_sin(z), c = m_cos(z);
+        a = c; d1 = -s; d2 = -c; d3 = s; d4 = c;
+      }
       return;
     }
   }

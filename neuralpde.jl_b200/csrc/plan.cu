@@ -37,7 +37,7 @@ long long plan_net(const char* what, int k, int n_layers, const int32_t* dims, c
   }
   if (n.dims[0] > PINN_MAX_IN) return fail("pinn_create: %s %d input dimension %d > %d", what, k, n.dims[0], PINN_MAX_IN), -1;
   for (int l = 0; l < n_layers; ++l) {
-    if (acts[l] < PINN_ACT_IDENTITY || acts[l] > PINN_ACT_LOGCOSH)
+    if (acts[l] < PINN_ACT_IDENTITY || acts[l] > PINN_ACT_COS)
       return fail("pinn_create: %s %d layer %d unknown activation %d", what, k, l, acts[l]), -1;
     n.acts[l] = acts[l];
     n.w_off[l] = off; off += (long long)n.dims[l] * n.dims[l + 1];
@@ -431,9 +431,10 @@ int check_tc_nets(const pinn_problem_desc* d, const DevProblem& P, Plan& p, int&
     if (n.acts[n.n_layers - 1] != PINN_ACT_IDENTITY)
       return fail("pinn_create(tc): net %d: the last layer must be linear (identity activation)", k);
     for (int l = 0; l < n.n_layers; ++l)
-      if (n.acts[l] == PINN_ACT_GELU || n.acts[l] == PINN_ACT_LOGCOSH)
+      if (n.acts[l] == PINN_ACT_GELU || n.acts[l] == PINN_ACT_LOGCOSH || n.acts[l] == PINN_ACT_COS)
         return fail("pinn_create(tc): net %d layer %d: %s layers run on the FFMA path (PINN_MODE_FFMA, or "
-                    "PINN_MODE_TC_F64 for Float64)", k, l, n.acts[l] == PINN_ACT_GELU ? "gelu" : "logcosh");
+                    "PINN_MODE_TC_F64 for Float64)", k, l,
+                    n.acts[l] == PINN_ACT_GELU ? "gelu" : n.acts[l] == PINN_ACT_LOGCOSH ? "logcosh" : "cos");
     for (int l = 1; l < n.n_layers; ++l) {
       if (n.dims[l] > 64) wide = true;
       if (n.dims[l] == 192 || n.dims[l] == 256) x256 = true;

@@ -35,7 +35,7 @@ __device__ __forceinline__ void add_at(float* v, int idx, float x) {
 
 // activation value and first three derivatives.  AK = 1: tanh, 2: sigmoid (branch-free, built on
 // ex2.approx + rcp.approx: absolute error ~1e-7, far below the bf16-split operand noise);
-// AK = 0: any activation through the accurate generic evaluator (gelu and logcosh excepted: check_tc_nets
+// AK = 0: any activation through the accurate generic evaluator (gelu, logcosh and cos excepted: check_tc_nets
 // refuses them).
 template <int AK>
 __device__ __forceinline__ void act_eval_tc(int act, float z, float& a, float& d1, float& d2, float& d3) {

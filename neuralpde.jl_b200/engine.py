@@ -25,7 +25,8 @@ F32, F64 = 0, 1
 # TC_SPLIT (hidden widths up to 64), TC_F64 (FFMA's shapes, fp64 only, layer products on DMMA); include/pinn_b200.h lists
 # the shapes each tensor-core mode accepts
 MODE_FFMA, MODE_TC_BF16, MODE_TC_SPLIT, MODE_TC_F64 = 0, 1, 2, 3
-ACT = {"identity": 0, "tanh": 1, "sigmoid": 2, "sin": 3, "softplus": 4, "swish": 5, "gelu": 6, "logcosh": 7}
+ACT = {"identity": 0, "tanh": 1, "sigmoid": 2, "sin": 3, "softplus": 4, "swish": 5, "gelu": 6, "logcosh": 7,
+       "cos": 8}
 OP = {
     "const": 0, "coord": 1, "tap": 2, "param": 3, "add": 4, "sub": 5, "mul": 6, "div": 7, "neg": 8,
     "pow": 9, "powi": 10, "sin": 11, "cos": 12, "exp": 13, "log": 14, "tanh": 15, "sqrt": 16, "abs": 17,

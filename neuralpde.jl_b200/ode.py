@@ -39,12 +39,13 @@ class ODEFunction:
 
 
 class _TrialProblem:
-    """What ODEProblem and SDEProblem share: the checks of their fields, ``scalar``, and the name and out-of-place
-    message of the solver that traces their functions of (u, p, t)"""
+    """What ODEProblem, SDEProblem and DAEProblem share: the checks of their fields, ``scalar``, and the name and
+    out-of-place message of the solver that traces their functions of (u, p, t) (DAEProblem: (du, u, p, t))"""
     _solver = "NNODE"
     _out_of_place = "The NNODE solver only supports out-of-place ODE definitions, i.e. du=f(u,p,t)."
     _components_note = ""      # appended to the component-count refusal
     _traced = ("f",)           # the functions of (u, p, t) the solver traces
+    _inplace_args = 4          # the argument count of an in-place function: f(du, u, p, t)
 
     def __post_init__(self):
         if not isinstance(self.f, ODEFunction):
@@ -55,8 +56,8 @@ class _TrialProblem:
             try:
                 n_args = len(inspect.signature(self._function(name)).parameters)
             except (TypeError, ValueError):
-                n_args = 3
-            if n_args == 4:
+                n_args = self._inplace_args - 1
+            if n_args == self._inplace_args:
                 raise ValueError(self._out_of_place)
         self.tspan = (float(self.tspan[0]), float(self.tspan[1]))
 
@@ -66,6 +67,9 @@ class _TrialProblem:
     @property
     def scalar(self) -> bool:
         return np.ndim(self.u0) == 0
+
+    def _analytic(self, t: float):
+        return self.f.analytic(self.u0, self.p, t)
 
 
 @dataclass
@@ -176,15 +180,20 @@ class _Lowering:
         else:
             self.p_arg, self.param_index = prob.p, {}
 
-    def _trace(self, name: str, comps: List[sp.Expr]) -> List[sp.Expr]:
+    def _trace(self, name: str, comps: List[sp.Expr], du: Optional[List[sp.Expr]] = None) -> List[sp.Expr]:
         """the problem's function `name` (f or g) of (u, p, t) at u = comps, with symbols: one expression per
-        component"""
+        component.  With `du`, f is a DAE residual f(du, u, p, t), and du and u are lists even for a scalar u0."""
         who = self.prob._solver
         try:
-            out = self.prob._function(name)(comps[0] if self.prob.scalar else list(comps), self.p_arg, T_SYM)
+            fn = self.prob._function(name)
+            if du is not None:
+                out = fn(list(du), list(comps), self.p_arg, T_SYM)
+            else:
+                out = fn(comps[0] if self.prob.scalar else list(comps), self.p_arg, T_SYM)
         except Exception as ex:      # noqa: BLE001 -- any failure to trace is the user's function, reported with its message
-            raise ValueError("%s: %s(u, p, t) could not be traced with symbolic u, p and t (write it with sympy "
-                             "functions such as sympy.cos): %s: %s" % (who, name, type(ex).__name__, ex)) from ex
+            args = "u, p" if du is None else "du, u, p"
+            raise ValueError("%s: %s(%s, t) could not be traced with symbolic %s and t (write it with sympy functions "
+                             "such as sympy.cos): %s: %s" % (who, name, args, args, type(ex).__name__, ex)) from ex
         if out is None:
             raise ValueError(self.prob._out_of_place)
         outs = list(np.ravel(np.asarray(out, dtype=object)))      # a number, or a sequence of one for a scalar u0
@@ -469,12 +478,13 @@ class NNODERepresentation(_TrialRepresentation):
 
 
 def _analytic_errors(prob: _TrialProblem, ts: np.ndarray, U: np.ndarray) -> dict:
-    """SciMLBase's timeseries errors of the (n, len(ts)) values U against prob.f.analytic: the final, maximum and
-    root-mean-square errors; empty without an analytic solution"""
+    """SciMLBase's timeseries errors of the (n, len(ts)) values U against prob.f.analytic (``analytic(u0, p, t)``;
+    DAEProblem: ``analytic(du0, u0, p, t)``): the final, maximum and root-mean-square errors; empty without an analytic
+    solution"""
     an = prob.f.analytic
     if an is None:
         return {}
-    A = np.stack([np.ravel(np.asarray(an(prob.u0, prob.p, float(ti)), dtype=np.float64)) for ti in ts], axis=1)
+    A = np.stack([np.ravel(np.asarray(prob._analytic(float(ti)), dtype=np.float64)) for ti in ts], axis=1)
     E = U - A
     return {"final": float(np.mean(np.abs(E[:, -1]))), "l∞": float(np.max(np.abs(E))),
             "l2": float(np.sqrt(np.mean(E ** 2)))}

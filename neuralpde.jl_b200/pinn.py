@@ -28,7 +28,7 @@ MODES = {"ffma": _eng.MODE_FFMA, "tc_bf16": _eng.MODE_TC_BF16, "tc_split": _eng.
 FFMA_KERNEL_MODES = (_eng.MODE_FFMA, _eng.MODE_TC_F64)
 
 _ACT_NAMES = {"identity": "identity", "tanh": "tanh", "sigmoid": "sigmoid", "σ": "sigmoid", "sin": "sin",
-              "softplus": "softplus", "swish": "swish", "gelu": "gelu", "logcosh": "logcosh",
+              "softplus": "softplus", "swish": "swish", "gelu": "gelu", "logcosh": "logcosh", "cos": "cos",
               None: "identity"}
 
 
@@ -1192,8 +1192,11 @@ def solve(prob: OptimizationProblem, opt: Union[Adam, LBFGS, BFGS], maxiters: in
     keywords of ``ode.solve``.  ``solve(prob::ODEProblem, alg::BNNODE; saveat)`` samples the Bayesian ODE posterior
     (bpinn_ode.py) and returns a BPINNsolution.  ``solve(prob::SDEProblem, alg::NNSDE; maxiters, dt, abstol, saveat,
     ...)`` trains an NNSDE (sde.py) and returns an SDEsol.  ``solve(prob::SDEProblem, alg::SDEPINN; maxiters = 200,
-    verbose)`` trains the density of the SDE's Fokker-Planck equation (sde_weak.py) and returns ``(res, phi)``."""
+    verbose)`` trains the density of the SDE's Fokker-Planck equation (sde_weak.py) and returns ``(res, phi)``.
+    ``solve(prob::DAEProblem, alg::NNDAE; maxiters, dt, abstol, saveat, ...)`` trains an NNDAE (dae.py) and returns a
+    DAESolution."""
     from .bpinn_ode import BNNODE, solve_bnnode
+    from .dae import DAEProblem, solve_nndae
     from .ode import ODEProblem, solve_nnode
     from .sde import SDEProblem, solve_nnsde
     from .sde_weak import SDEPINN, solve_sdepinn
@@ -1201,6 +1204,12 @@ def solve(prob: OptimizationProblem, opt: Union[Adam, LBFGS, BFGS], maxiters: in
         if callback is not None or chunk != 50 or device_loop:
             raise TypeError("solve(::SDEProblem, ::SDEPINN) takes no callback, chunk or device_loop")
         return solve_sdepinn(prob, opt, maxiters=200 if maxiters is _MAXITERS_DEFAULT else maxiters, **ode_kwargs)
+    if isinstance(prob, DAEProblem):
+        if callback is not None or chunk != 50:
+            raise TypeError("solve(::DAEProblem, ::NNDAE) takes no callback or chunk: it stops at abstol")
+        if maxiters is _MAXITERS_DEFAULT:
+            raise TypeError("solve(::DAEProblem, ::NNDAE) needs maxiters")
+        return solve_nndae(prob, opt, maxiters=maxiters, device_loop=device_loop, **ode_kwargs)
     if isinstance(prob, SDEProblem):
         if callback is not None or chunk != 50:
             raise TypeError("solve(::SDEProblem, ::NNSDE) takes no callback or chunk: it stops at abstol")
